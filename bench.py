@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — 1080p frames/sec of the Motion (Laplace, 6-level) hot path on N B200s.
+"""bench.py — 1080p frames/sec of the Motion (Laplace, 6-level) hot path on N H100s.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
   (N>1: launched by torchrun, one rank per GPU, NCCL; weak scaling — every rank serves its own
    `lanes` independent streams; the only collective on the data path is a one-time broadcast of the
    parameter block.)
@@ -11,7 +11,8 @@ lane-batched kernels).  `value` = frames/s with frames resident in HBM; `e2e` = 
 through the public host API (pinned host frames in, pinned host frames out, copies inside the
 timed region).  `--impl reference` times the reference's own CPU implementation of the path (its sources
 compiled in place into oracle/_ref, OpenCV kernels through cv2, all host threads; the oracle restatement if that
-module is absent) on the same workload.
+module is absent) on the same workload.  `--dump-outputs DIR` writes the frames the last timed step produced
+(float32 .npy, a fixed seeded sample when the whole batch exceeds DUMP_MAX_ELEMS) so two builds can be compared.
 """
 import argparse
 import ctypes as C
@@ -55,7 +56,7 @@ def measured_peaks():
             return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -259,8 +260,7 @@ def run_reference(args, rank, world):
 
 
 def kernel_table(prof, lanes, band_from_state=False):
-    """prof: {(kernel name, level): (launches, total ms)} from mc_profile_read -> (per-kernel table sorted by time share,
-    {kernel: ncu DRAM bytes per launch scaled to `lanes`} from profiles/traffic.json for captures that still apply)."""
+    """prof: {(kernel name, level): (launches, total ms)} from mc_profile_read -> per-kernel table sorted by time share."""
     px = level_pixels(W, H, LEVELS)
     total_ms = sum(v[1] for v in prof.values())
     table = []
@@ -295,18 +295,27 @@ def kernel_table(prof, lanes, band_from_state=False):
         table.append({"kernel": f"{name}[{lvl}]", "us_per_launch": us, "share": tms / total_ms,
                       "algorithmic_GBps": alg / (us * 1e-6) / 1e9, "interface_GBps": io / (us * 1e-6) / 1e9,
                       "interface_bytes": io})
-    # DRAM bytes per launch from the committed `ncu --set full` captures (profiles/traffic.json).  A capture only
-    # speaks for the kernel it was taken on: entries whose recorded interface model no longer matches the current
-    # kernel (e.g. after the band stopped being stored) are dropped -> traffic null until re-captured.
-    traffic = {}
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        model = {t["kernel"]: t["interface_bytes"] / lanes for t in table}
-        traffic = {k: (v["dram_read_bytes"] + v["dram_write_bytes"]) * lanes / v["lanes"] for k, v in tj.items()
-                   if k in model and abs(v.get("interface_bytes_per_lane", 0) - model[k]) <= 0.01 * model[k]}
-    except Exception:
-        pass
-    return table, traffic
+    return table
+
+
+DUMP_MAX_ELEMS = 8 << 20     # 32 MiB of float32
+
+
+def dump_outputs(out_dir, out_d):
+    """The u8 frames [lanes][H][W][3] of the last timed step as float32: all of them as frames.npy when they fit in
+    DUMP_MAX_ELEMS, else frames_sample.npy = the elements at DUMP_MAX_ELEMS sorted flat indices drawn with seed 0
+    (the same indices for the same arguments), plus lane 0's top rows in full as lane0_rows.npy."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    flat = out_d.reshape(-1)
+    if flat.numel() <= DUMP_MAX_ELEMS:
+        np.save(os.path.join(out_dir, "frames.npy"), flat.reshape(out_d.shape).float().cpu().numpy())
+        return
+    idx = np.sort(np.random.default_rng(0).integers(0, flat.numel(), DUMP_MAX_ELEMS, dtype=np.int64))
+    sample = flat[torch.from_numpy(idx).to(flat.device)].float().cpu().numpy()
+    np.save(os.path.join(out_dir, "frames_sample.npy"), sample)
+    rows = max(1, min(out_d.shape[1], (DUMP_MAX_ELEMS // 2) // (out_d.shape[2] * out_d.shape[3])))
+    np.save(os.path.join(out_dir, "lane0_rows.npy"), out_d[0, :rows].float().cpu().numpy())
 
 
 def run_ours(args, rank, world, local_rank):
@@ -315,7 +324,7 @@ def run_ours(args, rank, world, local_rank):
     from lvm_b200 import capi
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: the magnification core has no CPU fallback")
+        raise SystemExit("bench.py needs an H100: the magnification core has no CPU fallback")
     torch.cuda.set_device(local_rank)
     dist = None
     if world > 1:
@@ -378,6 +387,8 @@ def run_ours(args, rank, world, local_rank):
     e1.record(stream)
     barrier()
     sampler.window(t_w0, time.time())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out_d)
     ms = max_over_ranks(e0.elapsed_time(e1))
     from lvm_b200.shard import sum_over_ranks
     launches = int(sum_over_ranks(float(proc.launch_count - l0), dist, device="cuda"))
@@ -457,21 +468,21 @@ def run_ours(args, rank, world, local_rank):
             step_dev(3 + i)
         prof = proc.profile_read()
         proc.set_option("profile_kernels", 0)
-        table, traffic = kernel_table(prof, lanes, band_from_state=True)   # the library default
+        table = kernel_table(prof, lanes, band_from_state=True)   # the library default
         dom = table[0]
         fused = next(t for t in table if t["kernel"] == "level[1]")   # the fused Laplace-pyramid + IIR kernel
         roof = {"bound": "hbm", "kernel": dom["kernel"], "achieved": dom["algorithmic_GBps"], "peak": peak,
-                "unit": "GB/s", "frac": dom["algorithmic_GBps"] / peak, "traffic": traffic.get(dom["kernel"]),
+                "unit": "GB/s", "frac": dom["algorithmic_GBps"] / peak,
                 "peak_source": peak_src, "interface_frac": dom["interface_GBps"] / peak,
                 "bound_note": ("the step's largest kernels are the exact OpenCV colour conversions: BGR->Lab ingest is bound by "
-                               "the L1 data pipe (two divergent 32-byte LUT gathers per pixel; ncu: l1tex 82 %, dram 16 %), "
+                               "the L1 data pipe (two divergent 32-byte LUT gathers per pixel), "
                                "Lab->BGR egress by issue slots; their HBM fraction is low by construction.  The HBM-bound "
                                "kernel of the path is the fused per-level pyramid+IIR kernel reported under fused_level_kernel "
                                "(interface_frac = bytes its interface moves / time / peak)"),
                 "fused_level_kernel": {"kernel": "level[1]", "achieved": fused["algorithmic_GBps"],
                                        "frac": fused["algorithmic_GBps"] / peak,
                                        "interface_frac": fused["interface_GBps"] / peak,
-                                       "us_per_launch": fused["us_per_launch"], "traffic": traffic.get("level[1]")},
+                                       "us_per_launch": fused["us_per_launch"]},
                 "frame": {"a_min_bytes": a_min_bytes(W, H, CH, LEVELS),
                           "achieved": a_min_bytes(W, H, CH, LEVELS) * (fps / world) / 1e9,
                           "frac": a_min_bytes(W, H, CH, LEVELS) * (fps / world) / 1e9 / peak},
@@ -501,7 +512,7 @@ def run_ours(args, rank, world, local_rank):
             "config": {"workload": WORKLOAD, "lanes_per_gpu": lanes, "frames_per_step": lanes * world,
                        "clip_frames": T, "options": args.opt,
                        "device_io": "`value` is device-in / device-out (frames resident in HBM, the ceiling a decoder/encoder hand-off would see)",
-                       "l2": f"inputs {T * frame_bytes / 1e6:.0f} MB + per-lane state cycle through > L2 (126 MB); no flush needed"},
+                       "l2": f"inputs {T * frame_bytes / 1e6:.0f} MB + per-lane state cycle through > L2 (50 MB); no flush needed"},
             "e2e": {"value": e2e_fps, "unit": "frames/s", "h2d_bytes_per_step": frame_bytes,
                     "d2h_bytes_per_step": frame_bytes, "pipeline_depth": depth, "numa": numa,
                     "single_stream_blocking": single},
@@ -541,6 +552,8 @@ def main():
     ap.add_argument("--cpu-frames", type=int, default=64)
     ap.add_argument("--ref-frames-per-step", type=int, default=1)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the frames of the last timed step to DIR/*.npy (float32) for output comparison")
     ap.add_argument("--opt", action="append", default=[], help="library option key=value (mc_set_option), repeatable")
     ap.add_argument("--workload", default="1080p6", choices=["1080p6", "4k8"],
                     help="1080p6 = BASELINE.json configs[1] (the headline, default); 4k8 = configs[4]: 3840x2160, 8 levels")

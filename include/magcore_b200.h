@@ -1,5 +1,5 @@
 /*
- * magcore_b200.h — C ABI of the B200-native Eulerian video-magnification core.
+ * magcore_b200.h — C ABI of the H100-native Eulerian video-magnification core.
  *
  * Drop-in boundary: the reference's per-frame hot path sits behind
  *     livim::IProcessor::process(const FrameRef&, const ProcessorConfig&) / reset()
@@ -30,7 +30,7 @@ typedef enum mc_status {
     MC_OK = 0,
     MC_ERR_INVALID = 1,     /* bad argument */
     MC_ERR_CUDA = 2,        /* a CUDA runtime / cuFFT call failed; see mc_last_error() */
-    MC_ERR_NO_DEVICE = 3,   /* no usable sm_100 device: the core has no CPU fallback */
+    MC_ERR_NO_DEVICE = 3,   /* no usable sm_90 device: the core has no CPU fallback */
     MC_ERR_UNSUPPORTED = 4,
     MC_ERR_INTERNAL = 5     /* a C++ exception (std::bad_alloc, ...) was caught at the boundary; the handle's temporal
                                state has been dropped, as after any failed frame; see mc_last_error() */
@@ -118,7 +118,7 @@ mc_status mc_sync(mc_handle* h);
  * Replaces runChainOnce(chain, in, cfg, original) (reference src/processing/ChainBuilder.cpp:19-29) over
  * PreprocessProcessor (ROI crop + INTER_AREA downscale, PreprocessProcessor.cpp:10-51), GrayscaleProcessor
  * (BGR2GRAY, GrayscaleProcessor.cpp:7-16) and MagnificationProcessor: the raw frame is uploaded once, both
- * front stages run bit-exact on the B200, the magnification core runs on their result, and the processed frame
+ * front stages run bit-exact on the H100, the magnification core runs on their result, and the processed frame
  * plus the "original" tap (the pre-magnification frame, ChainBuilder.cpp:25) come back.  lanes must be 1.
  * `out` / `original` are written tight (step = width * channels); the *_is_input flags mirror the reference
  * returning the very same FrameRef (nothing written). */
@@ -163,7 +163,7 @@ void* mc_stream(mc_handle* h);
  *        the 128-bit LDG staging path (same results; kept for A/B measurements)
  *   "prefetch_state" (default 1; needs use_tma): the fused level kernel requests the tile's two state planes as TMA
  *        bulk copies at kernel entry, together with its input window, instead of loading them in its last phase
- *        (same results; measured on B200: level[1] 235 -> 205 us per 32-lane launch; 0 kept for A/B measurements)
+ *        (same results; 0 kept for A/B measurements)
  *   "lane_groups" (default 0 = automatic: min(2, lanes / 8), at least 1): Laplace — the lanes of the handle run as
  *        that many concurrent launch chains on separate CUDA streams, forked from and joined into mc_stream(); the
  *        L1-bound ingest, issue-bound egress and HBM-bound level kernels of different groups then share the SMs
@@ -177,8 +177,7 @@ void* mc_stream(mc_handle* h);
  *        *produced = 0; the cheap first pass of temporal sharding (SURVEY 8f-3)
  *   "band_from_state" (default 1): Laplace synthesis rebuilds each amplified band gain*(hi-lo) from the two
  *        state planes instead of reading a band plane stored by the level kernel (same results; takes 4 B/px off
- *        the level kernel's interface and adds them to the collapse / egress kernels; measured on B200 together
- *        with prefetch_state: level[1] 205 -> 177 us, egress +8 us, step -1.6 %; 0 kept for A/B measurements) */
+ *        the level kernel's interface and adds them to the collapse / egress kernels; 0 kept for A/B measurements) */
 mc_status mc_set_option(mc_handle* h, const char* key, int value);
 
 /* Test-only access to temporal state planes as dense f32 [lanes][channels][rows][cols].

@@ -1,4 +1,4 @@
-// Reference-side adapter: a livim::IProcessor that forwards the magnification stage to the B200 core
+// Reference-side adapter: a livim::IProcessor that forwards the magnification stage to the H100 core
 // through the C ABI (include/magcore_b200.h).  It is the ONLY file the reference application needs:
 //
 //     // src/processing/ChainBuilder.cpp:15

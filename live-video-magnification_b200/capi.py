@@ -1,5 +1,5 @@
 """ctypes binding of include/magcore_b200.h (libmagcore_b200.so, built in-tree by
-__graft_entry__.build()).  There is no CPU fallback: if the library is missing or no B200 is
+__graft_entry__.build()).  There is no CPU fallback: if the library is missing or no H100 is
 visible, constructing a processor raises."""
 from __future__ import annotations
 
@@ -77,7 +77,7 @@ def lib() -> C.CDLL:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). There is no CPU fallback for the magnification core.")
+                "(nvcc, sm_90a). There is no CPU fallback for the magnification core.")
         l = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(l, name)

@@ -244,7 +244,7 @@ __global__ void k_color_egress(const float* __restrict__ a, const float* __restr
 inline unsigned cdiv(int a, int b) { return (unsigned)((a + b - 1) / b); }
 inline unsigned gs_blocks(size_t n) {
     size_t b = (n + 255) / 256;
-    return (unsigned)(b < 1 ? 1 : (b > 148 * 16 ? 148 * 16 : b));
+    return (unsigned)(b < 1 ? 1 : (b > 132 * 16 ? 132 * 16 : b));
 }
 
 }  // namespace

@@ -1,4 +1,4 @@
-// The handle behind the C ABI: a B200-resident twin of livim::MagnificationProcessor
+// The handle behind the C ABI: an H100-resident twin of livim::MagnificationProcessor
 // (reference src/processing/MagnificationProcessor.cpp:10-67) — level clamp, structural reset,
 // mode dispatch, passthrough decisions — plus device memory, streams and the pinned pipeline.
 #include <algorithm>
@@ -343,9 +343,9 @@ mc_status mc_create_lanes(int device, int lanes, mc_handle** out) try {
         return MC_ERR_NO_DEVICE;
     }
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major < 10) {
+    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 9) {
         cudaGetLastError();
-        g_create_error = "device is not sm_100-class; kernels are built for sm_100a only";
+        g_create_error = "device is not sm_90-class; kernels are built for sm_90a only";
         return MC_ERR_NO_DEVICE;
     }
     debug_maybe_throw();

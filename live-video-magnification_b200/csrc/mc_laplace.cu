@@ -1,4 +1,4 @@
-// Motion (Laplace) kernels for sm_100a.
+// Motion (Laplace) kernels for sm_90a.
 //
 //   lab16   : u8 BGR -> Lab (OpenCV LUT, exact) stored as int16 planes            (MagnifyCore.hpp:87-93)
 //   level   : pyrDown + pyrUp + subtract + dual-EMA state update + gain, fused    (SpatialFilter.cpp:25-38,
@@ -151,8 +151,7 @@ struct LevelKArgs {
 };
 
 // PREFETCH (with USE_TMA): the tile's two state planes are requested as bulk-tensor copies at kernel entry, together
-// with the input window, and only waited for in the last phase — the fused kernel is latency-bound (B200 probe:
-// removing 16 % of its bytes did not shorten it), so what matters is how many bytes each CTA keeps in flight.
+// with the input window, and only waited for in the last phase — the fused kernel is latency-bound, so what matters is how many bytes each CTA keeps in flight.
 template <int KIND, bool USE_TMA, bool PREFETCH>
 __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_constant__ CUtensorMap tmap,
                                                const __grid_constant__ CUtensorMap tmap_hi,
@@ -1324,7 +1323,7 @@ cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16
 
 cudaError_t launch_copy_planes(float* dst, const float* src, size_t n, cudaStream_t s) {
     unsigned blocks = (unsigned)((n + 255) / 256);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     if (blocks == 0) blocks = 1;
     k_copy<<<blocks, 256, 0, s>>>(dst, src, n);
     return cudaGetLastError();

@@ -18,8 +18,8 @@ constexpr int kGammaTabSize = 1024;     // OpenCV GAMMA_TAB_SIZE
 
 // One packed LUT cell (32 B = one L1/L2 sector): the Lab int16 values of the lattice points (b, g..g+1, r..r+1),
 // interleaved so that one dp2a does the r-interpolation of a channel at one (b, g) corner.  A pixel needs two cells,
-// (b, g, r) and (b+1, g, r), each fetched with ONE 256-bit load (LDG.E.256 on sm_100) — the divergent LUT gathers are
-// what bounds the BGR->Lab kernels (L1 tag lookups per distinct sector), so bytes per gather instruction is the lever.
+// (b, g, r) and (b+1, g, r), each fetched as one 128-bit + one 64-bit load from its single sector (ldg_cell) — the
+// divergent LUT gathers are what bounds the BGR->Lab kernels (L1 tag lookups per distinct sector).
 // The table is [34][33][33]: g+1 / r+1 are clamped when the table is built and the b = 33 slab repeats b = 32, so the
 // device code needs no clamping (a clamped neighbour always has weight 0).
 struct alignas(32) LabLutCell { int16_t v[16]; };  // {L00,L01, a00,a01, b00,b01, L10,L11, a10,a11, b10,b11, 0,0,0,0}, index = (g-offset, r-offset)
@@ -93,14 +93,16 @@ MC_HD int lab_q_of_u8_float(int v) {   // the definition (float arithmetic of co
 MC_HD int lab_q_of_u8(int v) { return (v * 16448 + 128) >> 13; }
 
 #if defined(__CUDA_ARCH__)
-// one LUT cell = one 256-bit read-only load
-__device__ __forceinline__ void ldg_cell(const LabLutCell* p, int (&w)[8]) {
+// the 24 used bytes of one LUT cell: a 128-bit and a 64-bit read-only load from the same 32-byte sector
+// (sm_90 has no 256-bit load; the 8 pad bytes are never read)
+__device__ __forceinline__ void ldg_cell(const LabLutCell* p, int (&w)[6]) {
 #if defined(MC_CUDA_EMU)
     const int* q = reinterpret_cast<const int*>(p);
-    for (int i = 0; i < 8; ++i) w[i] = q[i];
+    for (int i = 0; i < 6; ++i) w[i] = q[i];
 #else
-    asm("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-        : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "l"(p));
+    asm("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%6];\n\t"
+        "ld.global.nc.v2.b32 {%4,%5}, [%6+16];"
+        : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]) : "l"(p));
 #endif
 }
 #endif
@@ -114,7 +116,7 @@ MC_HD void lab_fixed_from_q(int qb, int qg, int qr, const LabLutCell* __restrict
     const LabLutCell* c0 = lut + ((tb * kLabLutDim + tg) * kLabLutDim + tr);
     const int w01 = (16 - xb) * xg, w00 = ((16 - xb) << 4) - w01, w11 = xb * xg, w10 = (xb << 4) - w11;
 #if defined(__CUDA_ARCH__)
-    int u[8], v[8];
+    int u[6], v[6];
     ldg_cell(c0, u);
     ldg_cell(c0 + kLabLutSlab, v);
     const int wr = 16 + 255 * xr;                               // int8 pair for dp2a: lo * (16-x) + hi * x
@@ -249,7 +251,7 @@ __device__ __forceinline__ void lab_to_bgr_fast(float L, float a, float b, const
     if (NAN_AS_OPENCV) {
         // NOT fmaxf(fminf(v, 1), 0): ptxas folds that pair into the producing FFMA as .SAT, and .SAT turns NaN into 0
         // (black) where OpenCV's max(min(v,1),0) gives 1 (white).  The explicit NaN select survives the fold
-        // (round-1 GPUTEST failure; tools/check_sass.py asserts the FSETP.NAN/FSEL pair is in k_riesz_egress).
+        // (tools/check_sass.py asserts the FSETP.NAN test and its select are in k_riesz_egress).
         vb = (vb != vb) ? 1.0f : __saturatef(vb);
         vg = (vg != vg) ? 1.0f : __saturatef(vg);
         vr = (vr != vr) ? 1.0f : __saturatef(vr);

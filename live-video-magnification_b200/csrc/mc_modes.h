@@ -1,4 +1,4 @@
-// Per-mode device state + per-frame drivers: the B200 twins of magcore::MotionState / ColorState /
+// Per-mode device state + per-frame drivers: the H100 twins of magcore::MotionState / ColorState /
 // RieszState and magnifyMotion / magnifyColor / magnifyRiesz (reference
 // src/processing/magnification/MagnifyCore.hpp:24-40, :83-279).
 #pragma once
@@ -36,8 +36,7 @@ struct ModeCtx {
     float* float_out;  // optional [lanes][h][w][C] pre-quantisation tap
     Profiler* prof;    // optional
     bool use_tma;      // stage level-kernel tiles with cp.async.bulk.tensor (option "use_tma", default on)
-    bool prefetch_state;    // level kernel requests its state tiles by TMA at kernel entry (option "prefetch_state", default on:
-                            // B200, 32 lanes: level[1] 235 -> 205 us)
+    bool prefetch_state;    // level kernel requests its state tiles by TMA at kernel entry (option "prefetch_state", default on)
     int egress_strip;       // Laplace egress as the register/shuffle strip kernel (option "egress_strip": 0 = tile kernel,
                             // 16 / 20 / 24 = strip kernel compiled for that many resident warps per SM)
     int ingest_warps;       // warps per CTA of the fused ingest kernel (option "ingest_warps": 1, 2 or 4)

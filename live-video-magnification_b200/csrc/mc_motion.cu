@@ -53,10 +53,8 @@ void MotionMode::reset() {
 // (Re)builds the lane groups — their streams, events and TMA descriptors — over the existing buffers; the temporal state
 // is untouched, so the option can change between frames (profile_kernels forces one group).
 mc_status MotionMode::make_groups(const ModeCtx& ctx) {
-    // lane groups: automatic = two chains once each has >= 8 streams.  B200, 32 lanes x 1080p: 1 group 27.9 k frames/s,
-    // 2 groups 29.2 k, 4 groups 29.0 k, 8 groups 28.6 k; serialising the same stage of consecutive groups with events
-    // (so that different stages overlap by construction) was slower than one chain (24.1 k): the stages contend for the
-    // same L1 data pipe, so co-residency buys little beyond filling each other's tails.
+    // lane groups: automatic = two chains once each has >= 8 streams.  The stages contend for the same L1 data pipe,
+    // so co-residency buys little beyond filling each other's tails.
     drop_groups();
     groups_req = ctx.lane_groups;
     int ng = groups_req > 0 ? groups_req : std::min(2, lanes / 8);

@@ -52,8 +52,8 @@ __device__ __forceinline__ float mulr(float a, float b) { return __fmul_rn(a, b)
 __device__ __forceinline__ float addr(float a, float b) { return __fadd_rn(a, b); }
 __device__ __forceinline__ float subr(float a, float b) { return __fsub_rn(a, b); }
 
-// cv::filter2D's f32 engine (FilterVec_32f + scalar remainder; OpenCV 4.x, the AVX2 dispatch both this container and the
-// B200 boxes run, tools/probe_filter2d_order.py): every output accumulates its non-zero taps in raster order — with one
+// cv::filter2D's f32 engine (FilterVec_32f + scalar remainder; OpenCV 4.x, its AVX2 dispatch,
+// tools/probe_filter2d_order.py): every output accumulates its non-zero taps in raster order — with one
 // FMA per tap in the vectorised columns x < (w & ~7), with multiply-then-add in the scalar tail columns.  The device
 // kernels follow that rule column by column, which makes the band planes and the Riesz pair bit-identical to the
 // reference for every width (acos near 1 turns a last-ulp difference here into visible differences downstream).

@@ -7,7 +7,7 @@ Same names, argument meaning and error behaviour as the reference: ``process(fra
 the *same* frame object when the reference would return its input FrameRef (identity /
 passthrough), otherwise a fresh frame that never aliases the input; a failing core raises (the
 caller's firewall then calls ``reset()``, ProcessingChain.cpp:50-62).  All arithmetic happens on
-the B200 behind the C ABI (include/magcore_b200.h).
+the H100 behind the C ABI (include/magcore_b200.h).
 """
 from __future__ import annotations
 
@@ -130,7 +130,7 @@ class IProcessor:  # IProcessor.hpp:50-60
 
 
 class MagnificationProcessor(IProcessor):
-    """B200 drop-in for livim::MagnificationProcessor.  ``lanes`` > 1 steps that many independent
+    """H100 drop-in for livim::MagnificationProcessor.  ``lanes`` > 1 steps that many independent
     streams in lock-step (images then carry a leading lane axis)."""
 
     def __init__(self, device: int = 0, lanes: int = 1):
@@ -273,7 +273,7 @@ class MagnificationProcessor(IProcessor):
 class ProcessingChainB200:
     """The reference's per-frame chain ``runChainOnce(chain, in, cfg, original)`` (reference
     src/processing/ChainBuilder.cpp:11-29: PreprocessProcessor -> GrayscaleProcessor -> MagnificationProcessor)
-    executed on the B200 behind ``mc_chain_process``: the raw frame is uploaded once, ROI crop + INTER_AREA
+    executed on the H100 behind ``mc_chain_process``: the raw frame is uploaded once, ROI crop + INTER_AREA
     downscale and BGR2GRAY run bit-exact on the device, the magnification core runs on their result.
 
     ``run_chain_once(frame, cfg) -> (cur, original)`` returns the *same* frame object wherever the reference

@@ -1,7 +1,7 @@
 """Multi-GPU plumbing for the replica-parallel path (SURVEY.md §8e): one process per GPU, every rank
 serves its own independent streams.  The data path has NO per-frame collective; the only exchange is
 a one-time broadcast of the POD parameter block from rank 0, plus a MAX-reduction of the timings for
-reporting.  Works with any torch.distributed backend (NCCL on B200s, gloo in the CPU tests)."""
+reporting.  Works with any torch.distributed backend (NCCL on H100s, gloo in the CPU tests)."""
 from __future__ import annotations
 
 import ctypes as C

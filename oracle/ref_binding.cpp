@@ -84,7 +84,7 @@ struct RefChain {
 // The drop-in itself: the reference's chain exactly as buildProcessors() assembles it (ChainBuilder.cpp:11-17) with
 // the single substitution INTEGRATION.md describes at ChainBuilder.cpp:15 — MagnificationProcessorB200 (the adapter
 // over the C ABI) in place of MagnificationProcessor — driven by the reference's own runChainOnce().  The two
-// front stages are the reference's compiled code.  Needs a B200: the adapter's constructor throws without one.
+// front stages are the reference's compiled code.  Needs an H100: the adapter's constructor throws without one.
 struct DropInChain {
     std::vector<std::unique_ptr<IProcessor>> chain;
     std::uint64_t seq = 0;

@@ -391,8 +391,8 @@ cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int d) {
     if (d != 0) return cudaErrorInvalidValue;
     std::memset(p, 0, sizeof(*p));
     std::snprintf(p->name, sizeof(p->name), "cuda_emu (CPU fibers, not a GPU)");
-    p->major = 10; p->minor = 0; p->multiProcessorCount = 148; p->warpSize = 32; p->maxThreadsPerBlock = 1024;
-    p->totalGlobalMem = 8ull << 30; p->sharedMemPerBlock = 48 << 10; p->sharedMemPerBlockOptin = 227 << 10; p->l2CacheSize = 126 << 20;
+    p->major = 9; p->minor = 0; p->multiProcessorCount = 132; p->warpSize = 32; p->maxThreadsPerBlock = 1024;
+    p->totalGlobalMem = 8ull << 30; p->sharedMemPerBlock = 48 << 10; p->sharedMemPerBlockOptin = 227 << 10; p->l2CacheSize = 50 << 20;
     return cudaSuccess;
 }
 cudaError_t cudaDeviceSynchronize() { cuda_emu::drain_all(); return cudaSuccess; }

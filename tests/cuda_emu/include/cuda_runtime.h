@@ -2,7 +2,7 @@
 // (live-video-magnification_b200/csrc/*.cu) can be compiled with g++ and their *logic* exercised by the parity
 // tests in a container that has no GPU (tests/cuda_emu/build_emu.py -> tests/cuda_emu/libmagcore_emu.so).
 // It is never shipped, never loaded by the product (lvm_b200.capi loads libmagcore_b200.so only; mc_create in
-// that library still fails without an sm_100 device), and it says nothing about performance.
+// that library still fails without an sm_90 device), and it says nothing about performance.
 //
 // Model: a kernel launch runs its CTAs one after another; the threads of a CTA are cooperative fibers
 // (ucontext) scheduled round-robin by one OS thread, so __syncthreads / warp shuffles have their CUDA meaning,
@@ -187,7 +187,7 @@ constexpr unsigned long long cudaEnableDefault = 0;
 
 enum cudaFuncAttribute { cudaFuncAttributeMaxDynamicSharedMemorySize = 8, cudaFuncAttributePreferredSharedMemoryCarveout = 9 };
 template <typename F> inline cudaError_t cudaFuncSetAttribute(F, cudaFuncAttribute, int value) {
-    return value <= 227 * 1024 ? cudaSuccess : cudaErrorInvalidValue;   // sm_100: at most 227 KB per CTA
+    return value <= 227 * 1024 ? cudaSuccess : cudaErrorInvalidValue;   // sm_90: at most 227 KB per CTA
 }
 const char* cudaGetErrorString(cudaError_t e);
 cudaError_t cudaGetLastError();

@@ -1,10 +1,11 @@
 """bench.py contract checks that need no GPU: the reference arm runs on the host and prints exactly one JSON
-line with the keys the driver reads; the product arm refuses to run without a B200 (no CPU fallback)."""
+line with the keys the driver reads; the product arm refuses to run without an H100 (no CPU fallback)."""
 import json
 import os
 import subprocess
 import sys
 
+import numpy as np
 import pytest
 import torch
 
@@ -39,14 +40,13 @@ def test_product_arm_needs_a_gpu():
 
 def test_kernel_table_accounting():
     """bench.kernel_table: interface / algorithmic byte models per kernel (no GPU needed), for the default data flow
-    (level kernels store their band, option band_from_state = 0) and for the shipped default band_from_state = 1; ncu
-    captures are only quoted for kernels whose interface still matches the capture."""
+    (level kernels store their band, option band_from_state = 0) and for the shipped default band_from_state = 1."""
     sys.path.insert(0, ROOT)
     import bench
     px = bench.level_pixels(1920, 1080, 6)
     prof = {("ingest_lab", 0): (20, 10.3), ("egress", 0): (20, 8.0), ("level", 1): (20, 4.0), ("level", 2): (20, 1.3),
             ("collapse", 2): (20, 0.6), ("collapse", 4): (20, 0.2)}
-    table, traffic = bench.kernel_table(prof, 32)
+    table = bench.kernel_table(prof, 32)
     by = {t["kernel"]: t for t in table}
     assert [t["kernel"] for t in table][0] == "ingest_lab[0]"                       # sorted by time share
     assert by["level[1]"]["interface_bytes"] == 32 * 3 * (16 * px[1] + 8 * px[1] + 4 * px[2])
@@ -54,19 +54,17 @@ def test_kernel_table_accounting():
     assert by["egress[0]"]["interface_bytes"] == 32 * 3 * (3 * px[0] + 4 * px[1] + 4 * px[2])
     assert abs(by["level[1]"]["algorithmic_GBps"] - 16 * 3 * px[1] * 32 / 200e-6 / 1e9) < 1e-6
     assert abs(sum(t["share"] for t in table) - 1.0) < 1e-9
-    assert "ingest_lab[0]" in traffic and "level[1]" not in traffic and "egress[0]" not in traffic   # captures are of the shipped flow
-    table2, traffic2 = bench.kernel_table(prof, 32, band_from_state=True)
+    table2 = bench.kernel_table(prof, 32, band_from_state=True)
     by2 = {t["kernel"]: t for t in table2}
     assert by2["level[1]"]["interface_bytes"] == 32 * 3 * (16 * px[1] + 4 * px[1] + 4 * px[2])
     assert by2["collapse[2]"]["interface_bytes"] == 32 * 3 * (12 * px[2] + 4 * px[3])
     assert by2["collapse[4]"]["interface_bytes"] == 32 * 3 * (12 * px[4] + 8 * px[5])  # top band comes from state planes
     assert by2["egress[0]"]["interface_bytes"] == 32 * 3 * (3 * px[0] + 8 * px[1] + 4 * px[2])
-    assert {"ingest_lab[0]", "egress[0]", "level[1]", "level[2]"} <= set(traffic2)  # round-2 captures: band rebuilt from state
 
 
 @pytest.mark.emu
-def test_product_arm_dry_run_on_emulation(monkeypatch):
-    """bench.run_ours end to end (device-resident loop, pipelined e2e loop, per-kernel table, CPU baseline, JSON line)
+def test_product_arm_dry_run_on_emulation(monkeypatch, tmp_path):
+    """bench.run_ours end to end (device-resident loop, output dump, pipelined e2e loop, per-kernel table, CPU baseline, JSON line)
     with the kernels on the CUDA-on-CPU emulation and a stand-in for the handful of torch.cuda calls it makes, at a
     tiny frame size.  Guards the bench's own logic in the GPU-less container; the numbers mean nothing."""
     import time
@@ -105,7 +103,7 @@ def test_product_arm_dry_run_on_emulation(monkeypatch):
     monkeypatch.setitem(bench.UI, "levels", 4)
     try:
         args = types.SimpleNamespace(gpus=1, steps=3, warmup=3, lanes=2, clip_frames=2, cpu_frames=2, no_cpu_baseline=False,
-                                     ref_frames_per_step=1, opt=[], workload="1080p6")
+                                     ref_frames_per_step=1, opt=[], workload="1080p6", dump_outputs=str(tmp_path / "out"))
         d = json.loads(bench.run_ours(args, 0, 1, 0))
     finally:
         capi.LIB_PATH, capi._lib = saved
@@ -117,3 +115,6 @@ def test_product_arm_dry_run_on_emulation(monkeypatch):
     assert r["bound"] == "hbm" and 0 < r["frac"] and r["fused_level_kernel"]["kernel"] == "level[1]"
     assert {k["kernel"] for k in r["kernels"]} >= {"ingest_lab[0]", "egress[0]", "level[1]", "level[2]", "level[3]", "collapse[2]"}
     assert d["cpu_baseline"]["value"] > 0 and d["cpu_baseline"]["kind"] in ("reference", "port")
+    frames = np.load(tmp_path / "out" / "frames.npy")       # the last timed step's output frames, float32
+    assert frames.dtype == np.float32 and frames.shape == (2, 108, 192, 3) and sorted(os.listdir(tmp_path / "out")) == ["frames.npy"]
+    assert frames.min() >= 0 and frames.max() <= 255 and frames.max() > 0 and np.array_equal(frames, np.round(frames))

@@ -3,8 +3,8 @@
 The product's own kernel sources are compiled with g++ against an emulated CUDA runtime (CTA threads as cooperative
 fibers, emulated TMA / mbarrier / shuffles / cuFFT) into tests/cuda_emu/libmagcore_emu.so, and tiny clips of all
 three modes plus the fused front of the chain are checked against the oracle with the same tolerances as the
-`-m gpu` parity tests.  This catches indexing / border / staging / state-handling regressions in the kernels in
-the GPU-less container; it says nothing about performance or hardware behaviour — the `-m gpu` tests on a B200
+`-m gpu` parity tests.  This catches indexing / border / staging / state-handling regressions in the kernels on
+a machine without a GPU; it says nothing about performance or hardware behaviour — the `-m gpu` tests on an H100
 remain the parity gate.  The whole `-m gpu` suite can be pointed at the emulation with `MC_EMU=1` (tests/conftest.py).
 """
 import numpy as np
@@ -156,7 +156,7 @@ def test_color_many_lanes_and_frame_rate_sweep(emu):
 
 
 def test_round2_kernel_forms_agree_on_emulation(emu):
-    """Round-2 kernel forms, logic only (the B200 runs the same checks in test_gpu_laplace.py / test_gpu_riesz.py):
+    """Round-2 kernel forms, logic only (the H100 runs the same checks in test_gpu_laplace.py / test_gpu_riesz.py):
     (1) the shuffle-strip egress equals the shared-memory tile egress bit for bit over several strips and chunks, both band
     sources, float taps included; (2) lanes run as two launch chains (option lane_groups) equal one chain; (3) the 9x9 Riesz
     kernels give the same bits with TMA-staged and with LDG-staged tiles."""
@@ -198,7 +198,7 @@ def test_round2_kernel_forms_agree_on_emulation(emu):
 
 def test_riesz_band_planes_bit_identical_on_odd_widths_on_emulation(emu):
     """mc_riesz.cu::f2d — cv::filter2D's FMA / multiply-then-add column rule: band planes and Riesz pair equal the
-    oracle's bit for bit on a width that is not a multiple of 8 (the B200 runs the same check in test_gpu_riesz.py)."""
+    oracle's bit for bit on a width that is not a multiple of 8 (the H100 runs the same check in test_gpu_riesz.py)."""
     w, h, levels = 71, 76, 4
     cfg, ocfg = make_cfgs(O.MODE_PHASE, 50, 50.0, 0.4, 3.0, 0, levels, 30.0)
     proc, op = L.MagnificationProcessor(0), O.MagnificationProcessor()

@@ -1,4 +1,4 @@
-"""Motion (Laplace) parity: CUDA path (through the C ABI) vs the oracle, on a B200.
+"""Motion (Laplace) parity: CUDA path (through the C ABI) vs the oracle, on an H100.
 
 Tolerances (SURVEY.md §A.7 / BASELINE.md §3): f32 output in [0,1] units before 8-bit quantisation
 max-abs < 1e-4; u8 output <= 1 LSB; state planes (Lab scale, L in [0,100]) max-abs < 1e-3 absolute

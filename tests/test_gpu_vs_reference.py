@@ -1,7 +1,7 @@
-"""CUDA path (through the C ABI) checked DIRECTLY against the reference's own code on a B200.
+"""CUDA path (through the C ABI) checked DIRECTLY against the reference's own code on the GPU.
 
 The checker here is not the oracle restatement but oracle/_ref/_livim_ref: /root/reference/src/processing/**
-compiled unmodified (oracle/build_ref.py, prebuilt in the container and shipped to the GPU box) with OpenCV's
+compiled unmodified (oracle/build_ref.py, prebuilt under oracle/_ref/ where the reference sources are present) with OpenCV's
 kernels underneath.  Same tolerances as the oracle-based tests: Laplace / Color <= 1 LSB free-running,
 Phase <= 3 LSB and >= 99.5 % identical free-running; passthrough decisions identical."""
 import numpy as np
@@ -17,9 +17,9 @@ import os
 
 R = livim_ref.load()
 if R is None and os.environ.get("MC_REQUIRE_REF") == "1":
-    # a GPU round must not silently lose its reference-pinned tests (tools/gpu_round.sh sets this)
+    # a GPU run must not silently lose its reference-pinned tests
     raise RuntimeError("MC_REQUIRE_REF=1 but oracle/_ref/_livim_ref is missing: run __graft_entry__.build() where "
-                       "/root/reference exists; the prebuilt module ships to the GPU box with the snapshot")
+                       "the reference sources are present, and keep oracle/_ref/ with the tree")
 pytestmark = [pytest.mark.gpu, pytest.mark.skipif(R is None, reason="oracle/_ref/_livim_ref not present")]
 
 

@@ -226,9 +226,10 @@ def test_c_abi_is_an_exception_firewall(built):
 
 def test_sass_of_the_built_library_has_the_claimed_instructions():
     """cuobjdump works without a GPU: the fused level kernels use TMA (UTMALDG + mbarrier SYNCS, three bulk copies with
-    the state prefetch), the ingest gathers are 256-bit, the strip egress prefetches into L1 and has no barrier, and the
+    the state prefetch), each ingest LUT gather is one 128-bit + one 64-bit load, the strip egress prefetches into L1
+    and has no barrier, and the
     Phase egress clips NaN with an explicit select — ptxas folded fmaxf/fminf into FFMA.SAT (NaN -> 0) in round 1, which
-    the CPU emulation cannot see (tools/check_sass.py; evidence in profiles/r02_sass_evidence.txt)."""
+    the CPU emulation cannot see (tools/check_sass.py)."""
     import shutil
     import subprocess
     import sys

@@ -234,7 +234,7 @@ def test_chain_bit_exact(extra):
 
 
 # --------------------------------------------------------------------------------------------------
-# The drop-in: reference chain + reference headers + the product's adapter (needs a B200 to run)
+# The drop-in: reference chain + reference headers + the product's adapter (needs an H100 to run)
 # --------------------------------------------------------------------------------------------------
 def test_dropin_chain_builds_against_real_reference_headers_and_has_no_cpu_fallback(built):
     """oracle/_ref/_livim_ref also holds the reference's chain with the ONE substitution of INTEGRATION.md

@@ -3,7 +3,7 @@ handed from rank to rank through the linear recurrence (lvm_b200.shard.magnify_s
 equal the single-handle run of the whole clip up to f32 rounding of the carry (<= 1 LSB, >= 99.9 % identical).
 
 CPU variants run the product's kernels on the CUDA-on-CPU emulation (tests/cuda_emu): in-process with a queue as the
-transport, and as a real world_size-2 gloo job.  The `gpu` variant runs the same on a B200."""
+transport, and as a real world_size-2 gloo job.  The `gpu` variant runs the same on an H100."""
 import os
 import socket
 

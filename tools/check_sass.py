@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Static checks of the built library's SASS (cuobjdump works without a GPU) and the evidence file the docs cite:
-which kernels use the TMA path (UTMALDG + mbarrier SYNCS), that the ingest gathers are 256-bit, that the strip egress
+which kernels use the TMA path (UTMALDG + mbarrier SYNCS), that each ingest LUT gather is one 128-bit + one 64-bit load,
+that the strip egress
 prefetches into L1, and that the Phase egress clips NaN to 1.0 with an explicit select (OpenCV's max(min(v,1),0)) instead
 of a .SAT folded into the producing FFMA (round-1 hardware failure).  Usage: python tools/check_sass.py [out.txt]"""
 import collections
@@ -32,9 +33,9 @@ def main():
     count = lambda k, pat: sum(1 for l in body[k] if re.search(pat, l))
     lines, ok = [], True
     lines.append("SASS evidence of libmagcore_b200.so (cuobjdump -sass; tools/check_sass.py)\n")
-    lines.append(f"{'kernel':90s} instr  UTMALDG SYNCS LDG.256 CCTL.PF1 SHFL  BAR")
+    lines.append(f"{'kernel':90s} instr  UTMALDG SYNCS LDG.128 LDG.64 CCTL.PF1 SHFL  BAR")
     for k in body:
-        lines.append(f"{k[:90]:90s} {len(body[k]):5d}  {count(k, 'UTMALDG'):7d} {count(k, 'SYNCS'):5d} {count(k, r'LDG\.E\.\S*256'):7d} "
+        lines.append(f"{k[:90]:90s} {len(body[k]):5d}  {count(k, 'UTMALDG'):7d} {count(k, 'SYNCS'):5d} {count(k, r'LDG\.E\.128'):7d} {count(k, r'LDG\.E\.64'):6d} "
                      f"{count(k, r'CCTL\.E\.PF1'):8d} {count(k, 'SHFL'):4d} {count(k, r'BAR\.SYNC'):4d}")
 
     def need(cond, what):
@@ -50,12 +51,15 @@ def main():
     r9 = [k for k in body if k.startswith("k_riesz_analysis(") or k.startswith("k_riesz_collapse(")]
     need(len(r9) == 2 and all(count(k, "UTMALDG") == 1 and count(k, "SYNCS") >= 2 for k in r9), "k_riesz_analysis / k_riesz_collapse: 9x9 input tile by one bulk-tensor copy")
     ing = [k for k in body if k.startswith("void k_ingest_lab<")]
-    need(bool(ing) and all(count(k, r"LDG\.E\.\S*256") >= 8 for k in ing), "k_ingest_lab: 256-bit LUT gathers (LDG.E.*.256)")
+    need(bool(ing) and all(count(k, r"LDG\.E\.128") >= 8 and count(k, r"LDG\.E\.128") == count(k, r"LDG\.E\.64") for k in ing),
+         "k_ingest_lab: each LUT gather is one LDG.E.128 + one LDG.E.64 (the 24 used bytes of a 32-byte cell)")
     strip = [k for k in body if k.startswith("void k_egress_strip<3")]
     need(bool(strip) and all(count(k, r"CCTL\.E\.PF1") >= 8 and count(k, r"BAR\.SYNC") == 0 for k in strip), "k_egress_strip<3>: L1 prefetches, no barrier")
     rz = [k for k in body if k.startswith("k_riesz_egress") or "k_riesz_egress(" in k]
-    need(bool(rz) and all(count(k, r"FSETP\.NAN") >= 3 and count(k, "FSEL") >= 3 and count(k, r"FFMA\.SAT") == 0 for k in rz),
-         "k_riesz_egress: explicit NaN -> 1.0 select before the gamma (FSETP.NAN + FSEL), no FFMA.SAT")
+    # the select is either an FSEL per channel or a saturate predicated on the NaN test over a preset 1.0
+    nan_sel = lambda k: count(k, "FSEL") + count(k, r"@!P\d FADD\.SAT")
+    need(bool(rz) and all(count(k, r"FSETP\.NAN") >= 3 and nan_sel(k) >= 3 and count(k, r"FFMA\.SAT") == 0 for k in rz),
+         "k_riesz_egress: explicit NaN -> 1.0 select before the gamma (FSETP.NAN + FSEL or @!P FADD.SAT), no FFMA.SAT")
     text = "\n".join(lines) + "\n"
     if len(sys.argv) > 1:
         open(sys.argv[1], "w").write(text)

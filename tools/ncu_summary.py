@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Summarises .ncu-rep captures (key metrics per kernel) — used to write profiles/*.md."""
+"""Summarises .ncu-rep captures (key metrics per kernel)."""
 import csv, subprocess, sys
 WANT = ['gpu__time_duration.sum', 'dram__bytes_read.sum', 'dram__bytes_write.sum',
         'gpu__dram_throughput.avg.pct_of_peak_sustained_elapsed', 'sm__throughput.avg.pct_of_peak_sustained_elapsed',
