@@ -46,6 +46,9 @@ SIGNATURES = {
     "mc_create_lanes": (C.c_int, [C.c_int, C.c_int, C.POINTER(_vp)]),
     "mc_destroy": (None, [_vp]),
     "mc_reset": (C.c_int, [_vp]),
+    "mc_restart_lane": (C.c_int, [_vp, C.c_int]),
+    "mc_hold_lane": (C.c_int, [_vp, C.c_int, C.c_int]),
+    "mc_lane_produced": (C.c_int, [_vp, _u8p, C.c_int]),
     "mc_process": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t, C.POINTER(C.c_int)]),
     "mc_process_device": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t, C.POINTER(C.c_int)]),
     "mc_sync": (C.c_int, [_vp]),

@@ -25,6 +25,7 @@ struct Slot {  // one in-flight frame of the pinned pipeline
     size_t bytes = 0;
     cudaEvent_t ev_in = nullptr, ev_k = nullptr, ev_done = nullptr;
     int produced = 0;
+    std::vector<uint8_t> lane_produced;          // per lane: its bytes of `out` are written
     uint8_t* user_out = nullptr;                 // destination given to mc_submit
     size_t user_out_step = 0;
     bool direct_out = false;                     // D2H went straight into user_out (pinned)
@@ -70,6 +71,13 @@ struct mc_handle {
     std::vector<Slot> slots;
     std::deque<int> inflight;
     int next_slot = 0;
+
+    // Lane lifecycle: per lane, whether it has temporal state (cleared by mc_reset, structural changes, mode None and the
+    // error path, or for one lane by mc_restart_lane) and whether it is held (mc_hold_lane; sticky).  A frame call turns
+    // them into one LaneOp per lane.
+    std::vector<uint8_t> has_state, hold, ops;
+    std::vector<uint8_t> lane_produced;   // of the frame most recently returned / collected
+    uint8_t* d_ops = nullptr;             // device copy of a mixed frame's ops (the mode uploads it on the handle's stream)
 };
 
 namespace {
@@ -127,11 +135,14 @@ void tracker_reset(mc_handle* h) {
     tracker_disable(h);
     h->t_down = 1; h->t_roi = 0; h->t_rx = 0.f; h->t_ry = 0.f; h->t_rw = 1.f; h->t_rh = 1.f;
 }
+bool tracker_changes(const mc_handle* h, const mc_params* p, int lv, int ch, int w, int hh) {
+    return p->mode != h->t_mode || lv != h->t_levels || w != h->t_w || hh != h->t_h ||
+           ch != h->t_channels || p->pre_downscale != h->t_down ||
+           (p->pre_roiEnabled != 0) != (h->t_roi != 0) || p->pre_roiX != h->t_rx ||
+           p->pre_roiY != h->t_ry || p->pre_roiW != h->t_rw || p->pre_roiH != h->t_rh;
+}
 bool tracker_update(mc_handle* h, const mc_params* p, int lv, int ch, int w, int hh) {
-    const bool change = p->mode != h->t_mode || lv != h->t_levels || w != h->t_w || hh != h->t_h ||
-                        ch != h->t_channels || p->pre_downscale != h->t_down ||
-                        (p->pre_roiEnabled != 0) != (h->t_roi != 0) || p->pre_roiX != h->t_rx ||
-                        p->pre_roiY != h->t_ry || p->pre_roiW != h->t_rw || p->pre_roiH != h->t_rh;
+    const bool change = tracker_changes(h, p, lv, ch, w, hh);
     if (change) {
         h->t_mode = p->mode; h->t_levels = lv; h->t_w = w; h->t_h = hh; h->t_channels = ch;
         h->t_down = p->pre_downscale; h->t_roi = p->pre_roiEnabled != 0;
@@ -141,6 +152,7 @@ bool tracker_update(mc_handle* h, const mc_params* p, int lv, int ch, int w, int
 }
 
 void reset_modes(mc_handle* h) {
+    std::fill(h->has_state.begin(), h->has_state.end(), (uint8_t)0);
     h->motion.reset();
     h->color.reset();
     h->riesz.reset();
@@ -171,6 +183,7 @@ mc_status ensure_slots(mc_handle* h, size_t bytes) {
     h->slots.resize((size_t)h->depth);
     for (auto& s : h->slots) {
         s.bytes = bytes;
+        s.lane_produced.assign((size_t)h->lanes, 0);
         CK(cudaHostAlloc((void**)&s.h_in, bytes, cudaHostAllocDefault));
         CK(cudaHostAlloc((void**)&s.h_out, bytes, cudaHostAllocDefault));
         CK(cudaMalloc((void**)&s.d_in, bytes));
@@ -192,9 +205,11 @@ bool is_pinned(const void* p) {
 }
 
 // The body of MagnificationProcessor::process on device-resident frames.
+// lane_produced: `lanes` per-lane flags (written).
 mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, int channels, size_t in_step,
-                              const mc_params* p, uint8_t* d_out, size_t out_step, int* produced) {
+                              const mc_params* p, uint8_t* d_out, size_t out_step, int* produced, uint8_t* lane_produced) {
     *produced = 0;
+    std::fill(lane_produced, lane_produced + h->lanes, (uint8_t)0);
     debug_maybe_throw();
     if (!p) { h->err = "params is null"; return MC_ERR_INVALID; }
     // Identity when disabled / empty; free state so a later re-enable starts cleanly (:21-29).
@@ -212,7 +227,28 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
     const int max_levels = calculate_max_levels(w, hh);  // :32-33
     if (max_levels < 1) return MC_OK;
     const int levels = std::min(std::max((int)p->levels, 1), max_levels);  // :34
+    if (p->mode == MC_MODE_COLOR) {
+        // The Color window (ring head, length and the DFT plans cached per length) is shared by all lanes, so a lane
+        // cannot be held, or restarted while others run, on a multi-lane handle; refused before any state changes.
+        // A held 1-lane handle skips the call: its window stays as it is.
+        const bool change = tracker_changes(h, p, levels, channels, w, hh);
+        int n_hold = 0, n_state = 0;
+        for (int l = 0; l < h->lanes; ++l) { n_hold += h->hold[(size_t)l] != 0; n_state += h->has_state[(size_t)l] != 0; }
+        if (h->lanes == 1 && n_hold) return MC_OK;
+        if (n_hold) { h->err = "Color mode cannot hold a lane of a multi-lane handle"; return MC_ERR_UNSUPPORTED; }
+        if (!change && n_state != 0 && n_state != h->lanes) {
+            h->err = "Color mode cannot restart one lane of a multi-lane handle while the others run";
+            return MC_ERR_UNSUPPORTED;
+        }
+    }
     if (tracker_update(h, p, levels, channels, w, hh)) reset_modes(h);      // :39-43
+    int n_first = 0;
+    for (int l = 0; l < h->lanes; ++l) {
+        const uint8_t op = h->hold[(size_t)l] ? LANE_HOLD : h->has_state[(size_t)l] ? LANE_RUN : LANE_FIRST;
+        h->ops[(size_t)l] = op;
+        n_first += op == LANE_FIRST;
+    }
+    if (p->mode == MC_MODE_COLOR && n_first == h->lanes) h->color.reset();   // every lane restarted: a fresh window
 
     FrameIO io;
     io.in = d_in; io.in_step = in_step; io.in_lane_stride = in_step * (size_t)hh;
@@ -231,7 +267,9 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
         fout = h->float_out;
     }
 
-    ModeCtx ctx{h->stream, &h->tables, &h->launches, &h->err, h->faithful0, fout, h->profile ? &h->prof : nullptr, h->use_tma, h->prefetch_state, h->egress_strip, h->ingest_warps, h->band_from_state, h->profile ? 1 : h->lane_groups, h->analysis_only};
+    bool held_lost = false;
+    ModeCtx ctx{h->stream, &h->tables, &h->launches, &h->err, h->faithful0, fout, h->profile ? &h->prof : nullptr, h->use_tma, h->prefetch_state, h->egress_strip, h->ingest_warps, h->band_from_state, h->profile ? 1 : h->lane_groups, h->analysis_only,
+                h->ops.data(), h->d_ops, lane_produced, &held_lost};
     mc_status st = MC_OK;
     switch (p->mode) {
         case MC_MODE_LAPLACE: st = h->motion.process(ctx, io, *p, levels, produced); break;
@@ -245,6 +283,13 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
         reset_modes(h);
         tracker_reset(h);
         *produced = 0;
+        std::fill(lane_produced, lane_produced + h->lanes, (uint8_t)0);
+        return st;
+    }
+    if (p->mode == MC_MODE_COLOR) std::fill(lane_produced, lane_produced + h->lanes, (uint8_t)(*produced != 0));   // all lanes step together
+    for (int l = 0; l < h->lanes; ++l) {
+        if (h->ops[(size_t)l] != LANE_HOLD) h->has_state[(size_t)l] = 1;
+        else if (held_lost) h->has_state[(size_t)l] = 0;
     }
     return st;
 }
@@ -374,6 +419,11 @@ mc_status mc_create_lanes(int device, int lanes, mc_handle** out) try {
     if ((e = cudaMemcpy(h->tables.lab_lut, lut.data(), lut.size() * sizeof(LabLutCell), cudaMemcpyHostToDevice)) != cudaSuccess) return fail("copy lut", e);
     if ((e = cudaMemcpy(h->tables.inv_gamma, gam.data(), gam.size() * sizeof(float4), cudaMemcpyHostToDevice)) != cudaSuccess) return fail("copy gamma", e);
     h->motion.lanes = h->color.lanes = h->riesz.lanes = lanes;
+    h->has_state.assign((size_t)lanes, 0);
+    h->hold.assign((size_t)lanes, 0);
+    h->ops.assign((size_t)lanes, 0);
+    h->lane_produced.assign((size_t)lanes, 0);
+    if ((e = cudaMalloc((void**)&h->d_ops, (size_t)lanes)) != cudaSuccess) return fail("cudaMalloc lane ops", e);
     *out = h;
     return MC_OK;
     } catch (...) { mc_destroy(h); throw; }
@@ -397,6 +447,7 @@ void mc_destroy(mc_handle* h) try {
     if (h->c_tabs) cudaFree(h->c_tabs);
     if (h->tables.lab_lut) cudaFree(h->tables.lab_lut);
     if (h->tables.inv_gamma) cudaFree(h->tables.inv_gamma);
+    if (h->d_ops) cudaFree(h->d_ops);
     if (h->stream) cudaStreamDestroy(h->stream);
     if (h->s_in) cudaStreamDestroy(h->s_in);
     if (h->s_out) cudaStreamDestroy(h->s_out);
@@ -412,6 +463,28 @@ mc_status mc_reset(mc_handle* h) try {
     CK(cudaStreamSynchronize(h->stream));
     reset_modes(h);
     tracker_reset(h);
+    return MC_OK;
+} catch (...) { return on_exception(h); }
+
+mc_status mc_restart_lane(mc_handle* h, int lane) try {
+    if (!h) return MC_ERR_INVALID;
+    if (lane < 0 || lane >= h->lanes) { h->err = "lane out of range"; return MC_ERR_INVALID; }
+    if (h->lanes == 1) return mc_reset(h);
+    h->has_state[(size_t)lane] = 0;   // taken into the next frame call's ops; frames in flight are not affected
+    return MC_OK;
+} catch (...) { return on_exception(h); }
+
+mc_status mc_hold_lane(mc_handle* h, int lane, int hold) try {
+    if (!h) return MC_ERR_INVALID;
+    if (lane < 0 || lane >= h->lanes) { h->err = "lane out of range"; return MC_ERR_INVALID; }
+    h->hold[(size_t)lane] = hold != 0;
+    return MC_OK;
+} catch (...) { return on_exception(h); }
+
+mc_status mc_lane_produced(mc_handle* h, uint8_t* produced, int n) try {
+    if (!h || !produced) return MC_ERR_INVALID;
+    if (n != h->lanes) { h->err = "n must equal the handle's lanes"; return MC_ERR_INVALID; }
+    std::memcpy(produced, h->lane_produced.data(), (size_t)n);
     return MC_OK;
 } catch (...) { return on_exception(h); }
 
@@ -454,7 +527,7 @@ mc_status mc_process_device(mc_handle* h, const uint8_t* d_in, int width, int he
                             const mc_params* p, uint8_t* d_out, size_t out_step, int* produced) try {
     if (!h || !produced) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    return process_device_impl(h, d_in, width, height, channels, in_step, p, d_out, out_step, produced);
+    return process_device_impl(h, d_in, width, height, channels, in_step, p, d_out, out_step, produced, h->lane_produced.data());
 } catch (...) { return on_exception(h); }
 
 // submit with the destination known up front: when `in`/`out` are pinned (cudaHostAlloc /
@@ -477,7 +550,7 @@ mc_status mc_submit(mc_handle* h, const uint8_t* in, int width, int height, int 
     if (have && out && out_step < row) { h->err = "out_step too small"; return MC_ERR_INVALID; }
     if (!have) {
         int produced = 0;
-        st = process_device_impl(h, nullptr, 0, 0, channels, 0, p, nullptr, 0, &produced);
+        st = process_device_impl(h, nullptr, 0, 0, channels, 0, p, nullptr, 0, &produced, s.lane_produced.data());
         if (st != MC_OK) return st;
         CK(cudaEventRecord(s.ev_done, h->stream));
         h->inflight.push_back(si);
@@ -495,19 +568,32 @@ mc_status mc_submit(mc_handle* h, const uint8_t* in, int width, int height, int 
     CK(cudaEventRecord(s.ev_in, h->s_in));
     CK(cudaStreamWaitEvent(h->stream, s.ev_in, 0));
     int produced = 0;
-    st = process_device_impl(h, s.d_in, width, height, channels, row, p, s.d_out, row, &produced);
+    st = process_device_impl(h, s.d_in, width, height, channels, row, p, s.d_out, row, &produced, s.lane_produced.data());
     if (st != MC_OK) return st;
     s.produced = produced;
     CK(cudaEventRecord(s.ev_k, h->stream));
     if (produced) {
         CK(cudaStreamWaitEvent(h->s_out, s.ev_k, 0));
-        if (out && is_pinned(out)) {
-            if (out_step == row) CK(cudaMemcpyAsync(out, s.d_out, bytes, cudaMemcpyDeviceToHost, h->s_out));
-            else CK(cudaMemcpy2DAsync(out, out_step, s.d_out, row, row, rows, cudaMemcpyDeviceToHost, h->s_out));
-            s.direct_out = true;
-        } else if (out) {
-            CK(cudaMemcpyAsync(s.h_out, s.d_out, bytes, cudaMemcpyDeviceToHost, h->s_out));
+        // only the lanes that produced are downloaded: one copy per run of consecutive produced lanes (one in all when
+        // every lane produced); the bytes of the other lanes in `out` are left as they are
+        const bool direct = out && is_pinned(out);
+        const size_t lane_bytes = row * (size_t)height;
+        for (int a = 0; a < h->lanes && out;) {
+            if (!s.lane_produced[(size_t)a]) { ++a; continue; }
+            int b = a;
+            while (b < h->lanes && s.lane_produced[(size_t)b]) ++b;
+            const size_t n = (size_t)(b - a) * lane_bytes, run_rows = (size_t)(b - a) * height;
+            const uint8_t* src = s.d_out + (size_t)a * lane_bytes;
+            if (direct) {
+                uint8_t* dst = out + (size_t)a * height * out_step;
+                if (out_step == row) CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, h->s_out));
+                else CK(cudaMemcpy2DAsync(dst, out_step, src, row, row, run_rows, cudaMemcpyDeviceToHost, h->s_out));
+            } else {
+                CK(cudaMemcpyAsync(s.h_out + (size_t)a * lane_bytes, src, n, cudaMemcpyDeviceToHost, h->s_out));
+            }
+            a = b;
         }
+        s.direct_out = direct;
         CK(cudaEventRecord(s.ev_done, h->s_out));
     } else {
         CK(cudaEventRecord(s.ev_done, h->stream));
@@ -528,9 +614,13 @@ mc_status mc_collect(mc_handle* h, int* produced) try {
     Slot& s = h->slots[(size_t)si];
     CK(cudaEventSynchronize(s.ev_done));
     *produced = s.produced;
+    h->lane_produced = s.lane_produced;
     if (s.produced && !s.direct_out && s.user_out) {
-        const size_t row = (size_t)s.w * s.c, rows = (size_t)s.h * h->lanes;
-        for (size_t r = 0; r < rows; ++r) std::memcpy(s.user_out + r * s.user_out_step, s.h_out + r * row, row);
+        const size_t row = (size_t)s.w * s.c;
+        for (int l = 0; l < h->lanes; ++l) {
+            if (!s.lane_produced[(size_t)l]) continue;
+            for (size_t r = (size_t)l * s.h; r < (size_t)(l + 1) * s.h; ++r) std::memcpy(s.user_out + r * s.user_out_step, s.h_out + r * row, row);
+        }
     }
     return MC_OK;
 } catch (...) { return on_exception(h); }
@@ -655,9 +745,10 @@ extern "C" mc_status mc_chain_process(mc_handle* h, const uint8_t* in, int width
     CK(cudaSetDevice(h->device));
     if (h->lanes != 1) { h->err = "mc_chain_process needs a 1-lane handle"; return MC_ERR_INVALID; }
     if (!h->inflight.empty()) { h->err = "mc_chain_process called with pipelined frames in flight"; return MC_ERR_INVALID; }
+    if (h->hold[0]) { h->err = "mc_chain_process called while lane 0 is held"; return MC_ERR_INVALID; }
     int produced = 0;
     if (in == nullptr || width <= 0 || height <= 0) {   // empty image: every stage is an identity (PreprocessProcessor.cpp:11)
-        return process_device_impl(h, nullptr, 0, 0, channels, 0, p, nullptr, 0, &produced);
+        return process_device_impl(h, nullptr, 0, 0, channels, 0, p, nullptr, 0, &produced, h->lane_produced.data());
     }
     if (channels != 1 && channels != 3) { h->err = "channels must be 1 or 3"; return MC_ERR_INVALID; }
     const size_t row = (size_t)width * channels;
@@ -725,7 +816,7 @@ extern "C" mc_status mc_chain_process(mc_handle* h, const uint8_t* in, int width
     // ---- MagnificationProcessor::process on the chain's current frame
     const size_t crow = (size_t)cw * cc;
     if ((st = grow(h, &h->c_out, &h->c_out_b, crow * chh)) != MC_OK) return st;
-    st = process_device_impl(h, cur, cw, chh, cc, crow, p, h->c_out, crow, &produced);
+    st = process_device_impl(h, cur, cw, chh, cc, crow, p, h->c_out, crow, &produced, h->lane_produced.data());
     if (st != MC_OK) return st;
     info->magnified = produced;
     const uint8_t* result = produced ? h->c_out : cur;

@@ -45,6 +45,15 @@ void gaussian_kernel_13_3(float taps[13]);
 void build_area_tab(int ssize, int dsize, double scale, std::vector<AreaTap>& tab, std::vector<int>& ofs);
 void preprocess_roi(int cols, int rows, bool enabled, float rx, float ry, float rw, float rh, int& x, int& y, int& w, int& h);
 
+// What one frame call does to one lane (stream) of a multi-lane handle.  The kernels read a per-frame device array of
+// these, indexed by lane; a null array means every lane is RUN (the handle's uniform first frame is the `first` flag).
+enum LaneOp : uint8_t {
+    LANE_RUN = 0,     // the lane has temporal state: the ordinary frame
+    LANE_FIRST = 1,   // the lane has no state: this frame is its first frame
+    LANE_HOLD = 2,    // the lane is held: its state and its bytes of `out` are left untouched
+};
+__host__ __device__ __forceinline__ int lane_op(const uint8_t* ops, int lane) { return ops ? (int)ops[lane] : (int)LANE_RUN; }
+
 // ------------------------------------------------------------------------------------------------
 // Laplace launchers (mc_laplace.cu).  All take the handle's stream; every call is one kernel launch
 // and returns the launch's cudaError_t (cudaGetLastError()).
@@ -55,6 +64,7 @@ struct FrameIO {
     uint8_t* out = nullptr;
     size_t out_step = 0, out_lane_stride = 0;
     int w = 0, h = 0, channels = 0, lanes = 0;
+    const uint8_t* ops = nullptr;  // device LaneOp per lane of this FrameIO (already offset to its first lane) or null
 };
 
 // u8 BGR frame -> Lab int16 planes [lanes*3][h][pitch16] (exact OpenCV LUT values, SURVEY A.3)
@@ -84,6 +94,7 @@ struct LevelArgs {
     float gain = 0;
     const void* tmap = nullptr;   // CUtensorMap of the f32 input planes (TMA-staged tile) or null
     const void* tmap_hi = nullptr, *tmap_lo = nullptr;   // CUtensorMaps of the state planes: prefetch their tiles too
+    const uint8_t* ops = nullptr;   // device LaneOp per lane (plane / channels) or null: HOLD skips, FIRST acts as `first`
 };
 // 128-byte opaque CUtensorMap storage + encoder for the level kernel's (72 x 39 x 1) box
 struct alignas(64) TensorMapStorage { unsigned char bytes[128]; };
@@ -106,14 +117,16 @@ struct BandSrc {
 };
 
 // out_l = pyrUp(coarse) + fine (SpatialFilter.cpp:52-61); `out` may be the stored fine plane itself (in place)
+// (ops: device LaneOp per lane of `channels` planes, or null; HOLD lanes are skipped)
 cudaError_t launch_collapse(const Level& lf, const Level& lc, const BandSrc& fine, const BandSrc& coarse, float* out, int planes,
-                            cudaStream_t s);
+                            cudaStream_t s, const uint8_t* ops = nullptr, int channels = 1);
 
 // out = convert(input + chroma * pyrUp(pyrUp(c2) + m1)) (MagnifyCore.hpp:136-158).
 // m1.a == nullptr: no motion; c2.a == nullptr: cur_1 = m1.  C == 3 reads `lab`, C == 1 reads io.in.
+// io.ops: HOLD lanes are skipped, and with first_only also RUN lanes (analysis_only: only FIRST lanes are converted).
 cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16_t* lab, int pitch16, size_t plane16,
                           const BandSrc& m1, const Level& l1, const BandSrc& c2, const Level& l2, float chroma,
-                          float* float_out_or_null, cudaStream_t s, int strip = 20);
+                          float* float_out_or_null, cudaStream_t s, int strip = 20, bool first_only = false);
 
 // PreprocessProcessor + GrayscaleProcessor on the device (mc_preprocess.cu)
 cudaError_t launch_preprocess(const uint8_t* src_roi, size_t step, int cn, int sw, int sh, int dw, int dh, bool copy_only,

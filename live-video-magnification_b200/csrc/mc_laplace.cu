@@ -50,8 +50,9 @@ __device__ __forceinline__ float band_of(float hi, float lo, float gain) { retur
 __global__ void __launch_bounds__(256) k_lab16(const uint8_t* __restrict__ in, size_t in_step, size_t in_lane_stride,
                                                int w, int h, const LabLutCell* __restrict__ lut,
                                                int16_t* __restrict__ lab, int pitch16, size_t plane16, int aligned,
-                                               float* __restrict__ lf, int lf_pitch, size_t lf_plane) {
+                                               float* __restrict__ lf, int lf_pitch, size_t lf_plane, const uint8_t* __restrict__ ops) {
     const int lane = blockIdx.z;
+    if (lane_op(ops, lane) == LANE_HOLD) return;
     const int y = blockIdx.y;
     const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     if (x >= w) return;
@@ -148,6 +149,7 @@ struct LevelKArgs {
     double c_hi, omc_hi, c_lo, omc_lo;
     float gain;
     int in_vec_ok;            // u8 rows are 4-byte aligned
+    const uint8_t* ops;       // LaneOp per lane or null
 };
 
 // PREFETCH (with USE_TMA): the tile's two state planes are requested as bulk-tensor copies at kernel entry, together
@@ -162,8 +164,11 @@ __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_
     __shared__ __align__(128) float sS[PREFETCH ? 2 : 1][PREFETCH ? TH : 1][PREFETCH ? TW : 4];   // hi / lo tiles
     __shared__ __align__(8) uint64_t tma_bar;
     __shared__ __align__(8) uint64_t st_bar;
-    const bool prefetch = PREFETCH && a.band && !a.first;
     const int plane = blockIdx.z;
+    const int op = lane_op(a.ops, plane / a.channels);
+    if (op == LANE_HOLD) return;                     // held lane: state and G_{l+1} are left as they are
+    const bool first = a.first || op == LANE_FIRST;  // this lane's first frame: hi = lo = band
+    const bool prefetch = PREFETCH && a.band && !first;
     const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH;
     const int wf = a.lf.w, hf = a.lf.h, wc = a.lc.w, hc = a.lc.h;
     const bool interior = x0 >= 4 && x0 + TW + 4 <= wf && y0 >= 4 && y0 + TH + 3 <= hf && (KIND != IN_U8 || a.in_vec_ok);
@@ -304,10 +309,13 @@ __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_
         float band[4] = {gv.x - up[ry][0], gv.y - up[ry][1], gv.z - up[ry][2], gv.w - up[ry][3]};
         const size_t o = (size_t)gy * a.lf.pitch + gx;
         // rows are padded to a multiple of 32 floats, so a full float4 at gx < wf is always in-bounds
-        if (a.first) {
+        if (first) {
             const float4 b4 = make_float4(band[0], band[1], band[2], band[3]);
             *reinterpret_cast<float4*>(hi + o) = b4;
             *reinterpret_cast<float4*>(lo + o) = b4;
+            // a lane's first frame among running lanes: its stored amplified band is gain * (hi - lo) = +-0
+            if (m) *reinterpret_cast<float4*>(m + o) = make_float4((band[0] - band[0]) * a.gain, (band[1] - band[1]) * a.gain,
+                                                                   (band[2] - band[2]) * a.gain, (band[3] - band[3]) * a.gain);
         } else {
             float4 h4, l4;
             if (prefetch) {
@@ -385,12 +393,14 @@ struct DownArgs {
     Level lf, lc;
     float* g_next;
     int in_vec_ok;
+    const uint8_t* ops;   // LaneOp per lane or null
 };
 
 template <int KIND>
 __global__ void __launch_bounds__(32 * DS_WARPS) k_down_strip(const DownArgs a) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int plane = blockIdx.z;
+    if (lane_op(a.ops, plane / a.channels) == LANE_HOLD) return;
     const int wf = a.lf.w, hf = a.lf.h, wc = a.lc.w, hc = a.lc.h;
     const int gx = blockIdx.x * DS_COLS - 4 + lane * 4;               // first fine column of this lane (multiple of 4)
     const int k0 = (blockIdx.y * DS_WARPS + warp) * DS_ROWS;          // first coarse row of this warp
@@ -454,6 +464,7 @@ struct IngestArgs {
     const LabLutCell* lut;
     int16_t* lab; int pitch16; size_t plane16;
     float* g1; Level l1;
+    const uint8_t* ops;   // LaneOp per lane or null
 };
 
 struct IgRaw { uint32_t w0, w1, w2; };   // 4 BGR pixels of one lane
@@ -515,6 +526,7 @@ template <int WARPS>
 __global__ void __launch_bounds__(32 * WARPS) k_ingest_lab(const IngestArgs a) {
     const int lane_id = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int lane = blockIdx.z;                                       // stream
+    if (lane_op(a.ops, lane) == LANE_HOLD) return;
     const int gx = blockIdx.x * DS_COLS - 4 + lane_id * 4;
     const int k0 = (blockIdx.y * WARPS + warp) * IG_ROWS;
     const int wc = a.l1.w, hc = a.l1.h;
@@ -592,9 +604,11 @@ __device__ __forceinline__ float band_at(const BandSrc& b, size_t off) {
     return b.b ? band_of(v, __ldg(b.b + off), b.gain) : v;
 }
 
-__global__ void __launch_bounds__(256) k_collapse(Level lf, Level lc, BandSrc fine, BandSrc coarse, float* out) {
+__global__ void __launch_bounds__(256) k_collapse(Level lf, Level lc, BandSrc fine, BandSrc coarse, float* out,
+                                                  const uint8_t* __restrict__ ops, int channels) {
     __shared__ __align__(16) float sD[DH][DP];
     const int plane = blockIdx.z;
+    if (lane_op(ops, plane / channels) == LANE_HOLD) return;
     const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH;
     const size_t cbase = (size_t)plane * lc.plane;
     for (int i = threadIdx.x; i < DH * DW; i += 256) {
@@ -660,7 +674,14 @@ struct EgressArgs {
     BandSrc c2; Level l2;           // collapsed level 2 (or band 2 from state when it is the top band); a == null: cur_1 = m_1
     float chroma;
     float* fout;
+    const uint8_t* ops;             // LaneOp per lane or null: HOLD lanes are skipped
+    int first_only;                 // skip RUN lanes too (analysis_only frames convert only the lanes' first frames)
 };
+
+__device__ __forceinline__ bool egress_skips(const EgressArgs& a, int lane) {
+    const int op = lane_op(a.ops, lane);
+    return op == LANE_HOLD || (a.first_only && op == LANE_RUN);
+}
 
 // The pixel stage of egress for the 4 output pixels (gy, gx .. gx+3) of stream `lane`: input (+ motion `up`, the a / b
 // planes attenuated by chroma) -> Lab2BGR -> u8 (MagnifyCore.hpp:140-158).  Split into the load of the input samples
@@ -774,6 +795,7 @@ __global__ void __launch_bounds__(256) k_egress(const EgressArgs a) {
     __shared__ __align__(16) float sT[C][E2H][DP];    // horizontal pyrUp pass of the level-2 window rows
     __shared__ __align__(16) float sD[C][DH][DP];
     const int lane = blockIdx.z;
+    if (egress_skips(a, lane)) return;
     const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH;
     const int w1 = a.l1.w, h1 = a.l1.h;
     if (a.m1.a) {
@@ -931,7 +953,7 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
     const int lane = blockIdx.z;
     const int gx = blockIdx.x * DS_COLS - 4 + lane_id * 4;          // first output column of this lane (multiple of 4)
     const int f0 = blockIdx.y * EG_ROWS;
-    if (f0 >= a.h0) return;
+    if (f0 >= a.h0 || egress_skips(a, lane)) return;
     const int f_end = min(f0 + EG_ROWS, a.h0);
     const bool px_owner = lane_id >= 1 && lane_id <= 30 && gx < a.w0;
     if (!a.m1.a) {   // no motion (first frame, or fewer than two levels): conversion only
@@ -1235,7 +1257,7 @@ cudaError_t launch_lab16(const FrameIO& io, const DeviceTables& tb, int16_t* lab
                          cudaStream_t s, float* l_f32, int l_pitch, size_t l_plane) {
     const int aligned = (reinterpret_cast<uintptr_t>(io.in) % 4 == 0) && (io.in_step % 4 == 0) && (io.in_lane_stride % 4 == 0);
     dim3 grid(cdiv(cdiv(io.w, 4), 256), io.h, io.lanes);
-    k_lab16<<<grid, 256, 0, s>>>(io.in, io.in_step, io.in_lane_stride, io.w, io.h, tb.lab_lut, lab, pitch16, plane16, aligned, l_f32, l_pitch, l_plane);
+    k_lab16<<<grid, 256, 0, s>>>(io.in, io.in_step, io.in_lane_stride, io.w, io.h, tb.lab_lut, lab, pitch16, plane16, aligned, l_f32, l_pitch, l_plane, io.ops);
     return cudaGetLastError();
 }
 
@@ -1246,6 +1268,7 @@ cudaError_t launch_ingest_lab(const FrameIO& io, const DeviceTables& tb, int16_t
     a.w = io.w; a.h = io.h;
     a.aligned = (reinterpret_cast<uintptr_t>(io.in) % 4 == 0) && (io.in_step % 4 == 0) && (io.in_lane_stride % 4 == 0);
     a.lut = tb.lab_lut; a.lab = lab; a.pitch16 = pitch16; a.plane16 = plane16; a.g1 = g1; a.l1 = l1;
+    a.ops = io.ops;
     if (warps != 2 && warps != 4) warps = 1;
     dim3 grid(cdiv(io.w, DS_COLS), cdiv(l1.h, IG_ROWS * warps), io.lanes);
     if (warps == 4) k_ingest_lab<4><<<grid, 128, 0, s>>>(a);
@@ -1262,6 +1285,7 @@ cudaError_t launch_level(const LevelArgs& a, cudaStream_t s) {
     k.first = a.first; k.band = a.band;
     k.c_hi = a.c_hi; k.omc_hi = a.one_minus_c_hi; k.c_lo = a.c_lo; k.omc_lo = a.one_minus_c_lo;
     k.gain = a.gain;
+    k.ops = a.ops;
     k.in_vec_ok = a.in_kind == IN_U8 ? ((reinterpret_cast<uintptr_t>(a.g) % 4 == 0) && (a.in_row % 4 == 0) && (a.in_plane % 4 == 0)) : 1;
     dim3 grid(cdiv(a.lf.w, TW), cdiv(a.lf.h, TH), a.planes);
     static const CUtensorMap dummy{};
@@ -1281,6 +1305,7 @@ cudaError_t launch_down(const LevelArgs& a, cudaStream_t s) {
     k.g = a.g; k.in_plane = a.in_plane; k.in_row = a.in_row; k.channels = a.channels;
     for (int i = 0; i < 3; ++i) { k.sc[i] = a.sc[i]; k.of[i] = a.of[i]; }
     k.lf = a.lf; k.lc = a.lc; k.g_next = a.g_next;
+    k.ops = a.ops;
     k.in_vec_ok = a.in_kind == IN_U8 ? ((reinterpret_cast<uintptr_t>(a.g) % 4 == 0) && (a.in_row % 4 == 0) && (a.in_plane % 4 == 0)) : 1;
     dim3 grid(cdiv(a.lf.w, DS_COLS), cdiv(a.lc.h, DS_ROWS * DS_WARPS), a.planes);
     if (a.in_kind == IN_F32) k_down_strip<IN_F32><<<grid, 32 * DS_WARPS, 0, s>>>(k);
@@ -1290,15 +1315,15 @@ cudaError_t launch_down(const LevelArgs& a, cudaStream_t s) {
 }
 
 cudaError_t launch_collapse(const Level& lf, const Level& lc, const BandSrc& fine, const BandSrc& coarse, float* out, int planes,
-                            cudaStream_t s) {
+                            cudaStream_t s, const uint8_t* ops, int channels) {
     dim3 grid(cdiv(lf.w, TW), cdiv(lf.h, TH), planes);
-    k_collapse<<<grid, 256, 0, s>>>(lf, lc, fine, coarse, out);
+    k_collapse<<<grid, 256, 0, s>>>(lf, lc, fine, coarse, out, ops, channels);
     return cudaGetLastError();
 }
 
 cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16_t* lab, int pitch16, size_t plane16,
                           const BandSrc& m1, const Level& l1, const BandSrc& c2, const Level& l2, float chroma,
-                          float* fout, cudaStream_t s, int strip) {
+                          float* fout, cudaStream_t s, int strip, bool first_only) {
     EgressArgs a;
     a.in = io.in; a.in_step = io.in_step; a.in_lane_stride = io.in_lane_stride;
     a.lab = lab; a.pitch16 = pitch16; a.plane16 = plane16;
@@ -1306,6 +1331,7 @@ cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16
     a.w0 = io.w; a.h0 = io.h;
     a.gtab = tb.inv_gamma; a.coeffs = tb.inv_coeffs;
     a.m1 = m1; a.l1 = l1; a.c2 = c2; a.l2 = l2; a.chroma = chroma; a.fout = fout;
+    a.ops = io.ops; a.first_only = first_only ? 1 : 0;
     if (strip) {
         dim3 grid(cdiv(io.w, DS_COLS), cdiv(io.h, EG_ROWS), io.lanes);
         // the register cap (resident warps per SM) is an A/B knob: 16 -> <= 128 registers, 20 -> 96, 24 -> 80

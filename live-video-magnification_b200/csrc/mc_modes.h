@@ -45,6 +45,45 @@ struct ModeCtx {
     int lane_groups;        // Laplace: number of lane groups run as concurrent launch chains (option "lane_groups"; 0 = automatic)
     bool analysis_only;     // Laplace / Phase: update the temporal state but skip synthesis + egress (*produced = 0); used by the
                             // state-carry pass of temporal sharding (SURVEY 8f-3, lvm_b200.shard.magnify_segment)
+    // Lane lifecycle (mc_restart_lane / mc_hold_lane): the handle's LaneOp per lane for this frame, the device buffer the
+    // mode uploads its per-lane ops to (stream-ordered: the previous frame's kernels have read it before the copy runs),
+    // and the mode's answers: which lanes produced, and whether held lanes lost their state (reallocation, Phase cutoff change).
+    const uint8_t* lane_ops = nullptr;   // host, `lanes` entries
+    uint8_t* d_lane_ops = nullptr;       // device, `lanes` bytes
+    uint8_t* lane_produced = nullptr;    // host, `lanes` entries (written)
+    bool* held_lost = nullptr;           // (written)
+};
+
+// The per-lane ops of one frame as a mode runs it: the handle's ops, with every lane that is not held turned into FIRST
+// when the mode itself holds no state (first frame after allocation).
+struct LanePlan {
+    std::vector<uint8_t> op;
+    int n_run = 0, n_first = 0, n_hold = 0;
+    void make(const uint8_t* ops, int lanes, bool all_first) {
+        op.assign(ops, ops + lanes);
+        n_run = n_first = n_hold = 0;
+        for (uint8_t& o : op) {
+            if (all_first && o == LANE_RUN) o = LANE_FIRST;
+            (o == LANE_HOLD ? n_hold : o == LANE_FIRST ? n_first : n_run)++;
+        }
+    }
+    bool mixed() const { return n_hold > 0 || (n_run > 0 && n_first > 0); }
+    // Mixed frames upload the ops and return the device array; uniform frames return null (the kernels' default path).
+    cudaError_t upload(const ModeCtx& ctx, const uint8_t** d_ops) const {
+        *d_ops = nullptr;
+        if (!mixed()) return cudaSuccess;
+        *d_ops = ctx.d_lane_ops;
+        // pageable source: staged before the call returns, so `op` may change right after
+        return cudaMemcpyAsync(ctx.d_lane_ops, op.data(), op.size(), cudaMemcpyHostToDevice, ctx.stream);
+    }
+    void produced(const ModeCtx& ctx, bool run_produces, bool first_produces, int* any) const {
+        *any = 0;
+        for (size_t l = 0; l < op.size(); ++l) {
+            const bool p = op[l] == LANE_RUN ? run_produces : op[l] == LANE_FIRST ? first_produces : false;
+            ctx.lane_produced[l] = p ? 1 : 0;
+            *any |= p ? 1 : 0;
+        }
+    }
 };
 
 // Launch bookkeeping shared by the mode drivers: counts the launch, optionally brackets it with events.
@@ -118,6 +157,7 @@ struct MotionMode {
     cudaEvent_t ev_fork = nullptr;
     int groups_req = 0;                    // ModeCtx::lane_groups at allocation time
     std::vector<float> gains;              // per-level gains of the current frame (member: no per-frame allocation)
+    LanePlan plan;                         // per-lane ops of the current frame
 
     void reset();
     mc_status process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced);
@@ -180,13 +220,14 @@ struct RieszMode {
     // TMA descriptors of the 9x9 kernels' input tiles (72 x 24 boxes): octave i (analysis), amplified band i (collapse)
     std::vector<TensorMapStorage> tm_oct, tm_band;
     std::vector<char> tm_valid;
+    LanePlan plan;              // per-lane ops of the current frame
 
     void reset();
     mc_status process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced);
     void find_state(const char* name, int level, StateRef& out);
 
 private:
-    mc_status build_pyramid(const ModeCtx& ctx);
+    mc_status build_pyramid(const ModeCtx& ctx, const uint8_t* ops);
 };
 
 }  // namespace mc

@@ -128,15 +128,26 @@ mc_status MotionMode::allocate(const ModeCtx& ctx, const FrameIO& io, int nlevel
     return MC_OK;
 }
 
-mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int nlevels, int* produced) {
+mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_params& p, int nlevels, int* produced) {
+    *produced = 0;
     if (!allocated || faithful != ctx.faithful0 || from_state != ctx.band_from_state) {
-        mc_status st = allocate(ctx, io, nlevels);
+        if (allocated) *ctx.held_lost = true;
+        mc_status st = allocate(ctx, io_in, nlevels);
         if (st != MC_OK) return st;
     } else if (groups_req != ctx.lane_groups) {
         mc_status st = make_groups(ctx);
         if (st != MC_OK) return st;
     }
-    const bool first = empty;  // MagnifyCore.hpp:98
+    // Per-lane ops: a lane without state takes its first frame (MagnifyCore.hpp:98-103) while the others run; a held lane is
+    // skipped by every kernel.  Uniform frames pass no op array and `first` says which of the two paths all lanes take.
+    plan.make(ctx.lane_ops, lanes, empty);
+    if (plan.n_hold == lanes) {   // every lane held: nothing to do
+        plan.produced(ctx, false, false, produced);
+        return MC_OK;
+    }
+    const bool first = plan.n_first == lanes;  // MagnifyCore.hpp:98
+    FrameIO io = io_in;
+    MCK(plan.upload(ctx, &io.ops));
     motion_gains(p.amplification, p.coWavelength, levels, w, h, gains);
     double c_lo = p.coLow, c_hi = p.coHigh;
     if (c_lo == 0) c_lo = 0.01;  // TemporalFilter.cpp:11-12
@@ -158,12 +169,9 @@ mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_pa
             MCK(cudaStreamWaitEvent(ctx.stream, g.done, 0));
         }
     }
-    if (ctx.analysis_only && !first) {   // state-carry pass: the temporal state is up to date, no frame is produced
-        *produced = 0;
-        return MC_OK;
-    }
     empty = false;
-    *produced = 1;
+    // state-carry pass (analysis_only): the temporal state is up to date, only first frames are produced
+    plan.produced(ctx, !ctx.analysis_only || first, true, produced);
     return MC_OK;
 }
 
@@ -173,6 +181,7 @@ mc_status MotionMode::run_group(const ModeCtx& ctx, const FrameIO& io_all, const
     io.in = io_all.in + (size_t)g.lane0 * io_all.in_lane_stride;
     io.out = io_all.out + (size_t)g.lane0 * io_all.out_lane_stride;
     io.lanes = g.lanes;
+    if (io.ops) io.ops += g.lane0;   // the op array is indexed by the handle's lane
     const int planes = g.lanes * channels;
     const size_t p0 = (size_t)g.lane0 * channels;
     auto off = [&](float* base, int l) { return base ? base + p0 * lv[(size_t)l].plane : nullptr; };
@@ -215,6 +224,7 @@ mc_status MotionMode::run_group(const ModeCtx& ctx, const FrameIO& io_all, const
         a.band = (l >= 1 || faithful) ? 1 : 0;
         a.c_hi = c_hi; a.one_minus_c_hi = 1 - c_hi; a.c_lo = c_lo; a.one_minus_c_lo = 1 - c_lo;
         a.gain = gains[(size_t)l];
+        a.ops = io.ops;
         if (a.band) LAUNCH("level", l, launch_level(a, ctx.stream));
         else LAUNCH("down", l, launch_down(a, ctx.stream));
     }
@@ -223,8 +233,24 @@ mc_status MotionMode::run_group(const ModeCtx& ctx, const FrameIO& io_all, const
         const size_t n = (size_t)planes * lv[(size_t)levels].plane;
         LAUNCH("copy", levels, launch_copy_planes(off(hi[(size_t)levels], levels), off(G[(size_t)levels], levels), n, ctx.stream));
         LAUNCH("copy", levels, launch_copy_planes(off(lo[(size_t)levels], levels), off(G[(size_t)levels], levels), n, ctx.stream));
+    } else if (faithful && io.ops) {   // the same copy for each lane that takes its first frame among running lanes
+        const size_t n = (size_t)channels * lv[(size_t)levels].plane;
+        for (int ln = g.lane0; ln < g.lane0 + g.lanes; ++ln) {
+            if (plan.op[(size_t)ln] != LANE_FIRST) continue;
+            const size_t o = (size_t)ln * n;
+            LAUNCH("copy", levels, launch_copy_planes(hi[(size_t)levels] + o, G[(size_t)levels] + o, n, ctx.stream));
+            LAUNCH("copy", levels, launch_copy_planes(lo[(size_t)levels] + o, G[(size_t)levels] + o, n, ctx.stream));
+        }
     }
-    if (ctx.analysis_only && !first) return MC_OK;
+    const Level& l1 = lv[levels >= 1 ? 1 : 0];
+    const Level& l2 = lv[levels >= 2 ? 2 : 0];
+    if (ctx.analysis_only && !first) {
+        // state-carry pass: lanes on their first frame are still converted (no motion), the running lanes produce nothing
+        if (plan.n_first > 0)
+            LAUNCH("egress", 0, launch_egress(io, *ctx.tables, lab, pitch16, plane16, BandSrc{}, l1, BandSrc{}, l2, (float)p.chromAttenuation,
+                                              fout, ctx.stream, ctx.egress_strip, true));
+        return MC_OK;
+    }
     BandSrc m1, c2;
     if (!first && levels >= 2) {
         // synthesis: residual and finest band are zero (MagnifyCore.hpp:130-131), so the collapse starts from
@@ -234,12 +260,11 @@ mc_status MotionMode::run_group(const ModeCtx& ctx, const FrameIO& io_all, const
         };
         auto cur = [&](int l) { return l == levels - 1 ? band(l) : BandSrc{off(M[(size_t)l], l), nullptr, 1.0f}; };
         for (int l = levels - 2; l >= 2; --l)
-            LAUNCH("collapse", l, launch_collapse(lv[(size_t)l], lv[(size_t)l + 1], band(l), cur(l + 1), off(M[(size_t)l], l), planes, ctx.stream));
+            LAUNCH("collapse", l, launch_collapse(lv[(size_t)l], lv[(size_t)l + 1], band(l), cur(l + 1), off(M[(size_t)l], l), planes, ctx.stream,
+                                                  io.ops, channels));
         m1 = band(1);
         if (levels >= 3) c2 = cur(2);
     }
-    const Level& l1 = lv[levels >= 1 ? 1 : 0];
-    const Level& l2 = lv[levels >= 2 ? 2 : 0];
     LAUNCH("egress", 0, launch_egress(io, *ctx.tables, lab, pitch16, plane16, m1, l1, c2, l2, (float)p.chromAttenuation, fout,
                                       ctx.stream, ctx.egress_strip));
     return MC_OK;

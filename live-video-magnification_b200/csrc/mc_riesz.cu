@@ -103,10 +103,12 @@ __device__ __forceinline__ void r9_load_tile(float (*s)[R9_SW], const float* __r
 // hp = filter2D(oct, HP) ; next = subsample(filter2D(oct, 2*LP))   (REFLECT_101, correlation)
 __global__ void __launch_bounds__(256) k_riesz_analysis(Level l, Level ln, const float* __restrict__ oct,
                                                         float* __restrict__ hp, float* __restrict__ next,
-                                                        const __grid_constant__ CUtensorMap tm, int use_tma) {
+                                                        const __grid_constant__ CUtensorMap tm, int use_tma,
+                                                        const uint8_t* __restrict__ ops) {
     __shared__ __align__(128) float s[R9_SH][R9_SW];
     __shared__ __align__(8) uint64_t bar;
-    const int plane = blockIdx.z;
+    const int plane = blockIdx.z;   // one plane (L) per lane
+    if (lane_op(ops, plane) == LANE_HOLD) return;
     const int x0 = blockIdx.x * R9_W, y0 = blockIdx.y * R9_H;
     if (use_tma) {
         if (threadIdx.x == 0) mbar_init(&bar, 1);
@@ -184,6 +186,8 @@ struct PhaseArgs {
     float *lo_r0c, *lo_r0s, *lo_r1c, *lo_r1s, *hi_r0c, *hi_r0s, *hi_r1c, *hi_r1s;
     float *amp, *t_c, *t_s;                // amplitude, (hiIIR - loIIR) * amplitude
     Butter lo, hi;
+    float* cur_low;                        // == low, written only for held lanes
+    const uint8_t* ops;                    // LaneOp per lane or null
 };
 
 __device__ __forceinline__ float muld(float x, double s) { return (float)((double)x * s); }  // cv::multiply(Mat, double)
@@ -202,6 +206,26 @@ __global__ void __launch_bounds__(256) k_riesz_phase(const PhaseArgs a) {
     const int x0 = blockIdx.x * RT_W, y0 = blockIdx.y * RT_H;
     const Level l = a.l;
     const size_t pb = (size_t)plane * l.plane;
+    const int op = lane_op(a.ops, plane);
+    if (op != LANE_RUN) {
+        for (int i = threadIdx.x; i < RT_H * RT_W; i += 256) {
+            const int gy = y0 + i / RT_W, gx = x0 + i % RT_W;
+            if (gy >= l.h || gx >= l.w) continue;
+            const size_t o = pb + (size_t)gy * l.pitch + gx;
+            if (op == LANE_HOLD) {
+                // the cur <-> old swap after this kernel must hand the held lane its `old` pyramid back unchanged
+                if (a.plow) { a.cur_low[o] = a.plow[o]; a.rx[o] = a.prx[o]; a.ry[o] = a.pry[o]; }
+            } else {
+                // the lane's first frame (RieszPyramid.cpp:196-213, MagnifyCore.hpp:226-240): `old` becomes this frame's
+                // band with a zero Riesz pair, the phases and both filters' registers start at zero
+                a.rx[o] = 0.f; a.ry[o] = 0.f;
+                a.ph_c[o] = 0.f; a.ph_s[o] = 0.f;
+                a.lo_r0c[o] = 0.f; a.lo_r0s[o] = 0.f; a.lo_r1c[o] = 0.f; a.lo_r1s[o] = 0.f;
+                a.hi_r0c[o] = 0.f; a.hi_r0s[o] = 0.f; a.hi_r1c[o] = 0.f; a.hi_r1s[o] = 0.f;
+            }
+        }
+        return;
+    }
     for (int i = threadIdx.x; i < (RT_H + 4) * (RT_W + 4); i += 256) {
         const int r = i / (RT_W + 4), c = i - r * (RT_W + 4);
         s[r][c] = __ldg(a.low + pb + (size_t)reflect101(y0 - 2 + r, l.h) * l.pitch + reflect101(x0 - 2 + c, l.w));
@@ -279,6 +303,7 @@ struct AmpArgs {
     float* out;                            // amplified band
     Gauss13 g;
     float alpha, thresh;
+    const uint8_t* ops;                    // LaneOp per lane or null: only RUN lanes are amplified
 };
 
 // Tile 64 x 16, thread strip 1 x 4 (same row dealing as the 9x9 kernels is not needed here).  Row pass:
@@ -299,6 +324,7 @@ __global__ void __launch_bounds__(256) k_riesz_amplify(const AmpArgs a) {
     __shared__ __align__(16) float s[3][GA_H][GA_W];
     __shared__ __align__(16) float sr[3][GA_H][GA_TW];
     const int plane = blockIdx.z;
+    if (lane_op(a.ops, plane) != LANE_RUN) return;
     const int x0 = blockIdx.x * GA_TW, y0 = blockIdx.y * GA_TH;
     const Level l = a.l;
     const size_t pb = (size_t)plane * l.plane;
@@ -406,11 +432,13 @@ __device__ __forceinline__ void rc_lowpass(const float (*sc)[RC_CW], int y, int 
 
 __global__ void __launch_bounds__(256) k_riesz_collapse(Level l, Level lc, const float* __restrict__ band,
                                                         const float* __restrict__ coarse, float* __restrict__ out,
-                                                        const __grid_constant__ CUtensorMap tm, int use_tma) {
+                                                        const __grid_constant__ CUtensorMap tm, int use_tma,
+                                                        const uint8_t* __restrict__ ops) {
     __shared__ __align__(128) float sb[R9_SH][R9_SW];
     __shared__ __align__(16) float sc[RC_CH][RC_CW];
     __shared__ __align__(8) uint64_t bar;
     const int plane = blockIdx.z;
+    if (lane_op(ops, plane) != LANE_RUN) return;
     const int x0 = blockIdx.x * R9_W, y0 = blockIdx.y * R9_H;
     if (use_tma) {
         if (threadIdx.x == 0) mbar_init(&bar, 1);
@@ -468,9 +496,9 @@ __global__ void __launch_bounds__(256) k_riesz_collapse(Level l, Level lc, const
 __global__ void __launch_bounds__(256) k_riesz_egress(const float* __restrict__ Lp, Level l, const int16_t* __restrict__ lab,
                                                       int pitch16, size_t plane16, const float4* __restrict__ gtab,
                                                       LabInvCoeffs coeffs, uint8_t* __restrict__ out, size_t step,
-                                                      size_t lane_stride, float* __restrict__ fout) {
+                                                      size_t lane_stride, float* __restrict__ fout, const uint8_t* __restrict__ ops) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, lane = blockIdx.z;
-    if (x >= l.w) return;
+    if (x >= l.w || lane_op(ops, lane) != LANE_RUN) return;   // first frames pass through, held lanes are not written
     const float L = Lp[(size_t)lane * l.plane + (size_t)y * l.pitch + x];
     const int16_t* p = lab + (size_t)(lane * 3) * plane16 + (size_t)y * pitch16 + x;
     const float A = fmaf((float)p[plane16], 1.0f / 64.0f, -128.0f);
@@ -508,25 +536,31 @@ void RieszMode::reset() {
         ++*ctx.launches;                                                           \
     } while (0)
 
-mc_status RieszMode::build_pyramid(const ModeCtx& ctx) {
+mc_status RieszMode::build_pyramid(const ModeCtx& ctx, const uint8_t* ops) {
     // RieszPyramid::buildPyramid (RieszPyramid.cpp:215-238); the Riesz pair itself is formed in the phase kernel
     for (int i = 0; i < levels - 1; ++i) {
         const Level& l = lv[(size_t)i];
         dim3 grid(cdiv(l.w, R9_W), cdiv(l.h, R9_H), lanes);
         const int tma = ctx.use_tma && tm_valid[(size_t)i];
         KLAUNCH("riesz_analysis", i, k_riesz_analysis<<<grid, 256, 0, ctx.stream>>>(l, lv[(size_t)i + 1], oct[(size_t)i], cur_low[(size_t)i], oct[(size_t)i + 1],
-                                                                                    *reinterpret_cast<const CUtensorMap*>(&tm_oct[(size_t)i]), tma));
+                                                                                    *reinterpret_cast<const CUtensorMap*>(&tm_oct[(size_t)i]), tma, ops));
     }
     return MC_OK;
 }
 
-mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int nlevels, int* produced) {
+mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_params& p, int nlevels, int* produced) {
     *produced = 0;
-    if (io.channels < 3) return MC_OK;  // MagnifyCore.hpp:212: gray input is a silent passthrough
-    const bool first = !allocated || std::isnan(loA[0]) || std::isnan(hiA[0]);  // :226
+    if (io_in.channels < 3) return MC_OK;  // MagnifyCore.hpp:212: gray input is a silent passthrough
+    // Per-lane ops: lanes without state take their first frame while the others run, held lanes are skipped.  When every
+    // lane is on its first frame the handle's state is rebuilt from scratch, as for the reference's first frame.
+    const bool fresh = !allocated || std::isnan(loA[0]) || std::isnan(hiA[0]);  // :226
+    plan.make(ctx.lane_ops, lanes, fresh);
+    if (plan.n_hold == lanes) return MC_OK;   // every lane held: nothing to do
+    const bool first = fresh || plan.n_first == lanes;
     if (first) {
+        if (allocated) *ctx.held_lost = true;
         reset();
-        levels = nlevels; w = io.w; h = io.h;
+        levels = nlevels; w = io_in.w; h = io_in.h;
         lv.resize((size_t)levels);
         int cw = w, ch = h;
         for (int i = 0; i < levels; ++i) {
@@ -575,9 +609,11 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_par
         design(hi_freq, hiA, hiB);
         allocated = true;
     }
+    FrameIO io = io_in;
+    MCK(plan.upload(ctx, &io.ops));
     // BGR -> Lab; only L is magnified (MagnifyCore.hpp:217-222)
     LAUNCH("lab16", 0, launch_lab16(io, *ctx.tables, lab16, pitch16, plane16, ctx.stream, oct[0], lv[0].pitch, lv[0].plane));
-    mc_status st = build_pyramid(ctx);
+    mc_status st = build_pyramid(ctx, io.ops);
     if (st != MC_OK) return st;
     if (first) {
         // old = pyramid of the first frame with a zero Riesz pair; the frame itself is shown unmagnified (:239)
@@ -587,6 +623,7 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_par
     // cutoff changes re-design the filter, zero both filters' registers and rebuild `old` from this frame (:243-254)
     bool rebuild_old = false;
     auto zero_state = [&]() -> mc_status {
+        *ctx.held_lost = true;   // every lane's registers are zeroed and `old` is rebuilt: a held lane restarts on release
         for (auto* v : {&phase_c, &phase_s, &lo_r0c, &lo_r0s, &lo_r1c, &lo_r1s, &hi_r0c, &hi_r0s, &hi_r1c, &hi_r1s})
             for (int i = 0; i < levels - 1; ++i)
                 MCK(cudaMemsetAsync((*v)[(size_t)i], 0, (size_t)lanes * lv[(size_t)i].plane * sizeof(float), ctx.stream));
@@ -624,6 +661,8 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_par
         a.amp = amp[(size_t)i]; a.t_c = t_c[(size_t)i]; a.t_s = t_s[(size_t)i];
         a.lo = Butter{loB[0], loB[1], loB[2], loA[1], loA[2]};
         a.hi = Butter{hiB[0], hiB[1], hiB[2], hiA[1], hiA[2]};
+        a.cur_low = cur_low[(size_t)i];
+        a.ops = io.ops;
         dim3 grid(cdiv(a.l.w, RT_W), cdiv(a.l.h, RT_H), lanes);
         KLAUNCH("riesz_phase", i, k_riesz_phase<<<grid, 256, 0, ctx.stream>>>(a));
     }
@@ -637,6 +676,7 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_par
         *produced = 0;
         return MC_OK;
     }
+    if (plan.n_run == 0) return MC_OK;   // only first frames (passthrough) and held lanes
     // amplify (RieszPyramid.cpp:248-252) — this frame's band/pair now live in the old_* buffers
     const float alpha = (float)p.amplification;
     const float thresh = (float)(p.coWavelength * (3.14159265358979323846 / 100.0));  // PI_PERCENT, :214,:269
@@ -648,6 +688,7 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_par
         a.out = low_amp[(size_t)i];
         gaussian_kernel_13_3(a.g.k);
         a.alpha = alpha; a.thresh = thresh;
+        a.ops = io.ops;
         dim3 grid(cdiv(a.l.w, GA_TW), cdiv(a.l.h, GA_TH), lanes);
         KLAUNCH("riesz_amplify", i, k_riesz_amplify<<<grid, 256, 0, ctx.stream>>>(a));
     }
@@ -658,14 +699,14 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_par
         dim3 grid(cdiv(l.w, R9_W), cdiv(l.h, R9_H), lanes);
         const int tma = ctx.use_tma && tm_valid[(size_t)i];
         KLAUNCH("riesz_collapse", i, k_riesz_collapse<<<grid, 256, 0, ctx.stream>>>(l, lv[(size_t)i + 1], low_amp[(size_t)i], result, res[(size_t)i],
-                                                                                    *reinterpret_cast<const CUtensorMap*>(&tm_band[(size_t)i]), tma));
+                                                                                    *reinterpret_cast<const CUtensorMap*>(&tm_band[(size_t)i]), tma, io.ops));
         result = res[(size_t)i];
     }
     {
         dim3 grid(cdiv(w, 256), h, lanes);
-        KLAUNCH("riesz_egress", 0, k_riesz_egress<<<grid, 256, 0, ctx.stream>>>(result, lv[0], lab16, pitch16, plane16, ctx.tables->inv_gamma, ctx.tables->inv_coeffs, io.out, io.out_step, io.out_lane_stride, ctx.float_out));
+        KLAUNCH("riesz_egress", 0, k_riesz_egress<<<grid, 256, 0, ctx.stream>>>(result, lv[0], lab16, pitch16, plane16, ctx.tables->inv_gamma, ctx.tables->inv_coeffs, io.out, io.out_step, io.out_lane_stride, ctx.float_out, io.ops));
     }
-    *produced = 1;
+    plan.produced(ctx, true, false, produced);
     return MC_OK;
 }
 

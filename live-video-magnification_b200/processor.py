@@ -165,6 +165,23 @@ class MagnificationProcessor(IProcessor):
         """MagnificationProcessor::reset (MagnificationProcessor.cpp:10-15)."""
         self._check(self._lib.mc_reset(self._h))
 
+    # -- lane lifecycle (multi-stream serving) -----------------------------------------------
+    def restart_lane(self, lane: int) -> None:
+        """The lane's next frame is its first frame (a stream joins, or hits a scene cut); the other lanes run on.
+        On a 1-lane processor this is reset()."""
+        self._check(self._lib.mc_restart_lane(self._h, int(lane)))
+
+    def hold_lane(self, lane: int, hold: bool = True) -> None:
+        """While held, frame calls skip the lane: its temporal state stays as it is and its output is not written
+        (a stream without a new frame this step).  Holds survive reset()."""
+        self._check(self._lib.mc_hold_lane(self._h, int(lane), int(bool(hold))))
+
+    def lane_produced(self) -> np.ndarray:
+        """-> bool[lanes]: which lanes produced an output in the most recent frame call (or collect())."""
+        a = np.zeros(self.lanes, np.uint8)
+        self._check(self._lib.mc_lane_produced(self._h, a.ctypes.data_as(C.POINTER(C.c_uint8)), self.lanes))
+        return a.astype(bool)
+
     def process(self, frame: Frame, cfg: ProcessorConfig) -> Frame:
         """MagnificationProcessor::process (MagnificationProcessor.cpp:17-67)."""
         produced, out = self.process_image(frame.image, cfg)
@@ -181,7 +198,9 @@ class MagnificationProcessor(IProcessor):
         return w, h, c
 
     def process_image(self, image: Optional[np.ndarray], cfg: ProcessorConfig):
-        """-> (produced, out8u or the input image)."""
+        """-> (produced, out8u or the input image).  On a multi-lane processor ``produced`` means "some lane produced",
+        and the lanes that did not (held, or passing through) carry their input frame, as the reference returns the
+        input FrameRef of that stream."""
         p = _to_mc(cfg)
         produced = C.c_int(0)
         if image is None or image.size == 0:
@@ -195,7 +214,13 @@ class MagnificationProcessor(IProcessor):
         out = np.empty_like(img)
         self._check(self._lib.mc_process(self._h, img.ctypes.data, w, h, c, step, C.byref(p), out.ctypes.data, step,
                                          C.byref(produced)))
-        return (True, out) if produced.value else (False, image)
+        if not produced.value:
+            return False, image
+        if self.lanes > 1:
+            idle = ~self.lane_produced()
+            if idle.any():
+                out[idle] = img[idle]
+        return True, out
 
     # -- device-resident / pipelined forms (benchmarks, serving) -----------------------------
     def process_device(self, d_in: int, w: int, h: int, c: int, in_step: int, cfg_or_params, d_out: int,
