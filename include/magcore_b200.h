@@ -144,6 +144,27 @@ mc_status mc_process_device(mc_handle* h, const uint8_t* d_in, int width, int he
                             int* produced);
 mc_status mc_sync(mc_handle* h);
 
+/* --- clips: T = `frames` consecutive frames of every lane in one call (an exporter that knows its clip up front) -----
+ * in/out hold frame t of lane k at (t * lanes + k) * height * step.  produced: frames * lanes bytes, [t][lane].  The
+ * result (out bytes, produced flags, temporal state afterwards, mc_lane_produced = the last frame's flags) is exactly
+ * that of `frames` consecutive mc_process_device calls with the same params and no lifecycle calls in between:
+ * restarts and holds are taken at the clip's first frame, and a held lane is skipped for the whole clip.  A frame that
+ * did not produce leaves its bytes of out untouched.
+ *   Laplace: one launch set for the whole clip.  The spatial kernels run over frames * lanes "virtual lanes", and the
+ *            level kernel carries each tile's temporal state in registers from the first frame to the last, so the
+ *            state planes are read and written once per clip instead of once per frame.  The structural tracker runs
+ *            once, at the clip's first frame; analysis_only produces only the lanes' first frames, as frame calls do.
+ *   Phase, Color: one frame call per frame (same results; the clip call works whatever the mode).
+ * MC_ERR_INVALID, with the state untouched, when frames < 1, frames * lanes > MC_MAX_LANES, produced is NULL or frames of
+ * mc_submit are in flight; the parameter checks of mc_process_device apply unchanged.  Mode None and an empty image
+ * are the identity (all flags 0, state dropped).  A failed clip drops the state like a failed frame.  The clip path
+ * keeps device scratch for the largest clip seen (~29 MB per 1080p colour frame at 6 levels), released by mc_reset. */
+mc_status mc_process_clip_device(mc_handle* h, const uint8_t* d_in, int frames, int width, int height, int channels,
+                                 size_t in_step, const mc_params* p, uint8_t* d_out, size_t out_step, uint8_t* produced);
+/* The same on host pointers, blocking (upload, kernels, download of the produced frames only).  Pinned or pageable. */
+mc_status mc_process_clip(mc_handle* h, const uint8_t* in, int frames, int width, int height, int channels,
+                          size_t in_step, const mc_params* p, uint8_t* out, size_t out_step, uint8_t* produced);
+
 /* --- "next" row (SURVEY.md 8f-1): the whole processing chain of one frame on the device ---------------------
  * Replaces runChainOnce(chain, in, cfg, original) (reference src/processing/ChainBuilder.cpp:19-29) over
  * PreprocessProcessor (ROI crop + INTER_AREA downscale, PreprocessProcessor.cpp:10-51), GrayscaleProcessor

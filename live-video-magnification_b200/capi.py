@@ -52,6 +52,8 @@ SIGNATURES = {
     "mc_process": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t, C.POINTER(C.c_int)]),
     "mc_process_device": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t, C.POINTER(C.c_int)]),
     "mc_sync": (C.c_int, [_vp]),
+    "mc_process_clip_device": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t, _u8p]),
+    "mc_process_clip": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t, _u8p]),
     "mc_chain_process": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, C.c_int, _vp, C.c_size_t, _vp,
                                    C.c_size_t, C.POINTER(McChainInfo)]),
     "mc_pipeline_depth": (C.c_int, [_vp]),

@@ -67,6 +67,10 @@ struct mc_handle {
     void* c_tabs = nullptr;
     size_t c_tabs_b = 0;
 
+    // mc_process_clip device staging: the clip's frames in and out
+    uint8_t *k_in = nullptr, *k_out = nullptr;
+    size_t k_in_b = 0, k_out_b = 0;
+
     // pipeline
     std::vector<Slot> slots;
     std::deque<int> inflight;
@@ -205,11 +209,14 @@ bool is_pinned(const void* p) {
 }
 
 // The body of MagnificationProcessor::process on device-resident frames.
-// lane_produced: `lanes` per-lane flags (written).
+// lane_produced: `lanes` per-lane flags (written).  frames > 1 (Laplace only): a clip of that many consecutive frames
+// of every lane, [t][lane] in the lane stride, with frames * lanes flags.
 mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, int channels, size_t in_step,
-                              const mc_params* p, uint8_t* d_out, size_t out_step, int* produced, uint8_t* lane_produced) {
+                              const mc_params* p, uint8_t* d_out, size_t out_step, int* produced, uint8_t* lane_produced,
+                              int frames = 1) {
+    const size_t n_flags = (size_t)frames * h->lanes;
     *produced = 0;
-    std::fill(lane_produced, lane_produced + h->lanes, (uint8_t)0);
+    std::fill(lane_produced, lane_produced + n_flags, (uint8_t)0);
     debug_maybe_throw();
     if (!p) { h->err = "params is null"; return MC_ERR_INVALID; }
     // Identity when disabled / empty; free state so a later re-enable starts cleanly (:21-29).
@@ -272,7 +279,7 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
                 h->ops.data(), h->d_ops, lane_produced, &held_lost};
     mc_status st = MC_OK;
     switch (p->mode) {
-        case MC_MODE_LAPLACE: st = h->motion.process(ctx, io, *p, levels, produced); break;
+        case MC_MODE_LAPLACE: st = h->motion.process(ctx, io, *p, levels, produced, frames); break;
         case MC_MODE_COLOR: st = h->color.process(ctx, io, *p, levels, produced); break;
         case MC_MODE_PHASE: st = h->riesz.process(ctx, io, *p, levels, produced); break;
         default: break;
@@ -283,7 +290,7 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
         reset_modes(h);
         tracker_reset(h);
         *produced = 0;
-        std::fill(lane_produced, lane_produced + h->lanes, (uint8_t)0);
+        std::fill(lane_produced, lane_produced + n_flags, (uint8_t)0);
         return st;
     }
     if (p->mode == MC_MODE_COLOR) std::fill(lane_produced, lane_produced + h->lanes, (uint8_t)(*produced != 0));   // all lanes step together
@@ -445,6 +452,8 @@ void mc_destroy(mc_handle* h) try {
     if (h->c_gray) cudaFree(h->c_gray);
     if (h->c_out) cudaFree(h->c_out);
     if (h->c_tabs) cudaFree(h->c_tabs);
+    if (h->k_in) cudaFree(h->k_in);
+    if (h->k_out) cudaFree(h->k_out);
     if (h->tables.lab_lut) cudaFree(h->tables.lab_lut);
     if (h->tables.inv_gamma) cudaFree(h->tables.inv_gamma);
     if (h->d_ops) cudaFree(h->d_ops);
@@ -826,6 +835,74 @@ extern "C" mc_status mc_chain_process(mc_handle* h, const uint8_t* in, int width
             if (out_bytes < crow * chh) { h->err = "out buffer too small"; return MC_ERR_INVALID; }
             CK(cudaMemcpyAsync(out, result, crow * chh, cudaMemcpyDeviceToHost, h->stream));
         }
+    }
+    CK(cudaStreamSynchronize(h->stream));
+    return MC_OK;
+} catch (...) { return on_exception(h); }
+
+// ---- clips: `frames` consecutive frames of every lane in one call ----------------------------------------------------
+namespace {
+mc_status clip_impl(mc_handle* h, const uint8_t* d_in, int frames, int w, int hh, int channels, size_t in_step, const mc_params* p,
+                    uint8_t* d_out, size_t out_step, uint8_t* produced) {
+    if (frames < 1) { h->err = "frames must be >= 1"; return MC_ERR_INVALID; }
+    // frames * lanes * channels becomes a grid.z extent of the batched ingest / egress
+    if ((long long)frames * h->lanes > MC_MAX_LANES) { h->err = "frames * lanes exceeds MC_MAX_LANES"; return MC_ERR_INVALID; }
+    if (!produced) { h->err = "produced is null"; return MC_ERR_INVALID; }
+    if (!h->inflight.empty()) { h->err = "clip called with pipelined frames in flight"; return MC_ERR_INVALID; }
+    const size_t lanes = (size_t)h->lanes;
+    std::fill(produced, produced + (size_t)frames * lanes, (uint8_t)0);
+    int any = 0;
+    mc_status st = MC_OK;
+    if (p && p->mode == MC_MODE_LAPLACE && frames > 1) {
+        st = process_device_impl(h, d_in, w, hh, channels, in_step, p, d_out, out_step, &any, produced, frames);
+    } else {
+        // Phase, Color (and Laplace with one frame): the frame path, one call per frame
+        const size_t in_frame = in_step * (size_t)hh * lanes, out_frame = out_step * (size_t)hh * lanes;
+        for (int t = 0; t < frames && st == MC_OK; ++t)
+            st = process_device_impl(h, d_in ? d_in + (size_t)t * in_frame : nullptr, w, hh, channels, in_step, p,
+                                     d_out ? d_out + (size_t)t * out_frame : nullptr, out_step, &any, produced + (size_t)t * lanes);
+    }
+    if (st != MC_OK) std::fill(produced, produced + (size_t)frames * lanes, (uint8_t)0);   // the state was dropped
+    std::memcpy(h->lane_produced.data(), produced + (size_t)(frames - 1) * lanes, lanes);
+    return st;
+}
+}  // namespace
+
+extern "C" mc_status mc_process_clip_device(mc_handle* h, const uint8_t* d_in, int frames, int width, int height, int channels,
+                                            size_t in_step, const mc_params* p, uint8_t* d_out, size_t out_step, uint8_t* produced) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    return clip_impl(h, d_in, frames, width, height, channels, in_step, p, d_out, out_step, produced);
+} catch (...) { return on_exception(h); }
+
+extern "C" mc_status mc_process_clip(mc_handle* h, const uint8_t* in, int frames, int width, int height, int channels,
+                                     size_t in_step, const mc_params* p, uint8_t* out, size_t out_step, uint8_t* produced) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    const bool have = in != nullptr && width > 0 && height > 0 && (channels == 1 || channels == 3);
+    if (!have || frames < 1 || (long long)frames * h->lanes > MC_MAX_LANES || !produced || !h->inflight.empty())
+        return clip_impl(h, nullptr, frames, 0, 0, channels, 0, p, nullptr, 0, produced);   // argument errors, identity
+    const size_t row = (size_t)width * channels;
+    if (in_step < row || (out && out_step < row)) { h->err = "step too small"; return MC_ERR_INVALID; }
+    const size_t vl = (size_t)frames * h->lanes, rows = vl * height, frame_bytes = row * height;
+    mc_status st;
+    if ((st = grow(h, &h->k_in, &h->k_in_b, rows * row)) != MC_OK) return st;
+    if ((st = grow(h, &h->k_out, &h->k_out_b, rows * row)) != MC_OK) return st;
+    if (in_step == row) CK(cudaMemcpyAsync(h->k_in, in, rows * row, cudaMemcpyHostToDevice, h->stream));
+    else CK(cudaMemcpy2DAsync(h->k_in, row, in, in_step, row, rows, cudaMemcpyHostToDevice, h->stream));
+    st = clip_impl(h, h->k_in, frames, width, height, channels, row, p, h->k_out, row, produced);
+    if (st != MC_OK) return st;
+    // only the frames that produced are downloaded, one copy per run of consecutive ones ([t][lane] order); the bytes of
+    // the others in `out` are left as they are
+    for (size_t a = 0; a < vl && out;) {
+        if (!produced[a]) { ++a; continue; }
+        size_t b = a;
+        while (b < vl && produced[b]) ++b;
+        const uint8_t* src = h->k_out + a * frame_bytes;
+        uint8_t* dst = out + a * height * out_step;
+        if (out_step == row) CK(cudaMemcpyAsync(dst, src, (b - a) * frame_bytes, cudaMemcpyDeviceToHost, h->stream));
+        else CK(cudaMemcpy2DAsync(dst, out_step, src, row, row, (b - a) * height, cudaMemcpyDeviceToHost, h->stream));
+        a = b;
     }
     CK(cudaStreamSynchronize(h->stream));
     return MC_OK;

@@ -104,6 +104,11 @@ bool make_tensor_map_box(void* out_map, const float* base, const Level& l, int p
 // fused per level: pyrDown + pyrUp + subtract + dual-EMA update + gain (SpatialFilter.cpp:25-38,
 // TemporalFilter.cpp:9-22, MagnifyCore.hpp:127-134)
 cudaError_t launch_level(const LevelArgs& a, cudaStream_t s);
+// the same over a clip of `frames` consecutive frames (mc_process_clip_device): the grid covers a.planes = lanes * C
+// state planes, whose hi / lo tiles stay in registers for the whole clip.  Frame t of state plane p is virtual plane
+// t * a.planes + p of the input (a.g, a.tmap over all virtual planes), a.g_next and a.m.  a.first / a.ops describe
+// the clip's first frame; the later frames run.
+cudaError_t launch_level_clip(const LevelArgs& a, int frames, cudaStream_t s);
 // pure pyrDown of `a.g` into `a.g_next` (register/shuffle strip kernel; used when a.band == 0)
 cudaError_t launch_down(const LevelArgs& a, cudaStream_t s);
 

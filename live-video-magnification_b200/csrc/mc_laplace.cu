@@ -3,6 +3,7 @@
 //   lab16   : u8 BGR -> Lab (OpenCV LUT, exact) stored as int16 planes            (MagnifyCore.hpp:87-93)
 //   level   : pyrDown + pyrUp + subtract + dual-EMA state update + gain, fused    (SpatialFilter.cpp:25-38,
 //             per pyramid level; input f32 planes, Lab16 planes or u8 gray        TemporalFilter.cpp:9-22, MagnifyCore.hpp:127-134)
+//   level_clip: the same over a clip of consecutive frames, the state tile kept in registers across the clip
 //   collapse: pyrUp + add (small levels only)                                     (SpatialFilter.cpp:52-61)
 //   egress  : two pyrUp+add levels + chroma attenuation + input+motion +          (MagnifyCore.hpp:136-158)
 //             Lab2BGR + u8
@@ -152,6 +153,133 @@ struct LevelKArgs {
     const uint8_t* ops;       // LaneOp per lane or null
 };
 
+// ---- the level kernels' stencil stages, shared by k_level (one frame) and k_level_clip (a clip of frames) ----------
+
+template <int KIND>
+__device__ __forceinline__ const void* level_input(const LevelKArgs& a, size_t plane) {
+    if (KIND == IN_F32) return reinterpret_cast<const float*>(a.g) + plane * a.in_plane;
+    if (KIND == IN_LAB16) return reinterpret_cast<const short*>(a.g) + plane * a.in_plane;
+    return reinterpret_cast<const uint8_t*>(a.g) + plane * a.in_plane;
+}
+
+// A TMA-staged window of a border tile holds zeros outside the level: replace every cell with its BORDER_REFLECT_101
+// source, which lies inside the window.
+__device__ __forceinline__ void level_reflect_window(float (*sG)[GW], int x0, int y0, int wf, int hf) {
+    __syncthreads();
+    float fix[(GH * GW + 255) / 256];
+    int n = 0;
+    for (int i = threadIdx.x; i < GH * GW; i += 256, ++n) {
+        const int r = i / GW, c = i - r * GW;
+        const int gy = y0 - 4 + r, gx = x0 - 4 + c;
+        int rr = reflect101(gy, hf) - (y0 - 4), cc = reflect101(gx, wf) - (x0 - 4);
+        rr = rr < 0 ? 0 : (rr > GH - 1 ? GH - 1 : rr);
+        cc = cc < 0 ? 0 : (cc > GW - 1 ? GW - 1 : cc);
+        fix[n] = sG[rr][cc];
+    }
+    __syncthreads();
+    n = 0;
+    for (int i = threadIdx.x; i < GH * GW; i += 256, ++n) {
+        const int r = i / GW, c = i - r * GW;
+        sG[r][c] = fix[n];
+    }
+}
+
+// pyrDown of the staged window: row pass into sH, column pass into the coarse window sD (pyrUp's border rule
+// pre-applied), and the tile's pixels of G_{l+1} stored to gn.
+__device__ __forceinline__ void level_down(const float (*sG)[GW], float (*sH)[DP], float (*sD)[DP], float* __restrict__ gn,
+                                           int gn_pitch, int x0, int y0, int wc, int hc, bool interior) {
+    // row pass: sH[r][j] for the coarse columns of the window (pairs of columns per item)
+    if (interior) {
+        for (int i = threadIdx.x; i < GH * (DW / 2); i += 256) {
+            const int r = i / (DW / 2), jp = i - r * (DW / 2);
+            const float4 u = *reinterpret_cast<const float4*>(&sG[r][4 * jp]);
+            const float4 v = *reinterpret_cast<const float4*>(&sG[r][4 * jp + 4]);
+            float2 o;
+            o.x = down5(u.x, u.y, u.z, u.w, v.x);
+            o.y = down5(u.z, u.w, v.x, v.y, v.z);
+            *reinterpret_cast<float2*>(&sH[r][2 * jp]) = o;
+        }
+    } else {
+        for (int i = threadIdx.x; i < GH * DW; i += 256) {
+            const int r = i / DW, j = i - r * DW;
+            const int im = upsrc(x0 / 2 - 1 + j, wc);
+            int c = 2 * im - x0 + 4;
+            c = c < 2 ? 2 : (c > GW - 4 ? GW - 4 : c);
+            sH[r][j] = down5(sG[r][c - 2], sG[r][c - 1], sG[r][c], sG[r][c + 1], sG[r][c + 2]);
+        }
+    }
+    __syncthreads();
+    // column pass -> coarse window D; store G_{l+1}
+    if (interior) {
+        for (int i = threadIdx.x; i < (DH / 2) * DW; i += 256) {
+            const int kp = i / DW, j = i - kp * DW;
+            const int r = 4 * kp;  // rows r..r+6 feed coarse rows 2kp, 2kp+1
+            const float f0 = sH[r][j], f1 = sH[r + 1][j], f2 = sH[r + 2][j], f3 = sH[r + 3][j], f4 = sH[r + 4][j],
+                        f5 = sH[r + 5][j], f6 = sH[r + 6][j];
+            const float d0 = down5(f0, f1, f2, f3, f4) * kInv256, d1 = down5(f2, f3, f4, f5, f6) * kInv256;
+            sD[2 * kp][j] = d0;
+            sD[2 * kp + 1][j] = d1;
+            if (j >= 1 && j <= TW / 2) {
+                const int ix = x0 / 2 - 1 + j;
+                const int iy = y0 / 2 - 1 + 2 * kp;
+                if (kp >= 1) gn[(size_t)iy * gn_pitch + ix] = d0;             // k = 2kp in [1,16] <=> kp >= 1
+                if (kp <= DH / 2 - 2) gn[(size_t)(iy + 1) * gn_pitch + ix] = d1;  // k = 2kp+1 <= 16
+            }
+        }
+    } else {
+        for (int i = threadIdx.x; i < DH * DW; i += 256) {
+            const int k = i / DW, j = i - k * DW;
+            const int iy = y0 / 2 - 1 + k, ix = x0 / 2 - 1 + j;
+            const int imy = upsrc(iy, hc);
+            int r = 2 * imy - y0 + 4;
+            r = r < 2 ? 2 : (r > GH - 3 ? GH - 3 : r);
+            const float v = down5(sH[r - 2][j], sH[r - 1][j], sH[r][j], sH[r + 1][j], sH[r + 2][j]) * kInv256;
+            sD[k][j] = v;
+            if (k >= 1 && k <= TH / 2 && j >= 1 && j <= TW / 2 && iy < hc && ix < wc) gn[(size_t)iy * gn_pitch + ix] = v;
+        }
+    }
+}
+
+// pyrUp of the coarse window at thread (tx, ty)'s fine pixels x = 4tx..4tx+3, y = 2ty, 2ty+1
+__device__ __forceinline__ void level_up(const float (*sD)[DP], int tx, int ty, float (&up)[2][4]) {
+    float e[3][4];  // pyrUp row pass for coarse rows ty, ty+1, ty+2 (window rows), fine cols 4tx..4tx+3
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+        const float2 p0 = *reinterpret_cast<const float2*>(&sD[ty + q][2 * tx]);
+        const float2 p1 = *reinterpret_cast<const float2*>(&sD[ty + q][2 * tx + 2]);
+        e[q][0] = p0.x + p0.y * 6.0f + p1.x;
+        e[q][1] = (p0.y + p1.x) * 4.0f;
+        e[q][2] = p0.y + p1.x * 6.0f + p1.y;
+        e[q][3] = (p1.x + p1.y) * 4.0f;
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        up[0][i] = (e[0][i] + e[1][i] * 6.0f + e[2][i]) * kInv64;
+        up[1][i] = ((e[1][i] + e[2][i]) * 4.0f) * kInv64;
+    }
+}
+
+// The band of fine row 2ty+ry at the thread's 4 pixels and the temporal filter on it: a lane's first frame sets
+// hi = lo = band and m = gain * (band - band) = +-0 (MagnifyCore.hpp:98-103); otherwise both EMAs step
+// (TemporalFilter.cpp:9-22) and m = gain * (hi - lo).
+__device__ __forceinline__ void level_filter(const LevelKArgs& a, const float (*sG)[GW], const float (&up)[2][4], int tx, int ty,
+                                             int ry, bool first, float (&h)[4], float (&l)[4], float (&m)[4]) {
+    const float4 gv = *reinterpret_cast<const float4*>(&sG[2 * ty + ry + 4][4 * tx + 4]);
+    const float band[4] = {gv.x - up[ry][0], gv.y - up[ry][1], gv.z - up[ry][2], gv.w - up[ry][3]};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        if (first) {
+            h[i] = band[i];
+            l[i] = band[i];
+            m[i] = (band[i] - band[i]) * a.gain;
+        } else {
+            h[i] = ema(h[i], band[i], a.omc_hi, a.c_hi);
+            l[i] = ema(l[i], band[i], a.omc_lo, a.c_lo);
+            m[i] = (h[i] - l[i]) * a.gain;
+        }
+    }
+}
+
 // PREFETCH (with USE_TMA): the tile's two state planes are requested as bulk-tensor copies at kernel entry, together
 // with the input window, and only waited for in the last phase — the fused kernel is latency-bound, so what matters is how many bytes each CTA keeps in flight.
 template <int KIND, bool USE_TMA, bool PREFETCH>
@@ -173,10 +301,6 @@ __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_
     const int wf = a.lf.w, hf = a.lf.h, wc = a.lc.w, hc = a.lc.h;
     const bool interior = x0 >= 4 && x0 + TW + 4 <= wf && y0 >= 4 && y0 + TH + 3 <= hf && (KIND != IN_U8 || a.in_vec_ok);
     const int ch = plane % a.channels;
-    const void* base;
-    if (KIND == IN_F32) base = reinterpret_cast<const float*>(a.g) + (size_t)plane * a.in_plane;
-    else if (KIND == IN_LAB16) base = reinterpret_cast<const short*>(a.g) + (size_t)plane * a.in_plane;
-    else base = reinterpret_cast<const uint8_t*>(a.g) + (size_t)plane * a.in_plane;
     if (USE_TMA) {
         // The (GH x GW) window of this plane is fetched by ONE bulk-tensor copy issued by one thread; the
         // TMA unit zero-fills whatever lies outside the level, and border tiles then patch those cells with
@@ -196,106 +320,21 @@ __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_
             }
         }
         mbar_wait(&tma_bar, 0);
-        if (!interior) {
-            __syncthreads();
-            float fix[(GH * GW + 255) / 256];
-            int n = 0;
-            for (int i = threadIdx.x; i < GH * GW; i += 256, ++n) {
-                const int r = i / GW, c = i - r * GW;
-                const int gy = y0 - 4 + r, gx = x0 - 4 + c;
-                int rr = reflect101(gy, hf) - (y0 - 4), cc = reflect101(gx, wf) - (x0 - 4);
-                rr = rr < 0 ? 0 : (rr > GH - 1 ? GH - 1 : rr);
-                cc = cc < 0 ? 0 : (cc > GW - 1 ? GW - 1 : cc);
-                fix[n] = sG[rr][cc];
-            }
-            __syncthreads();
-            n = 0;
-            for (int i = threadIdx.x; i < GH * GW; i += 256, ++n) {
-                const int r = i / GW, c = i - r * GW;
-                sG[r][c] = fix[n];
-            }
-        }
+        if (!interior) level_reflect_window(sG, x0, y0, wf, hf);
     } else {
         const float scv = ch == 0 ? a.sc[0] : (ch == 1 ? a.sc[1] : a.sc[2]);
         const float ofv = ch == 0 ? a.of[0] : (ch == 1 ? a.of[1] : a.of[2]);
-        load_fine_window<KIND>(sG, base, a.in_row, wf, hf, x0, y0, interior, scv, ofv);
+        load_fine_window<KIND>(sG, level_input<KIND>(a, (size_t)plane), a.in_row, wf, hf, x0, y0, interior, scv, ofv);
     }
     __syncthreads();
-
-    // pyrDown row pass: sH[r][j] for the coarse columns of the window (pairs of columns per item)
-    if (interior) {
-        for (int i = threadIdx.x; i < GH * (DW / 2); i += 256) {
-            const int r = i / (DW / 2), jp = i - r * (DW / 2);
-            const float4 u = *reinterpret_cast<const float4*>(&sG[r][4 * jp]);
-            const float4 v = *reinterpret_cast<const float4*>(&sG[r][4 * jp + 4]);
-            float2 o;
-            o.x = down5(u.x, u.y, u.z, u.w, v.x);
-            o.y = down5(u.z, u.w, v.x, v.y, v.z);
-            *reinterpret_cast<float2*>(&sH[r][2 * jp]) = o;
-        }
-    } else {
-        for (int i = threadIdx.x; i < GH * DW; i += 256) {
-            const int r = i / DW, j = i - r * DW;
-            const int im = upsrc(x0 / 2 - 1 + j, wc);
-            int c = 2 * im - x0 + 4;
-            c = c < 2 ? 2 : (c > GW - 4 ? GW - 4 : c);
-            sH[r][j] = down5(sG[r][c - 2], sG[r][c - 1], sG[r][c], sG[r][c + 1], sG[r][c + 2]);
-        }
-    }
-    __syncthreads();
-    // pyrDown column pass -> coarse window D (pyrUp's border rule pre-applied); store G_{l+1}
-    float* __restrict__ gn = a.g_next + (size_t)plane * a.lc.plane;
-    if (interior) {
-        for (int i = threadIdx.x; i < (DH / 2) * DW; i += 256) {
-            const int kp = i / DW, j = i - kp * DW;
-            const int r = 4 * kp;  // rows r..r+6 feed coarse rows 2kp, 2kp+1
-            const float f0 = sH[r][j], f1 = sH[r + 1][j], f2 = sH[r + 2][j], f3 = sH[r + 3][j], f4 = sH[r + 4][j],
-                        f5 = sH[r + 5][j], f6 = sH[r + 6][j];
-            const float d0 = down5(f0, f1, f2, f3, f4) * kInv256, d1 = down5(f2, f3, f4, f5, f6) * kInv256;
-            sD[2 * kp][j] = d0;
-            sD[2 * kp + 1][j] = d1;
-            if (j >= 1 && j <= TW / 2) {
-                const int ix = x0 / 2 - 1 + j;
-                const int iy = y0 / 2 - 1 + 2 * kp;
-                if (kp >= 1) gn[(size_t)iy * a.lc.pitch + ix] = d0;             // k = 2kp in [1,16] <=> kp >= 1
-                if (kp <= DH / 2 - 2) gn[(size_t)(iy + 1) * a.lc.pitch + ix] = d1;  // k = 2kp+1 <= 16
-            }
-        }
-    } else {
-        for (int i = threadIdx.x; i < DH * DW; i += 256) {
-            const int k = i / DW, j = i - k * DW;
-            const int iy = y0 / 2 - 1 + k, ix = x0 / 2 - 1 + j;
-            const int imy = upsrc(iy, hc);
-            int r = 2 * imy - y0 + 4;
-            r = r < 2 ? 2 : (r > GH - 3 ? GH - 3 : r);
-            const float v = down5(sH[r - 2][j], sH[r - 1][j], sH[r][j], sH[r + 1][j], sH[r + 2][j]) * kInv256;
-            sD[k][j] = v;
-            if (k >= 1 && k <= TH / 2 && j >= 1 && j <= TW / 2 && iy < hc && ix < wc) gn[(size_t)iy * a.lc.pitch + ix] = v;
-        }
-    }
+    level_down(sG, sH, sD, a.g_next + (size_t)plane * a.lc.plane, a.lc.pitch, x0, y0, wc, hc, interior);
     if (!a.band) return;
     __syncthreads();
 
     // pyrUp + band + temporal filter: thread (tx, ty) owns fine pixels x = 4tx..4tx+3, y = 2ty, 2ty+1
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
     float up[2][4];
-    {
-        float e[3][4];  // pyrUp row pass for coarse rows ty, ty+1, ty+2 (window rows), fine cols 4tx..4tx+3
-#pragma unroll
-        for (int q = 0; q < 3; ++q) {
-            const float2 p0 = *reinterpret_cast<const float2*>(&sD[ty + q][2 * tx]);
-            const float2 p1 = *reinterpret_cast<const float2*>(&sD[ty + q][2 * tx + 2]);
-            e[q][0] = p0.x + p0.y * 6.0f + p1.x;
-            e[q][1] = (p0.y + p1.x) * 4.0f;
-            e[q][2] = p0.y + p1.x * 6.0f + p1.y;
-            e[q][3] = (p1.x + p1.y) * 4.0f;
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            up[0][i] = (e[0][i] + e[1][i] * 6.0f + e[2][i]) * kInv64;
-            up[1][i] = ((e[1][i] + e[2][i]) * 4.0f) * kInv64;
-        }
-    }
+    level_up(sD, tx, ty, up);
     float* __restrict__ hi = a.hi + (size_t)plane * a.lf.plane;
     float* __restrict__ lo = a.lo + (size_t)plane * a.lf.plane;
     float* __restrict__ m = a.m ? a.m + (size_t)plane * a.lf.plane : nullptr;
@@ -305,17 +344,12 @@ __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_
     for (int ry = 0; ry < 2; ++ry) {
         const int gy = y0 + 2 * ty + ry;
         if (gy >= hf || gx >= wf) continue;
-        const float4 gv = *reinterpret_cast<const float4*>(&sG[2 * ty + ry + 4][4 * tx + 4]);
-        float band[4] = {gv.x - up[ry][0], gv.y - up[ry][1], gv.z - up[ry][2], gv.w - up[ry][3]};
         const size_t o = (size_t)gy * a.lf.pitch + gx;
         // rows are padded to a multiple of 32 floats, so a full float4 at gx < wf is always in-bounds
+        float nh[4], nl[4], mm[4];
         if (first) {
-            const float4 b4 = make_float4(band[0], band[1], band[2], band[3]);
-            *reinterpret_cast<float4*>(hi + o) = b4;
-            *reinterpret_cast<float4*>(lo + o) = b4;
             // a lane's first frame among running lanes: its stored amplified band is gain * (hi - lo) = +-0
-            if (m) *reinterpret_cast<float4*>(m + o) = make_float4((band[0] - band[0]) * a.gain, (band[1] - band[1]) * a.gain,
-                                                                   (band[2] - band[2]) * a.gain, (band[3] - band[3]) * a.gain);
+            level_filter(a, sG, up, tx, ty, ry, true, nh, nl, mm);
         } else {
             float4 h4, l4;
             if (prefetch) {
@@ -325,17 +359,110 @@ __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_
                 h4 = *reinterpret_cast<const float4*>(hi + o);
                 l4 = *reinterpret_cast<const float4*>(lo + o);
             }
-            float nh[4] = {h4.x, h4.y, h4.z, h4.w}, nl[4] = {l4.x, l4.y, l4.z, l4.w}, mm[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                nh[i] = ema(nh[i], band[i], a.omc_hi, a.c_hi);
-                nl[i] = ema(nl[i], band[i], a.omc_lo, a.c_lo);
-                mm[i] = (nh[i] - nl[i]) * a.gain;
-            }
-            *reinterpret_cast<float4*>(hi + o) = make_float4(nh[0], nh[1], nh[2], nh[3]);
-            *reinterpret_cast<float4*>(lo + o) = make_float4(nl[0], nl[1], nl[2], nl[3]);
-            if (m) *reinterpret_cast<float4*>(m + o) = make_float4(mm[0], mm[1], mm[2], mm[3]);
+            nh[0] = h4.x; nh[1] = h4.y; nh[2] = h4.z; nh[3] = h4.w;
+            nl[0] = l4.x; nl[1] = l4.y; nl[2] = l4.z; nl[3] = l4.w;
+            level_filter(a, sG, up, tx, ty, ry, false, nh, nl, mm);
         }
+        *reinterpret_cast<float4*>(hi + o) = make_float4(nh[0], nh[1], nh[2], nh[3]);
+        *reinterpret_cast<float4*>(lo + o) = make_float4(nl[0], nl[1], nl[2], nl[3]);
+        if (m) *reinterpret_cast<float4*>(m + o) = make_float4(mm[0], mm[1], mm[2], mm[3]);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// level_clip: the level kernel over a clip of `frames` consecutive frames of every lane.  The grid is that of k_level
+// over the handle's lanes * C state planes; each CTA keeps its hi / lo tile in registers (16 floats per thread) from
+// the first frame to the last, so the state moves once per clip instead of once per frame.  Per frame t it stages the
+// input window of virtual plane t * frame_planes + plane and writes G_{l+1}(t) and the amplified band M_l(t) of that
+// virtual plane.  With USE_TMA the window of frame t+1 is requested into the second buffer while frame t is computed.
+// ------------------------------------------------------------------------------------------------
+template <int KIND, bool USE_TMA>
+__global__ void __launch_bounds__(256) k_level_clip(const LevelKArgs a, const int frames, const int frame_planes,
+                                                    const __grid_constant__ CUtensorMap tmap) {
+    __shared__ __align__(128) float sG0[GH][GW];
+    __shared__ __align__(128) float sG1[USE_TMA ? GH : 1][GW];
+    __shared__ __align__(16) float sH[GH][DP];
+    __shared__ __align__(16) float sD[DH][DP];
+    __shared__ __align__(8) uint64_t bar[2];
+    const int plane = blockIdx.z;
+    const int op = lane_op(a.ops, plane / a.channels);
+    if (op == LANE_HOLD) return;                     // held lane: skipped for the whole clip
+    const bool first = a.first || op == LANE_FIRST;  // the lane's first frame is the clip's first frame
+    const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH;
+    const int wf = a.lf.w, hf = a.lf.h, wc = a.lc.w, hc = a.lc.h;
+    const bool interior = x0 >= 4 && x0 + TW + 4 <= wf && y0 >= 4 && y0 + TH + 3 <= hf && (KIND != IN_U8 || a.in_vec_ok);
+    const int ch = plane % a.channels;
+    const float scv = ch == 0 ? a.sc[0] : (ch == 1 ? a.sc[1] : a.sc[2]);
+    const float ofv = ch == 0 ? a.of[0] : (ch == 1 ? a.of[1] : a.of[2]);
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    const int gx = x0 + 4 * tx;
+    float* __restrict__ hi = a.hi + (size_t)plane * a.lf.plane;
+    float* __restrict__ lo = a.lo + (size_t)plane * a.lf.plane;
+
+    float sh[2][4], sl[2][4];   // the tile's temporal state, carried through the clip
+#pragma unroll
+    for (int ry = 0; ry < 2; ++ry) {
+        const int gy = y0 + 2 * ty + ry;
+        float4 h4 = make_float4(0.f, 0.f, 0.f, 0.f), l4 = h4;
+        if (!first && gy < hf && gx < wf) {
+            const size_t o = (size_t)gy * a.lf.pitch + gx;
+            h4 = *reinterpret_cast<const float4*>(hi + o);
+            l4 = *reinterpret_cast<const float4*>(lo + o);
+        }
+        sh[ry][0] = h4.x; sh[ry][1] = h4.y; sh[ry][2] = h4.z; sh[ry][3] = h4.w;
+        sl[ry][0] = l4.x; sl[ry][1] = l4.y; sl[ry][2] = l4.z; sl[ry][3] = l4.w;
+    }
+    if (USE_TMA) {
+        if (threadIdx.x == 0) {
+            mbar_init(&bar[0], 1);
+            mbar_init(&bar[1], 1);
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            mbar_expect_tx(&bar[0], GH * GW * sizeof(float));
+            tma_load_3d(&sG0[0][0], &tmap, x0 - 4, y0 - 4, plane, &bar[0]);
+        }
+    }
+    for (int t = 0; t < frames; ++t) {
+        const size_t vplane = (size_t)t * frame_planes + plane;
+        float (*sG)[GW] = USE_TMA && (t & 1) ? sG1 : sG0;
+        if (USE_TMA) {
+            // the other buffer was last read in frame t-1, which every thread has finished (barrier at the loop's end)
+            if (threadIdx.x == 0 && t + 1 < frames) {
+                uint64_t* nb = &bar[(t + 1) & 1];
+                mbar_expect_tx(nb, GH * GW * sizeof(float));
+                tma_load_3d((t & 1) ? &sG0[0][0] : &sG1[0][0], &tmap, x0 - 4, y0 - 4, (int)(vplane + frame_planes), nb);
+            }
+            mbar_wait(&bar[t & 1], (t >> 1) & 1);
+            if (!interior) level_reflect_window(sG, x0, y0, wf, hf);
+        } else {
+            load_fine_window<KIND>(sG, level_input<KIND>(a, vplane), a.in_row, wf, hf, x0, y0, interior, scv, ofv);
+        }
+        __syncthreads();
+        level_down(sG, sH, sD, a.g_next + vplane * a.lc.plane, a.lc.pitch, x0, y0, wc, hc, interior);
+        __syncthreads();
+        float up[2][4];
+        level_up(sD, tx, ty, up);
+        float* __restrict__ m = a.m ? a.m + vplane * a.lf.plane : nullptr;
+#pragma unroll
+        for (int ry = 0; ry < 2; ++ry) {
+            const int gy = y0 + 2 * ty + ry;
+            if (gy >= hf || gx >= wf) continue;
+            float mm[4];
+            level_filter(a, sG, up, tx, ty, ry, first && t == 0, sh[ry], sl[ry], mm);
+            if (m) *reinterpret_cast<float4*>(m + (size_t)gy * a.lf.pitch + gx) = make_float4(mm[0], mm[1], mm[2], mm[3]);
+        }
+        // sG, sH and sD are refilled by the next frame; a border tile's generic writes to sG precede a later TMA write
+        if (USE_TMA && !interior) fence_proxy_async_shared();
+        __syncthreads();
+    }
+#pragma unroll
+    for (int ry = 0; ry < 2; ++ry) {
+        const int gy = y0 + 2 * ty + ry;
+        if (gy >= hf || gx >= wf) continue;
+        const size_t o = (size_t)gy * a.lf.pitch + gx;
+        *reinterpret_cast<float4*>(hi + o) = make_float4(sh[ry][0], sh[ry][1], sh[ry][2], sh[ry][3]);
+        *reinterpret_cast<float4*>(lo + o) = make_float4(sl[ry][0], sl[ry][1], sl[ry][2], sl[ry][3]);
     }
 }
 
@@ -1277,7 +1404,7 @@ cudaError_t launch_ingest_lab(const FrameIO& io, const DeviceTables& tb, int16_t
     return cudaGetLastError();
 }
 
-cudaError_t launch_level(const LevelArgs& a, cudaStream_t s) {
+static LevelKArgs level_kargs(const LevelArgs& a) {
     LevelKArgs k;
     k.g = a.g; k.in_plane = a.in_plane; k.in_row = a.in_row; k.channels = a.channels;
     for (int i = 0; i < 3; ++i) { k.sc[i] = a.sc[i]; k.of[i] = a.of[i]; }
@@ -1287,6 +1414,23 @@ cudaError_t launch_level(const LevelArgs& a, cudaStream_t s) {
     k.gain = a.gain;
     k.ops = a.ops;
     k.in_vec_ok = a.in_kind == IN_U8 ? ((reinterpret_cast<uintptr_t>(a.g) % 4 == 0) && (a.in_row % 4 == 0) && (a.in_plane % 4 == 0)) : 1;
+    return k;
+}
+
+cudaError_t launch_level_clip(const LevelArgs& a, int frames, cudaStream_t s) {
+    const LevelKArgs k = level_kargs(a);
+    dim3 grid(cdiv(a.lf.w, TW), cdiv(a.lf.h, TH), a.planes);
+    static const CUtensorMap dummy{};
+    const CUtensorMap* tg = reinterpret_cast<const CUtensorMap*>(a.tmap);
+    if (a.in_kind == IN_F32 && tg) k_level_clip<IN_F32, true><<<grid, 256, 0, s>>>(k, frames, a.planes, *tg);
+    else if (a.in_kind == IN_F32) k_level_clip<IN_F32, false><<<grid, 256, 0, s>>>(k, frames, a.planes, dummy);
+    else if (a.in_kind == IN_LAB16) k_level_clip<IN_LAB16, false><<<grid, 256, 0, s>>>(k, frames, a.planes, dummy);
+    else k_level_clip<IN_U8, false><<<grid, 256, 0, s>>>(k, frames, a.planes, dummy);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_level(const LevelArgs& a, cudaStream_t s) {
+    const LevelKArgs k = level_kargs(a);
     dim3 grid(cdiv(a.lf.w, TW), cdiv(a.lf.h, TH), a.planes);
     static const CUtensorMap dummy{};
     const CUtensorMap* tg = reinterpret_cast<const CUtensorMap*>(a.tmap);

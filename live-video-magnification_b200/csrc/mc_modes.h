@@ -50,7 +50,7 @@ struct ModeCtx {
     // and the mode's answers: which lanes produced, and whether held lanes lost their state (reallocation, Phase cutoff change).
     const uint8_t* lane_ops = nullptr;   // host, `lanes` entries
     uint8_t* d_lane_ops = nullptr;       // device, `lanes` bytes
-    uint8_t* lane_produced = nullptr;    // host, `lanes` entries (written)
+    uint8_t* lane_produced = nullptr;    // host, `lanes` entries, [t][lane] for a clip of t frames (written)
     bool* held_lost = nullptr;           // (written)
 };
 
@@ -159,8 +159,24 @@ struct MotionMode {
     std::vector<float> gains;              // per-level gains of the current frame (member: no per-frame allocation)
     LanePlan plan;                         // per-lane ops of the current frame
 
+    // Scratch of the clip path (mc_process_clip_device): the per-frame planes of `cap` virtual lanes (frame t of lane k
+    // is virtual lane t * lanes + k).  The temporal state stays in hi / lo above, so clip and frame calls interleave.
+    struct Clip {
+        int cap = 0;                          // virtual lanes the buffers hold (the largest clip seen)
+        std::vector<float*> G, M;             // per level: G_1 .. G_levels, amplified bands M_1 .. M_{levels-1}
+        int16_t* lab16 = nullptr;             // Lab planes (C == 3)
+        float* fout = nullptr;                // pre-quantisation tap of every frame (keep_float_output)
+        uint8_t* d_vops = nullptr;            // device LaneOp per virtual lane
+        std::vector<uint8_t> vops;
+        std::vector<TensorMapStorage> tmaps;  // per level: TMA descriptor of G_l over all virtual planes
+        std::vector<char> tmap_valid;
+        DeviceArena arena;
+    } clip;
+
     void reset();
-    mc_status process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced);
+    // frames > 1: `frames` consecutive frames of every lane ([t][lane] in io's lane stride); ctx.lane_produced then
+    // holds frames * lanes flags
+    mc_status process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced, int frames = 1);
     void find_state(const char* name, int level, StateRef& out);
 
 private:
@@ -168,6 +184,8 @@ private:
     mc_status make_groups(const ModeCtx& ctx);
     void drop_groups();
     mc_status run_group(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, Group& g, bool first, double c_lo, double c_hi);
+    mc_status ensure_clip(const ModeCtx& ctx, int vlanes);
+    mc_status run_clip(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int frames, bool first, double c_lo, double c_hi);
 };
 
 struct ColorMode {

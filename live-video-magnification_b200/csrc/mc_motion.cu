@@ -44,6 +44,8 @@ void MotionMode::drop_groups() {
 void MotionMode::reset() {
     drop_groups();
     arena.release();
+    clip.arena.release();
+    clip = Clip{};
     lv.clear(); G.clear(); hi.clear(); lo.clear(); M.clear();
     lab16 = nullptr;
     allocated = false;
@@ -128,7 +130,7 @@ mc_status MotionMode::allocate(const ModeCtx& ctx, const FrameIO& io, int nlevel
     return MC_OK;
 }
 
-mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_params& p, int nlevels, int* produced) {
+mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_params& p, int nlevels, int* produced, int frames) {
     *produced = 0;
     if (!allocated || faithful != ctx.faithful0 || from_state != ctx.band_from_state) {
         if (allocated) *ctx.held_lost = true;
@@ -152,6 +154,20 @@ mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc
     double c_lo = p.coLow, c_hi = p.coHigh;
     if (c_lo == 0) c_lo = 0.01;  // TemporalFilter.cpp:11-12
 
+    if (frames > 1) {
+        const mc_status st = run_clip(ctx, io, p, frames, first, c_lo, c_hi);
+        if (st != MC_OK) return st;
+        empty = false;
+        // frame 0 as a frame call; every later frame is RUN for the lanes that are not held
+        plan.produced(ctx, !ctx.analysis_only || first, true, produced);
+        for (int t = 1; t < frames; ++t)
+            for (int l = 0; l < lanes; ++l) {
+                const bool pr = plan.op[(size_t)l] != LANE_HOLD && !ctx.analysis_only;
+                ctx.lane_produced[(size_t)t * lanes + l] = pr ? 1 : 0;
+                *produced |= pr ? 1 : 0;
+            }
+        return MC_OK;
+    }
     if (groups.size() == 1) {
         const mc_status st = run_group(ctx, io, p, groups[0], first, c_lo, c_hi);
         if (st != MC_OK) return st;
@@ -267,6 +283,143 @@ mc_status MotionMode::run_group(const ModeCtx& ctx, const FrameIO& io_all, const
     }
     LAUNCH("egress", 0, launch_egress(io, *ctx.tables, lab, pitch16, plane16, m1, l1, c2, l2, (float)p.chromAttenuation, fout,
                                       ctx.stream, ctx.egress_strip));
+    return MC_OK;
+}
+
+// Grows the clip scratch to `vlanes` virtual lanes (and adds the float tap when keep_float_output asks for it).
+mc_status MotionMode::ensure_clip(const ModeCtx& ctx, int vlanes) {
+    const size_t vplanes = (size_t)vlanes * channels;
+    if (vlanes > clip.cap) {
+        clip.arena.release();   // cudaFree waits for the kernels still reading the old buffers
+        clip = Clip{};
+        clip.G.assign((size_t)levels + 1, nullptr);
+        clip.M.assign((size_t)levels + 1, nullptr);
+        clip.tmaps.assign((size_t)levels + 1, TensorMapStorage{});
+        clip.tmap_valid.assign((size_t)levels + 1, 0);
+        for (int l = 1; l <= levels; ++l) {
+            MCK(clip.arena.alloc(&clip.G[(size_t)l], vplanes * lv[(size_t)l].plane));
+            if (l < levels) MCK(clip.arena.alloc(&clip.M[(size_t)l], vplanes * lv[(size_t)l].plane));
+            if (l < levels) clip.tmap_valid[(size_t)l] = make_level_tensor_map(&clip.tmaps[(size_t)l], clip.G[(size_t)l], lv[(size_t)l], (int)vplanes) ? 1 : 0;
+        }
+        if (channels == 3) {
+            void* p = nullptr;
+            MCK(clip.arena.alloc_bytes(&p, vplanes * plane16 * sizeof(int16_t)));
+            clip.lab16 = (int16_t*)p;
+        }
+        void* p = nullptr;
+        MCK(clip.arena.alloc_bytes(&p, (size_t)vlanes));
+        clip.d_vops = (uint8_t*)p;
+        clip.cap = vlanes;
+    }
+    if (ctx.float_out && !clip.fout) MCK(clip.arena.alloc(&clip.fout, (size_t)clip.cap * w * h * channels));
+    return MC_OK;
+}
+
+// One clip: the launch set of run_group over V = frames * lanes virtual lanes, with the level kernels replaced by
+// k_level_clip (state in registers across the clip).  Synthesis reads the stored bands M_l; a lane's first frame has
+// M = +-0 there, which gives the first-frame output without a branch.  Lane groups do not apply: one chain.
+mc_status MotionMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_params& p, int frames, bool first, double c_lo, double c_hi) {
+    const int vl = frames * lanes;
+    MCK_ST(ensure_clip(ctx, vl));
+    const int planes = lanes * channels, vplanes = vl * channels;
+    FrameIO io = io0;   // every frame of every lane
+    io.lanes = vl;
+    io.ops = nullptr;
+    if (plan.mixed()) {   // virtual ops: HOLD for held lanes at every t, FIRST at t = 0 for lanes without state, RUN otherwise
+        clip.vops.resize((size_t)vl);
+        for (int t = 0; t < frames; ++t)
+            for (int l = 0; l < lanes; ++l) {
+                const uint8_t o = plan.op[(size_t)l];
+                clip.vops[(size_t)t * lanes + l] = o == LANE_HOLD ? LANE_HOLD : (t == 0 ? o : (uint8_t)LANE_RUN);
+            }
+        MCK(cudaMemcpyAsync(clip.d_vops, clip.vops.data(), (size_t)vl, cudaMemcpyHostToDevice, ctx.stream));
+        io.ops = clip.d_vops;
+    }
+
+    const bool fused_ingest = channels == 3 && !faithful && levels >= 2;
+    if (fused_ingest) LAUNCH("ingest_lab", 0, launch_ingest_lab(io, *ctx.tables, clip.lab16, pitch16, plane16, clip.G[1], lv[1], ctx.stream, ctx.ingest_warps));
+    else if (channels == 3) LAUNCH("lab16", 0, launch_lab16(io, *ctx.tables, clip.lab16, pitch16, plane16, ctx.stream));
+
+    const int l_begin = fused_ingest ? 1 : ((levels >= 2 || faithful) ? 0 : levels);
+    for (int l = l_begin; l < levels; ++l) {
+        LevelArgs a;
+        if (l == 0) {
+            if (channels == 3) {
+                a.in_kind = 1; a.g = clip.lab16; a.in_plane = plane16; a.in_row = pitch16;
+                a.sc[0] = 100.0f / 16384.0f; a.of[0] = 0.0f;
+                a.sc[1] = a.sc[2] = 1.0f / 64.0f; a.of[1] = a.of[2] = -128.0f;
+            } else {
+                a.in_kind = 2; a.g = io.in; a.in_plane = io.in_lane_stride; a.in_row = (int)io.in_step;
+                a.sc[0] = 0.003921568859368563f;
+            }
+        } else {
+            a.in_kind = 0; a.g = clip.G[(size_t)l]; a.in_plane = lv[(size_t)l].plane; a.in_row = lv[(size_t)l].pitch;
+            if (clip.tmap_valid[(size_t)l] && ctx.use_tma) a.tmap = &clip.tmaps[(size_t)l];
+        }
+        a.channels = channels;
+        a.lf = lv[(size_t)l]; a.lc = lv[(size_t)l + 1];
+        a.g_next = clip.G[(size_t)l + 1];
+        a.hi = hi[(size_t)l]; a.lo = lo[(size_t)l];
+        a.m = ctx.analysis_only ? nullptr : clip.M[(size_t)l];
+        a.first = first ? 1 : 0;
+        a.band = (l >= 1 || faithful) ? 1 : 0;
+        a.c_hi = c_hi; a.one_minus_c_hi = 1 - c_hi; a.c_lo = c_lo; a.one_minus_c_lo = 1 - c_lo;
+        a.gain = gains[(size_t)l];
+        if (a.band) {
+            a.planes = planes; a.ops = io0.ops;   // state planes, per-lane ops of the clip's first frame
+            LAUNCH("level_clip", l, launch_level_clip(a, frames, ctx.stream));
+        } else {
+            a.planes = vplanes; a.ops = io.ops;
+            LAUNCH("down", l, launch_down(a, ctx.stream));
+        }
+    }
+    if (faithful) {   // st.lowpassHi/Lo[levels] = residual of the lane's first frame (MagnifyCore.hpp:100-101)
+        const size_t n = (size_t)channels * lv[(size_t)levels].plane;
+        for (int ln = 0; ln < lanes; ++ln) {
+            if (!(first ? plan.op[(size_t)ln] != LANE_HOLD : plan.op[(size_t)ln] == LANE_FIRST)) continue;
+            const size_t o = (size_t)ln * n;
+            LAUNCH("copy", levels, launch_copy_planes(hi[(size_t)levels] + o, clip.G[(size_t)levels] + o, n, ctx.stream));
+            LAUNCH("copy", levels, launch_copy_planes(lo[(size_t)levels] + o, clip.G[(size_t)levels] + o, n, ctx.stream));
+        }
+    }
+    const Level& l1 = lv[levels >= 1 ? 1 : 0];
+    const Level& l2 = lv[levels >= 2 ? 2 : 0];
+    const float chroma = (float)p.chromAttenuation;
+    if (ctx.analysis_only) {
+        // state-carry pass: only the clip's first frame can produce (lanes on their first frame, converted without
+        // motion); it is frame 0's egress of a frame call, so the float tap is written in place
+        FrameIO f0 = io0;
+        if (first) LAUNCH("egress", 0, launch_egress(f0, *ctx.tables, clip.lab16, pitch16, plane16, BandSrc{}, l1, BandSrc{}, l2, chroma,
+                                                     ctx.float_out, ctx.stream, ctx.egress_strip));
+        else if (plan.n_first > 0)
+            LAUNCH("egress", 0, launch_egress(f0, *ctx.tables, clip.lab16, pitch16, plane16, BandSrc{}, l1, BandSrc{}, l2, chroma,
+                                              ctx.float_out, ctx.stream, ctx.egress_strip, true));
+        return MC_OK;
+    }
+    BandSrc m1, c2;
+    if (levels >= 2) {
+        auto band = [&](int l) { return BandSrc{clip.M[(size_t)l], nullptr, 1.0f}; };
+        for (int l = levels - 2; l >= 2; --l)
+            LAUNCH("collapse", l, launch_collapse(lv[(size_t)l], lv[(size_t)l + 1], band(l), band(l + 1), clip.M[(size_t)l], vplanes,
+                                                  ctx.stream, io.ops, channels));
+        m1 = band(1);
+        if (levels >= 3) c2 = band(2);
+    }
+    float* fout = ctx.float_out ? clip.fout : nullptr;
+    LAUNCH("egress", 0, launch_egress(io, *ctx.tables, clip.lab16, pitch16, plane16, m1, l1, c2, l2, chroma, fout, ctx.stream,
+                                      ctx.egress_strip));
+    if (fout) {   // the tap holds the clip's last frame: copy the lanes it wrote (all but the held ones)
+        const size_t lane_floats = (size_t)w * h * channels;
+        const float* last = fout + (size_t)(frames - 1) * lanes * lane_floats;
+        for (int a = 0; a < lanes;) {
+            if (plan.op[(size_t)a] == LANE_HOLD) { ++a; continue; }
+            int b = a;
+            while (b < lanes && plan.op[(size_t)b] != LANE_HOLD) ++b;
+            MCK(cudaMemcpyAsync(ctx.float_out + (size_t)a * lane_floats, last + (size_t)a * lane_floats, (size_t)(b - a) * lane_floats * sizeof(float),
+                                cudaMemcpyDeviceToDevice, ctx.stream));
+            a = b;
+        }
+    }
     return MC_OK;
 }
 

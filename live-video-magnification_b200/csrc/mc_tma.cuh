@@ -16,6 +16,7 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* tm, in
     const int c[3] = {x, y, z};
     cuda_emu::tma_load(dst, tm, c, bar);
 }
+__device__ __forceinline__ void fence_proxy_async_shared() {}
 #else
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, unsigned count) {
@@ -44,6 +45,8 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* tm, in
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
         ::"r"(smem_u32(dst)), "l"(tm), "r"(smem_u32(bar)), "r"(x), "r"(y), "r"(z) : "memory");
 }
+// orders this thread's generic-proxy accesses to shared memory before later async-proxy (bulk copy) accesses
+__device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 #endif
 

@@ -222,7 +222,38 @@ class MagnificationProcessor(IProcessor):
                 out[idle] = img[idle]
         return True, out
 
+    def process_clip(self, frames: np.ndarray, cfg: ProcessorConfig):
+        """Magnifies T consecutive frames in one call (mc_process_clip): ``frames`` is [T, H, W(, C)], or
+        [T, lanes, H, W(, C)] on a multi-lane processor.  -> (produced bool[T, lanes], out of the same shape).  The result
+        equals T process_image calls; frames that did not produce carry their input frame."""
+        if frames.dtype != np.uint8:
+            raise TypeError("frames must be uint8 (CV_8UC1 / CV_8UC3)")
+        img = np.ascontiguousarray(frames)
+        if self.lanes > 1 and (img.ndim < 4 or img.shape[1] != self.lanes):
+            raise ValueError("frames must be [T, lanes, H, W(, C)] on a multi-lane processor")
+        if img.ndim < 3:
+            raise ValueError("frames must be [T, H, W(, C)]")
+        n = img.shape[0]
+        per = img.shape[2:] if self.lanes > 1 else img.shape[1:]
+        h, w = per[:2]
+        c = 1 if len(per) == 2 else per[2]
+        p = _to_mc(cfg)
+        out = img.copy()
+        flags = np.zeros((n, self.lanes), np.uint8)
+        self._check(self._lib.mc_process_clip(self._h, img.ctypes.data, n, w, h, c, w * c, C.byref(p), out.ctypes.data,
+                                              w * c, flags.ctypes.data_as(C.POINTER(C.c_uint8))))
+        return flags.astype(bool), out
+
     # -- device-resident / pipelined forms (benchmarks, serving) -----------------------------
+    def process_clip_device(self, d_in: int, frames: int, w: int, h: int, c: int, in_step: int, cfg_or_params, d_out: int,
+                            out_step: int) -> np.ndarray:
+        """mc_process_clip_device on raw device pointers -> produced bool[frames, lanes]."""
+        p = cfg_or_params if isinstance(cfg_or_params, McParams) else _to_mc(cfg_or_params)
+        flags = np.zeros((int(frames), self.lanes), np.uint8)
+        self._check(self._lib.mc_process_clip_device(self._h, d_in, int(frames), w, h, c, in_step, C.byref(p), d_out, out_step,
+                                                     flags.ctypes.data_as(C.POINTER(C.c_uint8))))
+        return flags.astype(bool)
+
     def process_device(self, d_in: int, w: int, h: int, c: int, in_step: int, cfg_or_params, d_out: int,
                        out_step: int) -> bool:
         p = cfg_or_params if isinstance(cfg_or_params, McParams) else _to_mc(cfg_or_params)

@@ -28,6 +28,21 @@ def kernels():
     return body
 
 
+def clip_spills():
+    """-> {mangled k_level_clip instance: (spill store bytes, spill load bytes)} from the build's ptxas -v log."""
+    log = os.path.join(ROOT, "live-video-magnification_b200", "csrc", "mc_laplace.ptxas.log")
+    out, cur = {}, None
+    for line in open(log) if os.path.exists(log) else []:
+        m = re.search(r"Function properties for (\S+)", line)
+        if m:
+            cur = m.group(1) if "k_level_clip" in m.group(1) else None
+        m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", line)
+        if m and cur:
+            out[cur] = (int(m.group(1)), int(m.group(2)))
+            cur = None
+    return out
+
+
 def main():
     body = kernels()
     count = lambda k, pat: sum(1 for l in body[k] if re.search(pat, l))
@@ -48,6 +63,11 @@ def main():
     need(bool(tma) and all(count(k, "UTMALDG") >= 1 and count(k, "SYNCS") >= 2 for k in tma), "k_level<f32, TMA, *>: cp.async.bulk.tensor (UTMALDG) + mbarrier (SYNCS)")
     pre = [k for k in tma if k.startswith("void k_level<0, true, true")]
     need(bool(pre) and all(count(k, "UTMALDG") == 3 for k in pre), "k_level<f32, TMA, PREFETCH>: three bulk-tensor copies (input window + both state tiles)")
+    clip = [k for k in body if k.startswith("void k_level_clip<0, true>")]
+    need(len(clip) == 1 and count(clip[0], "UTMALDG") >= 1 and count(clip[0], "SYNCS") >= 2,
+         "k_level_clip<f32, TMA>: double-buffered cp.async.bulk.tensor (UTMALDG) + mbarrier (SYNCS)")
+    spills = clip_spills()
+    need(bool(spills) and all(s == (0, 0) for s in spills.values()), f"k_level_clip<*>: no local-memory spills (ptxas -v, {len(spills)} instances)")
     r9 = [k for k in body if k.startswith("k_riesz_analysis(") or k.startswith("k_riesz_collapse(")]
     need(len(r9) == 2 and all(count(k, "UTMALDG") == 1 and count(k, "SYNCS") >= 2 for k in r9), "k_riesz_analysis / k_riesz_collapse: 9x9 input tile by one bulk-tensor copy")
     ing = [k for k in body if k.startswith("void k_ingest_lab<")]
