@@ -154,11 +154,16 @@ mc_status mc_sync(mc_handle* h);
  *            level kernel carries each tile's temporal state in registers from the first frame to the last, so the
  *            state planes are read and written once per clip instead of once per frame.  The structural tracker runs
  *            once, at the clip's first frame; analysis_only produces only the lanes' first frames, as frame calls do.
- *   Phase, Color: one frame call per frame (same results; the clip call works whatever the mode).
+ *   Phase:   one launch set for the whole clip as well.  The analysis, amplification, collapse and egress run over
+ *            the virtual lanes, and the phase kernel carries each pixel's prior pyramid, phases and Butterworth
+ *            registers in registers across the clip.  A filter design that is not finite (every frame is a first frame)
+ *            runs as frame calls.  analysis_only updates the state and produces nothing, as frame calls do.
+ *   Color:   one frame call per frame (same results; the clip call works whatever the mode).
  * MC_ERR_INVALID, with the state untouched, when frames < 1, frames * lanes > MC_MAX_LANES, produced is NULL or frames of
  * mc_submit are in flight; the parameter checks of mc_process_device apply unchanged.  Mode None and an empty image
  * are the identity (all flags 0, state dropped).  A failed clip drops the state like a failed frame.  The clip path
- * keeps device scratch for the largest clip seen (~29 MB per 1080p colour frame at 6 levels), released by mc_reset. */
+ * keeps device scratch for the largest clip seen, released by mc_reset: ~29 MB (Laplace) or ~82 MB (Phase) per 1080p
+ * colour frame at 6 levels. */
 mc_status mc_process_clip_device(mc_handle* h, const uint8_t* d_in, int frames, int width, int height, int channels,
                                  size_t in_step, const mc_params* p, uint8_t* d_out, size_t out_step, uint8_t* produced);
 /* The same on host pointers, blocking (upload, kernels, download of the produced frames only).  Pinned or pageable. */

@@ -209,8 +209,8 @@ bool is_pinned(const void* p) {
 }
 
 // The body of MagnificationProcessor::process on device-resident frames.
-// lane_produced: `lanes` per-lane flags (written).  frames > 1 (Laplace only): a clip of that many consecutive frames
-// of every lane, [t][lane] in the lane stride, with frames * lanes flags.
+// lane_produced: `lanes` per-lane flags (written).  frames > 1 (Laplace and Phase): a clip of that many consecutive
+// frames of every lane, [t][lane] in the lane stride, with frames * lanes flags.
 mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, int channels, size_t in_step,
                               const mc_params* p, uint8_t* d_out, size_t out_step, int* produced, uint8_t* lane_produced,
                               int frames = 1) {
@@ -281,7 +281,7 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
     switch (p->mode) {
         case MC_MODE_LAPLACE: st = h->motion.process(ctx, io, *p, levels, produced, frames); break;
         case MC_MODE_COLOR: st = h->color.process(ctx, io, *p, levels, produced); break;
-        case MC_MODE_PHASE: st = h->riesz.process(ctx, io, *p, levels, produced); break;
+        case MC_MODE_PHASE: st = h->riesz.process(ctx, io, *p, levels, produced, frames); break;
         default: break;
     }
     if (st != MC_OK) {
@@ -853,10 +853,10 @@ mc_status clip_impl(mc_handle* h, const uint8_t* d_in, int frames, int w, int hh
     std::fill(produced, produced + (size_t)frames * lanes, (uint8_t)0);
     int any = 0;
     mc_status st = MC_OK;
-    if (p && p->mode == MC_MODE_LAPLACE && frames > 1) {
+    if (p && (p->mode == MC_MODE_LAPLACE || p->mode == MC_MODE_PHASE) && frames > 1) {
         st = process_device_impl(h, d_in, w, hh, channels, in_step, p, d_out, out_step, &any, produced, frames);
     } else {
-        // Phase, Color (and Laplace with one frame): the frame path, one call per frame
+        // Color (and every mode with one frame): the frame path, one call per frame
         const size_t in_frame = in_step * (size_t)hh * lanes, out_frame = out_step * (size_t)hh * lanes;
         for (int t = 0; t < frames && st == MC_OK; ++t)
             st = process_device_impl(h, d_in ? d_in + (size_t)t * in_frame : nullptr, w, hh, channels, in_step, p,

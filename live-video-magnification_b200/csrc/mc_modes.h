@@ -240,12 +240,38 @@ struct RieszMode {
     std::vector<char> tm_valid;
     LanePlan plan;              // per-lane ops of the current frame
 
+    // Scratch of the clip path (mc_process_clip_device): the per-frame planes of `cap` virtual lanes (frame t of lane k
+    // is virtual lane t * lanes + k).  The temporal state stays in the planes above, so clip and frame calls interleave.
+    struct Clip {
+        int cap = 0;                          // virtual lanes the buffers hold (the largest clip seen)
+        std::vector<float*> oct;              // per level: octave i of every frame (oct[levels-1]: the residual)
+        std::vector<float*> band, rx, ry;     // per band level: band and Riesz pair of every frame; after amplify, rx
+                                              // holds the amplified band and band the collapse result
+        float *amp = nullptr, *t_c = nullptr, *t_s = nullptr;   // one band level (the largest): phase_clip(i) and
+                                                                // amplify(i) are issued back to back
+        int16_t* lab16 = nullptr;             // Lab planes of every frame
+        float* fout = nullptr;                // pre-quantisation tap of every frame (keep_float_output)
+        uint8_t* d_vops = nullptr;            // device LaneOp per virtual lane
+        std::vector<uint8_t> vops;
+        // per band level: TMA descriptors over all virtual planes of octave i (analysis), the band (phase_clip's
+        // 40 x 20 window) and the amplified band (collapse)
+        std::vector<TensorMapStorage> tm_oct, tm_band, tm_amp;
+        std::vector<char> tm_valid;
+        DeviceArena arena;
+    } clip;
+
     void reset();
-    mc_status process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced);
+    // frames > 1: `frames` consecutive frames of every lane ([t][lane] in io's lane stride); ctx.lane_produced then
+    // holds frames * lanes flags
+    mc_status process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced, int frames = 1);
     void find_state(const char* name, int level, StateRef& out);
 
 private:
     mc_status build_pyramid(const ModeCtx& ctx, const uint8_t* ops);
+    mc_status apply_cutoffs(const ModeCtx& ctx, const mc_params& p, bool* rebuild_old);
+    mc_status frame_loop(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced, int frames);
+    mc_status ensure_clip(const ModeCtx& ctx, int vlanes);
+    mc_status run_clip(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int frames, bool first, int* produced);
 };
 
 }  // namespace mc

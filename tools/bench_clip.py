@@ -11,7 +11,12 @@ sequence the same number of times, so the per-frame and clip outputs of the last
 A separate run with profile_kernels gives per-kernel times.  Reported: frames/s, the level kernels' counted bytes
 (from shapes, SURVEY 8d) and roofline.frame = A_min(T) * fps / peak, with the card's name and power limit.
 
-    python tools/bench_clip.py [--seconds 1.0] [--rounds 3] [--out result.json]
+With --mode phase the workload is tools/mode_bench.py's `phase` config instead: Phase (Riesz) 1920x1080x3, 6 levels,
+UI amplification 50, wavelength 50, 0.4-3 Hz @30fps, timed the same way.  Reported: frames/s, bit equality, per-kernel
+times, the phase kernels' bytes per frame counted from shapes, and the clip scratch per frame.  A Phase handle's first
+frame passes through, so only the handle's first frame is allowed not to produce.
+
+    python tools/bench_clip.py [--mode laplace|phase] [--seconds 1.0] [--rounds 3] [--out result.json]
 """
 import argparse
 import ctypes as C
@@ -49,6 +54,37 @@ def a_min(t_frames):
     return 2 * CH * p[0] + 16 * CH * sum(p[1:LEVELS]) / t_frames
 
 
+PHASE_UI = (50, 50.0, 0.4, 3.0, 0, LEVELS, 30.0)   # amplification, wavelength, low, high, chroma, levels, fps
+PHASE_WORKLOAD = "Phase (Riesz) 1920x1080x3 BGR, 6 levels, UI amplification 50, wavelength 50, 0.4-3 Hz @30fps"
+
+
+def riesz_levels(w, h, levels):
+    """(w, h, pitch) of the Phase octaves 0 .. levels-1 (subsample(): ceil halving; rows padded to 32 floats)"""
+    out = []
+    for _ in range(levels):
+        out.append((w, h, (w + 31) // 32 * 32))
+        w, h = w // 2 + w % 2, h // 2 + h % 2
+    return out
+
+
+def phase_counted_bytes(t_frames):
+    """The phase kernels' bytes per frame from shapes, per pitched band-level pixel (one L plane).  k_riesz_phase reads
+    the band (4), the prior {low, Rx, Ry} (12) and the state (2 phases + 8 registers, 40) and writes Rx, Ry (8), the state
+    (40) and amp, t_c, t_s (12): 116 B.  k_riesz_phase_clip moves per frame the band (4), Rx, Ry (8) and amp, t_c, t_s
+    (12), and once per clip the prior and the state in (52) and out (52): 24 + 104 / T B."""
+    px = sum(h * pitch for (_, h, pitch) in riesz_levels(W, H, LEVELS)[:LEVELS - 1])
+    return px, 116 * px, (24 + 104 / t_frames) * px
+
+
+def phase_clip_scratch_bytes():
+    """Device scratch of a Phase clip per frame of one lane (RieszMode::Clip): every octave, the band and the Riesz
+    pair of every band level, amp / t_c / t_s of the largest level, and the Lab int16 planes."""
+    lv = riesz_levels(W, H, LEVELS)
+    planes = [h * pitch for (_, h, pitch) in lv]
+    floats = sum(planes) + 3 * sum(planes[:LEVELS - 1]) + 3 * planes[0]
+    return 4 * floats + 2 * 3 * H * ((W + 63) // 64 * 64)
+
+
 def card():
     try:
         r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -64,7 +100,9 @@ def main():
     ap.add_argument("--seconds", type=float, default=1.0, help="least length of one timed window")
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--out", default=None, help="also write the JSON result here")
+    ap.add_argument("--mode", choices=["laplace", "phase"], default="laplace")
     args = ap.parse_args()
+    phase = args.mode == "phase"
 
     import torch
     import lvm_b200 as L
@@ -73,8 +111,11 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_clip.py needs an H100: the magnification core has no CPU fallback")
     p = capi.McParams()
-    capi.lib().mc_params_from_ui(C.byref(p), capi.MODE_LAPLACE, UI["amplification"], UI["wavelength"], UI["low"], UI["high"],
-                                 UI["chroma"], UI["levels"], UI["fps"])
+    if phase:
+        capi.lib().mc_params_from_ui(C.byref(p), capi.MODE_PHASE, *PHASE_UI)
+    else:
+        capi.lib().mc_params_from_ui(C.byref(p), capi.MODE_LAPLACE, UI["amplification"], UI["wavelength"], UI["low"], UI["high"],
+                                     UI["chroma"], UI["levels"], UI["fps"])
     row = W * CH
     frame_bytes = H * row
     d_in = torch.from_numpy(make_clip(N, 1)).cuda()                    # [N][1][H][W][3]
@@ -87,20 +128,24 @@ def main():
             self.stream = torch.cuda.ExternalStream(self.proc.stream)
             self.out = torch.empty_like(d_in)
             self.fps = []
+            self.fresh = phase   # Phase: the handle's first frame passes through
 
         def step(self):
             """the N-frame sequence once"""
             o = self.out.data_ptr()
             if self.name == "frame":
                 for i in range(N):
-                    assert self.proc.process_device(base + i * frame_bytes, W, H, CH, row, p, o + i * frame_bytes, row)
+                    assert self.proc.process_device(base + i * frame_bytes, W, H, CH, row, p, o + i * frame_bytes, row) or self.fresh
+                    self.fresh = False
             elif self.name == "clip":
                 for i in range(0, N, self.t):
                     f = self.proc.process_clip_device(base + i * frame_bytes, self.t, W, H, CH, row, p, o + i * frame_bytes, row)
-                    assert f.all()
+                    assert f.all() or (self.fresh and f[1:].all())
+                    self.fresh = False
             else:   # T lanes per launch set: N / T steps of T streams
                 for i in range(0, N, self.lanes):
-                    assert self.proc.process_device(base + i * frame_bytes, W, H, CH, row, p, o + i * frame_bytes, row)
+                    assert self.proc.process_device(base + i * frame_bytes, W, H, CH, row, p, o + i * frame_bytes, row) or self.fresh
+                    self.fresh = False
 
         def time(self, steps):
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -141,6 +186,37 @@ def main():
             prof = pr.profile_read()   # the second pass is kept
         kernels[label] = {f"{k}[{lvl}]": round(ms * 1e3 / N, 2) for (k, lvl), (n, ms) in sorted(prof.items(), key=lambda x: -x[1][1])}
         pr.close()
+
+    if phase:
+        rates = {}
+        for m in methods:
+            key = "frame" if m.name == "frame" else f"{m.name} T={m.t if m.name == 'clip' else m.lanes}"
+            rates[key] = {"fps": round(statistics.median(m.fps), 1), "fps_rounds": [round(x, 1) for x in m.fps]}
+        px, frame_b, _ = phase_counted_bytes(1)
+        result = {
+            "workload": PHASE_WORKLOAD + ", one stream, frames in HBM",
+            "card": card(),
+            "unit": "frames/s (device-resident, CUDA events on the handle's stream, median of rounds)",
+            "window_s_min": args.seconds, "passes_per_window": steps, "frames_per_pass": N,
+            "rates": rates,
+            "bit_equal_to_frame_calls": equal,
+            "band_level_pixels": px,
+            "counted_bytes_phase_kernels_MB_per_frame": {"frame_kernel": round(frame_b / 1e6, 1),
+                                                         **{f"clip_kernel T={t}": round(phase_counted_bytes(t)[2] / 1e6, 1) for t in TS}},
+            "clip_scratch_MB_per_frame": round(phase_clip_scratch_bytes() / 1e6, 1),
+            "kernel_us_per_frame": kernels,
+        }
+        line = json.dumps(result)
+        print(line, flush=True)
+        if args.out:
+            os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+            with open(args.out, "w") as f:
+                f.write(line + "\n")
+        for m in methods:
+            m.proc.close()
+        if not all(equal.values()):
+            raise SystemExit("clip outputs differ from per-frame outputs")
+        return
 
     peak, peak_src = measured_peaks()
     frame_b, clip_b = counted_bytes(16)

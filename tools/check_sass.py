@@ -28,14 +28,14 @@ def kernels():
     return body
 
 
-def clip_spills():
-    """-> {mangled k_level_clip instance: (spill store bytes, spill load bytes)} from the build's ptxas -v log."""
-    log = os.path.join(ROOT, "live-video-magnification_b200", "csrc", "mc_laplace.ptxas.log")
+def clip_spills(kernel="k_level_clip", source="mc_laplace"):
+    """-> {mangled `kernel` instance: (spill store bytes, spill load bytes)} from the build's ptxas -v log of `source`."""
+    log = os.path.join(ROOT, "live-video-magnification_b200", "csrc", source + ".ptxas.log")
     out, cur = {}, None
     for line in open(log) if os.path.exists(log) else []:
         m = re.search(r"Function properties for (\S+)", line)
         if m:
-            cur = m.group(1) if "k_level_clip" in m.group(1) else None
+            cur = m.group(1) if kernel in m.group(1) else None
         m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", line)
         if m and cur:
             out[cur] = (int(m.group(1)), int(m.group(2)))
@@ -68,6 +68,12 @@ def main():
          "k_level_clip<f32, TMA>: double-buffered cp.async.bulk.tensor (UTMALDG) + mbarrier (SYNCS)")
     spills = clip_spills()
     need(bool(spills) and all(s == (0, 0) for s in spills.values()), f"k_level_clip<*>: no local-memory spills (ptxas -v, {len(spills)} instances)")
+    pclip = [k for k in body if k.startswith("void k_riesz_phase_clip<true>")]
+    need(len(pclip) == 1 and count(pclip[0], "UTMALDG") >= 1 and count(pclip[0], "SYNCS") >= 2,
+         "k_riesz_phase_clip<TMA>: double-buffered cp.async.bulk.tensor (UTMALDG) + mbarrier (SYNCS)")
+    pspills = clip_spills("k_riesz_phase_clip", "mc_riesz")
+    need(len(pspills) == 2 and all(s == (0, 0) for s in pspills.values()),
+         f"k_riesz_phase_clip<*>: no local-memory spills (ptxas -v, {len(pspills)} instances)")
     r9 = [k for k in body if k.startswith("k_riesz_analysis(") or k.startswith("k_riesz_collapse(")]
     need(len(r9) == 2 and all(count(k, "UTMALDG") == 1 and count(k, "SYNCS") >= 2 for k in r9), "k_riesz_analysis / k_riesz_collapse: 9x9 input tile by one bulk-tensor copy")
     ing = [k for k in body if k.startswith("void k_ingest_lab<")]
