@@ -587,21 +587,20 @@ mc_status mc_submit(mc_handle* h, const uint8_t* in, int width, int height, int 
         // every lane produced); the bytes of the other lanes in `out` are left as they are
         const bool direct = out && is_pinned(out);
         const size_t lane_bytes = row * (size_t)height;
-        for (int a = 0; a < h->lanes && out;) {
-            if (!s.lane_produced[(size_t)a]) { ++a; continue; }
-            int b = a;
-            while (b < h->lanes && s.lane_produced[(size_t)b]) ++b;
-            const size_t n = (size_t)(b - a) * lane_bytes, run_rows = (size_t)(b - a) * height;
-            const uint8_t* src = s.d_out + (size_t)a * lane_bytes;
-            if (direct) {
-                uint8_t* dst = out + (size_t)a * height * out_step;
-                if (out_step == row) CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, h->s_out));
-                else CK(cudaMemcpy2DAsync(dst, out_step, src, row, row, run_rows, cudaMemcpyDeviceToHost, h->s_out));
-            } else {
-                CK(cudaMemcpyAsync(s.h_out + (size_t)a * lane_bytes, src, n, cudaMemcpyDeviceToHost, h->s_out));
-            }
-            a = b;
-        }
+        if (out)
+            st = for_each_run(h->lanes, [&](size_t l) { return s.lane_produced[l] != 0; }, [&](size_t a, size_t b) -> mc_status {
+                const size_t n = (b - a) * lane_bytes, run_rows = (b - a) * height;
+                const uint8_t* src = s.d_out + a * lane_bytes;
+                if (direct) {
+                    uint8_t* dst = out + a * height * out_step;
+                    if (out_step == row) CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, h->s_out));
+                    else CK(cudaMemcpy2DAsync(dst, out_step, src, row, row, run_rows, cudaMemcpyDeviceToHost, h->s_out));
+                } else {
+                    CK(cudaMemcpyAsync(s.h_out + a * lane_bytes, src, n, cudaMemcpyDeviceToHost, h->s_out));
+                }
+                return MC_OK;
+            });
+        if (st != MC_OK) return st;
         s.direct_out = direct;
         CK(cudaEventRecord(s.ev_done, h->s_out));
     } else {
@@ -894,16 +893,15 @@ extern "C" mc_status mc_process_clip(mc_handle* h, const uint8_t* in, int frames
     if (st != MC_OK) return st;
     // only the frames that produced are downloaded, one copy per run of consecutive ones ([t][lane] order); the bytes of
     // the others in `out` are left as they are
-    for (size_t a = 0; a < vl && out;) {
-        if (!produced[a]) { ++a; continue; }
-        size_t b = a;
-        while (b < vl && produced[b]) ++b;
-        const uint8_t* src = h->k_out + a * frame_bytes;
-        uint8_t* dst = out + a * height * out_step;
-        if (out_step == row) CK(cudaMemcpyAsync(dst, src, (b - a) * frame_bytes, cudaMemcpyDeviceToHost, h->stream));
-        else CK(cudaMemcpy2DAsync(dst, out_step, src, row, row, (b - a) * height, cudaMemcpyDeviceToHost, h->stream));
-        a = b;
-    }
+    if (out)
+        st = for_each_run(vl, [&](size_t i) { return produced[i] != 0; }, [&](size_t a, size_t b) -> mc_status {
+            const uint8_t* src = h->k_out + a * frame_bytes;
+            uint8_t* dst = out + a * height * out_step;
+            if (out_step == row) CK(cudaMemcpyAsync(dst, src, (b - a) * frame_bytes, cudaMemcpyDeviceToHost, h->stream));
+            else CK(cudaMemcpy2DAsync(dst, out_step, src, row, row, (b - a) * height, cudaMemcpyDeviceToHost, h->stream));
+            return MC_OK;
+        });
+    if (st != MC_OK) return st;
     CK(cudaStreamSynchronize(h->stream));
     return MC_OK;
 } catch (...) { return on_exception(h); }

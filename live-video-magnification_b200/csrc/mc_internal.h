@@ -54,6 +54,20 @@ enum LaneOp : uint8_t {
 };
 __host__ __device__ __forceinline__ int lane_op(const uint8_t* ops, int lane) { return ops ? (int)ops[lane] : (int)LANE_RUN; }
 
+// Calls f(a, b) once per run [a, b) of consecutive indices in [0, n) for which keep(i) holds, so that lanes (or frames)
+// stored back to back move in one copy.  Stops at the first call that returns an error (non-zero) and returns it.
+template <class Keep, class F>
+auto for_each_run(size_t n, Keep keep, F f) -> decltype(f(n, n)) {
+    for (size_t a = 0; a < n;) {
+        if (!keep(a)) { ++a; continue; }
+        size_t b = a;
+        while (b < n && keep(b)) ++b;
+        if (const auto r = f(a, b)) return r;
+        a = b;
+    }
+    return {};
+}
+
 // ------------------------------------------------------------------------------------------------
 // Laplace launchers (mc_laplace.cu).  All take the handle's stream; every call is one kernel launch
 // and returns the launch's cudaError_t (cudaGetLastError()).

@@ -76,13 +76,17 @@ struct LanePlan {
         // pageable source: staged before the call returns, so `op` may change right after
         return cudaMemcpyAsync(ctx.d_lane_ops, op.data(), op.size(), cudaMemcpyHostToDevice, ctx.stream);
     }
-    void produced(const ModeCtx& ctx, bool run_produces, bool first_produces, int* any) const {
+    // The flags of `frames` frames ([t][lane]): frame 0 by each lane's op, every later frame `later_produces` for the
+    // lanes that are not held (a clip's later frames run).
+    void produced(const ModeCtx& ctx, bool run_produces, bool first_produces, int* any, int frames = 1,
+                  bool later_produces = false) const {
         *any = 0;
-        for (size_t l = 0; l < op.size(); ++l) {
-            const bool p = op[l] == LANE_RUN ? run_produces : op[l] == LANE_FIRST ? first_produces : false;
-            ctx.lane_produced[l] = p ? 1 : 0;
-            *any |= p ? 1 : 0;
-        }
+        for (int t = 0; t < frames; ++t)
+            for (size_t l = 0; l < op.size(); ++l) {
+                const bool p = op[l] == LANE_HOLD ? false : t > 0 ? later_produces : op[l] == LANE_RUN ? run_produces : first_produces;
+                ctx.lane_produced[(size_t)t * op.size() + l] = p ? 1 : 0;
+                *any |= p ? 1 : 0;
+            }
     }
 };
 
@@ -127,6 +131,49 @@ struct DeviceArena {
     void release();
 };
 
+// Scratch of a mode's clip path (mc_process_clip_device): the per-frame buffers of `cap` virtual lanes (frame t of lane k
+// is virtual lane t * lanes + k).  The temporal state stays in the mode's own planes, so clip and frame calls interleave.
+// A mode's Clip derives from this and adds its own planes and tensor maps.
+struct ClipScratch {
+    int cap = 0;                  // virtual lanes the buffers hold (the largest clip seen)
+    int16_t* lab16 = nullptr;     // Lab planes of every frame (C == 3)
+    float* fout = nullptr;        // pre-quantisation tap of every frame (keep_float_output)
+    uint8_t* d_vops = nullptr;    // device LaneOp per virtual lane
+    std::vector<uint8_t> vops;
+    DeviceArena arena;
+
+    // Grows `clip` to `vlanes` virtual lanes of `lane_floats` tap floats and `lab_bytes` Lab16 bytes (none when 0).  On
+    // growth every buffer is released (cudaFree waits for the kernels still reading the old ones), `clip` starts over and
+    // `alloc_planes()` allocates the mode's own planes.  The tap is added when keep_float_output first asks for it.
+    template <class Clip, class AllocPlanes>
+    static mc_status grow(Clip& clip, const ModeCtx& ctx, int vlanes, size_t lab_bytes, size_t lane_floats, AllocPlanes alloc_planes) {
+        if (vlanes > clip.cap) {
+            clip.arena.release();
+            clip = Clip{};
+            MCK_ST(alloc_planes());
+            void* p = nullptr;
+            if (lab_bytes) {
+                MCK(clip.arena.alloc_bytes(&p, lab_bytes));
+                clip.lab16 = (int16_t*)p;
+            }
+            MCK(clip.arena.alloc_bytes(&p, (size_t)vlanes));
+            clip.d_vops = (uint8_t*)p;
+            clip.cap = vlanes;
+        }
+        if (ctx.float_out && !clip.fout) MCK(clip.arena.alloc(&clip.fout, (size_t)clip.cap * lane_floats));
+        return MC_OK;
+    }
+    // The ops of the clip's virtual lanes: HOLD for held lanes at every t, the plan's op at t = 0, RUN after.  With
+    // `upload` they go to d_vops and *d_ops points there; otherwise *d_ops is null and every virtual lane runs.  Laplace
+    // uploads for mixed plans only: a first frame is produced (its stored band is +-0), so when every lane takes one,
+    // `first` alone describes the clip.  Phase uploads whenever a lane is not RUN: a first frame passes through, so the
+    // kernels after the analysis must not write frame 0 of a FIRST lane, even when every lane is FIRST.
+    cudaError_t upload_vops(const ModeCtx& ctx, const LanePlan& plan, int frames, bool upload, const uint8_t** d_ops);
+    // The tap holds every frame of the clip: ctx.float_out gets the last frame of each lane that is not held, one copy
+    // per run of such lanes.
+    mc_status copy_last_tap(const ModeCtx& ctx, const LanePlan& plan, int frames, size_t lane_floats) const;
+};
+
 struct MotionMode {
     int lanes = 1;
     bool empty = true;       // MotionState::empty()
@@ -159,18 +206,11 @@ struct MotionMode {
     std::vector<float> gains;              // per-level gains of the current frame (member: no per-frame allocation)
     LanePlan plan;                         // per-lane ops of the current frame
 
-    // Scratch of the clip path (mc_process_clip_device): the per-frame planes of `cap` virtual lanes (frame t of lane k
-    // is virtual lane t * lanes + k).  The temporal state stays in hi / lo above, so clip and frame calls interleave.
-    struct Clip {
-        int cap = 0;                          // virtual lanes the buffers hold (the largest clip seen)
+    // Scratch of the clip path; the temporal state stays in hi / lo above.
+    struct Clip : ClipScratch {
         std::vector<float*> G, M;             // per level: G_1 .. G_levels, amplified bands M_1 .. M_{levels-1}
-        int16_t* lab16 = nullptr;             // Lab planes (C == 3)
-        float* fout = nullptr;                // pre-quantisation tap of every frame (keep_float_output)
-        uint8_t* d_vops = nullptr;            // device LaneOp per virtual lane
-        std::vector<uint8_t> vops;
         std::vector<TensorMapStorage> tmaps;  // per level: TMA descriptor of G_l over all virtual planes
         std::vector<char> tmap_valid;
-        DeviceArena arena;
     } clip;
 
     void reset();
@@ -184,8 +224,18 @@ private:
     mc_status make_groups(const ModeCtx& ctx);
     void drop_groups();
     mc_status run_group(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, Group& g, bool first, double c_lo, double c_hi);
-    mc_status ensure_clip(const ModeCtx& ctx, int vlanes);
     mc_status run_clip(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int frames, bool first, double c_lo, double c_hi);
+    // the launch set around the level kernels, shared by run_group and run_clip
+    bool fused_ingest() const;
+    int first_level() const;
+    mc_status ingest(const ModeCtx& ctx, const FrameIO& io, int16_t* lab, float* g1);
+    LevelArgs level_args(int l, const std::vector<float*>& g, size_t p0, const int16_t* lab, const FrameIO& io, bool first,
+                         double c_lo, double c_hi) const;
+    mc_status copy_residual(const ModeCtx& ctx, const float* g_res, int lane0, int n);
+    mc_status egress_first_frames(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, const int16_t* lab, float* fout, bool first);
+    template <class Band, class Out>
+    mc_status synthesize(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, const int16_t* lab, float* fout, bool motion,
+                         Band band, Out out);
 };
 
 struct ColorMode {
@@ -240,24 +290,17 @@ struct RieszMode {
     std::vector<char> tm_valid;
     LanePlan plan;              // per-lane ops of the current frame
 
-    // Scratch of the clip path (mc_process_clip_device): the per-frame planes of `cap` virtual lanes (frame t of lane k
-    // is virtual lane t * lanes + k).  The temporal state stays in the planes above, so clip and frame calls interleave.
-    struct Clip {
-        int cap = 0;                          // virtual lanes the buffers hold (the largest clip seen)
+    // Scratch of the clip path; the temporal state stays in the planes above.
+    struct Clip : ClipScratch {
         std::vector<float*> oct;              // per level: octave i of every frame (oct[levels-1]: the residual)
         std::vector<float*> band, rx, ry;     // per band level: band and Riesz pair of every frame; after amplify, rx
                                               // holds the amplified band and band the collapse result
         float *amp = nullptr, *t_c = nullptr, *t_s = nullptr;   // one band level (the largest): phase_clip(i) and
                                                                 // amplify(i) are issued back to back
-        int16_t* lab16 = nullptr;             // Lab planes of every frame
-        float* fout = nullptr;                // pre-quantisation tap of every frame (keep_float_output)
-        uint8_t* d_vops = nullptr;            // device LaneOp per virtual lane
-        std::vector<uint8_t> vops;
         // per band level: TMA descriptors over all virtual planes of octave i (analysis), the band (phase_clip's
         // 40 x 20 window) and the amplified band (collapse)
         std::vector<TensorMapStorage> tm_oct, tm_band, tm_amp;
         std::vector<char> tm_valid;
-        DeviceArena arena;
     } clip;
 
     void reset();
@@ -267,11 +310,18 @@ struct RieszMode {
     void find_state(const char* name, int level, StateRef& out);
 
 private:
-    mc_status build_pyramid(const ModeCtx& ctx, const uint8_t* ops);
+    mc_status allocate(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels);
     mc_status apply_cutoffs(const ModeCtx& ctx, const mc_params& p, bool* rebuild_old);
     mc_status frame_loop(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced, int frames);
-    mc_status ensure_clip(const ModeCtx& ctx, int vlanes);
     mc_status run_clip(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int frames, bool first, int* produced);
+    // the kernels shared by the frame and the clip path, over io.lanes lanes with io.ops
+    mc_status build_pyramid(const ModeCtx& ctx, const FrameIO& io, int16_t* lab, const std::vector<float*>& octs,
+                            const std::vector<float*>& bands, const std::vector<TensorMapStorage>& tm, const std::vector<char>& valid);
+    mc_status amplify(const ModeCtx& ctx, const mc_params& p, int i, int n, const uint8_t* ops, const float* a, const float* tc,
+                      const float* ts, const float* low, const float* rx, const float* ry, float* out);
+    mc_status collapse_egress(const ModeCtx& ctx, const FrameIO& io, const int16_t* lab, const float* residual,
+                              const std::vector<float*>& bands, const std::vector<float*>& out, const std::vector<TensorMapStorage>& tm,
+                              const std::vector<char>& valid, float* fout);
 };
 
 }  // namespace mc

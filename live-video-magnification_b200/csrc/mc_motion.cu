@@ -32,6 +32,30 @@ void DeviceArena::release() {
     blocks.clear();
 }
 
+cudaError_t ClipScratch::upload_vops(const ModeCtx& ctx, const LanePlan& plan, int frames, bool upload, const uint8_t** d_ops) {
+    *d_ops = nullptr;
+    if (!upload) return cudaSuccess;
+    const size_t lanes = plan.op.size();
+    vops.resize((size_t)frames * lanes);
+    for (int t = 0; t < frames; ++t)
+        for (size_t l = 0; l < lanes; ++l) {
+            const uint8_t o = plan.op[l];
+            vops[(size_t)t * lanes + l] = o == LANE_HOLD ? LANE_HOLD : (t == 0 ? o : (uint8_t)LANE_RUN);
+        }
+    *d_ops = d_vops;
+    return cudaMemcpyAsync(d_vops, vops.data(), vops.size(), cudaMemcpyHostToDevice, ctx.stream);
+}
+
+mc_status ClipScratch::copy_last_tap(const ModeCtx& ctx, const LanePlan& plan, int frames, size_t lane_floats) const {
+    if (!ctx.float_out) return MC_OK;
+    const float* last = fout + (size_t)(frames - 1) * plan.op.size() * lane_floats;
+    return for_each_run(plan.op.size(), [&](size_t l) { return plan.op[l] != LANE_HOLD; }, [&](size_t a, size_t b) -> mc_status {
+        MCK(cudaMemcpyAsync(ctx.float_out + a * lane_floats, last + a * lane_floats, (b - a) * lane_floats * sizeof(float),
+                            cudaMemcpyDeviceToDevice, ctx.stream));
+        return MC_OK;
+    });
+}
+
 void MotionMode::drop_groups() {
     for (Group& g : groups) {
         if (g.stream) { cudaStreamSynchronize(g.stream); cudaStreamDestroy(g.stream); }
@@ -155,22 +179,9 @@ mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc
     if (c_lo == 0) c_lo = 0.01;  // TemporalFilter.cpp:11-12
 
     if (frames > 1) {
-        const mc_status st = run_clip(ctx, io, p, frames, first, c_lo, c_hi);
-        if (st != MC_OK) return st;
-        empty = false;
-        // frame 0 as a frame call; every later frame is RUN for the lanes that are not held
-        plan.produced(ctx, !ctx.analysis_only || first, true, produced);
-        for (int t = 1; t < frames; ++t)
-            for (int l = 0; l < lanes; ++l) {
-                const bool pr = plan.op[(size_t)l] != LANE_HOLD && !ctx.analysis_only;
-                ctx.lane_produced[(size_t)t * lanes + l] = pr ? 1 : 0;
-                *produced |= pr ? 1 : 0;
-            }
-        return MC_OK;
-    }
-    if (groups.size() == 1) {
-        const mc_status st = run_group(ctx, io, p, groups[0], first, c_lo, c_hi);
-        if (st != MC_OK) return st;
+        MCK_ST(run_clip(ctx, io, p, frames, first, c_lo, c_hi));
+    } else if (groups.size() == 1) {
+        MCK_ST(run_group(ctx, io, p, groups[0], first, c_lo, c_hi));
     } else {
         // fork: every group's chain starts after whatever the caller queued on the handle's stream (the frame upload),
         // join: the handle's stream continues after all of them (the download / the caller's next use of `out`)
@@ -186,8 +197,95 @@ mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc
         }
     }
     empty = false;
-    // state-carry pass (analysis_only): the temporal state is up to date, only first frames are produced
-    plan.produced(ctx, !ctx.analysis_only || first, true, produced);
+    // state-carry pass (analysis_only): the temporal state is up to date, only first frames are produced; a clip's later
+    // frames run for the lanes that are not held
+    plan.produced(ctx, !ctx.analysis_only || first, true, produced, frames, !ctx.analysis_only);
+    return MC_OK;
+}
+
+// ---- the launch set around the level kernels, shared by run_group (io: one group's lanes) and run_clip (io: every
+// frame's lanes) ----
+
+// production path, >= 2 levels: one fused kernel converts u8 BGR to Lab16 planes and also builds G1; otherwise the
+// level-0 kernel builds G1 (from the Lab16 planes, or from gray frames directly)
+bool MotionMode::fused_ingest() const { return channels == 3 && !faithful && levels >= 2; }
+// the first level the level loop runs: level 0 only builds G1 unless the faithful option is on
+int MotionMode::first_level() const { return fused_ingest() ? 1 : ((levels >= 2 || faithful) ? 0 : levels); }
+
+mc_status MotionMode::ingest(const ModeCtx& ctx, const FrameIO& io, int16_t* lab, float* g1) {
+    if (fused_ingest()) LAUNCH("ingest_lab", 0, launch_ingest_lab(io, *ctx.tables, lab, pitch16, plane16, g1, lv[1], ctx.stream, ctx.ingest_warps));
+    else if (channels == 3) LAUNCH("lab16", 0, launch_lab16(io, *ctx.tables, lab, pitch16, plane16, ctx.stream));
+    return MC_OK;
+}
+
+// The level kernel's arguments that do not depend on the path: level l reads g[l] (level 0: the Lab16 planes or the
+// gray frames) and writes g[l + 1], from plane p0 on; the state planes hi / lo likewise.
+LevelArgs MotionMode::level_args(int l, const std::vector<float*>& g, size_t p0, const int16_t* lab, const FrameIO& io, bool first,
+                                 double c_lo, double c_hi) const {
+    LevelArgs a;
+    if (l == 0) {
+        if (channels == 3) {
+            a.in_kind = 1; a.g = lab; a.in_plane = plane16; a.in_row = pitch16;
+            a.sc[0] = 100.0f / 16384.0f; a.of[0] = 0.0f;
+            a.sc[1] = a.sc[2] = 1.0f / 64.0f; a.of[1] = a.of[2] = -128.0f;
+        } else {
+            a.in_kind = 2; a.g = io.in; a.in_plane = io.in_lane_stride; a.in_row = (int)io.in_step;
+            a.sc[0] = 0.003921568859368563f;
+        }
+    } else {
+        a.in_kind = 0; a.g = g[(size_t)l] + p0 * lv[(size_t)l].plane; a.in_plane = lv[(size_t)l].plane; a.in_row = lv[(size_t)l].pitch;
+    }
+    auto off = [&](float* base, int k) { return base ? base + p0 * lv[(size_t)k].plane : nullptr; };
+    a.channels = channels;
+    a.lf = lv[(size_t)l]; a.lc = lv[(size_t)l + 1];
+    a.g_next = off(g[(size_t)l + 1], l + 1);
+    a.hi = off(hi[(size_t)l], l); a.lo = off(lo[(size_t)l], l);
+    a.first = first ? 1 : 0;
+    a.band = (l >= 1 || faithful) ? 1 : 0;
+    a.c_hi = c_hi; a.one_minus_c_hi = 1 - c_hi; a.c_lo = c_lo; a.one_minus_c_lo = 1 - c_lo;
+    a.gain = gains[(size_t)l];
+    return a;
+}
+
+// faithful_level0: st.lowpassHi/Lo[levels] = the residual g_res of a lane's first frame (MagnifyCore.hpp:100-101), for the
+// lanes [lane0, lane0 + n) that take it; one copy pair per run of such lanes.
+mc_status MotionMode::copy_residual(const ModeCtx& ctx, const float* g_res, int lane0, int n) {
+    if (!faithful) return MC_OK;
+    const size_t lane_floats = (size_t)channels * lv[(size_t)levels].plane;
+    return for_each_run((size_t)n, [&](size_t i) { return plan.op[(size_t)lane0 + i] == LANE_FIRST; }, [&](size_t a, size_t b) -> mc_status {
+        const size_t o = ((size_t)lane0 + a) * lane_floats, len = (b - a) * lane_floats;
+        LAUNCH("copy", levels, launch_copy_planes(hi[(size_t)levels] + o, g_res + o, len, ctx.stream));
+        LAUNCH("copy", levels, launch_copy_planes(lo[(size_t)levels] + o, g_res + o, len, ctx.stream));
+        return MC_OK;
+    });
+}
+
+// analysis_only (state-carry pass): lanes on their first frame are still converted (no motion), running lanes produce
+// nothing.
+mc_status MotionMode::egress_first_frames(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, const int16_t* lab, float* fout, bool first) {
+    if (first || plan.n_first > 0)
+        LAUNCH("egress", 0, launch_egress(io, *ctx.tables, lab, pitch16, plane16, BandSrc{}, lv[levels >= 1 ? 1 : 0], BandSrc{},
+                                          lv[levels >= 2 ? 2 : 0], (float)p.chromAttenuation, fout, ctx.stream, ctx.egress_strip, !first));
+    return MC_OK;
+}
+
+// Synthesis: residual and finest band are zero (MagnifyCore.hpp:130-131), so the collapse starts from band levels-1
+// (cur_{levels-1} = 0 + m_{levels-1}) and writes cur_l to out(l) down to level 2; levels 1 and 0 are folded into egress.
+// band(l) is where level l's amplified band is found.  Without motion (first frames) egress converts the input as it is.
+template <class Band, class Out>
+mc_status MotionMode::synthesize(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, const int16_t* lab, float* fout, bool motion,
+                                 Band band, Out out) {
+    BandSrc m1, c2;
+    if (motion && levels >= 2) {
+        auto cur = [&](int l) { return l == levels - 1 ? band(l) : BandSrc{out(l), nullptr, 1.0f}; };
+        for (int l = levels - 2; l >= 2; --l)
+            LAUNCH("collapse", l, launch_collapse(lv[(size_t)l], lv[(size_t)l + 1], band(l), cur(l + 1), out(l), io.lanes * channels,
+                                                  ctx.stream, io.ops, channels));
+        m1 = band(1);
+        if (levels >= 3) c2 = cur(2);
+    }
+    LAUNCH("egress", 0, launch_egress(io, *ctx.tables, lab, pitch16, plane16, m1, lv[levels >= 1 ? 1 : 0], c2, lv[levels >= 2 ? 2 : 0],
+                                      (float)p.chromAttenuation, fout, ctx.stream, ctx.egress_strip));
     return MC_OK;
 }
 
@@ -198,100 +296,40 @@ mc_status MotionMode::run_group(const ModeCtx& ctx, const FrameIO& io_all, const
     io.out = io_all.out + (size_t)g.lane0 * io_all.out_lane_stride;
     io.lanes = g.lanes;
     if (io.ops) io.ops += g.lane0;   // the op array is indexed by the handle's lane
-    const int planes = g.lanes * channels;
     const size_t p0 = (size_t)g.lane0 * channels;
     auto off = [&](float* base, int l) { return base ? base + p0 * lv[(size_t)l].plane : nullptr; };
     int16_t* lab = lab16 ? lab16 + p0 * plane16 : nullptr;
     float* fout = ctx.float_out ? ctx.float_out + (size_t)g.lane0 * w * h * channels : nullptr;
 
-    // ingest: u8 BGR -> Lab16 planes (gray frames are read directly by the level-0 kernel)
-    // (production path, >= 2 levels: one fused kernel also builds G1; otherwise Lab16 alone)
-    const bool fused_ingest = channels == 3 && !faithful && levels >= 2;
-    if (fused_ingest) LAUNCH("ingest_lab", 0, launch_ingest_lab(io, *ctx.tables, lab, pitch16, plane16, off(G[1], 1), lv[1], ctx.stream, ctx.ingest_warps));
-    else if (channels == 3) LAUNCH("lab16", 0, launch_lab16(io, *ctx.tables, lab, pitch16, plane16, ctx.stream));
-
-    // analysis: one fused kernel per level (level 0 only builds G1 unless the faithful option is on)
-    const int l_begin = fused_ingest ? 1 : ((levels >= 2 || faithful) ? 0 : levels);
-    for (int l = l_begin; l < levels; ++l) {
-        LevelArgs a;
-        if (l == 0) {
-            if (channels == 3) {
-                a.in_kind = 1; a.g = lab; a.in_plane = plane16; a.in_row = pitch16;
-                a.sc[0] = 100.0f / 16384.0f; a.of[0] = 0.0f;
-                a.sc[1] = a.sc[2] = 1.0f / 64.0f; a.of[1] = a.of[2] = -128.0f;
-            } else {
-                a.in_kind = 2; a.g = io.in; a.in_plane = io.in_lane_stride; a.in_row = (int)io.in_step;
-                a.sc[0] = 0.003921568859368563f;
-            }
-        } else {
-            a.in_kind = 0; a.g = off(G[(size_t)l], l); a.in_plane = lv[(size_t)l].plane; a.in_row = lv[(size_t)l].pitch;
-            if (g.tmap_valid[(size_t)l] && ctx.use_tma) {
-                a.tmap = &g.tmaps[(size_t)l];
-                if (ctx.prefetch_state) { a.tmap_hi = &g.tmaps_hi[(size_t)l]; a.tmap_lo = &g.tmaps_lo[(size_t)l]; }
-            }
+    MCK_ST(ingest(ctx, io, lab, off(G[1], 1)));
+    for (int l = first_level(); l < levels; ++l) {
+        LevelArgs a = level_args(l, G, p0, lab, io, first, c_lo, c_hi);
+        if (l >= 1 && g.tmap_valid[(size_t)l] && ctx.use_tma) {
+            a.tmap = &g.tmaps[(size_t)l];
+            if (ctx.prefetch_state) { a.tmap_hi = &g.tmaps_hi[(size_t)l]; a.tmap_lo = &g.tmaps_lo[(size_t)l]; }
         }
-        a.channels = channels;
-        a.lf = lv[(size_t)l]; a.lc = lv[(size_t)l + 1];
-        a.g_next = off(G[(size_t)l + 1], l + 1);
-        a.hi = off(hi[(size_t)l], l); a.lo = off(lo[(size_t)l], l);
         a.m = (first || from_state) ? nullptr : off(M[(size_t)l], l);
-        a.planes = planes;
-        a.first = first ? 1 : 0;
-        a.band = (l >= 1 || faithful) ? 1 : 0;
-        a.c_hi = c_hi; a.one_minus_c_hi = 1 - c_hi; a.c_lo = c_lo; a.one_minus_c_lo = 1 - c_lo;
-        a.gain = gains[(size_t)l];
+        a.planes = g.lanes * channels;
         a.ops = io.ops;
         if (a.band) LAUNCH("level", l, launch_level(a, ctx.stream));
         else LAUNCH("down", l, launch_down(a, ctx.stream));
     }
-    if (first && faithful)  // st.lowpassHi/Lo[levels] = residual (MagnifyCore.hpp:100-101)
-    {
-        const size_t n = (size_t)planes * lv[(size_t)levels].plane;
-        LAUNCH("copy", levels, launch_copy_planes(off(hi[(size_t)levels], levels), off(G[(size_t)levels], levels), n, ctx.stream));
-        LAUNCH("copy", levels, launch_copy_planes(off(lo[(size_t)levels], levels), off(G[(size_t)levels], levels), n, ctx.stream));
-    } else if (faithful && io.ops) {   // the same copy for each lane that takes its first frame among running lanes
-        const size_t n = (size_t)channels * lv[(size_t)levels].plane;
-        for (int ln = g.lane0; ln < g.lane0 + g.lanes; ++ln) {
-            if (plan.op[(size_t)ln] != LANE_FIRST) continue;
-            const size_t o = (size_t)ln * n;
-            LAUNCH("copy", levels, launch_copy_planes(hi[(size_t)levels] + o, G[(size_t)levels] + o, n, ctx.stream));
-            LAUNCH("copy", levels, launch_copy_planes(lo[(size_t)levels] + o, G[(size_t)levels] + o, n, ctx.stream));
-        }
-    }
-    const Level& l1 = lv[levels >= 1 ? 1 : 0];
-    const Level& l2 = lv[levels >= 2 ? 2 : 0];
-    if (ctx.analysis_only && !first) {
-        // state-carry pass: lanes on their first frame are still converted (no motion), the running lanes produce nothing
-        if (plan.n_first > 0)
-            LAUNCH("egress", 0, launch_egress(io, *ctx.tables, lab, pitch16, plane16, BandSrc{}, l1, BandSrc{}, l2, (float)p.chromAttenuation,
-                                              fout, ctx.stream, ctx.egress_strip, true));
-        return MC_OK;
-    }
-    BandSrc m1, c2;
-    if (!first && levels >= 2) {
-        // synthesis: residual and finest band are zero (MagnifyCore.hpp:130-131), so the collapse starts from
-        // band levels-1 (cur_{levels-1} = 0 + m_{levels-1}); levels 1 and 0 are folded into egress.
-        auto band = [&](int l) {
-            return from_state ? BandSrc{off(hi[(size_t)l], l), off(lo[(size_t)l], l), gains[(size_t)l]} : BandSrc{off(M[(size_t)l], l), nullptr, 1.0f};
-        };
-        auto cur = [&](int l) { return l == levels - 1 ? band(l) : BandSrc{off(M[(size_t)l], l), nullptr, 1.0f}; };
-        for (int l = levels - 2; l >= 2; --l)
-            LAUNCH("collapse", l, launch_collapse(lv[(size_t)l], lv[(size_t)l + 1], band(l), cur(l + 1), off(M[(size_t)l], l), planes, ctx.stream,
-                                                  io.ops, channels));
-        m1 = band(1);
-        if (levels >= 3) c2 = cur(2);
-    }
-    LAUNCH("egress", 0, launch_egress(io, *ctx.tables, lab, pitch16, plane16, m1, l1, c2, l2, (float)p.chromAttenuation, fout,
-                                      ctx.stream, ctx.egress_strip));
-    return MC_OK;
+    MCK_ST(copy_residual(ctx, G[(size_t)levels], g.lane0, g.lanes));
+    if (ctx.analysis_only) return egress_first_frames(ctx, io, p, lab, fout, first);
+    auto band = [&](int l) {
+        return from_state ? BandSrc{off(hi[(size_t)l], l), off(lo[(size_t)l], l), gains[(size_t)l]} : BandSrc{off(M[(size_t)l], l), nullptr, 1.0f};
+    };
+    return synthesize(ctx, io, p, lab, fout, !first, band, [&](int l) { return off(M[(size_t)l], l); });
 }
 
-// Grows the clip scratch to `vlanes` virtual lanes (and adds the float tap when keep_float_output asks for it).
-mc_status MotionMode::ensure_clip(const ModeCtx& ctx, int vlanes) {
-    const size_t vplanes = (size_t)vlanes * channels;
-    if (vlanes > clip.cap) {
-        clip.arena.release();   // cudaFree waits for the kernels still reading the old buffers
-        clip = Clip{};
+// One clip: the launch set of run_group over V = frames * lanes virtual lanes, with the level kernels replaced by
+// k_level_clip (state in registers across the clip).  Synthesis reads the stored bands M_l; a lane's first frame has
+// M = +-0 there, which gives the first-frame output without a branch.  Lane groups do not apply: one chain.
+mc_status MotionMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_params& p, int frames, bool first, double c_lo, double c_hi) {
+    const int vl = frames * lanes;
+    MCK_ST(ClipScratch::grow(clip, ctx, vl, channels == 3 ? (size_t)vl * channels * plane16 * sizeof(int16_t) : 0, (size_t)w * h * channels,
+                             [&]() -> mc_status {
+        const size_t vplanes = (size_t)vl * channels;
         clip.G.assign((size_t)levels + 1, nullptr);
         clip.M.assign((size_t)levels + 1, nullptr);
         clip.tmaps.assign((size_t)levels + 1, TensorMapStorage{});
@@ -301,126 +339,32 @@ mc_status MotionMode::ensure_clip(const ModeCtx& ctx, int vlanes) {
             if (l < levels) MCK(clip.arena.alloc(&clip.M[(size_t)l], vplanes * lv[(size_t)l].plane));
             if (l < levels) clip.tmap_valid[(size_t)l] = make_level_tensor_map(&clip.tmaps[(size_t)l], clip.G[(size_t)l], lv[(size_t)l], (int)vplanes) ? 1 : 0;
         }
-        if (channels == 3) {
-            void* p = nullptr;
-            MCK(clip.arena.alloc_bytes(&p, vplanes * plane16 * sizeof(int16_t)));
-            clip.lab16 = (int16_t*)p;
-        }
-        void* p = nullptr;
-        MCK(clip.arena.alloc_bytes(&p, (size_t)vlanes));
-        clip.d_vops = (uint8_t*)p;
-        clip.cap = vlanes;
-    }
-    if (ctx.float_out && !clip.fout) MCK(clip.arena.alloc(&clip.fout, (size_t)clip.cap * w * h * channels));
-    return MC_OK;
-}
-
-// One clip: the launch set of run_group over V = frames * lanes virtual lanes, with the level kernels replaced by
-// k_level_clip (state in registers across the clip).  Synthesis reads the stored bands M_l; a lane's first frame has
-// M = +-0 there, which gives the first-frame output without a branch.  Lane groups do not apply: one chain.
-mc_status MotionMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_params& p, int frames, bool first, double c_lo, double c_hi) {
-    const int vl = frames * lanes;
-    MCK_ST(ensure_clip(ctx, vl));
-    const int planes = lanes * channels, vplanes = vl * channels;
+        return MC_OK;
+    }));
     FrameIO io = io0;   // every frame of every lane
     io.lanes = vl;
-    io.ops = nullptr;
-    if (plan.mixed()) {   // virtual ops: HOLD for held lanes at every t, FIRST at t = 0 for lanes without state, RUN otherwise
-        clip.vops.resize((size_t)vl);
-        for (int t = 0; t < frames; ++t)
-            for (int l = 0; l < lanes; ++l) {
-                const uint8_t o = plan.op[(size_t)l];
-                clip.vops[(size_t)t * lanes + l] = o == LANE_HOLD ? LANE_HOLD : (t == 0 ? o : (uint8_t)LANE_RUN);
-            }
-        MCK(cudaMemcpyAsync(clip.d_vops, clip.vops.data(), (size_t)vl, cudaMemcpyHostToDevice, ctx.stream));
-        io.ops = clip.d_vops;
-    }
+    MCK(clip.upload_vops(ctx, plan, frames, plan.mixed(), &io.ops));
 
-    const bool fused_ingest = channels == 3 && !faithful && levels >= 2;
-    if (fused_ingest) LAUNCH("ingest_lab", 0, launch_ingest_lab(io, *ctx.tables, clip.lab16, pitch16, plane16, clip.G[1], lv[1], ctx.stream, ctx.ingest_warps));
-    else if (channels == 3) LAUNCH("lab16", 0, launch_lab16(io, *ctx.tables, clip.lab16, pitch16, plane16, ctx.stream));
-
-    const int l_begin = fused_ingest ? 1 : ((levels >= 2 || faithful) ? 0 : levels);
-    for (int l = l_begin; l < levels; ++l) {
-        LevelArgs a;
-        if (l == 0) {
-            if (channels == 3) {
-                a.in_kind = 1; a.g = clip.lab16; a.in_plane = plane16; a.in_row = pitch16;
-                a.sc[0] = 100.0f / 16384.0f; a.of[0] = 0.0f;
-                a.sc[1] = a.sc[2] = 1.0f / 64.0f; a.of[1] = a.of[2] = -128.0f;
-            } else {
-                a.in_kind = 2; a.g = io.in; a.in_plane = io.in_lane_stride; a.in_row = (int)io.in_step;
-                a.sc[0] = 0.003921568859368563f;
-            }
-        } else {
-            a.in_kind = 0; a.g = clip.G[(size_t)l]; a.in_plane = lv[(size_t)l].plane; a.in_row = lv[(size_t)l].pitch;
-            if (clip.tmap_valid[(size_t)l] && ctx.use_tma) a.tmap = &clip.tmaps[(size_t)l];
-        }
-        a.channels = channels;
-        a.lf = lv[(size_t)l]; a.lc = lv[(size_t)l + 1];
-        a.g_next = clip.G[(size_t)l + 1];
-        a.hi = hi[(size_t)l]; a.lo = lo[(size_t)l];
+    MCK_ST(ingest(ctx, io, clip.lab16, clip.G[1]));
+    for (int l = first_level(); l < levels; ++l) {
+        LevelArgs a = level_args(l, clip.G, 0, clip.lab16, io, first, c_lo, c_hi);
+        if (l >= 1 && clip.tmap_valid[(size_t)l] && ctx.use_tma) a.tmap = &clip.tmaps[(size_t)l];
         a.m = ctx.analysis_only ? nullptr : clip.M[(size_t)l];
-        a.first = first ? 1 : 0;
-        a.band = (l >= 1 || faithful) ? 1 : 0;
-        a.c_hi = c_hi; a.one_minus_c_hi = 1 - c_hi; a.c_lo = c_lo; a.one_minus_c_lo = 1 - c_lo;
-        a.gain = gains[(size_t)l];
         if (a.band) {
-            a.planes = planes; a.ops = io0.ops;   // state planes, per-lane ops of the clip's first frame
+            a.planes = lanes * channels; a.ops = io0.ops;   // state planes, per-lane ops of the clip's first frame
             LAUNCH("level_clip", l, launch_level_clip(a, frames, ctx.stream));
         } else {
-            a.planes = vplanes; a.ops = io.ops;
+            a.planes = vl * channels; a.ops = io.ops;
             LAUNCH("down", l, launch_down(a, ctx.stream));
         }
     }
-    if (faithful) {   // st.lowpassHi/Lo[levels] = residual of the lane's first frame (MagnifyCore.hpp:100-101)
-        const size_t n = (size_t)channels * lv[(size_t)levels].plane;
-        for (int ln = 0; ln < lanes; ++ln) {
-            if (!(first ? plan.op[(size_t)ln] != LANE_HOLD : plan.op[(size_t)ln] == LANE_FIRST)) continue;
-            const size_t o = (size_t)ln * n;
-            LAUNCH("copy", levels, launch_copy_planes(hi[(size_t)levels] + o, clip.G[(size_t)levels] + o, n, ctx.stream));
-            LAUNCH("copy", levels, launch_copy_planes(lo[(size_t)levels] + o, clip.G[(size_t)levels] + o, n, ctx.stream));
-        }
-    }
-    const Level& l1 = lv[levels >= 1 ? 1 : 0];
-    const Level& l2 = lv[levels >= 2 ? 2 : 0];
-    const float chroma = (float)p.chromAttenuation;
-    if (ctx.analysis_only) {
-        // state-carry pass: only the clip's first frame can produce (lanes on their first frame, converted without
-        // motion); it is frame 0's egress of a frame call, so the float tap is written in place
-        FrameIO f0 = io0;
-        if (first) LAUNCH("egress", 0, launch_egress(f0, *ctx.tables, clip.lab16, pitch16, plane16, BandSrc{}, l1, BandSrc{}, l2, chroma,
-                                                     ctx.float_out, ctx.stream, ctx.egress_strip));
-        else if (plan.n_first > 0)
-            LAUNCH("egress", 0, launch_egress(f0, *ctx.tables, clip.lab16, pitch16, plane16, BandSrc{}, l1, BandSrc{}, l2, chroma,
-                                              ctx.float_out, ctx.stream, ctx.egress_strip, true));
-        return MC_OK;
-    }
-    BandSrc m1, c2;
-    if (levels >= 2) {
-        auto band = [&](int l) { return BandSrc{clip.M[(size_t)l], nullptr, 1.0f}; };
-        for (int l = levels - 2; l >= 2; --l)
-            LAUNCH("collapse", l, launch_collapse(lv[(size_t)l], lv[(size_t)l + 1], band(l), band(l + 1), clip.M[(size_t)l], vplanes,
-                                                  ctx.stream, io.ops, channels));
-        m1 = band(1);
-        if (levels >= 3) c2 = band(2);
-    }
-    float* fout = ctx.float_out ? clip.fout : nullptr;
-    LAUNCH("egress", 0, launch_egress(io, *ctx.tables, clip.lab16, pitch16, plane16, m1, l1, c2, l2, chroma, fout, ctx.stream,
-                                      ctx.egress_strip));
-    if (fout) {   // the tap holds the clip's last frame: copy the lanes it wrote (all but the held ones)
-        const size_t lane_floats = (size_t)w * h * channels;
-        const float* last = fout + (size_t)(frames - 1) * lanes * lane_floats;
-        for (int a = 0; a < lanes;) {
-            if (plan.op[(size_t)a] == LANE_HOLD) { ++a; continue; }
-            int b = a;
-            while (b < lanes && plan.op[(size_t)b] != LANE_HOLD) ++b;
-            MCK(cudaMemcpyAsync(ctx.float_out + (size_t)a * lane_floats, last + (size_t)a * lane_floats, (size_t)(b - a) * lane_floats * sizeof(float),
-                                cudaMemcpyDeviceToDevice, ctx.stream));
-            a = b;
-        }
-    }
-    return MC_OK;
+    MCK_ST(copy_residual(ctx, clip.G[(size_t)levels], 0, lanes));   // frame 0 is the first `lanes` virtual lanes
+    // state-carry pass: only the clip's first frame can produce; it is frame 0's egress of a frame call, so the float
+    // tap is written in place
+    if (ctx.analysis_only) return egress_first_frames(ctx, io0, p, clip.lab16, ctx.float_out, first);
+    MCK_ST(synthesize(ctx, io, p, clip.lab16, ctx.float_out ? clip.fout : nullptr, true,
+                      [&](int l) { return BandSrc{clip.M[(size_t)l], nullptr, 1.0f}; }, [&](int l) { return clip.M[(size_t)l]; }));
+    return clip.copy_last_tap(ctx, plan, frames, (size_t)w * h * channels);
 }
 
 void MotionMode::find_state(const char* name, int level, StateRef& out) {
