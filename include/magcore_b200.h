@@ -244,6 +244,11 @@ mc_status mc_set_option(mc_handle* h, const char* key, int value);
  *   "lo.r1.s", "hi.r0.c", "hi.r0.s", "hi.r1.c", "hi.r1.s" (itsRegister0/1 of the low / high cutoff filters,
  *   TemporalFilter.cpp:299-317);
  * Color keeps its rolling window in a device ring buffer that is not exposed.
+ * Laplace and Phase, level 0, three channels, read-only: "lab16", the BGR->Lab conversion of the last frame call as
+ *   the kernels hold it, the raw fixed-point values L*2^14/100, (a+128)*64, (b+128)*64 widened (exactly) to f32.  It
+ *   exists only after a frame call on 3-channel input; before the first frame, after mc_reset and after a clip call it
+ *   is absent (clips convert into their own scratch).  A held lane keeps the planes of its last converted frame.
+ *   mc_set_state on it returns MC_ERR_INVALID.
  * mc_state_dims reports rows/cols/channels for a name+level (0 rows if absent). */
 mc_status mc_state_dims(mc_handle* h, const char* name, int level, int* rows, int* cols, int* channels);
 mc_status mc_get_state(mc_handle* h, const char* name, int level, float* dst, size_t dst_floats);

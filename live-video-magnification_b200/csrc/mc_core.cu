@@ -650,7 +650,7 @@ mc_status mc_state_dims(mc_handle* h, const char* name, int level, int* rows, in
     if (h->t_mode == MC_MODE_LAPLACE) h->motion.find_state(name, level, r);
     else if (h->t_mode == MC_MODE_COLOR) h->color.find_state(name, level, r);
     else if (h->t_mode == MC_MODE_PHASE) h->riesz.find_state(name, level, r);
-    if (r.ptr) { *rows = r.rows; *cols = r.cols; *channels = r.channels; }
+    if (r.found()) { *rows = r.rows; *cols = r.cols; *channels = r.channels; }
     return MC_OK;
 } catch (...) { return on_exception(h); }
 
@@ -661,10 +661,20 @@ static mc_status state_xfer(mc_handle* h, const char* name, int level, float* ho
     if (h->t_mode == MC_MODE_LAPLACE) h->motion.find_state(name, level, r);
     else if (h->t_mode == MC_MODE_COLOR) h->color.find_state(name, level, r);
     else if (h->t_mode == MC_MODE_PHASE) h->riesz.find_state(name, level, r);
-    if (!r.ptr) { h->err = std::string("no such state: ") + name; return MC_ERR_INVALID; }
+    if (!r.found()) { h->err = std::string("no such state: ") + name; return MC_ERR_INVALID; }
+    if (r.ptr16 && !get) { h->err = std::string("read-only state: ") + name; return MC_ERR_INVALID; }
     const size_t planes = (size_t)h->lanes * r.channels;
     if (n < planes * r.rows * r.cols) { h->err = "state buffer too small"; return MC_ERR_INVALID; }
     CK(cudaStreamSynchronize(h->stream));
+    if (r.ptr16) {   // int16 planes: download, then widen (exact)
+        std::vector<int16_t> tmp((size_t)r.rows * r.cols);
+        for (size_t pl = 0; pl < planes; ++pl) {
+            CK(cudaMemcpy2D(tmp.data(), (size_t)r.cols * 2, r.ptr16 + pl * r.plane_stride, (size_t)r.pitch * 2, (size_t)r.cols * 2, r.rows,
+                            cudaMemcpyDeviceToHost));
+            std::copy(tmp.begin(), tmp.end(), host + pl * (size_t)r.rows * r.cols);
+        }
+        return MC_OK;
+    }
     for (size_t pl = 0; pl < planes; ++pl) {
         float* d = r.ptr + pl * r.plane_stride;
         float* hp = host + pl * (size_t)r.rows * r.cols;

@@ -118,9 +118,18 @@ struct LanePlan {
 
 struct StateRef {  // a named state plane set for mc_get_state / mc_set_state
     float* ptr = nullptr;
+    const int16_t* ptr16 = nullptr;   // read-only int16 planes ("lab16"), widened to f32 on download
     int rows = 0, cols = 0, channels = 0, pitch = 0;
     size_t plane_stride = 0;
+    bool found() const { return ptr || ptr16; }
 };
+
+// "lab16" (level 0, 3 channels): a mode's Lab16 planes of the last frame call, while they are current
+inline void lab16_state(const int16_t* lab16, bool current, int w, int h, int pitch16, size_t plane16, StateRef& out) {
+    out = StateRef{};
+    if (!lab16 || !current) return;
+    out.ptr16 = lab16; out.rows = h; out.cols = w; out.channels = 3; out.pitch = pitch16; out.plane_stride = plane16;
+}
 
 // Simple owner of cudaMalloc'ed float buffers (freed together on reset()).
 struct DeviceArena {
@@ -186,6 +195,7 @@ struct MotionMode {
     int16_t* lab16 = nullptr;           // Lab planes of the current frame (C == 3)
     int pitch16 = 0;
     size_t plane16 = 0;
+    bool lab16_frame = false;           // lab16 holds the last frame call's Lab (clips write their own scratch)
     DeviceArena arena;
 
     // Lane groups (option "lane_groups"): the streams of a handle are independent, so their launch sets are issued as
@@ -285,6 +295,7 @@ struct RieszMode {
     int16_t* lab16 = nullptr;
     int pitch16 = 0;
     size_t plane16 = 0;
+    bool lab16_frame = false;   // lab16 holds the last frame call's Lab (clips write their own scratch)
     // TMA descriptors of the 9x9 kernels' input tiles (72 x 24 boxes): octave i (analysis), amplified band i (collapse)
     std::vector<TensorMapStorage> tm_oct, tm_band;
     std::vector<char> tm_valid;

@@ -72,6 +72,7 @@ void MotionMode::reset() {
     clip = Clip{};
     lv.clear(); G.clear(); hi.clear(); lo.clear(); M.clear();
     lab16 = nullptr;
+    lab16_frame = false;
     allocated = false;
     empty = true;
 }
@@ -178,6 +179,7 @@ mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc
     double c_lo = p.coLow, c_hi = p.coHigh;
     if (c_lo == 0) c_lo = 0.01;  // TemporalFilter.cpp:11-12
 
+    lab16_frame = false;   // a clip converts into its own scratch; a frame call rewrites lab16 below
     if (frames > 1) {
         MCK_ST(run_clip(ctx, io, p, frames, first, c_lo, c_hi));
     } else if (groups.size() == 1) {
@@ -197,6 +199,7 @@ mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc
         }
     }
     empty = false;
+    lab16_frame = frames == 1 && lab16;
     // state-carry pass (analysis_only): the temporal state is up to date, only first frames are produced; a clip's later
     // frames run for the lanes that are not held
     plan.produced(ctx, !ctx.analysis_only || first, true, produced, frames, !ctx.analysis_only);
@@ -369,6 +372,10 @@ mc_status MotionMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_
 
 void MotionMode::find_state(const char* name, int level, StateRef& out) {
     out = StateRef{};
+    if (!std::strcmp(name, "lab16")) {
+        if (level == 0) lab16_state(lab16, lab16_frame, w, h, pitch16, plane16, out);
+        return;
+    }
     if (!allocated || empty || level < 0 || level > levels) return;
     float* p = nullptr;
     if (!std::strcmp(name, "lowpassHi")) p = hi[(size_t)level];

@@ -667,6 +667,7 @@ void RieszMode::reset() {
                     &lo_r1c, &lo_r1s, &hi_r0c, &hi_r0s, &hi_r1c, &hi_r1s, &amp, &t_c, &t_s, &low_amp, &res})
         v->clear();
     lab16 = nullptr;
+    lab16_frame = false;
     clip.arena.release();
     clip = Clip{};
     allocated = false;
@@ -816,7 +817,10 @@ mc_status RieszMode::allocate(const ModeCtx& ctx, const FrameIO& io, const mc_pa
 
 mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_params& p, int nlevels, int* produced, int frames) {
     *produced = 0;
-    if (io_in.channels < 3) return MC_OK;  // MagnifyCore.hpp:212: gray input is a silent passthrough
+    if (io_in.channels < 3) {   // MagnifyCore.hpp:212: gray input is a silent passthrough
+        lab16_frame = false;
+        return MC_OK;
+    }
     // Per-lane ops: lanes without state take their first frame while the others run, held lanes are skipped.  When every
     // lane is on its first frame the handle's state is rebuilt from scratch, as for the reference's first frame.
     const bool fresh = !allocated || std::isnan(loA[0]) || std::isnan(hiA[0]);  // :226
@@ -836,10 +840,12 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_
         if (allocated) *ctx.held_lost = true;
         MCK_ST(allocate(ctx, io_in, p, nlevels));
     }
+    lab16_frame = false;   // a clip converts into its own scratch; a frame call rewrites lab16 below
     if (frames > 1) return run_clip(ctx, io_in, p, frames, first, produced);
     FrameIO io = io_in;
     MCK(plan.upload(ctx, &io.ops));
     MCK_ST(build_pyramid(ctx, io, lab16, oct, cur_low, tm_oct, tm_valid));
+    lab16_frame = true;
     if (first) {
         // old = pyramid of the first frame with a zero Riesz pair; the frame itself is shown unmagnified (:239)
         for (int i = 0; i < levels - 1; ++i) std::swap(cur_low[(size_t)i], old_low[(size_t)i]);
@@ -902,6 +908,7 @@ mc_status RieszMode::frame_loop(const ModeCtx& ctx, const FrameIO& io, const mc_
         MCK_ST(process(c, f, p, nlevels, &any));
         *produced |= any;
     }
+    lab16_frame = false;   // a clip call, even one run as frame calls
     return MC_OK;
 }
 
@@ -988,6 +995,10 @@ mc_status RieszMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_p
 
 void RieszMode::find_state(const char* name, int level, StateRef& out) {
     out = StateRef{};
+    if (!std::strcmp(name, "lab16")) {   // before the band-level guard: a 1-level pyramid has no band level
+        if (level == 0) lab16_state(lab16, lab16_frame, w, h, pitch16, plane16, out);
+        return;
+    }
     if (!allocated || level < 0 || level >= levels - 1) return;
     struct { const char* n; std::vector<float*>* v; } map[] = {
         {"old.lowpass", &old_low}, {"old.rx", &old_rx}, {"old.ry", &old_ry}, {"phase.c", &phase_c}, {"phase.s", &phase_s},

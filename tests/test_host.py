@@ -88,12 +88,17 @@ def test_motion_gains_bit_identical(built):
     assert np.allclose(ref, [0, -0.0725, 1.855, 5.710, 13.420, 20, 0], atol=2e-3)
 
 
+def all_colours():
+    """Every 24-bit colour once, as (b, g, r) = (i >> 16, (i >> 8) & 255, i & 255)."""
+    i = np.arange(1 << 24, dtype=np.uint32)
+    return np.stack([i >> 16, (i >> 8) & 255, i & 255], -1).astype(np.uint8)
+
+
 def test_bgr2lab_device_function_is_bit_exact_with_cv2(hc):
+    """Every colour: this pins the whole LUT, including the clamped neighbours at the top of the lattice."""
     assert hc.hc_lut_entries() == 34 * 33 * 33   # LabLutCell table: one padded b slab
-    rng = np.random.default_rng(0)
-    px = rng.integers(0, 256, (50000, 3), dtype=np.uint8)
     edge = np.array([[0, 0, 0], [255, 255, 255], [255, 0, 0], [0, 255, 0], [0, 0, 255], [8, 8, 8], [7, 9, 247]], np.uint8)
-    px = np.concatenate([px, edge])
+    px = np.concatenate([all_colours(), edge])
     got = np.empty((len(px), 3), np.float32)
     hc.hc_bgr_to_lab(px.ctypes.data_as(C.c_void_p), len(px), got.ctypes.data_as(C.c_void_p))
     ref = cv2.cvtColor((px.astype(np.float32) * np.float32(1 / 255.0))[None], cv2.COLOR_BGR2Lab)[0]
@@ -102,9 +107,9 @@ def test_bgr2lab_device_function_is_bit_exact_with_cv2(hc):
 
 def test_lab2bgr_device_function_matches_cv2(hc):
     rng = np.random.default_rng(1)
-    px = rng.integers(0, 256, (40000, 3), dtype=np.uint8)
+    px = all_colours()
     lab = cv2.cvtColor((px.astype(np.float32) * np.float32(1 / 255.0))[None], cv2.COLOR_BGR2Lab)[0]
-    lab = np.concatenate([lab, lab + rng.normal(0, 4, lab.shape).astype(np.float32),
+    lab = np.concatenate([lab, lab[rng.integers(0, len(lab), 40000)] + rng.normal(0, 4, (40000, 3)).astype(np.float32),
                           np.stack([rng.uniform(-10, 110, 5000), rng.uniform(-150, 150, 5000), rng.uniform(-150, 150, 5000)], -1).astype(np.float32)])
     lab = np.ascontiguousarray(lab, np.float32)
     got = np.empty_like(lab)
