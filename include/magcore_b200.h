@@ -201,6 +201,39 @@ mc_status mc_submit(mc_handle* h, const uint8_t* in, int width, int height, int 
                     size_t in_step, const mc_params* p, uint8_t* out, size_t out_step);
 mc_status mc_collect(mc_handle* h, int* produced);
 
+/* --- NV12 frames: the hand-off format of hardware video decoders and encoders ---------------------------------------
+ * NV12 is 4:2:0 YCbCr in two planes: a luma plane (height rows of width bytes) and a plane of interleaved Cb,Cr pairs
+ * (height/2 rows of width bytes), one pair per 2x2 pixel block.  The matrix is ITU-R BT.601, limited range (Y 16..235,
+ * Cb/Cr 16..240); chroma is sited at the top-left pixel of each block.  The core converts on the device exactly as
+ * OpenCV does (u8, 20-bit fixed point): the input with cvtColor(COLOR_YUV2BGR_NV12), which gives every pixel of a block
+ * the block's Cb,Cr; the output with cvtColor(COLOR_BGR2YUV_I420), whose Cb,Cr are those of each block's top-left pixel,
+ * stored interleaved.  The magnifier in between sees 3-channel BGR frames, so for any NV12 input X an NV12 call gives
+ *     out = to_nv12(bgr_call(to_bgr(X)))
+ * bit for bit: the output bytes, the produced flags and the temporal state afterwards.  NV12 and BGR calls of the same
+ * geometry interleave on one handle without a structural reset (the tracker sees channels = 3).  A lane or frame that
+ * did not produce leaves both of its planes of `out` untouched.  keep_float_output, profile_kernels ("nv12_to_bgr",
+ * "bgr_to_nv12"), the lane lifecycle and the clip rules apply unchanged.  MC_ERR_INVALID, with the state untouched, when
+ * width or height is odd or < 2, pitch < width, a plane pointer is NULL, or (more than one lane) lane_stride is less
+ * than pitch * height.  Each call keeps device BGR staging for the largest frame set seen. */
+typedef struct mc_nv12 {
+    uint8_t* y;          /* luma plane of lane 0 (of frame 0 of lane 0 in a clip): height rows of width bytes */
+    uint8_t* uv;         /* interleaved Cb,Cr plane of the same frame: height/2 rows of width bytes; it need not follow
+                            the luma plane (decoders put it at pitch * aligned height, e.g. 1088 rows for 1080p H.264) */
+    size_t pitch;        /* bytes per row, both planes */
+    size_t lane_stride;  /* bytes from one (virtual) lane's planes to the next, the same for y and uv */
+} mc_nv12;
+/* mc_process_device on NV12 device planes. */
+mc_status mc_process_nv12_device(mc_handle* h, const mc_nv12* in, int width, int height, const mc_params* p,
+                                 const mc_nv12* out, int* produced);
+/* mc_process_clip_device on NV12 device planes: frame t of lane k is virtual lane t * lanes + k of in / out;
+ * produced: frames * lanes bytes, [t][lane]. */
+mc_status mc_process_clip_nv12_device(mc_handle* h, const mc_nv12* in, int frames, int width, int height,
+                                      const mc_params* p, const mc_nv12* out, uint8_t* produced);
+/* mc_submit on NV12 host planes, pinned or pageable; collected by mc_collect.  Only NV12 bytes cross PCIe (1.5 B/px
+ * each way); pageable planes go through NV12-sized pinned staging.  There is no blocking host NV12 call: submit and
+ * collect. */
+mc_status mc_submit_nv12(mc_handle* h, const mc_nv12* in, int width, int height, const mc_params* p, const mc_nv12* out);
+
 /* Pinned host memory for frames (so FramePool buffers can be DMA'd directly). */
 void* mc_host_alloc(size_t bytes);
 void mc_host_free(void* p);

@@ -30,9 +30,15 @@ class McChainInfo(C.Structure):
                 ("magnified", C.c_int32)]
 
 
+class McNv12(C.Structure):
+    """mc_nv12: one NV12 frame set (plane pointers are host or device addresses as integers)."""
+    _fields_ = [("y", C.c_void_p), ("uv", C.c_void_p), ("pitch", C.c_size_t), ("lane_stride", C.c_size_t)]
+
+
 # name -> (restype, argtypes); every symbol include/magcore_b200.h declares
 _u8p, _f32p, _vp = C.POINTER(C.c_uint8), C.POINTER(C.c_float), C.c_void_p
 _PP = C.POINTER(McParams)
+_NV = C.POINTER(McNv12)
 SIGNATURES = {
     "mc_abi_version": (C.c_int, []),
     "mc_device_count": (C.c_int, []),
@@ -59,6 +65,9 @@ SIGNATURES = {
     "mc_pipeline_depth": (C.c_int, [_vp]),
     "mc_submit": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t]),
     "mc_collect": (C.c_int, [_vp, C.POINTER(C.c_int)]),
+    "mc_process_nv12_device": (C.c_int, [_vp, _NV, C.c_int, C.c_int, _PP, _NV, C.POINTER(C.c_int)]),
+    "mc_process_clip_nv12_device": (C.c_int, [_vp, _NV, C.c_int, C.c_int, C.c_int, _PP, _NV, _u8p]),
+    "mc_submit_nv12": (C.c_int, [_vp, _NV, C.c_int, C.c_int, _PP, _NV]),
     "mc_host_alloc": (_vp, [C.c_size_t]),
     "mc_host_free": (None, [_vp]),
     "mc_stream": (_vp, [_vp]),

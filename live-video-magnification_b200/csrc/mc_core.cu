@@ -30,6 +30,8 @@ struct Slot {  // one in-flight frame of the pinned pipeline
     size_t user_out_step = 0;
     bool direct_out = false;                     // D2H went straight into user_out (pinned)
     int w = 0, h = 0, c = 0;
+    bool nv12 = false;                           // an mc_submit_nv12 frame: the buffers hold NV12, user_nv12 is `out`
+    mc_nv12 user_nv12{};
 };
 }  // namespace
 
@@ -70,6 +72,10 @@ struct mc_handle {
     // mc_process_clip device staging: the clip's frames in and out
     uint8_t *k_in = nullptr, *k_out = nullptr;
     size_t k_in_b = 0, k_out_b = 0;
+
+    // NV12 calls: the magnifier's BGR input and output, and the produced flags of a call where only some lanes produced
+    uint8_t *n_in = nullptr, *n_out = nullptr, *n_flags = nullptr;
+    size_t n_in_b = 0, n_out_b = 0, n_flags_b = 0;
 
     // pipeline
     std::vector<Slot> slots;
@@ -206,6 +212,21 @@ bool is_pinned(const void* p) {
         return false;
     }
     return at.type == cudaMemoryTypeHost;
+}
+
+// The NV12 frame set of a pipeline slot: every lane a packed frame (luma rows, then Cb,Cr rows, pitch = width), lanes
+// back to back.
+mc_nv12 slot_nv12(uint8_t* base, int w, int hh) {
+    const size_t luma = (size_t)w * hh;
+    return mc_nv12{base, base + luma, (size_t)w, luma + luma / 2};
+}
+
+// Both planes of one lane, host to host.
+void host_copy_nv12(const mc_nv12& dst, const mc_nv12& src, int w, int hh, size_t lane) {
+    for (int r = 0; r < hh; ++r)
+        std::memcpy(dst.y + lane * dst.lane_stride + r * dst.pitch, src.y + lane * src.lane_stride + r * src.pitch, (size_t)w);
+    for (int r = 0; r < hh / 2; ++r)
+        std::memcpy(dst.uv + lane * dst.lane_stride + r * dst.pitch, src.uv + lane * src.lane_stride + r * src.pitch, (size_t)w);
 }
 
 // The body of MagnificationProcessor::process on device-resident frames.
@@ -454,6 +475,9 @@ void mc_destroy(mc_handle* h) try {
     if (h->c_tabs) cudaFree(h->c_tabs);
     if (h->k_in) cudaFree(h->k_in);
     if (h->k_out) cudaFree(h->k_out);
+    if (h->n_in) cudaFree(h->n_in);
+    if (h->n_out) cudaFree(h->n_out);
+    if (h->n_flags) cudaFree(h->n_flags);
     if (h->tables.lab_lut) cudaFree(h->tables.lab_lut);
     if (h->tables.inv_gamma) cudaFree(h->tables.inv_gamma);
     if (h->d_ops) cudaFree(h->d_ops);
@@ -555,7 +579,7 @@ mc_status mc_submit(mc_handle* h, const uint8_t* in, int width, int height, int 
     const int si = h->next_slot;
     Slot& s = h->slots[(size_t)si];
     s.w = width; s.h = height; s.c = channels; s.produced = 0;
-    s.user_out = out; s.user_out_step = out_step; s.direct_out = false;
+    s.user_out = out; s.user_out_step = out_step; s.direct_out = false; s.nv12 = false;
     if (have && out && out_step < row) { h->err = "out_step too small"; return MC_ERR_INVALID; }
     if (!have) {
         int produced = 0;
@@ -623,7 +647,11 @@ mc_status mc_collect(mc_handle* h, int* produced) try {
     CK(cudaEventSynchronize(s.ev_done));
     *produced = s.produced;
     h->lane_produced = s.lane_produced;
-    if (s.produced && !s.direct_out && s.user_out) {
+    if (s.produced && !s.direct_out && s.nv12) {
+        const mc_nv12 staged = slot_nv12(s.h_out, s.w, s.h);
+        for (int l = 0; l < h->lanes; ++l)
+            if (s.lane_produced[(size_t)l]) host_copy_nv12(s.user_nv12, staged, s.w, s.h, (size_t)l);
+    } else if (s.produced && !s.direct_out && s.user_out) {
         const size_t row = (size_t)s.w * s.c;
         for (int l = 0; l < h->lanes; ++l) {
             if (!s.lane_produced[(size_t)l]) continue;
@@ -915,3 +943,174 @@ extern "C" mc_status mc_process_clip(mc_handle* h, const uint8_t* in, int frames
     CK(cudaStreamSynchronize(h->stream));
     return MC_OK;
 } catch (...) { return on_exception(h); }
+
+// ---- NV12 frames: converted into BGR staging, magnified as BGR, converted back into the caller's planes ---------------
+namespace {
+mc_status check_nv12(mc_handle* h, const mc_nv12* in, const mc_nv12* out, int w, int hh, int vlanes, const mc_params* p) {
+    if (!p) { h->err = "params is null"; return MC_ERR_INVALID; }
+    if (w < 2 || hh < 2 || (w & 1) || (hh & 1)) { h->err = "NV12 width and height must be even and >= 2"; return MC_ERR_INVALID; }
+    for (const mc_nv12* f : {in, out}) {
+        if (!f || !f->y || !f->uv) { h->err = "NV12 plane is null"; return MC_ERR_INVALID; }
+        if (f->pitch < (size_t)w) { h->err = "NV12 pitch < width"; return MC_ERR_INVALID; }
+        if (vlanes > 1 && f->lane_stride < f->pitch * hh) { h->err = "NV12 lane_stride < pitch * height"; return MC_ERR_INVALID; }
+    }
+    return MC_OK;
+}
+
+Nv12Planes planes_of(const mc_nv12& f) { return Nv12Planes{f.y, f.uv, f.pitch, f.lane_stride}; }
+
+// Row pitch of the BGR staging: 16-byte rows keep the conversions on their 64-bit path.
+size_t bgr_step_of(int w) { return (size_t)round_up(3 * w, 16); }
+
+// `in` -> h->n_in (BGR, bgr_step_of(w)) for `vlanes` virtual lanes.  Mode None does not read its input: no launch.
+mc_status nv12_ingest(mc_handle* h, const mc_nv12& in, int w, int hh, int vlanes, const mc_params* p) {
+    const size_t bytes = bgr_step_of(w) * hh * vlanes;
+    mc_status st;
+    if ((st = grow(h, &h->n_in, &h->n_in_b, bytes)) != MC_OK) return st;
+    if ((st = grow(h, &h->n_out, &h->n_out_b, bytes)) != MC_OK) return st;
+    if (p->mode == MC_MODE_NONE) return MC_OK;
+    const bool prof = h->profile && h->prof.begin("nv12_to_bgr", 0, h->stream);
+    const cudaError_t e = launch_nv12_to_bgr(planes_of(in), w, hh, vlanes, h->n_in, bgr_step_of(w), h->stream);
+    if (prof) h->prof.end(h->stream);
+    CK(e);
+    ++h->launches;
+    return MC_OK;
+}
+
+// h->n_out -> `out` for the virtual lanes whose flag (host, vlanes bytes) is set.  When only some produced, the flags go
+// to the device on the handle's stream, as the modes upload their lane ops: no host synchronisation.
+mc_status nv12_egress(mc_handle* h, const mc_nv12& out, int w, int hh, int vlanes, const uint8_t* flags) {
+    const int n = (int)std::count_if(flags, flags + vlanes, [](uint8_t f) { return f != 0; });
+    if (n == 0) return MC_OK;
+    const uint8_t* d_flags = nullptr;
+    if (n < vlanes) {
+        mc_status st;
+        if ((st = grow(h, &h->n_flags, &h->n_flags_b, (size_t)vlanes)) != MC_OK) return st;
+        CK(cudaMemcpyAsync(h->n_flags, flags, (size_t)vlanes, cudaMemcpyHostToDevice, h->stream));
+        d_flags = h->n_flags;
+    }
+    const bool prof = h->profile && h->prof.begin("bgr_to_nv12", 0, h->stream);
+    const cudaError_t e = launch_bgr_to_nv12(h->n_out, bgr_step_of(w), w, hh, vlanes, d_flags, out.y, out.uv, out.pitch,
+                                             out.lane_stride, h->stream);
+    if (prof) h->prof.end(h->stream);
+    CK(e);
+    ++h->launches;
+    return MC_OK;
+}
+
+// Lanes [a, b) of both planes between host and device: one 2D copy for the run when both sides hold packed frames back
+// to back (the Cb,Cr rows right after the luma rows), otherwise two per lane.
+bool packed_nv12(const mc_nv12& f, int hh, size_t lanes) {
+    return f.uv == f.y + f.pitch * hh && (lanes == 1 || f.lane_stride == f.pitch * hh / 2 * 3);
+}
+mc_status copy_nv12(mc_handle* h, const mc_nv12& dst, const mc_nv12& src, int w, int hh, size_t a, size_t b, cudaMemcpyKind kind,
+                    cudaStream_t s) {
+    if (packed_nv12(dst, hh, b - a) && packed_nv12(src, hh, b - a)) {
+        CK(cudaMemcpy2DAsync(dst.y + a * dst.lane_stride, dst.pitch, src.y + a * src.lane_stride, src.pitch, (size_t)w,
+                             (b - a) * hh / 2 * 3, kind, s));
+        return MC_OK;
+    }
+    for (size_t l = a; l < b; ++l) {
+        CK(cudaMemcpy2DAsync(dst.y + l * dst.lane_stride, dst.pitch, src.y + l * src.lane_stride, src.pitch, (size_t)w, (size_t)hh, kind, s));
+        CK(cudaMemcpy2DAsync(dst.uv + l * dst.lane_stride, dst.pitch, src.uv + l * src.lane_stride, src.pitch, (size_t)w, (size_t)hh / 2,
+                             kind, s));
+    }
+    return MC_OK;
+}
+}  // namespace
+
+extern "C" mc_status mc_process_nv12_device(mc_handle* h, const mc_nv12* in, int width, int height, const mc_params* p,
+                                            const mc_nv12* out, int* produced) try {
+    if (!h || !produced) return MC_ERR_INVALID;
+    *produced = 0;
+    CK(cudaSetDevice(h->device));
+    mc_status st = check_nv12(h, in, out, width, height, h->lanes, p);
+    if (st != MC_OK) return st;
+    if ((st = nv12_ingest(h, *in, width, height, h->lanes, p)) != MC_OK) return st;
+    const size_t step = bgr_step_of(width);
+    st = process_device_impl(h, h->n_in, width, height, 3, step, p, h->n_out, step, produced, h->lane_produced.data());
+    if (st != MC_OK) return st;
+    return nv12_egress(h, *out, width, height, h->lanes, h->lane_produced.data());
+} catch (...) { return on_exception(h); }
+
+extern "C" mc_status mc_process_clip_nv12_device(mc_handle* h, const mc_nv12* in, int frames, int width, int height,
+                                                 const mc_params* p, const mc_nv12* out, uint8_t* produced) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    if (frames < 1 || (long long)frames * h->lanes > MC_MAX_LANES || !produced || !h->inflight.empty())
+        return clip_impl(h, nullptr, frames, 0, 0, 3, 0, p, nullptr, 0, produced);   // the clip's argument errors
+    const int vlanes = frames * h->lanes;
+    mc_status st = check_nv12(h, in, out, width, height, vlanes, p);
+    if (st != MC_OK) return st;
+    if ((st = nv12_ingest(h, *in, width, height, vlanes, p)) != MC_OK) return st;
+    const size_t step = bgr_step_of(width);
+    st = clip_impl(h, h->n_in, frames, width, height, 3, step, p, h->n_out, step, produced);
+    if (st != MC_OK) return st;
+    return nv12_egress(h, *out, width, height, vlanes, produced);
+} catch (...) { return on_exception(h); }
+
+// mc_submit on NV12 planes: the slot buffers hold NV12 (slot_nv12), so PCIe moves 1.5 B/px each way; the conversions run
+// on the compute stream around the magnifier, through the handle's BGR staging (stream-ordered, shared by the slots).
+extern "C" mc_status mc_submit_nv12(mc_handle* h, const mc_nv12* in, int width, int height, const mc_params* p,
+                                    const mc_nv12* out) try {
+    if (!h || !p) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    if ((int)h->inflight.size() >= h->depth) { h->err = "pipeline full: call mc_collect first"; return MC_ERR_INVALID; }
+    mc_status st = check_nv12(h, in, out, width, height, h->lanes, p);
+    if (st != MC_OK) return st;
+    const size_t lanes = (size_t)h->lanes, lane_bytes = (size_t)width * height / 2 * 3;
+    if ((st = ensure_slots(h, lane_bytes * lanes)) != MC_OK) return st;
+    const int si = h->next_slot;
+    Slot& s = h->slots[(size_t)si];
+    s.w = width; s.h = height; s.c = 3; s.produced = 0;
+    s.user_out = nullptr; s.user_out_step = 0; s.direct_out = false; s.nv12 = true; s.user_nv12 = *out;
+    const mc_nv12 d_in = slot_nv12(s.d_in, width, height), d_out = slot_nv12(s.d_out, width, height);
+    if (is_pinned(in->y) && is_pinned(in->uv)) {
+        if ((st = copy_nv12(h, d_in, *in, width, height, 0, lanes, cudaMemcpyHostToDevice, h->s_in)) != MC_OK) return st;
+    } else {
+        const mc_nv12 staged = slot_nv12(s.h_in, width, height);
+        for (size_t l = 0; l < lanes; ++l) host_copy_nv12(staged, *in, width, height, l);
+        CK(cudaMemcpyAsync(s.d_in, s.h_in, lane_bytes * lanes, cudaMemcpyHostToDevice, h->s_in));
+    }
+    CK(cudaEventRecord(s.ev_in, h->s_in));
+    CK(cudaStreamWaitEvent(h->stream, s.ev_in, 0));
+    if ((st = nv12_ingest(h, d_in, width, height, h->lanes, p)) != MC_OK) return st;
+    const size_t step = bgr_step_of(width);
+    int produced = 0;
+    st = process_device_impl(h, h->n_in, width, height, 3, step, p, h->n_out, step, &produced, s.lane_produced.data());
+    if (st != MC_OK) return st;
+    if ((st = nv12_egress(h, d_out, width, height, h->lanes, s.lane_produced.data())) != MC_OK) return st;
+    s.produced = produced;
+    CK(cudaEventRecord(s.ev_k, h->stream));
+    if (produced) {
+        CK(cudaStreamWaitEvent(h->s_out, s.ev_k, 0));
+        // only the lanes that produced are downloaded, one run of consecutive lanes at a time
+        const bool direct = is_pinned(out->y) && is_pinned(out->uv);
+        st = for_each_run(lanes, [&](size_t l) { return s.lane_produced[l] != 0; }, [&](size_t a, size_t b) -> mc_status {
+            if (direct) return copy_nv12(h, *out, d_out, width, height, a, b, cudaMemcpyDeviceToHost, h->s_out);
+            CK(cudaMemcpyAsync(s.h_out + a * lane_bytes, s.d_out + a * lane_bytes, (b - a) * lane_bytes, cudaMemcpyDeviceToHost, h->s_out));
+            return MC_OK;
+        });
+        if (st != MC_OK) return st;
+        s.direct_out = direct;
+        CK(cudaEventRecord(s.ev_done, h->s_out));
+    } else {
+        CK(cudaEventRecord(s.ev_done, h->stream));
+    }
+    h->inflight.push_back(si);
+    h->next_slot = (si + 1) % h->depth;
+    return MC_OK;
+} catch (...) { return on_exception(h); }
+
+/* test hooks, not declared in the public header: the two conversion kernels alone on device buffers (default stream,
+ * synchronised); they return the cudaError_t */
+extern "C" int mc_debug_nv12_to_bgr(const mc_nv12* in, int width, int height, int lanes, uint8_t* d_bgr, size_t bgr_step) {
+    cudaError_t e = launch_nv12_to_bgr(planes_of(*in), width, height, lanes, d_bgr, bgr_step, nullptr);
+    return (int)(e != cudaSuccess ? e : cudaStreamSynchronize(nullptr));
+}
+extern "C" int mc_debug_bgr_to_nv12(const uint8_t* d_bgr, size_t bgr_step, int width, int height, int lanes, const uint8_t* d_flags,
+                                    const mc_nv12* out) {
+    cudaError_t e = launch_bgr_to_nv12(d_bgr, bgr_step, width, height, lanes, d_flags, out->y, out->uv, out->pitch, out->lane_stride,
+                                       nullptr);
+    return (int)(e != cudaSuccess ? e : cudaStreamSynchronize(nullptr));
+}

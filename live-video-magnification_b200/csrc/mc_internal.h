@@ -152,6 +152,20 @@ cudaError_t launch_preprocess(const uint8_t* src_roi, size_t step, int cn, int s
                               const AreaTap* xtab, const int* xofs, const AreaTap* ytab, const int* yofs, uint8_t* dst,
                               uint8_t* gray, cudaStream_t s);
 
+// NV12 hand-off (mc_preprocess.cu).  An NV12 frame set: `lanes` frames, lane k's luma plane at y + k * lane_stride (h rows of
+// w bytes) and its interleaved Cb,Cr plane at uv + k * lane_stride (h / 2 rows); both planes `pitch` bytes per row.
+// BGR frames are packed u8 BGR, lane k at bgr + k * bgr_step * h.  w and h are even.
+struct Nv12Planes {
+    const uint8_t* y = nullptr;
+    const uint8_t* uv = nullptr;
+    size_t pitch = 0, lane_stride = 0;
+};
+// cvtColor(YUV2BGR_NV12) of every lane
+cudaError_t launch_nv12_to_bgr(const Nv12Planes& in, int w, int h, int lanes, uint8_t* bgr, size_t bgr_step, cudaStream_t s);
+// cvtColor(BGR2YUV_I420) of every lane whose flag is set (flags: one byte per lane, or null for all), chroma interleaved
+cudaError_t launch_bgr_to_nv12(const uint8_t* bgr, size_t bgr_step, int w, int h, int lanes, const uint8_t* flags,
+                               uint8_t* y, uint8_t* uv, size_t pitch, size_t lane_stride, cudaStream_t s);
+
 // plane copy helpers
 cudaError_t launch_copy_planes(float* dst, const float* src, size_t n, cudaStream_t s);
 

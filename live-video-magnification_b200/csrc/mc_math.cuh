@@ -276,6 +276,27 @@ __device__ __forceinline__ void lab_to_bgr_fast(float L, float a, float b, const
 // cv::cvtColor(COLOR_BGR2GRAY) on u8 (GrayscaleProcessor.cpp:13): 15-bit fixed point, round to nearest.
 MC_HD uint8_t bgr_to_gray_u8(int b, int g, int r) { return (uint8_t)((b * 3735 + g * 19235 + r * 9798 + 16384) >> 15); }
 
+// NV12 hand-off (ITU-R BT.601, limited range): OpenCV's u8 fixed point with 20 fractional bits, restated exactly.
+MC_HD uint8_t sat_u8(int v) { return (uint8_t)(v < 0 ? 0 : (v > 255 ? 255 : v)); }
+
+// cv::cvtColor(COLOR_YUV2BGR_NV12) of one pixel: luma y, and the Cb, Cr sample u, v of its 2x2 block.
+MC_HD void nv12_to_bgr_px(int y, int u, int v, uint8_t& b, uint8_t& g, uint8_t& r) {
+    const int yy = (y > 16 ? y - 16 : 0) * 1220542 + (1 << 19);
+    u -= 128;
+    v -= 128;
+    b = sat_u8((yy + 2116026 * u) >> 20);
+    g = sat_u8((yy - 409993 * u - 852492 * v) >> 20);
+    r = sat_u8((yy + 1673527 * v) >> 20);
+}
+
+// cv::cvtColor(COLOR_BGR2YUV_I420) of one pixel: its Y, and the Cb, Cr that OpenCV stores for a 2x2 block whose
+// top-left pixel it is (the other three pixels of the block do not contribute).
+MC_HD void bgr_to_ycc_px(int b, int g, int r, uint8_t& y, uint8_t& cb, uint8_t& cr) {
+    y = sat_u8((269484 * r + 528482 * g + 102760 * b + (16 << 20) + (1 << 19)) >> 20);
+    cb = sat_u8((-155188 * r - 305135 * g + 460324 * b + (128 << 20) + (1 << 19)) >> 20);
+    cr = sat_u8((460324 * r - 385875 * g - 74448 * b + (128 << 20) + (1 << 19)) >> 20);
+}
+
 #if defined(__CUDA_ARCH__)
 #define MC_FMUL(a, b) __fmul_rn((a), (b))
 #define MC_FADD(a, b) __fadd_rn((a), (b))

@@ -279,6 +279,28 @@ class MagnificationProcessor(IProcessor):
         self._check(self._lib.mc_collect(self._h, C.byref(produced)))
         return bool(produced.value)
 
+    # -- NV12 frames (video decoder / encoder hand-off); planes are capi.McNv12 -------------------
+    def process_nv12_device(self, d_in: capi.McNv12, w: int, h: int, cfg_or_params, d_out: capi.McNv12) -> bool:
+        """mc_process_nv12_device on NV12 device planes."""
+        p = cfg_or_params if isinstance(cfg_or_params, McParams) else _to_mc(cfg_or_params)
+        produced = C.c_int(0)
+        self._check(self._lib.mc_process_nv12_device(self._h, C.byref(d_in), w, h, C.byref(p), C.byref(d_out), C.byref(produced)))
+        return bool(produced.value)
+
+    def process_clip_nv12_device(self, d_in: capi.McNv12, frames: int, w: int, h: int, cfg_or_params,
+                                 d_out: capi.McNv12) -> np.ndarray:
+        """mc_process_clip_nv12_device -> produced bool[frames, lanes]."""
+        p = cfg_or_params if isinstance(cfg_or_params, McParams) else _to_mc(cfg_or_params)
+        flags = np.zeros((int(frames), self.lanes), np.uint8)
+        self._check(self._lib.mc_process_clip_nv12_device(self._h, C.byref(d_in), int(frames), w, h, C.byref(p), C.byref(d_out),
+                                                          flags.ctypes.data_as(C.POINTER(C.c_uint8))))
+        return flags.astype(bool)
+
+    def submit_nv12(self, in_planes: capi.McNv12, w: int, h: int, cfg_or_params, out_planes: capi.McNv12):
+        """mc_submit_nv12 on NV12 host planes (pinned or pageable); collect() returns the frame."""
+        p = cfg_or_params if isinstance(cfg_or_params, McParams) else _to_mc(cfg_or_params)
+        self._check(self._lib.mc_submit_nv12(self._h, C.byref(in_planes), w, h, C.byref(p), C.byref(out_planes)))
+
     def sync(self):
         self._check(self._lib.mc_sync(self._h))
 
