@@ -257,9 +257,9 @@ void* mc_stream(mc_handle* h);
  *        that many concurrent launch chains on separate CUDA streams, forked from and joined into mc_stream(); the
  *        L1-bound ingest, issue-bound egress and HBM-bound level kernels of different groups then share the SMs
  *        instead of running back to back (same results; profile_kernels forces 1)
- *   "egress_strip" (default 20): Laplace egress runs as the shuffle strip kernel (one warp per 128-column strip,
+ *   "egress_strip" (default 16): Laplace egress runs as the shuffle strip kernel (one warp per 128-column strip,
  *        sliding windows in per-lane shared-memory rings; the value 16 / 20 / 24 picks the register cap = resident
- *        warps per SM); 0 selects the shared-memory tile kernel (bit-identical results; kept for A/B)
+ *        warps per SM, 1 means the default); 0 selects the shared-memory tile kernel (bit-identical results; kept for A/B)
  *   "ingest_warps" (default 1): warps per CTA (1, 2 or 4) of the fused BGR->Lab ingest kernel (same results; A/B)
  *   "analysis_only" (default 0): Laplace and Phase — frames after the first update the temporal state (EMA planes;
  *        Riesz pyramids, phase accumulators and Butterworth registers) but skip synthesis and egress and report

@@ -51,7 +51,7 @@ struct mc_handle {
     // options
     bool faithful0 = false, keep_float = false, profile = false, use_tma = true, prefetch_state = true, band_from_state = true, analysis_only = false;
     int ingest_warps = 1;
-    int egress_strip = 20;
+    int egress_strip = 16;
     int lane_groups = 0;
     Profiler prof;
     int depth = 3;
@@ -529,7 +529,7 @@ mc_status mc_set_option(mc_handle* h, const char* key, int value) try {
     if (!std::strcmp(key, "use_tma")) { h->use_tma = value != 0; return MC_OK; }
     if (!std::strcmp(key, "prefetch_state")) { h->prefetch_state = value != 0; return MC_OK; }
     if (!std::strcmp(key, "lane_groups")) { h->lane_groups = value < 0 ? 0 : value; return MC_OK; }
-    if (!std::strcmp(key, "egress_strip")) { h->egress_strip = value == 1 ? 20 : value; return MC_OK; }
+    if (!std::strcmp(key, "egress_strip")) { h->egress_strip = value == 1 ? 16 : value; return MC_OK; }
     if (!std::strcmp(key, "ingest_warps")) { h->ingest_warps = value; return MC_OK; }
     if (!std::strcmp(key, "band_from_state")) { h->band_from_state = value != 0; return MC_OK; }
     if (!std::strcmp(key, "analysis_only")) { h->analysis_only = value != 0; return MC_OK; }

@@ -839,6 +839,60 @@ __device__ __forceinline__ EgressIn<1> egress_load<1>(const EgressArgs& a, int l
     return r;
 }
 
+// the input sample of one pixel as float Lab, plus its motion when `motion` (u0..u2: the pyrUp tap sums, see below)
+__device__ __forceinline__ void egress_lab_in(short l, short av, short bv, bool motion, float u0, float u1, float u2,
+                                              float chroma64, float& L, float& A, float& B) {
+    L = (float)l * (100.0f / 16384.0f);
+    A = fmaf((float)av, 1.0f / 64.0f, -128.0f);
+    B = fmaf((float)bv, 1.0f / 64.0f, -128.0f);
+    if (motion) {
+        // a,b motion planes *= chromAttenuation, then output = input + motion (MagnifyCore.hpp:140-148)
+        L = __fmaf_rn(u0, kInv64, L);
+        A = __fadd_rn(A, __fmul_rn(u1, chroma64));   // the reference scales the plane, then adds
+        B = __fadd_rn(B, __fmul_rn(u2, chroma64));
+    }
+}
+
+// lab_to_bgr_fast for the two Motion egress kernels, split so that the strip kernel can take the dark end once per warp:
+// lab_lin gives the clipped linear values, gamma_fast the analytic curve, kGammaDark is where the spline takes over.
+// The products of the XYZ -> BGR matrix are pinned to one contraction (blue fuses Y, then Z, into c*X; green and red
+// fuse X, then Z, into c*Y: the form nvcc chose for the tile kernel), so that both kernels give the same bits whatever
+// the surrounding code lets the compiler fuse.
+constexpr float kGammaDark = 8.0f / 1024.0f;
+
+__device__ __forceinline__ void lab_lin(float L, float a, float b, const LabInvCoeffs& k, float& vb, float& vg, float& vr) {
+    const float y_lin = L * (1.0f / 903.3f);
+    const float fy_lin = 7.787f * y_lin + 16.0f / 116.0f;
+    const float fy_cub = (L + 16.0f) * (1.0f / 116.0f);
+    const bool lo = L <= 8.0f;
+    const float fy = lo ? fy_lin : fy_cub;
+    const float Y = lo ? y_lin : fy_cub * fy_cub * fy_cub;
+    const float fx = a * (1.0f / 500.0f) + fy;
+    const float fz = fy - b * (1.0f / 200.0f);
+    const float fth = 6.0f / 29.0f;
+    const float X = fx <= fth ? (fx - 16.0f / 116.0f) * (1.0f / 7.787f) : fx * fx * fx;
+    const float Z = fz <= fth ? (fz - 16.0f / 116.0f) * (1.0f / 7.787f) : fz * fz * fz;
+    vb = __saturatef(__fmaf_rn(k.c[2], Z, __fmaf_rn(k.c[1], Y, __fmul_rn(k.c[0], X))));
+    vg = __saturatef(__fmaf_rn(k.c[5], Z, __fmaf_rn(k.c[3], X, __fmul_rn(k.c[4], Y))));
+    vr = __saturatef(__fmaf_rn(k.c[8], Z, __fmaf_rn(k.c[6], X, __fmul_rn(k.c[7], Y))));
+}
+
+__device__ __forceinline__ float gamma_fast(float v) { return fmaf(1.055f, mc_ex2(mc_lg2(v) * (1.0f / 2.4f)), -0.055f); }
+
+__device__ __forceinline__ void lab_to_bgr_egress(float L, float a, float b, const LabInvCoeffs& k, const float4* __restrict__ gtab,
+                                                  float& ob, float& og, float& orr) {
+    float vb, vg, vr;
+    lab_lin(L, a, b, k, vb, vg, vr);
+    ob = gamma_fast(vb);
+    og = gamma_fast(vg);
+    orr = gamma_fast(vr);
+    if (fminf(vb, fminf(vg, vr)) < kGammaDark) {   // dark end: OpenCV's spline, per channel
+        if (vb < kGammaDark) ob = spline_gamma(vb, gtab);
+        if (vg < kGammaDark) og = spline_gamma(vg, gtab);
+        if (vr < kGammaDark) orr = spline_gamma(vr, gtab);
+    }
+}
+
 // `up` holds the pyrUp tap sums BEFORE their 1/64 scale: the scale is exact, so it is folded into the add (L) and
 // into the chroma factor (a, b) without changing a bit.  q / f: the row's output pointers at column gx (f may be null).
 template <int C>
@@ -851,17 +905,10 @@ __device__ __forceinline__ void egress_convert<3>(const EgressArgs& a, uint8_t* 
     const short vL[4] = {in.L.x, in.L.y, in.L.z, in.L.w}, vA[4] = {in.A.x, in.A.y, in.A.z, in.A.w}, vB[4] = {in.B.x, in.B.y, in.B.z, in.B.w};
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-        float L = (float)vL[i] * (100.0f / 16384.0f);
-        float A = fmaf((float)vA[i], 1.0f / 64.0f, -128.0f);
-        float B = fmaf((float)vB[i], 1.0f / 64.0f, -128.0f);
-        if (a.m1.a) {
-            // a,b motion planes *= chromAttenuation, then output = input + motion (MagnifyCore.hpp:140-148)
-            L = __fmaf_rn(up[0][i], kInv64, L);
-            A = __fadd_rn(A, __fmul_rn(up[1][i], chroma64));   // the reference scales the plane, then adds
-            B = __fadd_rn(B, __fmul_rn(up[2][i], chroma64));
-        }
+        float L, A, B;
+        egress_lab_in(vL[i], vA[i], vB[i], a.m1.a != nullptr, up[0][i], up[1][i], up[2][i], chroma64, L, A, B);
         float ob, og, orr;
-        lab_to_bgr_fast(L, A, B, a.coeffs, a.gtab, ob, og, orr);
+        lab_to_bgr_egress(L, A, B, a.coeffs, a.gtab, ob, og, orr);
         of[3 * i] = ob; of[3 * i + 1] = og; of[3 * i + 2] = orr;
         // lab_to_bgr clips to [0,1] before the gamma spline, so the saturating branches of
         // convertTo reduce to a min with 255 (NaN -> 0 by the conversion itself)
@@ -1038,26 +1085,13 @@ __global__ void __launch_bounds__(256) k_egress(const EgressArgs a) {
 // vertical passes are register sliding windows — three horizontally expanded level-2 rows (H2) and three horizontally
 // expanded cur_1 rows (E).  Every value is computed by the same operations in the same order as in k_egress (and as
 // cv::pyrUp: row pass first), so the two kernels agree bit for bit; pyrUp's border rule (s[-1] := s[1],
-// s[n] := s[n-1]) is applied to the shuffled / streamed neighbours.  The kernel is issue-bound (Lab2BGR), not HBM-bound.
+// s[n] := s[n-1]) is applied to the shuffled / streamed neighbours.  The kernel is issue-bound (Lab2BGR), not HBM-bound,
+// so the main loop is kept to the pixel stage: the sources are addressed by one 32-bit offset per lane and warp-uniform
+// plane strides, every lane runs the pixel stage (the halo lanes' results are not stored, so no lane waits on a branch
+// around it), the dark end of the gamma is one vote per output row, and the float tap is a template parameter.
 // ------------------------------------------------------------------------------------------------
-// input samples of one row from running pointers (strip kernel): the three Lab16 plane rows at byte/element offset `off`,
-// or four gray bytes of a row
-template <int C>
-__device__ __forceinline__ EgressIn<C> egress_rows3(const int16_t* const (&p)[C], size_t off);
-template <>
-__device__ __forceinline__ EgressIn<3> egress_rows3<3>(const int16_t* const (&p)[3], size_t off) {
-    EgressIn<3> r;
-    r.L = __ldg(reinterpret_cast<const short4*>(p[0] + off));
-    r.A = __ldg(reinterpret_cast<const short4*>(p[1] + off));
-    r.B = __ldg(reinterpret_cast<const short4*>(p[2] + off));
-    return r;
-}
-template <>
-__device__ __forceinline__ EgressIn<1> egress_rows3<1>(const int16_t* const (&)[1], size_t) { return EgressIn<1>{0}; }
-template <int C>
-__device__ __forceinline__ EgressIn<C> egress_row1(const uint8_t* row, int gx, int w0);
-template <>
-__device__ __forceinline__ EgressIn<1> egress_row1<1>(const uint8_t* row, int gx, int w0) {
+// four gray input bytes of a row (strip kernel)
+__device__ __forceinline__ EgressIn<1> egress_row1(const uint8_t* row, int gx, int w0) {
     EgressIn<1> r;
     r.g = 0;
 #pragma unroll
@@ -1065,15 +1099,93 @@ __device__ __forceinline__ EgressIn<1> egress_row1<1>(const uint8_t* row, int gx
         if (gx >= 0 && gx + i < w0) r.g |= (uint32_t)__ldg(row + gx + i) << (8 * i);
     return r;
 }
-template <>
-__device__ __forceinline__ EgressIn<3> egress_row1<3>(const uint8_t*, int, int) { return EgressIn<3>{}; }
 
 constexpr int EG_ROWS = 64;   // output rows per warp (a multiple of 4)
 
 template <int C> struct StripM1 { float2 h[C], l[C]; };   // band-1 source of one cur_1 row at the lane's two columns
 template <int C> struct StripH2 { float v[C], vb[C], vr[C], vrb[C]; };   // one level-2 row at the lane's column (+ lane 31's right neighbour); b: lo state
 
-template <int C, int MINB>
+// true on every lane when `p` is true on one (the CUDA emulation has shuffles but no vote instruction)
+__device__ __forceinline__ bool warp_any(bool p) {
+#if defined(MC_CUDA_EMU)
+    int v = p ? 1 : 0;
+    for (int m = 16; m; m >>= 1) v |= __shfl_xor_sync(0xffffffffu, v, m);
+    return v != 0;
+#else
+    return __any_sync(0xffffffffu, p);
+#endif
+}
+
+// The strip kernel's pixel stage for the 4 pixels of one output row: the expressions of egress_convert with motion,
+// the u8 samples packed into C little-endian words.  The gamma is the analytic curve everywhere; `dark` says that a
+// linear value `v` lies below kGammaDark, where strip_dark puts OpenCV's spline in its place.
+template <int C> struct StripPx { uint32_t w[C]; float v[4 * C], f[4 * C]; bool dark; };
+
+template <int C>
+__device__ __forceinline__ StripPx<C> strip_px(const EgressArgs& a, float chroma64, const EgressIn<C>& in, const float (&up)[C][4]) {
+    StripPx<C> o;
+    uint32_t b[4 * C];
+    if constexpr (C == 3) {
+        const short vL[4] = {in.L.x, in.L.y, in.L.z, in.L.w}, vA[4] = {in.A.x, in.A.y, in.A.z, in.A.w}, vB[4] = {in.B.x, in.B.y, in.B.z, in.B.w};
+        float lo = 1.0f;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            float L, A, B;
+            egress_lab_in(vL[i], vA[i], vB[i], true, up[0][i], up[1][i], up[2][i], chroma64, L, A, B);
+            lab_lin(L, A, B, a.coeffs, o.v[3 * i], o.v[3 * i + 1], o.v[3 * i + 2]);
+            lo = fminf(lo, fminf(o.v[3 * i], fminf(o.v[3 * i + 1], o.v[3 * i + 2])));
+        }
+#pragma unroll
+        for (int k = 0; k < 12; ++k) {
+            o.f[k] = gamma_fast(o.v[k]);
+            b[k] = unit01_to_u8(o.f[k]);
+        }
+        o.dark = lo < kGammaDark;
+    } else {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            o.f[i] = __fmaf_rn(up[0][i], kInv64, u8_to_unit((uint8_t)((in.g >> (8 * i)) & 0xff)));
+            b[i] = unit_to_u8(o.f[i]);
+        }
+        o.dark = false;
+    }
+#pragma unroll
+    for (int wd = 0; wd < C; ++wd) o.w[wd] = b[4 * wd] | (b[4 * wd + 1] << 8) | (b[4 * wd + 2] << 16) | (b[4 * wd + 3] << 24);
+    return o;
+}
+
+// the dark end, per sample: OpenCV's spline replaces the analytic value (the same select as in lab_to_bgr_egress)
+template <int C>
+__device__ __forceinline__ void strip_dark(const float4* __restrict__ gtab, StripPx<C>& o) {
+#pragma unroll
+    for (int k = 0; k < 4 * C; ++k)
+        if (o.v[k] < kGammaDark) {
+            o.f[k] = spline_gamma(o.v[k], gtab);
+            const int sh = 8 * (k & 3);
+            o.w[k >> 2] = (o.w[k >> 2] & ~(0xffu << sh)) | ((uint32_t)unit01_to_u8(o.f[k]) << sh);
+        }
+}
+
+// one row's samples: C word stores when the lane's 4 pixels lie inside a 4-byte aligned row (`words`, fixed per lane
+// for the whole strip), else bytes up to the row's end (`bytes`); the float tap sample by sample
+template <int C, bool FOUT>
+__device__ __forceinline__ void strip_store(const StripPx<C>& o, uint8_t* q, float* f, int gx, int w0, bool words, bool bytes) {
+    if (words) {
+#pragma unroll
+        for (int wd = 0; wd < C; ++wd) reinterpret_cast<uint32_t*>(q)[wd] = o.w[wd];
+    } else if (bytes) {
+#pragma unroll
+        for (int i = 0; i < 4 * C; ++i)
+            if (gx + i / C < w0) q[i] = (uint8_t)(o.w[i >> 2] >> (8 * (i & 3)));
+    }
+    if (FOUT && (words || bytes)) {
+#pragma unroll
+        for (int i = 0; i < 4 * C; ++i)
+            if (gx + i / C < w0) f[i] = o.f[i];
+    }
+}
+
+template <int C, int MINB, bool FOUT>
 __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
     const unsigned full = 0xffffffffu;
     const int lane_id = threadIdx.x;
@@ -1102,64 +1214,64 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
     const int x2l = x2 < 0 ? 0 : (x2 >= w2 ? w2 - 1 : x2);
     const int x2r = x2l + 1 >= w2 ? w2 - 1 : x2l + 1;                // lane 31's right neighbour column
     const int gxl = px_owner ? gx : 0;                               // input column for the (unused) loads of non-owners
-    size_t base1[C], base2[C];
-#pragma unroll
-    for (int ch = 0; ch < C; ++ch) {
-        base1[ch] = (size_t)(lane * C + ch) * a.l1.plane + x1l;
-        base2[ch] = (size_t)(lane * C + ch) * a.l2.plane;
-    }
+    // The stream's source planes (warp-uniform): channel ch lies ch plane strides after channel 0; a lane addresses its
+    // row and columns by one 32-bit offset inside a plane.
+    const size_t pl1 = a.l1.plane, pl2 = a.l2.plane, pl16 = a.plane16;
+    const float* const m1a = a.m1.a + (size_t)(lane * C) * pl1;
+    const float* const m1b = from_state ? a.m1.b + (size_t)(lane * C) * pl1 : m1a;
+    const float* const c2a = has2 ? a.c2.a + (size_t)(lane * C) * pl2 : a.m1.a;
+    const float* const c2b = st2 ? a.c2.b + (size_t)(lane * C) * pl2 : c2a;
+    const int16_t* const lab = C == 3 ? a.lab + (size_t)(lane * 3) * pl16 : nullptr;
 
     // ---- loads; the lines of the next iteration are requested into L1 while the current one is computed ----
-    auto row1 = [&](int y1) { return (size_t)(y1 < h1 ? y1 : h1 - 1) * a.l1.pitch; };   // rows past the end are border copies
-    auto ld_m1 = [&](int y1) {
+    auto row1 = [&](int y1) { return (y1 < h1 ? y1 : h1 - 1) * a.l1.pitch; };   // rows past the end are border copies
+    auto ld_m1 = [&](int o) {   // o: offset of the row at the lane's columns
         StripM1<C> m;
-        const size_t ro = row1(y1);
 #pragma unroll
         for (int ch = 0; ch < C; ++ch) {
-            m.h[ch] = __ldg(reinterpret_cast<const float2*>(a.m1.a + base1[ch] + ro));
-            m.l[ch] = from_state ? __ldg(reinterpret_cast<const float2*>(a.m1.b + base1[ch] + ro)) : make_float2(0.f, 0.f);
+            m.h[ch] = __ldg(reinterpret_cast<const float2*>(m1a + ch * pl1 + o));
+            m.l[ch] = from_state ? __ldg(reinterpret_cast<const float2*>(m1b + ch * pl1 + o)) : make_float2(0.f, 0.f);
         }
         return m;
     };
-    auto pf_m1 = [&](int y1) {
-        const size_t ro = row1(y1);
+    auto pf_m1 = [&](int o) {
 #pragma unroll
         for (int ch = 0; ch < C; ++ch) {
-            prefetch_l1(a.m1.a + base1[ch] + ro);
-            if (from_state) prefetch_l1(a.m1.b + base1[ch] + ro);
+            prefetch_l1(m1a + ch * pl1 + o);
+            if (from_state) prefetch_l1(m1b + ch * pl1 + o);
         }
     };
     auto ld_h2 = [&](int y2) {
         StripH2<C> r;
-        const size_t ro = (size_t)upsrc(y2, h2) * a.l2.pitch;
+        const int ro = upsrc(y2, h2) * a.l2.pitch;
 #pragma unroll
         for (int ch = 0; ch < C; ++ch) {
             r.v[ch] = r.vb[ch] = r.vr[ch] = r.vrb[ch] = 0.f;
             if (has2) {
-                r.v[ch] = __ldg(a.c2.a + base2[ch] + ro + x2l);
-                if (st2) r.vb[ch] = __ldg(a.c2.b + base2[ch] + ro + x2l);
+                r.v[ch] = __ldg(c2a + ch * pl2 + ro + x2l);
+                if (st2) r.vb[ch] = __ldg(c2b + ch * pl2 + ro + x2l);
                 if (lane_id == 31) {
-                    r.vr[ch] = __ldg(a.c2.a + base2[ch] + ro + x2r);
-                    if (st2) r.vrb[ch] = __ldg(a.c2.b + base2[ch] + ro + x2r);
+                    r.vr[ch] = __ldg(c2a + ch * pl2 + ro + x2r);
+                    if (st2) r.vrb[ch] = __ldg(c2b + ch * pl2 + ro + x2r);
                 }
             }
         }
         return r;
     };
     auto pf_h2 = [&](int y2) {
-        const size_t ro = (size_t)upsrc(y2, h2) * a.l2.pitch;
+        const int ro = upsrc(y2, h2) * a.l2.pitch + x2l;
         if (has2) {
 #pragma unroll
             for (int ch = 0; ch < C; ++ch) {
-                prefetch_l1(a.c2.a + base2[ch] + ro + x2l);
-                if (st2) prefetch_l1(a.c2.b + base2[ch] + ro + x2l);
+                prefetch_l1(c2a + ch * pl2 + ro);
+                if (st2) prefetch_l1(c2b + ch * pl2 + ro);
             }
         }
     };
     auto pf_in = [&](int gy) {
         if (C == 3) {
-            const int16_t* lp = a.lab + (size_t)(lane * 3) * a.plane16 + (size_t)gy * a.pitch16 + gxl;
-            prefetch_l1(lp); prefetch_l1(lp + a.plane16); prefetch_l1(lp + 2 * a.plane16);
+            const int16_t* lp = lab + gy * a.pitch16 + gxl;
+            prefetch_l1(lp); prefetch_l1(lp + pl16); prefetch_l1(lp + 2 * pl16);
         } else {
             prefetch_l1(a.in + (size_t)lane * a.in_lane_stride + (size_t)gy * a.in_step + gxl);
         }
@@ -1223,8 +1335,8 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
     {
         const int ic = j0 >> 1;
         const StripH2<C> ra = ld_h2(ic - 1), rb = ld_h2(ic), rc = ld_h2(ic + 1);
-        const StripM1<C> mp = ld_m1(j0 > 0 ? j0 - 1 : 1), m0 = ld_m1(j0);
-        pf_m1(j0 + 1);
+        const StripM1<C> mp = ld_m1(row1(j0 > 0 ? j0 - 1 : 1) + x1l), m0 = ld_m1(row1(j0) + x1l);
+        pf_m1(row1(j0 + 1) + x1l);
         pf_in(2 * j0);
         pf_in(min(2 * j0 + 1, a.h0 - 1));
         expand_h2(ra, ic - 1);
@@ -1237,58 +1349,58 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
         put_E(j0, E);
     }
     const int j_end = (f_end + 1) >> 1;
-    // Running row pointers (advanced once per iteration instead of rebuilt per access): band-1 source rows at the lane's
-    // level-1 columns, the input rows at the lane's output columns, the output row.
-    const size_t st1 = (size_t)a.l1.pitch, st16 = (size_t)a.pitch16;
-    const float* ph[C];
-    const float* pl[C];
-    const int16_t* pin[C];
-#pragma unroll
-    for (int ch = 0; ch < C; ++ch) {
-        const size_t ro = row1(j0 + 1);
-        ph[ch] = a.m1.a + base1[ch] + ro;
-        pl[ch] = from_state ? a.m1.b + base1[ch] + ro : ph[ch];
-        pin[ch] = C == 3 ? a.lab + (size_t)(lane * 3 + ch) * a.plane16 + (size_t)(2 * j0) * st16 + gxl : nullptr;
-    }
+    // Running offsets, advanced once per iteration: the band-1 source row j+1 at the lane's level-1 columns and the input
+    // rows 2j, 2j+1 at the lane's output columns; the output row 2j (and the float tap's).
+    const int st1 = a.l1.pitch, st16 = a.pitch16;
+    int o1 = row1(j0 + 1) + x1l;
+    int o16 = 2 * j0 * st16 + gxl;
     const uint8_t* pg = C == 1 ? a.in + (size_t)lane * a.in_lane_stride + (size_t)(2 * j0) * a.in_step : nullptr;   // gray input row
     uint8_t* pq = a.out + (size_t)lane * a.out_lane_stride + (size_t)(2 * j0) * a.out_step + (size_t)gx * C;
+    float* pf = FOUT ? a.fout + (((size_t)lane * a.h0 + 2 * j0) * a.w0 + gx) * C : nullptr;
+    // word stores for every row of the strip when the rows are 4-byte aligned (gx * C is a multiple of 4)
+    const bool words = px_owner && gx + 4 <= a.w0 &&
+                       ((reinterpret_cast<uintptr_t>(a.out + (size_t)lane * a.out_lane_stride) | a.out_step) & 3) == 0;
+    const bool bytes = px_owner && !words;
+    const float chroma64 = a.chroma * kInv64;
     int sm = slot(j0 - 1), s0 = slot(j0), sp = slot(j0 + 1);           // ring slots of cur_1 rows j-1, j, j+1
     for (int j = j0; j < j_end; ++j) {
         const int jn = j + 1;
         const bool two = 2 * j + 1 < f_end;                            // the chunk may end on an even row
         // what this iteration consumes (requested into L1 by the previous one) ...
-        StripM1<C> cm;
-#pragma unroll
-        for (int ch = 0; ch < C; ++ch) {
-            cm.h[ch] = __ldg(reinterpret_cast<const float2*>(ph[ch]));
-            cm.l[ch] = from_state ? __ldg(reinterpret_cast<const float2*>(pl[ch])) : make_float2(0.f, 0.f);
-        }
+        const StripM1<C> cm = ld_m1(o1);
         StripH2<C> chh;
         if (!(jn & 1) && jn < h1) chh = ld_h2((jn >> 1) + 1);
         EgressIn<C> in0, in1;
-        if (C == 3) {
-            in0 = egress_rows3<C>(pin, 0);
-            in1 = egress_rows3<C>(pin, two ? st16 : 0);
+        if constexpr (C == 3) {
+            const int16_t* p = lab + o16;
+            in0.L = __ldg(reinterpret_cast<const short4*>(p));
+            in0.A = __ldg(reinterpret_cast<const short4*>(p + pl16));
+            in0.B = __ldg(reinterpret_cast<const short4*>(p + 2 * pl16));
+            if (two) p += st16;
+            in1.L = __ldg(reinterpret_cast<const short4*>(p));
+            in1.A = __ldg(reinterpret_cast<const short4*>(p + pl16));
+            in1.B = __ldg(reinterpret_cast<const short4*>(p + 2 * pl16));
         } else {
-            in0 = egress_row1<C>(pg, gx, a.w0);
-            in1 = egress_row1<C>(two ? pg + a.in_step : pg, gx, a.w0);
+            in0 = egress_row1(pg, gx, a.w0);
+            in1 = egress_row1(two ? pg + a.in_step : pg, gx, a.w0);
         }
         // ... and the requests for the next one: cur_1 row j+2, the level-2 row that enters the window with it, the inputs
         if (jn < j_end) {
-            const bool adv1 = jn + 1 < h1;
             if (jn & 1) pf_h2(((jn + 1) >> 1) + 1);
+            if (jn + 1 < h1) o1 += st1;
+            pf_m1(o1);
+            if constexpr (C == 3) {
+                o16 += 2 * st16;
+                const bool nxt = 2 * jn + 1 < a.h0;
 #pragma unroll
-            for (int ch = 0; ch < C; ++ch) {
-                if (adv1) { ph[ch] += st1; pl[ch] += st1; }
-                prefetch_l1(ph[ch]);
-                if (from_state) prefetch_l1(pl[ch]);
-                if (C == 3) {
-                    pin[ch] += 2 * st16;
-                    prefetch_l1(pin[ch]);
-                    if (2 * jn + 1 < a.h0) prefetch_l1(pin[ch] + st16);
+                for (int ch = 0; ch < C; ++ch) {
+                    prefetch_l1(lab + ch * pl16 + o16);
+                    if (nxt) prefetch_l1(lab + ch * pl16 + o16 + st16);
                 }
+            } else {
+                pg += 2 * a.in_step;
+                prefetch_l1(pg + gxl);
             }
-            if (C == 1) { pg += 2 * a.in_step; prefetch_l1(pg + gxl); }
         }
         // row j+1 of cur_1 (or its border copy) -> Ep
         float Ep[C][4];
@@ -1308,28 +1420,32 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
 #pragma unroll
             for (int ch = 0; ch < C; ++ch) sE[sm][ch][lane_id] = make_float4(Ep[ch][0], Ep[ch][1], Ep[ch][2], Ep[ch][3]);
         }
-        if (px_owner) {
-            float up[C][4], t0[C][4];
+        // the vertical pyrUp pass for output rows 2j (up0) and 2j+1 (up1), then the pixel stage of both rows
+        float up0[C][4], up1[C][4];
 #pragma unroll
-            for (int ch = 0; ch < C; ++ch) {
-                const float4 em = sE[sm][ch][lane_id], e0 = sE[s0][ch][lane_id];
-                t0[ch][0] = e0.x; t0[ch][1] = e0.y; t0[ch][2] = e0.z; t0[ch][3] = e0.w;
-                up[ch][0] = up3(em.x, e0.x, Ep[ch][0]);
-                up[ch][1] = up3(em.y, e0.y, Ep[ch][1]);
-                up[ch][2] = up3(em.z, e0.z, Ep[ch][2]);
-                up[ch][3] = up3(em.w, e0.w, Ep[ch][3]);
-            }
-            float* f = a.fout ? a.fout + (((size_t)lane * a.h0 + 2 * j) * a.w0 + gx) * C : nullptr;
-            egress_convert<C>(a, pq, f, gx, in0, up);
-            if (two) {
-#pragma unroll
-                for (int ch = 0; ch < C; ++ch)
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) up[ch][i] = up2(t0[ch][i], Ep[ch][i]);
-                egress_convert<C>(a, pq + a.out_step, f ? f + (size_t)a.w0 * C : nullptr, gx, in1, up);
-            }
+        for (int ch = 0; ch < C; ++ch) {
+            const float4 em = sE[sm][ch][lane_id], e0 = sE[s0][ch][lane_id];
+            up0[ch][0] = up3(em.x, e0.x, Ep[ch][0]);
+            up0[ch][1] = up3(em.y, e0.y, Ep[ch][1]);
+            up0[ch][2] = up3(em.z, e0.z, Ep[ch][2]);
+            up0[ch][3] = up3(em.w, e0.w, Ep[ch][3]);
+            up1[ch][0] = up2(e0.x, Ep[ch][0]);
+            up1[ch][1] = up2(e0.y, Ep[ch][1]);
+            up1[ch][2] = up2(e0.z, Ep[ch][2]);
+            up1[ch][3] = up2(e0.w, Ep[ch][3]);
+        }
+        {
+            StripPx<C> o = strip_px<C>(a, chroma64, in0, up0);
+            if (C == 3 && warp_any(px_owner && o.dark)) strip_dark<C>(a.gtab, o);
+            strip_store<C, FOUT>(o, pq, pf, gx, a.w0, words, bytes);
+        }
+        {
+            StripPx<C> o = strip_px<C>(a, chroma64, in1, up1);
+            if (C == 3 && warp_any(px_owner && o.dark)) strip_dark<C>(a.gtab, o);
+            strip_store<C, FOUT>(o, pq + a.out_step, FOUT ? pf + (size_t)a.w0 * C : nullptr, gx, a.w0, two && words, two && bytes);
         }
         pq += 2 * a.out_step;
+        if (FOUT) pf += (size_t)(2 * a.w0) * C;
         const int t = sm; sm = s0; s0 = sp; sp = t;
     }
 }
@@ -1465,6 +1581,14 @@ cudaError_t launch_collapse(const Level& lf, const Level& lc, const BandSrc& fin
     return cudaGetLastError();
 }
 
+// the float tap (keep_float_output, a test hook) has one instance per channel count: its extra stores do not fit the
+// tighter register caps without spilling, and the cap does not change a result
+template <int C, int MINB>
+static void launch_egress_strip(const EgressArgs& a, dim3 grid, cudaStream_t s) {
+    if (a.fout) k_egress_strip<C, C == 3 ? 16 : MINB, true><<<grid, 32, 0, s>>>(a);
+    else k_egress_strip<C, MINB, false><<<grid, 32, 0, s>>>(a);
+}
+
 cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16_t* lab, int pitch16, size_t plane16,
                           const BandSrc& m1, const Level& l1, const BandSrc& c2, const Level& l2, float chroma,
                           float* fout, cudaStream_t s, int strip, bool first_only) {
@@ -1478,11 +1602,11 @@ cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16
     a.ops = io.ops; a.first_only = first_only ? 1 : 0;
     if (strip) {
         dim3 grid(cdiv(io.w, DS_COLS), cdiv(io.h, EG_ROWS), io.lanes);
-        // the register cap (resident warps per SM) is an A/B knob: 16 -> <= 128 registers, 20 -> 96, 24 -> 80
-        if (io.channels != 3) k_egress_strip<1, 24><<<grid, 32, 0, s>>>(a);
-        else if (strip == 16) k_egress_strip<3, 16><<<grid, 32, 0, s>>>(a);
-        else if (strip == 24) k_egress_strip<3, 24><<<grid, 32, 0, s>>>(a);
-        else k_egress_strip<3, 20><<<grid, 32, 0, s>>>(a);
+        // the register cap (resident warps per SM): 16 -> <= 128 registers (default, the fastest on an H100), 20 -> 96, 24 -> 80
+        if (io.channels != 3) launch_egress_strip<1, 24>(a, grid, s);
+        else if (strip == 16) launch_egress_strip<3, 16>(a, grid, s);
+        else if (strip == 24) launch_egress_strip<3, 24>(a, grid, s);
+        else launch_egress_strip<3, 20>(a, grid, s);
     } else {
         dim3 grid(cdiv(io.w, TW), cdiv(io.h, TH), io.lanes);
         if (io.channels == 3) k_egress<3><<<grid, 256, 0, s>>>(a);

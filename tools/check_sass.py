@@ -2,7 +2,7 @@
 """Static checks of the built library's SASS (cuobjdump works without a GPU) and the evidence file the docs cite:
 which kernels use the TMA path (UTMALDG + mbarrier SYNCS), that each ingest LUT gather is one 128-bit + one 64-bit load,
 that the strip egress
-prefetches into L1, and that the Phase egress clips NaN to 1.0 with an explicit select (OpenCV's max(min(v,1),0)) instead
+prefetches into L1 and has no local memory, spill or barrier (it also prints the length of its main loop), and that the Phase egress clips NaN to 1.0 with an explicit select (OpenCV's max(min(v,1),0)) instead
 of a .SAT folded into the producing FFMA (round-1 hardware failure).  Usage: python tools/check_sass.py [out.txt]"""
 import collections
 import os
@@ -43,6 +43,34 @@ def clip_spills(kernel="k_level_clip", source="mc_laplace"):
     return out
 
 
+def main_loop(lines):
+    """-> (first, last) line of a kernel's longest loop: the target of its longest backward branch and that branch
+    (cuobjdump prints one 16-byte instruction per line, from offset 0)."""
+    best = (0, -1)
+    for i, l in enumerate(lines):
+        m = re.search(r"\bBRA\b.*?0x([0-9a-f]+)", l)
+        if m and int(m.group(1), 16) // 16 < i and i - int(m.group(1), 16) // 16 > best[1] - best[0]:
+            best = (int(m.group(1), 16) // 16, i)
+    return best
+
+
+def loop_counts(lines):
+    """-> (instructions of the longest loop, those of them that a warp-vote branch skips: the strip egress's dark-end
+    spline, which runs only when a lane of the warp needs it)"""
+    s, e = main_loop(lines)
+    rare = 0
+    for i in range(s, e + 1):
+        m = re.match(r"VOTE\.ANY (P\d)", lines[i])
+        if not m:
+            continue
+        for j in range(i + 1, e + 1):
+            b = re.match(r"@!" + m.group(1) + r" BRA 0x([0-9a-f]+)", lines[j])
+            if b:
+                rare += max(0, int(b.group(1), 16) // 16 - j - 1)
+                break
+    return e - s + 1, rare
+
+
 def main():
     body = kernels()
     count = lambda k, pat: sum(1 for l in body[k] if re.search(pat, l))
@@ -80,7 +108,15 @@ def main():
     need(bool(ing) and all(count(k, r"LDG\.E\.128") >= 8 and count(k, r"LDG\.E\.128") == count(k, r"LDG\.E\.64") for k in ing),
          "k_ingest_lab: each LUT gather is one LDG.E.128 + one LDG.E.64 (the 24 used bytes of a 32-byte cell)")
     strip = [k for k in body if k.startswith("void k_egress_strip<3")]
-    need(bool(strip) and all(count(k, r"CCTL\.E\.PF1") >= 8 and count(k, r"BAR\.SYNC") == 0 for k in strip), "k_egress_strip<3>: L1 prefetches, no barrier")
+    need(bool(strip) and all(count(k, r"CCTL\.E\.PF1") >= 8 and count(k, r"BAR\.SYNC") == 0 for k in strip), "k_egress_strip<3,*>: L1 prefetches, no barrier")
+    need(bool(strip) and all(count(k, r"\b(STL|LDL)\b") == 0 for k in strip), "k_egress_strip<3,*>: no local memory (STL / LDL)")
+    espills = clip_spills("k_egress_strip")
+    need(len(espills) == len(strip) + 2 and all(s == (0, 0) for s in espills.values()),
+         f"k_egress_strip<*>: no spills (ptxas -v, {len(espills)} instances)")
+    for k in strip:
+        n, rare = loop_counts(body[k])
+        lines.append(f"     {k}: main loop {n} instructions ({n - rare} outside the warp-voted dark-end spline) "
+                     f"per 2 output rows x 4 columns per lane")
     rz = [k for k in body if k.startswith("k_riesz_egress") or "k_riesz_egress(" in k]
     # the select is either an FSEL per channel or a saturate predicated on the NaN test over a preset 1.0
     nan_sel = lambda k: count(k, "FSEL") + count(k, r"@!P\d FADD\.SAT")
