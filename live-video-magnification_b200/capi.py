@@ -62,6 +62,11 @@ SIGNATURES = {
     "mc_process_clip": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t, _u8p]),
     "mc_chain_process": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, C.c_int, _vp, C.c_size_t, _vp,
                                    C.c_size_t, C.POINTER(McChainInfo)]),
+    "mc_chain_geometry": (C.c_int, [_PP, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(McChainInfo)]),
+    "mc_chain_process_device": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, C.c_int, _vp, C.c_size_t,
+                                          _vp, C.c_size_t, _u8p, C.POINTER(McChainInfo)]),
+    "mc_chain_process_nv12_device": (C.c_int, [_vp, _NV, C.c_int, C.c_int, C.c_int, _PP, C.c_int, _vp, C.c_size_t, _vp,
+                                               C.c_size_t, _u8p, C.POINTER(McChainInfo)]),
     "mc_pipeline_depth": (C.c_int, [_vp]),
     "mc_submit": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t]),
     "mc_collect": (C.c_int, [_vp, C.POINTER(C.c_int)]),

@@ -147,10 +147,23 @@ cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16
                           const BandSrc& m1, const Level& l1, const BandSrc& c2, const Level& l2, float chroma,
                           float* float_out_or_null, cudaStream_t s, int strip = 20, bool first_only = false);
 
-// PreprocessProcessor + GrayscaleProcessor on the device (mc_preprocess.cu)
-cudaError_t launch_preprocess(const uint8_t* src_roi, size_t step, int cn, int sw, int sh, int dw, int dh, bool copy_only,
-                              const AreaTap* xtab, const int* xofs, const AreaTap* ytab, const int* yofs, uint8_t* dst,
-                              uint8_t* gray, cudaStream_t s);
+// PreprocessProcessor + GrayscaleProcessor on the device (mc_preprocess.cu): one launch over `vlanes` virtual lanes.
+enum FrontSrc { FRONT_BGR = 0, FRONT_GRAY = 1, FRONT_NV12 = 2 };
+enum FrontKind { FRONT_COPY = 0, FRONT_AREA_FAST = 1, FRONT_AREA = 2 };   // crop only / integer INTER_AREA / general INTER_AREA
+struct FrontArgs {
+    const uint8_t* src = nullptr;   // lane 0's frame (BGR / gray) or luma plane (NV12)
+    const uint8_t* uv = nullptr;    // NV12: lane 0's Cb,Cr plane
+    size_t step = 0, lane_stride = 0;   // row pitch and virtual-lane stride of the source (both NV12 planes)
+    int rx = 0, ry = 0;             // ROI origin in the source
+    int dw = 0, dh = 0;             // output size
+    int kind = FRONT_COPY, isx = 1, isy = 1;
+    const AreaTap* xtab = nullptr; const int* xofs = nullptr; const AreaTap* ytab = nullptr; const int* yofs = nullptr;
+    uint8_t* dst = nullptr;         // preprocessed frames [v][dh][dst_step] (source channels), or null
+    size_t dst_step = 0, dst_lane_stride = 0;
+    uint8_t* gray = nullptr;        // their BGR2GRAY, tight [v][dh][dw], or null (3-channel sources only)
+    const uint8_t* flags = nullptr; // per virtual lane, 0 = skip (held); null = every lane
+};
+cudaError_t launch_chain_front(const FrontArgs& a, int src, int vlanes, cudaStream_t s);
 
 // NV12 hand-off (mc_preprocess.cu).  An NV12 frame set: `lanes` frames, lane k's luma plane at y + k * lane_stride (h rows of
 // w bytes) and its interleaved Cb,Cr plane at uv + k * lane_stride (h / 2 rows); both planes `pitch` bytes per row.

@@ -355,14 +355,45 @@ class ProcessingChainB200:
     downscale and BGR2GRAY run bit-exact on the device, the magnification core runs on their result.
 
     ``run_chain_once(frame, cfg) -> (cur, original)`` returns the *same* frame object wherever the reference
-    returns the same FrameRef (identity stages / passthrough)."""
+    returns the same FrameRef (identity stages / passthrough); it needs ``lanes == 1``.  ``process_device`` and
+    ``process_nv12_device`` run the chain on device frames of every lane, for one frame or a clip."""
 
-    def __init__(self, device: int = 0):
-        self.magnifier = MagnificationProcessor(device=device, lanes=1)
+    def __init__(self, device: int = 0, lanes: int = 1):
+        self.magnifier = MagnificationProcessor(device=device, lanes=lanes)
+        self.lanes = lanes
 
     def reset(self) -> None:
         """ProcessingChain's recovery path resets every stage (ProcessingChain.cpp:50-62); only the magnifier has state."""
         self.magnifier.reset()
+
+    @staticmethod
+    def geometry(cfg: ProcessorConfig, w: int, h: int, c: int) -> "capi.McChainInfo":
+        """mc_chain_geometry: what the chain gives a w x h x c frame under cfg, when the magnifier does not produce."""
+        p, info = _to_mc(cfg), capi.McChainInfo()
+        st = capi.lib().mc_chain_geometry(C.byref(p), int(w), int(h), int(c), int(cfg.grayscale), C.byref(info))
+        if st != capi.MC_OK:
+            raise MagcoreError(st, "mc_chain_geometry")
+        return info
+
+    def process_device(self, d_in: int, frames: int, w: int, h: int, c: int, in_step: int, cfg: ProcessorConfig, d_out: int,
+                       out_step: int, d_original: int = 0, original_step: int = 0):
+        """mc_chain_process_device on raw device pointers -> (produced bool[frames, lanes], McChainInfo)."""
+        m, p, info = self.magnifier, _to_mc(cfg), capi.McChainInfo()
+        flags = np.zeros((int(frames), self.lanes), np.uint8)
+        m._check(m._lib.mc_chain_process_device(m._h, d_in, int(frames), w, h, c, in_step, C.byref(p), int(cfg.grayscale), d_out,
+                                                out_step, d_original or None, original_step,
+                                                flags.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(info)))
+        return flags.astype(bool), info
+
+    def process_nv12_device(self, d_in: capi.McNv12, frames: int, w: int, h: int, cfg: ProcessorConfig, d_out: int,
+                            out_step: int, d_original: int = 0, original_step: int = 0):
+        """mc_chain_process_nv12_device on NV12 device planes -> (produced bool[frames, lanes], McChainInfo)."""
+        m, p, info = self.magnifier, _to_mc(cfg), capi.McChainInfo()
+        flags = np.zeros((int(frames), self.lanes), np.uint8)
+        m._check(m._lib.mc_chain_process_nv12_device(m._h, C.byref(d_in), int(frames), w, h, C.byref(p), int(cfg.grayscale),
+                                                     d_out, out_step, d_original or None, original_step,
+                                                     flags.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(info)))
+        return flags.astype(bool), info
 
     def run_chain_once(self, frame: Frame, cfg: ProcessorConfig):
         m = self.magnifier
