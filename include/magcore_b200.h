@@ -312,7 +312,10 @@ mc_status mc_set_option(mc_handle* h, const char* key, int value);
 
 /* Test-only access to temporal state planes as dense f32 [lanes][channels][rows][cols].
  * Names: Laplace "lowpassHi" / "lowpassLo" (MotionState, MagnifyCore.hpp:24-29), level 0..levels (levels 0 and
- *   `levels` exist only with option faithful_level0);
+ *   `levels` exist only with option faithful_level0); Laplace "band", the frame path's band planes of a level: the
+ *   amplified band gain * (hi - lo) the level kernel stores (levels 1..levels-1 with band_from_state 0), overwritten by
+ *   the collapse sum cur_l at levels 2..levels-2.  When a frame synthesises L only (zero chroma, see DESIGN.md
+ *   §4) their a / b planes are left as they are;
  * Phase, per band level 0..levels-2, one channel: "old.lowpass", "old.rx", "old.ry" (RieszState::old),
  *   "phase.c", "phase.s" (itsPhase — the two filters' copies are identical), "lo.r0.c", "lo.r0.s", "lo.r1.c",
  *   "lo.r1.s", "hi.r0.c", "hi.r0.s", "hi.r1.c", "hi.r1.s" (itsRegister0/1 of the low / high cutoff filters,

@@ -703,6 +703,9 @@ static mc_status state_xfer(mc_handle* h, const char* name, int level, float* ho
     const size_t planes = (size_t)h->lanes * r.channels;
     if (n < planes * r.rows * r.cols) { h->err = "state buffer too small"; return MC_ERR_INVALID; }
     CK(cudaStreamSynchronize(h->stream));
+    // Laplace EMA state written from outside is not known to be bounded: L-only synthesis stays off until every lane's state is
+    // dropped (DESIGN §4)
+    if (!get && h->t_mode == MC_MODE_LAPLACE && std::strncmp(name, "lowpass", 7) == 0) h->motion.ab_bounded = false;
     if (r.ptr16) {   // int16 planes: download, then widen (exact)
         std::vector<int16_t> tmp((size_t)r.rows * r.cols);
         for (size_t pl = 0; pl < planes; ++pl) {

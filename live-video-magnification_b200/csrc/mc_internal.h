@@ -101,6 +101,7 @@ struct LevelArgs {
     float* g_next = nullptr;   // G_{l+1} planes (written)
     float* hi = nullptr; float* lo = nullptr;     // state planes of this level
     float* m = nullptr;        // gain * (hi - lo), may be null
+    int m_luma = 0;            // 1: m is stored for the L planes (channel 0) only: L-only synthesis reads no other
     int planes = 0;
     int first = 0;             // 1: hi = lo = band (MagnifyCore.hpp:98-103)
     int band = 1;              // 0: only pyrDown (the level-0 band never reaches the output)
@@ -136,16 +137,20 @@ struct BandSrc {
 };
 
 // out_l = pyrUp(coarse) + fine (SpatialFilter.cpp:52-61); `out` may be the stored fine plane itself (in place)
+// over `planes` planes, the k-th being plane k * plane_stride of every source and of `out`
 // (ops: device LaneOp per lane of `channels` planes, or null; HOLD lanes are skipped)
 cudaError_t launch_collapse(const Level& lf, const Level& lc, const BandSrc& fine, const BandSrc& coarse, float* out, int planes,
-                            cudaStream_t s, const uint8_t* ops = nullptr, int channels = 1);
+                            cudaStream_t s, const uint8_t* ops = nullptr, int channels = 1, int plane_stride = 1);
 
 // out = convert(input + chroma * pyrUp(pyrUp(c2) + m1)) (MagnifyCore.hpp:136-158).
 // m1.a == nullptr: no motion; c2.a == nullptr: cur_1 = m1.  C == 3 reads `lab`, C == 1 reads io.in.
 // io.ops: HOLD lanes are skipped, and with first_only also RUN lanes (analysis_only: only FIRST lanes are converted).
+// luma_only (strip kernel, C == 3): only the L planes of m1 and c2 are read, a and b are the input's (a zero chroma
+// factor; the caller guarantees that the a / b motion it skips is finite).
 cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16_t* lab, int pitch16, size_t plane16,
                           const BandSrc& m1, const Level& l1, const BandSrc& c2, const Level& l2, float chroma,
-                          float* float_out_or_null, cudaStream_t s, int strip = 20, bool first_only = false);
+                          float* float_out_or_null, cudaStream_t s, int strip = 20, bool first_only = false,
+                          bool luma_only = false);
 
 // PreprocessProcessor + GrayscaleProcessor on the device (mc_preprocess.cu): one launch over `vlanes` virtual lanes.
 enum FrontSrc { FRONT_BGR = 0, FRONT_GRAY = 1, FRONT_NV12 = 2 };

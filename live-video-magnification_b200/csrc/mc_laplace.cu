@@ -149,6 +149,7 @@ struct LevelKArgs {
     int first, band;
     double c_hi, omc_hi, c_lo, omc_lo;
     float gain;
+    int m_luma;               // store m for channel 0 only
     int in_vec_ok;            // u8 rows are 4-byte aligned
     const uint8_t* ops;       // LaneOp per lane or null
 };
@@ -337,7 +338,7 @@ __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_
     level_up(sD, tx, ty, up);
     float* __restrict__ hi = a.hi + (size_t)plane * a.lf.plane;
     float* __restrict__ lo = a.lo + (size_t)plane * a.lf.plane;
-    float* __restrict__ m = a.m ? a.m + (size_t)plane * a.lf.plane : nullptr;
+    float* __restrict__ m = a.m && (!a.m_luma || ch == 0) ? a.m + (size_t)plane * a.lf.plane : nullptr;
     const int gx = x0 + 4 * tx;
     if (prefetch) mbar_wait(&st_bar, 0);   // every thread observes the copy's completion itself before reading sS
 #pragma unroll
@@ -443,7 +444,7 @@ __global__ void __launch_bounds__(256) k_level_clip(const LevelKArgs a, const in
         __syncthreads();
         float up[2][4];
         level_up(sD, tx, ty, up);
-        float* __restrict__ m = a.m ? a.m + vplane * a.lf.plane : nullptr;
+        float* __restrict__ m = a.m && (!a.m_luma || ch == 0) ? a.m + vplane * a.lf.plane : nullptr;
 #pragma unroll
         for (int ry = 0; ry < 2; ++ry) {
             const int gy = y0 + 2 * ty + ry;
@@ -724,7 +725,8 @@ __global__ void __launch_bounds__(32 * WARPS) k_ingest_lab(const IngestArgs a) {
 // (TemporalFilter.cpp:21, MagnifyCore.hpp:127-134) is either the plane the level kernel stored (then `out` may be
 // that same plane: every thread reads its pixels before it writes them) or, with option band_from_state, rebuilt
 // from the two state planes the level kernel has just written (same f32 subtract and multiply).  Tile 64 x 32,
-// thread block 4 x 2 (same register pyrUp as the level kernel), 128-bit accesses.
+// thread block 4 x 2 (same register pyrUp as the level kernel), 128-bit accesses.  Grid z runs over every
+// plane_stride-th plane: 1 for every plane, `channels` for the L planes only (L-only synthesis).
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float band_at(const BandSrc& b, size_t off) {
     const float v = __ldg(b.a + off);
@@ -732,9 +734,9 @@ __device__ __forceinline__ float band_at(const BandSrc& b, size_t off) {
 }
 
 __global__ void __launch_bounds__(256) k_collapse(Level lf, Level lc, BandSrc fine, BandSrc coarse, float* out,
-                                                  const uint8_t* __restrict__ ops, int channels) {
+                                                  const uint8_t* __restrict__ ops, int channels, int plane_stride) {
     __shared__ __align__(16) float sD[DH][DP];
-    const int plane = blockIdx.z;
+    const int plane = blockIdx.z * plane_stride;
     if (lane_op(ops, plane / channels) == LANE_HOLD) return;
     const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH;
     const size_t cbase = (size_t)plane * lc.plane;
@@ -1121,8 +1123,9 @@ __device__ __forceinline__ bool warp_any(bool p) {
 // linear value `v` lies below kGammaDark, where strip_dark puts OpenCV's spline in its place.
 template <int C> struct StripPx { uint32_t w[C]; float v[4 * C], f[4 * C]; bool dark; };
 
-template <int C>
-__device__ __forceinline__ StripPx<C> strip_px(const EgressArgs& a, float chroma64, const EgressIn<C>& in, const float (&up)[C][4]) {
+// NS: the channels whose motion `up` holds (C, or 1 = L only: a and b are the input's, see k_egress_strip).
+template <int C, int NS>
+__device__ __forceinline__ StripPx<C> strip_px(const EgressArgs& a, float chroma64, const EgressIn<C>& in, const float (&up)[NS][4]) {
     StripPx<C> o;
     uint32_t b[4 * C];
     if constexpr (C == 3) {
@@ -1131,7 +1134,12 @@ __device__ __forceinline__ StripPx<C> strip_px(const EgressArgs& a, float chroma
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             float L, A, B;
-            egress_lab_in(vL[i], vA[i], vB[i], true, up[0][i], up[1][i], up[2][i], chroma64, L, A, B);
+            if constexpr (NS == 3) {
+                egress_lab_in(vL[i], vA[i], vB[i], true, up[0][i], up[1][i], up[2][i], chroma64, L, A, B);
+            } else {
+                egress_lab_in(vL[i], vA[i], vB[i], false, 0.0f, 0.0f, 0.0f, 0.0f, L, A, B);
+                L = __fmaf_rn(up[0][i], kInv64, L);   // egress_lab_in's L motion
+            }
             lab_lin(L, A, B, a.coeffs, o.v[3 * i], o.v[3 * i + 1], o.v[3 * i + 2]);
             lo = fminf(lo, fminf(o.v[3 * i], fminf(o.v[3 * i + 1], o.v[3 * i + 2])));
         }
@@ -1185,8 +1193,13 @@ __device__ __forceinline__ void strip_store(const StripPx<C>& o, uint8_t* q, flo
     }
 }
 
-template <int C, int MINB, bool FOUT>
+// NS: the channels synthesised, C or (C == 3) 1.  With NS == 1 only the L planes of the band-1 source, of cur_2 and of
+// the rings are touched, and a, b go from Lab16 to the pixel stage unchanged.  This is the full synthesis bit for bit
+// when the a / b motion is finite and the chroma factor is zero: u * 0 = +-0, and a + (+-0) = a for a = v/64 - 128, which
+// is never -0 (the driver's condition, DESIGN §4).
+template <int C, int NS, int MINB, bool FOUT>
 __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
+    static_assert(NS == C || NS == 1, "L-only or full synthesis");
     const unsigned full = 0xffffffffu;
     const int lane_id = threadIdx.x;
     const int lane = blockIdx.z;
@@ -1226,9 +1239,9 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
     // ---- loads; the lines of the next iteration are requested into L1 while the current one is computed ----
     auto row1 = [&](int y1) { return (y1 < h1 ? y1 : h1 - 1) * a.l1.pitch; };   // rows past the end are border copies
     auto ld_m1 = [&](int o) {   // o: offset of the row at the lane's columns
-        StripM1<C> m;
+        StripM1<NS> m;
 #pragma unroll
-        for (int ch = 0; ch < C; ++ch) {
+        for (int ch = 0; ch < NS; ++ch) {
             m.h[ch] = __ldg(reinterpret_cast<const float2*>(m1a + ch * pl1 + o));
             m.l[ch] = from_state ? __ldg(reinterpret_cast<const float2*>(m1b + ch * pl1 + o)) : make_float2(0.f, 0.f);
         }
@@ -1236,16 +1249,16 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
     };
     auto pf_m1 = [&](int o) {
 #pragma unroll
-        for (int ch = 0; ch < C; ++ch) {
+        for (int ch = 0; ch < NS; ++ch) {
             prefetch_l1(m1a + ch * pl1 + o);
             if (from_state) prefetch_l1(m1b + ch * pl1 + o);
         }
     };
     auto ld_h2 = [&](int y2) {
-        StripH2<C> r;
+        StripH2<NS> r;
         const int ro = upsrc(y2, h2) * a.l2.pitch;
 #pragma unroll
-        for (int ch = 0; ch < C; ++ch) {
+        for (int ch = 0; ch < NS; ++ch) {
             r.v[ch] = r.vb[ch] = r.vr[ch] = r.vrb[ch] = 0.f;
             if (has2) {
                 r.v[ch] = __ldg(c2a + ch * pl2 + ro + x2l);
@@ -1262,7 +1275,7 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
         const int ro = upsrc(y2, h2) * a.l2.pitch + x2l;
         if (has2) {
 #pragma unroll
-            for (int ch = 0; ch < C; ++ch) {
+            for (int ch = 0; ch < NS; ++ch) {
                 prefetch_l1(c2a + ch * pl2 + ro);
                 if (st2) prefetch_l1(c2b + ch * pl2 + ro);
             }
@@ -1282,13 +1295,13 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
     // pixel stage and halve the number of resident warps of an issue-bound kernel.
     //   sH[i % 3]: horizontally expanded level-2 row i at the lane's two level-1 columns (even, odd)
     //   sE[j % 3]: horizontally expanded cur_1 row j at the lane's four output columns
-    __shared__ float2 sH[3][C][32];
-    __shared__ float4 sE[3][C][32];
+    __shared__ float2 sH[3][NS][32];
+    __shared__ float4 sE[3][NS][32];
     auto slot = [](int r) { return (r + 3) % 3; };      // rows >= -1
-    auto expand_h2 = [&](const StripH2<C>& in, int i) {
+    auto expand_h2 = [&](const StripH2<NS>& in, int i) {
         const int sl = slot(i);
 #pragma unroll
-        for (int ch = 0; ch < C; ++ch) {
+        for (int ch = 0; ch < NS; ++ch) {
             const float v = st2 ? band_of(in.v[ch], in.vb[ch], g2) : in.v[ch];
             float l = __shfl_up_sync(full, v, 1), r = __shfl_down_sync(full, v, 1);
             if (lane_id == 31) r = st2 ? band_of(in.vr[ch], in.vrb[ch], g2) : in.vr[ch];
@@ -1299,12 +1312,12 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
     };
     // cur_1 row y1 at the lane's two columns = pyrUp(cur_2) + m_1, then its horizontal expansion at the lane's four
     // output columns.  An even row 2i takes level-2 rows (i-1, i, i+1), an odd row 2i+1 rows (i, i+1).
-    auto cur1_row = [&](const StripM1<C>& m, int y1, float (&E)[C][4]) {
+    auto cur1_row = [&](const StripM1<NS>& m, int y1, float (&E)[NS][4]) {
         const bool odd = y1 & 1;
         const int i = y1 >> 1;
         const int sp = slot(odd ? i : i - 1), sq = slot(odd ? i + 1 : i), sr = slot(i + 1);
 #pragma unroll
-        for (int ch = 0; ch < C; ++ch) {
+        for (int ch = 0; ch < NS; ++ch) {
             float ca = m.h[ch].x, cb = m.h[ch].y;
             if (from_state) {
                 ca = band_of(ca, m.l[ch].x, g1);
@@ -1325,24 +1338,24 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
             E[ch][3] = up2(cb, right);
         }
     };
-    auto put_E = [&](int j, const float (&E)[C][4]) {
+    auto put_E = [&](int j, const float (&E)[NS][4]) {
         const int sl = slot(j);
 #pragma unroll
-        for (int ch = 0; ch < C; ++ch) sE[sl][ch][lane_id] = make_float4(E[ch][0], E[ch][1], E[ch][2], E[ch][3]);
+        for (int ch = 0; ch < NS; ++ch) sE[sl][ch][lane_id] = make_float4(E[ch][0], E[ch][1], E[ch][2], E[ch][3]);
     };
 
     const int j0 = f0 >> 1;                       // first level-1 row of the chunk (even)
     {
         const int ic = j0 >> 1;
-        const StripH2<C> ra = ld_h2(ic - 1), rb = ld_h2(ic), rc = ld_h2(ic + 1);
-        const StripM1<C> mp = ld_m1(row1(j0 > 0 ? j0 - 1 : 1) + x1l), m0 = ld_m1(row1(j0) + x1l);
+        const StripH2<NS> ra = ld_h2(ic - 1), rb = ld_h2(ic), rc = ld_h2(ic + 1);
+        const StripM1<NS> mp = ld_m1(row1(j0 > 0 ? j0 - 1 : 1) + x1l), m0 = ld_m1(row1(j0) + x1l);
         pf_m1(row1(j0 + 1) + x1l);
         pf_in(2 * j0);
         pf_in(min(2 * j0 + 1, a.h0 - 1));
         expand_h2(ra, ic - 1);
         expand_h2(rb, ic);
         expand_h2(rc, ic + 1);
-        float E[C][4];
+        float E[NS][4];
         // row j0-1 (odd, level-2 rows ic-1, ic); at the top of the image the slot of row -1 is filled with row 1 below
         if (j0 > 0) { cur1_row(mp, j0 - 1, E); put_E(j0 - 1, E); }
         cur1_row(m0, j0, E);
@@ -1367,8 +1380,8 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
         const int jn = j + 1;
         const bool two = 2 * j + 1 < f_end;                            // the chunk may end on an even row
         // what this iteration consumes (requested into L1 by the previous one) ...
-        const StripM1<C> cm = ld_m1(o1);
-        StripH2<C> chh;
+        const StripM1<NS> cm = ld_m1(o1);
+        StripH2<NS> chh;
         if (!(jn & 1) && jn < h1) chh = ld_h2((jn >> 1) + 1);
         EgressIn<C> in0, in1;
         if constexpr (C == 3) {
@@ -1403,10 +1416,10 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
             }
         }
         // row j+1 of cur_1 (or its border copy) -> Ep
-        float Ep[C][4];
+        float Ep[NS][4];
         if (jn >= h1) {
 #pragma unroll
-            for (int ch = 0; ch < C; ++ch) {
+            for (int ch = 0; ch < NS; ++ch) {
                 const float4 e = sE[s0][ch][lane_id];
                 Ep[ch][0] = e.x; Ep[ch][1] = e.y; Ep[ch][2] = e.z; Ep[ch][3] = e.w;
             }
@@ -1415,15 +1428,15 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
             cur1_row(cm, jn, Ep);
         }
 #pragma unroll
-        for (int ch = 0; ch < C; ++ch) sE[sp][ch][lane_id] = make_float4(Ep[ch][0], Ep[ch][1], Ep[ch][2], Ep[ch][3]);
+        for (int ch = 0; ch < NS; ++ch) sE[sp][ch][lane_id] = make_float4(Ep[ch][0], Ep[ch][1], Ep[ch][2], Ep[ch][3]);
         if (j == 0) {                                         // cur_1[-1] := cur_1[1]
 #pragma unroll
-            for (int ch = 0; ch < C; ++ch) sE[sm][ch][lane_id] = make_float4(Ep[ch][0], Ep[ch][1], Ep[ch][2], Ep[ch][3]);
+            for (int ch = 0; ch < NS; ++ch) sE[sm][ch][lane_id] = make_float4(Ep[ch][0], Ep[ch][1], Ep[ch][2], Ep[ch][3]);
         }
         // the vertical pyrUp pass for output rows 2j (up0) and 2j+1 (up1), then the pixel stage of both rows
-        float up0[C][4], up1[C][4];
+        float up0[NS][4], up1[NS][4];
 #pragma unroll
-        for (int ch = 0; ch < C; ++ch) {
+        for (int ch = 0; ch < NS; ++ch) {
             const float4 em = sE[sm][ch][lane_id], e0 = sE[s0][ch][lane_id];
             up0[ch][0] = up3(em.x, e0.x, Ep[ch][0]);
             up0[ch][1] = up3(em.y, e0.y, Ep[ch][1]);
@@ -1435,12 +1448,12 @@ __global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
             up1[ch][3] = up2(e0.w, Ep[ch][3]);
         }
         {
-            StripPx<C> o = strip_px<C>(a, chroma64, in0, up0);
+            StripPx<C> o = strip_px<C, NS>(a, chroma64, in0, up0);
             if (C == 3 && warp_any(px_owner && o.dark)) strip_dark<C>(a.gtab, o);
             strip_store<C, FOUT>(o, pq, pf, gx, a.w0, words, bytes);
         }
         {
-            StripPx<C> o = strip_px<C>(a, chroma64, in1, up1);
+            StripPx<C> o = strip_px<C, NS>(a, chroma64, in1, up1);
             if (C == 3 && warp_any(px_owner && o.dark)) strip_dark<C>(a.gtab, o);
             strip_store<C, FOUT>(o, pq + a.out_step, FOUT ? pf + (size_t)a.w0 * C : nullptr, gx, a.w0, two && words, two && bytes);
         }
@@ -1528,6 +1541,7 @@ static LevelKArgs level_kargs(const LevelArgs& a) {
     k.first = a.first; k.band = a.band;
     k.c_hi = a.c_hi; k.omc_hi = a.one_minus_c_hi; k.c_lo = a.c_lo; k.omc_lo = a.one_minus_c_lo;
     k.gain = a.gain;
+    k.m_luma = a.m_luma;
     k.ops = a.ops;
     k.in_vec_ok = a.in_kind == IN_U8 ? ((reinterpret_cast<uintptr_t>(a.g) % 4 == 0) && (a.in_row % 4 == 0) && (a.in_plane % 4 == 0)) : 1;
     return k;
@@ -1575,23 +1589,31 @@ cudaError_t launch_down(const LevelArgs& a, cudaStream_t s) {
 }
 
 cudaError_t launch_collapse(const Level& lf, const Level& lc, const BandSrc& fine, const BandSrc& coarse, float* out, int planes,
-                            cudaStream_t s, const uint8_t* ops, int channels) {
+                            cudaStream_t s, const uint8_t* ops, int channels, int plane_stride) {
     dim3 grid(cdiv(lf.w, TW), cdiv(lf.h, TH), planes);
-    k_collapse<<<grid, 256, 0, s>>>(lf, lc, fine, coarse, out, ops, channels);
+    k_collapse<<<grid, 256, 0, s>>>(lf, lc, fine, coarse, out, ops, channels, plane_stride);
     return cudaGetLastError();
 }
 
-// the float tap (keep_float_output, a test hook) has one instance per channel count: its extra stores do not fit the
+// the float tap (keep_float_output, a test hook) has one instance per synthesis: its extra stores do not fit the
 // tighter register caps without spilling, and the cap does not change a result
-template <int C, int MINB>
+template <int C, int NS, int MINB>
 static void launch_egress_strip(const EgressArgs& a, dim3 grid, cudaStream_t s) {
-    if (a.fout) k_egress_strip<C, C == 3 ? 16 : MINB, true><<<grid, 32, 0, s>>>(a);
-    else k_egress_strip<C, MINB, false><<<grid, 32, 0, s>>>(a);
+    if (a.fout) k_egress_strip<C, NS, C == 3 ? 16 : MINB, true><<<grid, 32, 0, s>>>(a);
+    else k_egress_strip<C, NS, MINB, false><<<grid, 32, 0, s>>>(a);
+}
+
+// colour frames: the register cap (resident warps per SM) 16 -> <= 128 registers, 20 -> 96, 24 -> 80
+template <int NS>
+static void launch_egress_strip3(const EgressArgs& a, int cap, dim3 grid, cudaStream_t s) {
+    if (cap == 16) launch_egress_strip<3, NS, 16>(a, grid, s);
+    else if (cap == 24) launch_egress_strip<3, NS, 24>(a, grid, s);
+    else launch_egress_strip<3, NS, 20>(a, grid, s);
 }
 
 cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16_t* lab, int pitch16, size_t plane16,
                           const BandSrc& m1, const Level& l1, const BandSrc& c2, const Level& l2, float chroma,
-                          float* fout, cudaStream_t s, int strip, bool first_only) {
+                          float* fout, cudaStream_t s, int strip, bool first_only, bool luma_only) {
     EgressArgs a;
     a.in = io.in; a.in_step = io.in_step; a.in_lane_stride = io.in_lane_stride;
     a.lab = lab; a.pitch16 = pitch16; a.plane16 = plane16;
@@ -1602,11 +1624,9 @@ cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16
     a.ops = io.ops; a.first_only = first_only ? 1 : 0;
     if (strip) {
         dim3 grid(cdiv(io.w, DS_COLS), cdiv(io.h, EG_ROWS), io.lanes);
-        // the register cap (resident warps per SM): 16 -> <= 128 registers (default, the fastest on an H100), 20 -> 96, 24 -> 80
-        if (io.channels != 3) launch_egress_strip<1, 24>(a, grid, s);
-        else if (strip == 16) launch_egress_strip<3, 16>(a, grid, s);
-        else if (strip == 24) launch_egress_strip<3, 24>(a, grid, s);
-        else launch_egress_strip<3, 20>(a, grid, s);
+        if (io.channels != 3) launch_egress_strip<1, 1, 24>(a, grid, s);
+        else if (luma_only) launch_egress_strip3<1>(a, strip, grid, s);
+        else launch_egress_strip3<3>(a, strip, grid, s);
     } else {
         dim3 grid(cdiv(io.w, TW), cdiv(io.h, TH), io.lanes);
         if (io.channels == 3) k_egress<3><<<grid, 256, 0, s>>>(a);

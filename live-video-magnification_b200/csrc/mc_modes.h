@@ -196,6 +196,9 @@ struct MotionMode {
     int pitch16 = 0;
     size_t plane16 = 0;
     bool lab16_frame = false;           // lab16 holds the last frame call's Lab (clips write their own scratch)
+    // Every EMA step of the state since the state of all lanes was last dropped used cutoffs in [0, 1], so the a / b
+    // state is bounded by the bands (a condition of L-only synthesis, DESIGN §4)
+    bool ab_bounded = true;
     DeviceArena arena;
 
     // Lane groups (option "lane_groups"): the streams of a handle are independent, so their launch sets are issued as
@@ -233,8 +236,11 @@ private:
     mc_status allocate(const ModeCtx& ctx, const FrameIO& io, int levels);
     mc_status make_groups(const ModeCtx& ctx);
     void drop_groups();
-    mc_status run_group(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, Group& g, bool first, double c_lo, double c_hi);
-    mc_status run_clip(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int frames, bool first, double c_lo, double c_hi);
+    bool luma_only(const ModeCtx& ctx, const mc_params& p) const;
+    mc_status run_group(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, Group& g, bool first, double c_lo, double c_hi,
+                        bool luma);
+    mc_status run_clip(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int frames, bool first, double c_lo, double c_hi,
+                       bool luma);
     // the launch set around the level kernels, shared by run_group and run_clip
     bool fused_ingest() const;
     int first_level() const;
@@ -245,7 +251,7 @@ private:
     mc_status egress_first_frames(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, const int16_t* lab, float* fout, bool first);
     template <class Band, class Out>
     mc_status synthesize(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, const int16_t* lab, float* fout, bool motion,
-                         Band band, Out out);
+                         bool luma, Band band, Out out);
 };
 
 struct ColorMode {

@@ -75,6 +75,7 @@ void MotionMode::reset() {
     lab16_frame = false;
     allocated = false;
     empty = true;
+    ab_bounded = true;
 }
 
 // (Re)builds the lane groups — their streams, events and TMA descriptors — over the existing buffers; the temporal state
@@ -178,12 +179,15 @@ mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc
     motion_gains(p.amplification, p.coWavelength, levels, w, h, gains);
     double c_lo = p.coLow, c_hi = p.coHigh;
     if (c_lo == 0) c_lo = 0.01;  // TemporalFilter.cpp:11-12
+    // a frame of a lane with state steps the EMAs (a clip's later frames always do); NaN is outside [0, 1]
+    if ((plan.n_run > 0 || frames > 1) && !(c_lo >= 0 && c_lo <= 1 && c_hi >= 0 && c_hi <= 1)) ab_bounded = false;
+    const bool luma = luma_only(ctx, p);
 
     lab16_frame = false;   // a clip converts into its own scratch; a frame call rewrites lab16 below
     if (frames > 1) {
-        MCK_ST(run_clip(ctx, io, p, frames, first, c_lo, c_hi));
+        MCK_ST(run_clip(ctx, io, p, frames, first, c_lo, c_hi, luma));
     } else if (groups.size() == 1) {
-        MCK_ST(run_group(ctx, io, p, groups[0], first, c_lo, c_hi));
+        MCK_ST(run_group(ctx, io, p, groups[0], first, c_lo, c_hi, luma));
     } else {
         // fork: every group's chain starts after whatever the caller queued on the handle's stream (the frame upload),
         // join: the handle's stream continues after all of them (the download / the caller's next use of `out`)
@@ -192,7 +196,7 @@ mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc
             MCK(cudaStreamWaitEvent(g.stream, ev_fork, 0));
             ModeCtx gctx = ctx;
             gctx.stream = g.stream;
-            const mc_status st = run_group(gctx, io, p, g, first, c_lo, c_hi);
+            const mc_status st = run_group(gctx, io, p, g, first, c_lo, c_hi, luma);
             if (st != MC_OK) return st;
             MCK(cudaEventRecord(g.done, g.stream));
             MCK(cudaStreamWaitEvent(ctx.stream, g.done, 0));
@@ -272,28 +276,44 @@ mc_status MotionMode::egress_first_frames(const ModeCtx& ctx, const FrameIO& io,
     return MC_OK;
 }
 
+// L-only synthesis (DESIGN §4).  The egress adds chroma/64 * u to a and b, u being the a / b motion; when that factor is
+// zero and u is finite the sum is a, b bit for bit, so only the L planes need to be synthesised.  u is finite when every
+// gain is finite with |g| <= 2^64 and the a / b state is bounded: EMAs with cutoffs in [0, 1] are convex combinations of
+// bands (|band| <= 256), so |m_l| <= 512 * 2^64 and the collapse sums stay far below FLT_MAX.  The strip egress alone has
+// an L-only form; the tile egress always synthesises every channel.
+bool MotionMode::luma_only(const ModeCtx& ctx, const mc_params& p) const {
+    if (channels != 3 || !ctx.egress_strip || !ab_bounded) return false;
+    if ((float)p.chromAttenuation * (1.0f / 64.0f) != 0.0f) return false;   // the egress's chroma64, as the device forms it
+    for (float g : gains)
+        if (!(std::fabs(g) <= 0x1p64f)) return false;
+    return true;
+}
+
 // Synthesis: residual and finest band are zero (MagnifyCore.hpp:130-131), so the collapse starts from band levels-1
 // (cur_{levels-1} = 0 + m_{levels-1}) and writes cur_l to out(l) down to level 2; levels 1 and 0 are folded into egress.
 // band(l) is where level l's amplified band is found.  Without motion (first frames) egress converts the input as it is.
+// luma: L-only synthesis, the collapses run over each lane's L plane only.
 template <class Band, class Out>
 mc_status MotionMode::synthesize(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, const int16_t* lab, float* fout, bool motion,
-                                 Band band, Out out) {
+                                 bool luma, Band band, Out out) {
     BandSrc m1, c2;
     if (motion && levels >= 2) {
         auto cur = [&](int l) { return l == levels - 1 ? band(l) : BandSrc{out(l), nullptr, 1.0f}; };
+        const int planes = luma ? io.lanes : io.lanes * channels, stride = luma ? channels : 1;
         for (int l = levels - 2; l >= 2; --l)
-            LAUNCH("collapse", l, launch_collapse(lv[(size_t)l], lv[(size_t)l + 1], band(l), cur(l + 1), out(l), io.lanes * channels,
-                                                  ctx.stream, io.ops, channels));
+            LAUNCH("collapse", l, launch_collapse(lv[(size_t)l], lv[(size_t)l + 1], band(l), cur(l + 1), out(l), planes,
+                                                  ctx.stream, io.ops, channels, stride));
         m1 = band(1);
         if (levels >= 3) c2 = cur(2);
     }
     LAUNCH("egress", 0, launch_egress(io, *ctx.tables, lab, pitch16, plane16, m1, lv[levels >= 1 ? 1 : 0], c2, lv[levels >= 2 ? 2 : 0],
-                                      (float)p.chromAttenuation, fout, ctx.stream, ctx.egress_strip));
+                                      (float)p.chromAttenuation, fout, ctx.stream, ctx.egress_strip, false, luma));
     return MC_OK;
 }
 
 // One group's launch set for one frame: lanes [g.lane0, g.lane0 + g.lanes) on ctx.stream.
-mc_status MotionMode::run_group(const ModeCtx& ctx, const FrameIO& io_all, const mc_params& p, Group& g, bool first, double c_lo, double c_hi) {
+mc_status MotionMode::run_group(const ModeCtx& ctx, const FrameIO& io_all, const mc_params& p, Group& g, bool first, double c_lo, double c_hi,
+                                bool luma) {
     FrameIO io = io_all;
     io.in = io_all.in + (size_t)g.lane0 * io_all.in_lane_stride;
     io.out = io_all.out + (size_t)g.lane0 * io_all.out_lane_stride;
@@ -312,6 +332,7 @@ mc_status MotionMode::run_group(const ModeCtx& ctx, const FrameIO& io_all, const
             if (ctx.prefetch_state) { a.tmap_hi = &g.tmaps_hi[(size_t)l]; a.tmap_lo = &g.tmaps_lo[(size_t)l]; }
         }
         a.m = (first || from_state) ? nullptr : off(M[(size_t)l], l);
+        a.m_luma = luma;
         a.planes = g.lanes * channels;
         a.ops = io.ops;
         if (a.band) LAUNCH("level", l, launch_level(a, ctx.stream));
@@ -322,13 +343,14 @@ mc_status MotionMode::run_group(const ModeCtx& ctx, const FrameIO& io_all, const
     auto band = [&](int l) {
         return from_state ? BandSrc{off(hi[(size_t)l], l), off(lo[(size_t)l], l), gains[(size_t)l]} : BandSrc{off(M[(size_t)l], l), nullptr, 1.0f};
     };
-    return synthesize(ctx, io, p, lab, fout, !first, band, [&](int l) { return off(M[(size_t)l], l); });
+    return synthesize(ctx, io, p, lab, fout, !first, luma, band, [&](int l) { return off(M[(size_t)l], l); });
 }
 
 // One clip: the launch set of run_group over V = frames * lanes virtual lanes, with the level kernels replaced by
 // k_level_clip (state in registers across the clip).  Synthesis reads the stored bands M_l; a lane's first frame has
 // M = +-0 there, which gives the first-frame output without a branch.  Lane groups do not apply: one chain.
-mc_status MotionMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_params& p, int frames, bool first, double c_lo, double c_hi) {
+mc_status MotionMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_params& p, int frames, bool first, double c_lo, double c_hi,
+                               bool luma) {
     const int vl = frames * lanes;
     MCK_ST(ClipScratch::grow(clip, ctx, vl, channels == 3 ? (size_t)vl * channels * plane16 * sizeof(int16_t) : 0, (size_t)w * h * channels,
                              [&]() -> mc_status {
@@ -353,6 +375,7 @@ mc_status MotionMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_
         LevelArgs a = level_args(l, clip.G, 0, clip.lab16, io, first, c_lo, c_hi);
         if (l >= 1 && clip.tmap_valid[(size_t)l] && ctx.use_tma) a.tmap = &clip.tmaps[(size_t)l];
         a.m = ctx.analysis_only ? nullptr : clip.M[(size_t)l];
+        a.m_luma = luma;
         if (a.band) {
             a.planes = lanes * channels; a.ops = io0.ops;   // state planes, per-lane ops of the clip's first frame
             LAUNCH("level_clip", l, launch_level_clip(a, frames, ctx.stream));
@@ -365,7 +388,7 @@ mc_status MotionMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_
     // state-carry pass: only the clip's first frame can produce; it is frame 0's egress of a frame call, so the float
     // tap is written in place
     if (ctx.analysis_only) return egress_first_frames(ctx, io0, p, clip.lab16, ctx.float_out, first);
-    MCK_ST(synthesize(ctx, io, p, clip.lab16, ctx.float_out ? clip.fout : nullptr, true,
+    MCK_ST(synthesize(ctx, io, p, clip.lab16, ctx.float_out ? clip.fout : nullptr, true, luma,
                       [&](int l) { return BandSrc{clip.M[(size_t)l], nullptr, 1.0f}; }, [&](int l) { return clip.M[(size_t)l]; }));
     return clip.copy_last_tap(ctx, plan, frames, (size_t)w * h * channels);
 }
@@ -380,6 +403,7 @@ void MotionMode::find_state(const char* name, int level, StateRef& out) {
     float* p = nullptr;
     if (!std::strcmp(name, "lowpassHi")) p = hi[(size_t)level];
     else if (!std::strcmp(name, "lowpassLo")) p = lo[(size_t)level];
+    else if (!std::strcmp(name, "band")) p = M[(size_t)level];
     if (!p) return;
     const Level& l = lv[(size_t)level];
     out.ptr = p; out.rows = l.h; out.cols = l.w; out.channels = channels; out.pitch = l.pitch; out.plane_stride = l.plane;

@@ -113,6 +113,8 @@ def main():
     espills = clip_spills("k_egress_strip")
     need(len(espills) == len(strip) + 2 and all(s == (0, 0) for s in espills.values()),
          f"k_egress_strip<*>: no spills (ptxas -v, {len(espills)} instances)")
+    luma = [k for k in strip if k.startswith("void k_egress_strip<3, 1,")]
+    need(len(luma) == 4, f"k_egress_strip<3, 1, *>: L-only synthesis at every register cap and with the float tap ({len(luma)} instances)")
     for k in strip:
         n, rare = loop_counts(body[k])
         lines.append(f"     {k}: main loop {n} instructions ({n - rare} outside the warp-voted dark-end spline) "
