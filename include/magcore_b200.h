@@ -107,9 +107,13 @@ mc_status mc_reset(mc_handle* h);
  *   Phase:   FIRST passes the lane through (not produced) and makes this frame its `old` pyramid with a zero Riesz pair and
  *            zeroed phases / filter registers (MagnifyCore.hpp:226-240).  A cutoff change while a lane is held drops that
  *            lane's state: its first frame after release is FIRST.
- *   Color:   the window is shared by the lanes.  With lanes > 1 a frame call while a lane is held, or while some lanes
- *            are restarted and others run, returns MC_ERR_UNSUPPORTED and changes nothing.  With lanes == 1 a held
- *            handle skips frame calls entirely (the window is unchanged). */
+ *   Color:   each lane has its own rolling window.  FIRST restarts it empty and appends the frame: one column, not
+ *            produced (MagnifyCore.hpp:180).  RUN appends; the lane produces from two columns on.  HOLD leaves the
+ *            window as it is.  A frame-rate change applies to each lane's own window when the lane next runs.  With
+ *            option "color_lane_lifecycle" = 1 every lane then equals, bit for bit, its own 1-lane handle fed its
+ *            frames.  Without it (the default) a frame call on a handle with lanes > 1 while a lane is held, or while
+ *            some lanes are restarted and others run, returns MC_ERR_UNSUPPORTED and changes nothing.  With lanes == 1
+ *            a held handle skips frame calls entirely (the window is unchanged). */
 
 /* The lane's next frame is its first frame: the lane's temporal state is dropped, the other lanes are untouched.
  * On a 1-lane handle this is mc_reset().  MC_ERR_INVALID if lane is out of range. */
@@ -203,7 +207,7 @@ mc_status mc_chain_geometry(const mc_params* p, int width, int height, int chann
  *     Phase batched, Color a loop of frame calls).
  *   Equivalence: every virtual lane gets, bit for bit, what mc_chain_process on a 1-lane handle gives when fed that
  *     lane's frames in order: the processed frame, the original tap, the info and the temporal state afterwards (held
- *     lanes and Color's shared window as in the lane lifecycle above).
+ *     lanes and Color's lanes as in the lane lifecycle above).
  *   What is written: `info` is mc_chain_geometry's, except that `magnified` is "at least one frame produced".  Virtual
  *     lane v's processed frame is written to d_out when produced[v] is set or when info.cur_is_input == 0 (a front
  *     stage ran); otherwise the input is the result, as the reference returns the same FrameRef.  d_original is written
@@ -212,8 +216,8 @@ mc_status mc_chain_geometry(const mc_params* p, int width, int height, int chann
  *   Errors, returned before any kernel runs and with no caller buffer or state changed: MC_ERR_INVALID for steps smaller
  *     than a row, a NULL d_out when the call would write to it (a front stage is on or the mode is not None), frames < 1,
  *     frames * lanes > MC_MAX_LANES, NULL produced / info / params, or frames of mc_submit in flight; MC_ERR_UNSUPPORTED
- *     for Color's multi-lane refusals.  Mode None and an empty image are the identity for the magnifier: the front stages
- *     still run when they are on.
+ *     for Color's multi-lane refusals (without option "color_lane_lifecycle").  Mode None and an empty image are the
+ *     identity for the magnifier: the front stages still run when they are on.
  *   Device scratch: the front keeps staging for its output (the preprocessed frames when d_original is NULL, the gray
  *   frames) and the INTER_AREA tap tables, which are uploaded on mc_stream() only when the crop or output size changes. */
 mc_status mc_chain_process_device(mc_handle* h, const uint8_t* d_in, int frames, int width, int height, int channels,
@@ -307,7 +311,10 @@ void* mc_stream(mc_handle* h);
  *        *produced = 0; the cheap first pass of temporal sharding (SURVEY 8f-3)
  *   "band_from_state" (default 1): Laplace synthesis rebuilds each amplified band gain*(hi-lo) from the two
  *        state planes instead of reading a band plane stored by the level kernel (same results; takes 4 B/px off
- *        the level kernel's interface and adds them to the collapse / egress kernels; 0 kept for A/B measurements) */
+ *        the level kernel's interface and adds them to the collapse / egress kernels; 0 kept for A/B measurements)
+ *   "color_lane_lifecycle" (default 0): Color on a handle with lanes > 1 accepts mc_hold_lane and single-lane
+ *        mc_restart_lane (see the lane lifecycle above) instead of refusing them with MC_ERR_UNSUPPORTED; lanes that
+ *        run in lock-step give the same results either way */
 mc_status mc_set_option(mc_handle* h, const char* key, int value);
 
 /* Test-only access to temporal state planes as dense f32 [lanes][channels][rows][cols].

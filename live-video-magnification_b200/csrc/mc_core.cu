@@ -54,6 +54,7 @@ struct mc_handle {
     int ingest_warps = 1;
     int egress_strip = 16;
     int lane_groups = 0;
+    bool color_lane_lifecycle = false;
     Profiler prof;
     int depth = 3;
 
@@ -235,9 +236,10 @@ void host_copy_nv12(const mc_nv12& dst, const mc_nv12& src, int w, int hh, size_
         std::memcpy(dst.uv + lane * dst.lane_stride + r * dst.pitch, src.uv + lane * src.lane_stride + r * src.pitch, (size_t)w);
 }
 
-// The Color window (ring head, length and the DFT plans cached per length) is shared by all lanes, so a lane cannot be
-// held, or restarted while others run, on a multi-lane handle: MC_ERR_UNSUPPORTED, checked before any state changes.
+// Without option "color_lane_lifecycle" a multi-lane Color handle keeps its lanes in lock-step: a frame call while a lane
+// is held, or restarted while others run, is MC_ERR_UNSUPPORTED, checked before any state changes.
 mc_status color_lane_check(mc_handle* h, const mc_params* p, int levels, int channels, int w, int hh) {
+    if (h->color_lane_lifecycle) return MC_OK;
     const bool change = tracker_changes(h, p, levels, channels, w, hh);
     int n_hold = 0, n_state = 0;
     for (int l = 0; l < h->lanes; ++l) { n_hold += h->hold[(size_t)l] != 0; n_state += h->has_state[(size_t)l] != 0; }
@@ -326,7 +328,6 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
         std::fill(lane_produced, lane_produced + n_flags, (uint8_t)0);
         return st;
     }
-    if (p->mode == MC_MODE_COLOR) std::fill(lane_produced, lane_produced + h->lanes, (uint8_t)(*produced != 0));   // all lanes step together
     for (int l = 0; l < h->lanes; ++l) {
         if (h->ops[(size_t)l] != LANE_HOLD) h->has_state[(size_t)l] = 1;
         else if (held_lost) h->has_state[(size_t)l] = 0;
@@ -542,6 +543,7 @@ mc_status mc_set_option(mc_handle* h, const char* key, int value) try {
     if (!std::strcmp(key, "ingest_warps")) { h->ingest_warps = value; return MC_OK; }
     if (!std::strcmp(key, "band_from_state")) { h->band_from_state = value != 0; return MC_OK; }
     if (!std::strcmp(key, "analysis_only")) { h->analysis_only = value != 0; return MC_OK; }
+    if (!std::strcmp(key, "color_lane_lifecycle")) { h->color_lane_lifecycle = value != 0; return MC_OK; }
     if (!std::strcmp(key, "pipeline_depth")) {
         if (value < 1 || value > 16 || !h->inflight.empty()) { h->err = "bad pipeline_depth"; return MC_ERR_INVALID; }
         h->depth = value;

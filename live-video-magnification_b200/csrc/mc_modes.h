@@ -254,12 +254,25 @@ private:
                          bool luma, Band band, Out out);
 };
 
+// One lane's row of the Color kernels' per-lane table (uploaded on the handle's stream when the lanes are not uniform)
+struct ColorLane {
+    int src_head, src_mod, copy_n;   // relayout: destination slot t < copy_n <- source slot (src_head + t) % src_mod
+    int append;                      // slot the frame is appended to; -1: held
+    int n;                           // DFT length this frame; 0: the lane does not run the filter (does not produce)
+    int sel;                         // physical slot of the reconstructed column (logical min(1, n - 1))
+    float sc;                        // DFT scale of both transforms, 1 / n^2
+    double fl, fh;                   // the CCS mask's packed index range for this n
+};
+
 struct ColorMode {
     int lanes = 1;
     bool allocated = false;
     int levels = 0, channels = 0, w = 0, h = 0;
-    int count = 0;          // frames currently in the window
-    int head = 0;           // physical slot of the OLDEST column
+    // Per lane: the rolling window's length, the physical slot of its OLDEST column and its logical ring size
+    // max(getOptimalBufferSize(int(framerate)), length, 2).  head == 0 or count == mod, lane by lane.
+    std::vector<int> count, head, mod;
+    std::vector<ColorLane> table;   // host copy of this frame's per-lane table
+    ColorLane* d_table = nullptr;
     std::vector<Level> lv;  // gaussian chain levels 0..levels
     std::vector<float*> G;  // pyrDown chain scratch (levels 1..levels-1) ; small level goes to the ring
     std::vector<float*> U;  // up-chain scratch
@@ -269,18 +282,23 @@ struct ColorMode {
     cufftComplex* spec = nullptr;
     float* minmax = nullptr;    // device scalars
     int small_rows = 0;         // pixels of the small level
-    int ring_cap = 0;           // physical slots allocated
-    int ring_mod = 0;           // logical ring size (<= ring_cap): max(getOptimalBufferSize(int(framerate)), window length)
+    int ring_cap = 0;           // physical slots allocated (>= every lane's mod)
     struct FftPlans { cufftHandle r2c = 0, c2r = 0; size_t work_bytes = 0; void* bound = nullptr; };
-    std::map<int, FftPlans> plans;   // per DFT length (the window length: 2 ... cap during warm-up), for plan_signals signals
+    // per (DFT length, one lane): the window length (2 ... cap during warm-up) over all plan_signals signals, or over one
+    // lane's channels * pixels signals (lanes whose windows differ in length)
+    std::map<std::pair<int, bool>, FftPlans> plans;
     size_t plan_signals = 0;
     void* fft_work = nullptr;        // one work area shared by all cached plans (they run back to back on one stream)
     size_t fft_work_bytes = 0;
     DeviceArena arena;
+    LanePlan plan;                   // per-lane ops of the current frame
 
     void reset();
     mc_status process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced);
     void find_state(const char* name, int level, StateRef& out);
+
+private:
+    mc_status fft_plan(const ModeCtx& ctx, int n, bool one_lane, FftPlans** out);
 };
 
 struct RieszMode {
