@@ -20,19 +20,63 @@ using namespace mc;
 namespace {
 thread_local std::string g_create_error;
 
-struct Slot {  // one in-flight frame of the pinned pipeline
-    uint8_t *h_in = nullptr, *h_out = nullptr;   // pinned staging (lanes frames)
-    uint8_t *d_in = nullptr, *d_out = nullptr;   // device frames
-    size_t bytes = 0;
+// A grow-only device buffer of T, freed with its owner.  grow(need) frees the old allocation before it allocates the
+// larger one.
+template <class T = uint8_t>
+struct DeviceBuffer {
+    T* p = nullptr;
+    size_t n = 0;   // capacity in T
+    DeviceBuffer() = default;
+    DeviceBuffer(const DeviceBuffer&) = delete;
+    DeviceBuffer& operator=(const DeviceBuffer&) = delete;
+    ~DeviceBuffer() { if (p) cudaFree(p); }
+    cudaError_t grow(size_t need) {
+        if (need <= n) return cudaSuccess;
+        if (p) cudaFree(p);
+        p = nullptr; n = 0;
+        const cudaError_t e = cudaMalloc((void**)&p, need * sizeof(T));
+        if (e == cudaSuccess) n = need;
+        return e;
+    }
+};
+
+// A frame set: one plane per lane (BGR or gray: height rows of w * c bytes) or two (NV12: height luma rows and height / 2
+// Cb,Cr rows of w bytes).  Rows hold `row` bytes and are `pitch` apart; lane l starts l * lane_stride after lane 0.
+struct Planes {
+    uint8_t* base[2] = {nullptr, nullptr};
+    size_t rows[2] = {0, 0};   // rows per lane; 0: no second plane
+    size_t row = 0, pitch = 0, lane_stride = 0;
+
+    size_t lane_rows() const { return rows[0] + rows[1]; }
+    size_t lane_bytes() const { return lane_rows() * row; }
+    // the same shape packed at `p`: no row padding, the second plane right after the first, lanes back to back
+    Planes packed(uint8_t* p) const { return Planes{{p, p + rows[0] * row}, {rows[0], rows[1]}, row, row, lane_bytes()}; }
+    // `lanes` consecutive lanes are one run of lanes * lane_rows() rows `pitch` apart
+    bool one_run(size_t lanes) const {
+        return (!rows[1] || base[1] == base[0] + rows[0] * pitch) && (lanes == 1 || lane_stride == lane_rows() * pitch);
+    }
+};
+
+Planes bgr_planes(const uint8_t* p, int w, int hh, int c, size_t step) {
+    return Planes{{const_cast<uint8_t*>(p), nullptr}, {(size_t)hh, 0}, (size_t)w * c, step, step * hh};
+}
+Planes nv12_planes(const mc_nv12& f, int w, int hh) {
+    return Planes{{f.y, f.uv}, {(size_t)hh, (size_t)hh / 2}, (size_t)w, f.pitch, f.lane_stride};
+}
+mc_nv12 nv12_of(const Planes& f) { return mc_nv12{f.base[0], f.base[1], f.pitch, f.lane_stride}; }
+
+struct Slot {  // one in-flight frame of the pinned pipeline; frees what it holds
+    uint8_t *h_in = nullptr, *h_out = nullptr;   // pinned staging (lanes frames, packed)
+    DeviceBuffer<> d_in, d_out;                  // device frames (packed)
     cudaEvent_t ev_in = nullptr, ev_k = nullptr, ev_done = nullptr;
     int produced = 0;
     std::vector<uint8_t> lane_produced;          // per lane: its bytes of `out` are written
-    uint8_t* user_out = nullptr;                 // destination given to mc_submit
-    size_t user_out_step = 0;
-    bool direct_out = false;                     // D2H went straight into user_out (pinned)
-    int w = 0, h = 0, c = 0;
-    bool nv12 = false;                           // an mc_submit_nv12 frame: the buffers hold NV12, user_nv12 is `out`
-    mc_nv12 user_nv12{};
+    Planes out;                                  // the caller's destination (base null: none)
+    bool direct_out = false;                     // D2H went straight into `out` (pinned)
+    ~Slot() {
+        for (uint8_t* p : {h_in, h_out}) if (p) cudaFreeHost(p);
+        for (cudaEvent_t e : {ev_in, ev_k, ev_done}) if (e) cudaEventDestroy(e);
+    }
 };
 }  // namespace
 
@@ -49,12 +93,7 @@ struct mc_handle {
     int t_down = 1, t_roi = 0;
     float t_rx = 0.f, t_ry = 0.f, t_rw = 1.f, t_rh = 1.f;
 
-    // options
-    bool faithful0 = false, keep_float = false, profile = false, use_tma = true, prefetch_state = true, band_from_state = true, analysis_only = false;
-    int ingest_warps = 1;
-    int egress_strip = 16;
-    int lane_groups = 0;
-    bool color_lane_lifecycle = false;
+    Options opt;
     Profiler prof;
     int depth = 3;
 
@@ -62,27 +101,22 @@ struct mc_handle {
     ColorMode color;
     RieszMode riesz;
 
-    float* float_out = nullptr;
-    size_t float_out_floats = 0;
+    DeviceBuffer<float> float_out;   // keep_float_output: the tap of the last frame call
 
     // chain calls: the front's staging (preprocessed frames when no tap is wanted, gray frames), the held-lane flags, and
     // the INTER_AREA tap tables with the geometry (rw, dw, rh, dh) they were built for and their host copy
-    uint8_t *f_pre = nullptr, *f_gray = nullptr, *f_flags = nullptr, *f_tabs = nullptr;
-    size_t f_pre_b = 0, f_gray_b = 0, f_flags_b = 0, f_tabs_b = 0;
+    DeviceBuffer<> f_pre, f_gray, f_flags, f_tabs;
     int f_tab_key[4] = {-1, -1, -1, -1};
     size_t f_tab_ofs[3] = {0, 0, 0};   // byte offsets of the y taps, x offsets, y offsets
     std::vector<uint8_t> f_tabs_host, f_flags_host;
     // mc_chain_process: device copies of its host frame, processed frame and original tap
-    uint8_t *c_raw = nullptr, *c_out = nullptr, *c_orig = nullptr;
-    size_t c_raw_b = 0, c_out_b = 0, c_orig_b = 0;
+    DeviceBuffer<> c_raw, c_out, c_orig;
 
     // mc_process_clip device staging: the clip's frames in and out
-    uint8_t *k_in = nullptr, *k_out = nullptr;
-    size_t k_in_b = 0, k_out_b = 0;
+    DeviceBuffer<> k_in, k_out;
 
     // NV12 calls: the magnifier's BGR input and output, and the produced flags of a call where only some lanes produced
-    uint8_t *n_in = nullptr, *n_out = nullptr, *n_flags = nullptr;
-    size_t n_in_b = 0, n_out_b = 0, n_flags_b = 0;
+    DeviceBuffer<> n_in, n_out, n_flags;
 
     // pipeline
     std::vector<Slot> slots;
@@ -176,35 +210,25 @@ void reset_modes(mc_handle* h) {
 }
 
 void free_slots(mc_handle* h) {
-    for (auto& s : h->slots) {
-        if (s.h_in) cudaFreeHost(s.h_in);
-        if (s.h_out) cudaFreeHost(s.h_out);
-        if (s.d_in) cudaFree(s.d_in);
-        if (s.d_out) cudaFree(s.d_out);
-        if (s.ev_in) cudaEventDestroy(s.ev_in);
-        if (s.ev_k) cudaEventDestroy(s.ev_k);
-        if (s.ev_done) cudaEventDestroy(s.ev_done);
-    }
     h->slots.clear();
     h->inflight.clear();
     h->next_slot = 0;
 }
 
 mc_status ensure_slots(mc_handle* h, size_t bytes) {
-    if ((int)h->slots.size() == h->depth && !h->slots.empty() && h->slots[0].bytes >= bytes) return MC_OK;
+    if ((int)h->slots.size() == h->depth && h->slots[0].d_in.n >= bytes) return MC_OK;
     if (!h->inflight.empty()) {
         h->err = "pipeline geometry changed with frames in flight";
         return MC_ERR_INVALID;
     }
     free_slots(h);
-    h->slots.resize((size_t)h->depth);
+    h->slots = std::vector<Slot>((size_t)h->depth);
     for (auto& s : h->slots) {
-        s.bytes = bytes;
         s.lane_produced.assign((size_t)h->lanes, 0);
         CK(cudaHostAlloc((void**)&s.h_in, bytes, cudaHostAllocDefault));
         CK(cudaHostAlloc((void**)&s.h_out, bytes, cudaHostAllocDefault));
-        CK(cudaMalloc((void**)&s.d_in, bytes));
-        CK(cudaMalloc((void**)&s.d_out, bytes));
+        CK(s.d_in.grow(bytes));
+        CK(s.d_out.grow(bytes));
         CK(cudaEventCreateWithFlags(&s.ev_in, cudaEventDisableTiming));
         CK(cudaEventCreateWithFlags(&s.ev_k, cudaEventDisableTiming));
         CK(cudaEventCreateWithFlags(&s.ev_done, cudaEventDisableTiming));
@@ -220,26 +244,38 @@ bool is_pinned(const void* p) {
     }
     return at.type == cudaMemoryTypeHost;
 }
+bool is_pinned(const Planes& f) { return is_pinned(f.base[0]) && (!f.rows[1] || is_pinned(f.base[1])); }
 
-// The NV12 frame set of a pipeline slot: every lane a packed frame (luma rows, then Cb,Cr rows, pitch = width), lanes
-// back to back.
-mc_nv12 slot_nv12(uint8_t* base, int w, int hh) {
-    const size_t luma = (size_t)w * hh;
-    return mc_nv12{base, base + luma, (size_t)w, luma + luma / 2};
+// Lane l of every plane, host to host, row by row.
+void host_copy(const Planes& dst, const Planes& src, size_t l) {
+    for (int k = 0; k < 2; ++k)
+        for (size_t r = 0; r < src.rows[k]; ++r)
+            std::memcpy(dst.base[k] + l * dst.lane_stride + r * dst.pitch, src.base[k] + l * src.lane_stride + r * src.pitch, src.row);
 }
 
-// Both planes of one lane, host to host.
-void host_copy_nv12(const mc_nv12& dst, const mc_nv12& src, int w, int hh, size_t lane) {
-    for (int r = 0; r < hh; ++r)
-        std::memcpy(dst.y + lane * dst.lane_stride + r * dst.pitch, src.y + lane * src.lane_stride + r * src.pitch, (size_t)w);
-    for (int r = 0; r < hh / 2; ++r)
-        std::memcpy(dst.uv + lane * dst.lane_stride + r * dst.pitch, src.uv + lane * src.lane_stride + r * src.pitch, (size_t)w);
+// Lanes [a, b) of every plane between host and device: one copy when both sides hold them as one run of rows (a plain
+// copy when neither side pads its rows), otherwise one 2D copy per plane and lane.
+mc_status copy_planes(mc_handle* h, const Planes& dst, const Planes& src, size_t a, size_t b, cudaMemcpyKind kind, cudaStream_t s) {
+    if (dst.one_run(b - a) && src.one_run(b - a)) {
+        uint8_t* d = dst.base[0] + a * dst.lane_stride;
+        const uint8_t* from = src.base[0] + a * src.lane_stride;
+        const size_t rows = (b - a) * src.lane_rows();
+        if (dst.pitch == src.row && src.pitch == src.row) CK(cudaMemcpyAsync(d, from, rows * src.row, kind, s));
+        else CK(cudaMemcpy2DAsync(d, dst.pitch, from, src.pitch, src.row, rows, kind, s));
+        return MC_OK;
+    }
+    for (size_t l = a; l < b; ++l)
+        for (int k = 0; k < 2; ++k)
+            if (src.rows[k])
+                CK(cudaMemcpy2DAsync(dst.base[k] + l * dst.lane_stride, dst.pitch, src.base[k] + l * src.lane_stride, src.pitch, src.row,
+                                     src.rows[k], kind, s));
+    return MC_OK;
 }
 
 // Without option "color_lane_lifecycle" a multi-lane Color handle keeps its lanes in lock-step: a frame call while a lane
 // is held, or restarted while others run, is MC_ERR_UNSUPPORTED, checked before any state changes.
 mc_status color_lane_check(mc_handle* h, const mc_params* p, int levels, int channels, int w, int hh) {
-    if (h->color_lane_lifecycle) return MC_OK;
+    if (h->opt.color_lane_lifecycle) return MC_OK;
     const bool change = tracker_changes(h, p, levels, channels, w, hh);
     int n_hold = 0, n_state = 0;
     for (int l = 0; l < h->lanes; ++l) { n_hold += h->hold[(size_t)l] != 0; n_state += h->has_state[(size_t)l] != 0; }
@@ -297,21 +333,15 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
     io.out = d_out; io.out_step = out_step; io.out_lane_stride = out_step * (size_t)hh;
     io.w = w; io.h = hh; io.channels = channels; io.lanes = h->lanes;
 
-    float* fout = nullptr;
-    if (h->keep_float) {
-        const size_t need = (size_t)h->lanes * w * hh * channels;
-        if (need > h->float_out_floats) {
-            if (h->float_out) cudaFree(h->float_out);
-            h->float_out = nullptr;
-            CK(cudaMalloc((void**)&h->float_out, need * sizeof(float)));
-            h->float_out_floats = need;
-        }
-        fout = h->float_out;
-    }
+    if (h->opt.keep_float_output) CK(h->float_out.grow((size_t)h->lanes * w * hh * channels));
 
     bool held_lost = false;
-    ModeCtx ctx{h->stream, &h->tables, &h->launches, &h->err, h->faithful0, fout, h->profile ? &h->prof : nullptr, h->use_tma, h->prefetch_state, h->egress_strip, h->ingest_warps, h->band_from_state, h->profile ? 1 : h->lane_groups, h->analysis_only,
-                h->ops.data(), h->d_ops, lane_produced, &held_lost};
+    Options opt = h->opt;
+    if (opt.profile_kernels) opt.lane_groups = 1;   // one launch chain: the events time one kernel at a time
+    const ModeCtx ctx{.stream = h->stream, .tables = &h->tables, .launches = &h->launches, .err = &h->err, .opt = opt,
+                      .float_out = opt.keep_float_output ? h->float_out.p : nullptr,
+                      .prof = opt.profile_kernels ? &h->prof : nullptr,
+                      .lane_ops = h->ops.data(), .d_lane_ops = h->d_ops, .lane_produced = lane_produced, .held_lost = &held_lost};
     mc_status st = MC_OK;
     switch (p->mode) {
         case MC_MODE_LAPLACE: st = h->motion.process(ctx, io, *p, levels, produced, frames); break;
@@ -333,6 +363,55 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
         else if (held_lost) h->has_state[(size_t)l] = 0;
     }
     return st;
+}
+
+// One frame set into the pipeline.  `in` is uploaded on the input stream into the next slot's packed device copy:
+// directly when it is pinned, through the slot's pinned staging when not.  `run(d_in, d_out, produced, lane_produced)`
+// then fills the slot's packed output on the handle's stream (with no buffers when `in` is empty: the identity).  Only
+// the lanes that produced are downloaded on the output stream, one copy per run of consecutive ones, into `out` when it
+// is pinned and into the staging, which mc_collect copies out, when not; the other lanes' bytes of `out` stay as they
+// are.  The slot's d_in is not overwritten before its kernels ran: the next upload into it follows mc_collect of this
+// frame, which waits on ev_done.
+template <class Run>
+mc_status submit_impl(mc_handle* h, const Planes& in, const Planes& out, Run run) {
+    const size_t lanes = (size_t)h->lanes, bytes = in.lane_bytes() * lanes;
+    mc_status st = ensure_slots(h, std::max<size_t>(bytes, 1));
+    if (st != MC_OK) return st;
+    if (out.base[0] && out.pitch < out.row) { h->err = "out_step too small"; return MC_ERR_INVALID; }
+    const int si = h->next_slot;
+    Slot& s = h->slots[(size_t)si];
+    s.produced = 0; s.out = out; s.direct_out = false;
+    const Planes none, d_in = bytes ? in.packed(s.d_in.p) : none, d_out = bytes ? in.packed(s.d_out.p) : none;
+    if (bytes) {
+        const bool pinned = is_pinned(in);
+        const Planes src = pinned ? in : in.packed(s.h_in);
+        if (!pinned)
+            for (size_t l = 0; l < lanes; ++l) host_copy(src, in, l);
+        if ((st = copy_planes(h, d_in, src, 0, lanes, cudaMemcpyHostToDevice, h->s_in)) != MC_OK) return st;
+        CK(cudaEventRecord(s.ev_in, h->s_in));
+        CK(cudaStreamWaitEvent(h->stream, s.ev_in, 0));
+    }
+    int produced = 0;
+    if ((st = run(d_in, d_out, &produced, s.lane_produced.data())) != MC_OK) return st;
+    s.produced = produced;
+    if (produced) {
+        CK(cudaEventRecord(s.ev_k, h->stream));
+        CK(cudaStreamWaitEvent(h->s_out, s.ev_k, 0));
+        if (out.base[0]) {
+            s.direct_out = is_pinned(out);
+            const Planes dst = s.direct_out ? out : out.packed(s.h_out);
+            st = for_each_run(lanes, [&](size_t l) { return s.lane_produced[l] != 0; }, [&](size_t a, size_t b) {
+                return copy_planes(h, dst, d_out, a, b, cudaMemcpyDeviceToHost, h->s_out);
+            });
+            if (st != MC_OK) return st;
+        }
+        CK(cudaEventRecord(s.ev_done, h->s_out));
+    } else {
+        CK(cudaEventRecord(s.ev_done, h->stream));
+    }
+    h->inflight.push_back(si);
+    h->next_slot = (si + 1) % h->depth;
+    return MC_OK;
 }
 
 }  // namespace
@@ -479,22 +558,13 @@ void mc_destroy(mc_handle* h) try {
     if (h->s_in) cudaStreamSynchronize(h->s_in);
     if (h->s_out) cudaStreamSynchronize(h->s_out);
     reset_modes(h);
-    free_slots(h);
-    if (h->float_out) cudaFree(h->float_out);
-    for (uint8_t* b : {h->f_pre, h->f_gray, h->f_flags, h->f_tabs, h->c_raw, h->c_out, h->c_orig})
-        if (b) cudaFree(b);
-    if (h->k_in) cudaFree(h->k_in);
-    if (h->k_out) cudaFree(h->k_out);
-    if (h->n_in) cudaFree(h->n_in);
-    if (h->n_out) cudaFree(h->n_out);
-    if (h->n_flags) cudaFree(h->n_flags);
     if (h->tables.lab_lut) cudaFree(h->tables.lab_lut);
     if (h->tables.inv_gamma) cudaFree(h->tables.inv_gamma);
     if (h->d_ops) cudaFree(h->d_ops);
     if (h->stream) cudaStreamDestroy(h->stream);
     if (h->s_in) cudaStreamDestroy(h->s_in);
     if (h->s_out) cudaStreamDestroy(h->s_out);
-    delete h;
+    delete h;   // the pipeline slots and the scratch buffers free themselves
 } catch (...) {}
 
 /* test hook, not declared in the public header: the n-th guarded entry on this thread throws std::bad_alloc */
@@ -533,17 +603,18 @@ mc_status mc_lane_produced(mc_handle* h, uint8_t* produced, int n) try {
 
 mc_status mc_set_option(mc_handle* h, const char* key, int value) try {
     if (!h || !key) return MC_ERR_INVALID;
-    if (!std::strcmp(key, "faithful_level0")) { h->faithful0 = value != 0; return MC_OK; }
-    if (!std::strcmp(key, "keep_float_output")) { h->keep_float = value != 0; return MC_OK; }
-    if (!std::strcmp(key, "profile_kernels")) { h->profile = value != 0; return MC_OK; }
-    if (!std::strcmp(key, "use_tma")) { h->use_tma = value != 0; return MC_OK; }
-    if (!std::strcmp(key, "prefetch_state")) { h->prefetch_state = value != 0; return MC_OK; }
-    if (!std::strcmp(key, "lane_groups")) { h->lane_groups = value < 0 ? 0 : value; return MC_OK; }
-    if (!std::strcmp(key, "egress_strip")) { h->egress_strip = value == 1 ? 16 : value; return MC_OK; }
-    if (!std::strcmp(key, "ingest_warps")) { h->ingest_warps = value; return MC_OK; }
-    if (!std::strcmp(key, "band_from_state")) { h->band_from_state = value != 0; return MC_OK; }
-    if (!std::strcmp(key, "analysis_only")) { h->analysis_only = value != 0; return MC_OK; }
-    if (!std::strcmp(key, "color_lane_lifecycle")) { h->color_lane_lifecycle = value != 0; return MC_OK; }
+    Options& o = h->opt;
+    if (!std::strcmp(key, "faithful_level0")) { o.faithful_level0 = value != 0; return MC_OK; }
+    if (!std::strcmp(key, "keep_float_output")) { o.keep_float_output = value != 0; return MC_OK; }
+    if (!std::strcmp(key, "profile_kernels")) { o.profile_kernels = value != 0; return MC_OK; }
+    if (!std::strcmp(key, "use_tma")) { o.use_tma = value != 0; return MC_OK; }
+    if (!std::strcmp(key, "prefetch_state")) { o.prefetch_state = value != 0; return MC_OK; }
+    if (!std::strcmp(key, "lane_groups")) { o.lane_groups = value < 0 ? 0 : value; return MC_OK; }
+    if (!std::strcmp(key, "egress_strip")) { o.egress_strip = value == 1 ? 16 : value; return MC_OK; }
+    if (!std::strcmp(key, "ingest_warps")) { o.ingest_warps = value; return MC_OK; }
+    if (!std::strcmp(key, "band_from_state")) { o.band_from_state = value != 0; return MC_OK; }
+    if (!std::strcmp(key, "analysis_only")) { o.analysis_only = value != 0; return MC_OK; }
+    if (!std::strcmp(key, "color_lane_lifecycle")) { o.color_lane_lifecycle = value != 0; return MC_OK; }
     if (!std::strcmp(key, "pipeline_depth")) {
         if (value < 1 || value > 16 || !h->inflight.empty()) { h->err = "bad pipeline_depth"; return MC_ERR_INVALID; }
         h->depth = value;
@@ -582,70 +653,14 @@ mc_status mc_submit(mc_handle* h, const uint8_t* in, int width, int height, int 
     CK(cudaSetDevice(h->device));
     if ((int)h->inflight.size() >= h->depth) { h->err = "pipeline full: call mc_collect first"; return MC_ERR_INVALID; }
     const bool have = in != nullptr && width > 0 && height > 0 && (channels == 1 || channels == 3);
-    const size_t row = have ? (size_t)width * channels : 0;
-    const size_t bytes = row * (size_t)(have ? height : 0) * h->lanes;
-    if (have && in_step < row) { h->err = "step too small"; return MC_ERR_INVALID; }
-    mc_status st = ensure_slots(h, std::max<size_t>(bytes, 1));
-    if (st != MC_OK) return st;
-    const int si = h->next_slot;
-    Slot& s = h->slots[(size_t)si];
-    s.w = width; s.h = height; s.c = channels; s.produced = 0;
-    s.user_out = out; s.user_out_step = out_step; s.direct_out = false; s.nv12 = false;
-    if (have && out && out_step < row) { h->err = "out_step too small"; return MC_ERR_INVALID; }
-    if (!have) {
-        int produced = 0;
-        st = process_device_impl(h, nullptr, 0, 0, channels, 0, p, nullptr, 0, &produced, s.lane_produced.data());
-        if (st != MC_OK) return st;
-        CK(cudaEventRecord(s.ev_done, h->stream));
-        h->inflight.push_back(si);
-        h->next_slot = (si + 1) % h->depth;
-        return MC_OK;
-    }
-    const size_t rows = (size_t)height * h->lanes;
-    if (is_pinned(in)) {
-        if (in_step == row) CK(cudaMemcpyAsync(s.d_in, in, bytes, cudaMemcpyHostToDevice, h->s_in));
-        else CK(cudaMemcpy2DAsync(s.d_in, row, in, in_step, row, rows, cudaMemcpyHostToDevice, h->s_in));
-    } else {
-        for (size_t r = 0; r < rows; ++r) std::memcpy(s.h_in + r * row, in + r * in_step, row);
-        CK(cudaMemcpyAsync(s.d_in, s.h_in, bytes, cudaMemcpyHostToDevice, h->s_in));
-    }
-    CK(cudaEventRecord(s.ev_in, h->s_in));
-    CK(cudaStreamWaitEvent(h->stream, s.ev_in, 0));
-    int produced = 0;
-    st = process_device_impl(h, s.d_in, width, height, channels, row, p, s.d_out, row, &produced, s.lane_produced.data());
-    if (st != MC_OK) return st;
-    s.produced = produced;
-    CK(cudaEventRecord(s.ev_k, h->stream));
-    if (produced) {
-        CK(cudaStreamWaitEvent(h->s_out, s.ev_k, 0));
-        // only the lanes that produced are downloaded: one copy per run of consecutive produced lanes (one in all when
-        // every lane produced); the bytes of the other lanes in `out` are left as they are
-        const bool direct = out && is_pinned(out);
-        const size_t lane_bytes = row * (size_t)height;
-        if (out)
-            st = for_each_run(h->lanes, [&](size_t l) { return s.lane_produced[l] != 0; }, [&](size_t a, size_t b) -> mc_status {
-                const size_t n = (b - a) * lane_bytes, run_rows = (b - a) * height;
-                const uint8_t* src = s.d_out + a * lane_bytes;
-                if (direct) {
-                    uint8_t* dst = out + a * height * out_step;
-                    if (out_step == row) CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, h->s_out));
-                    else CK(cudaMemcpy2DAsync(dst, out_step, src, row, row, run_rows, cudaMemcpyDeviceToHost, h->s_out));
-                } else {
-                    CK(cudaMemcpyAsync(s.h_out + a * lane_bytes, src, n, cudaMemcpyDeviceToHost, h->s_out));
-                }
-                return MC_OK;
-            });
-        if (st != MC_OK) return st;
-        s.direct_out = direct;
-        CK(cudaEventRecord(s.ev_done, h->s_out));
-    } else {
-        CK(cudaEventRecord(s.ev_done, h->stream));
-    }
-    // d_in of this slot must not be overwritten before its kernels ran: the next H2D into this slot
-    // happens only after collect() of this frame, which waits on ev_done (>= ev_k).
-    h->inflight.push_back(si);
-    h->next_slot = (si + 1) % h->depth;
-    return MC_OK;
+    if (have && in_step < (size_t)width * channels) { h->err = "step too small"; return MC_ERR_INVALID; }
+    const Planes none;
+    return submit_impl(h, have ? bgr_planes(in, width, height, channels, in_step) : none,
+                       have ? bgr_planes(out, width, height, channels, out_step) : none,
+                       [&](const Planes& d_in, const Planes& d_out, int* produced, uint8_t* lane_produced) {
+                           return process_device_impl(h, d_in.base[0], width, height, channels, d_in.pitch, p, d_out.base[0],
+                                                      d_out.pitch, produced, lane_produced);
+                       });
 } catch (...) { return on_exception(h); }
 
 mc_status mc_collect(mc_handle* h, int* produced) try {
@@ -658,16 +673,10 @@ mc_status mc_collect(mc_handle* h, int* produced) try {
     CK(cudaEventSynchronize(s.ev_done));
     *produced = s.produced;
     h->lane_produced = s.lane_produced;
-    if (s.produced && !s.direct_out && s.nv12) {
-        const mc_nv12 staged = slot_nv12(s.h_out, s.w, s.h);
-        for (int l = 0; l < h->lanes; ++l)
-            if (s.lane_produced[(size_t)l]) host_copy_nv12(s.user_nv12, staged, s.w, s.h, (size_t)l);
-    } else if (s.produced && !s.direct_out && s.user_out) {
-        const size_t row = (size_t)s.w * s.c;
-        for (int l = 0; l < h->lanes; ++l) {
-            if (!s.lane_produced[(size_t)l]) continue;
-            for (size_t r = (size_t)l * s.h; r < (size_t)(l + 1) * s.h; ++r) std::memcpy(s.user_out + r * s.user_out_step, s.h_out + r * row, row);
-        }
+    if (s.produced && !s.direct_out && s.out.base[0]) {
+        const Planes staged = s.out.packed(s.h_out);
+        for (size_t l = 0; l < (size_t)h->lanes; ++l)
+            if (s.lane_produced[l]) host_copy(s.out, staged, l);
     }
     return MC_OK;
 } catch (...) { return on_exception(h); }
@@ -736,9 +745,9 @@ mc_status mc_set_state(mc_handle* h, const char* name, int level, const float* s
 mc_status mc_get_float_output(mc_handle* h, float* dst, size_t n) try {
     if (!h || !dst) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    if (!h->float_out || n < h->float_out_floats) { h->err = "no float output kept (set keep_float_output) or buffer too small"; return MC_ERR_INVALID; }
+    if (!h->float_out.p || n < h->float_out.n) { h->err = "no float output kept (set keep_float_output) or buffer too small"; return MC_ERR_INVALID; }
     CK(cudaStreamSynchronize(h->stream));
-    CK(cudaMemcpy(dst, h->float_out, h->float_out_floats * sizeof(float), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(dst, h->float_out.p, h->float_out.n * sizeof(float), cudaMemcpyDeviceToHost));
     return MC_OK;
 } catch (...) { return on_exception(h); }
 
@@ -784,30 +793,26 @@ extern "C" mc_status mc_profile_read(mc_handle* h, char* buf, size_t cap) try {
     return MC_OK;
 } catch (...) { return on_exception(h); }
 
-namespace {
-mc_status grow(mc_handle* h, uint8_t** p, size_t* cap, size_t need) {
-    if (need <= *cap) return MC_OK;
-    if (*p) cudaFree(*p);
-    *p = nullptr; *cap = 0;
-    CK(cudaMalloc((void**)p, need));
-    *cap = need;
-    return MC_OK;
-}
-}  // namespace
-
 // ---- clips: `frames` consecutive frames of every lane in one call ----------------------------------------------------
 namespace {
-mc_status clip_impl(mc_handle* h, const uint8_t* d_in, int frames, int w, int hh, int channels, size_t in_step, const mc_params* p,
-                    uint8_t* d_out, size_t out_step, uint8_t* produced) {
+// The argument errors of a clip call, before anything changes.
+mc_status check_clip(mc_handle* h, int frames, const uint8_t* produced) {
     if (frames < 1) { h->err = "frames must be >= 1"; return MC_ERR_INVALID; }
     // frames * lanes * channels becomes a grid.z extent of the batched ingest / egress
     if ((long long)frames * h->lanes > MC_MAX_LANES) { h->err = "frames * lanes exceeds MC_MAX_LANES"; return MC_ERR_INVALID; }
     if (!produced) { h->err = "produced is null"; return MC_ERR_INVALID; }
     if (!h->inflight.empty()) { h->err = "clip called with pipelined frames in flight"; return MC_ERR_INVALID; }
+    return MC_OK;
+}
+
+// d_in null: the identity (no frame produces; a handle that was magnifying drops its state)
+mc_status clip_impl(mc_handle* h, const uint8_t* d_in, int frames, int w, int hh, int channels, size_t in_step, const mc_params* p,
+                    uint8_t* d_out, size_t out_step, uint8_t* produced) {
+    mc_status st = check_clip(h, frames, produced);
+    if (st != MC_OK) return st;
     const size_t lanes = (size_t)h->lanes;
     std::fill(produced, produced + (size_t)frames * lanes, (uint8_t)0);
     int any = 0;
-    mc_status st = MC_OK;
     if (p && (p->mode == MC_MODE_LAPLACE || p->mode == MC_MODE_PHASE) && frames > 1) {
         st = process_device_impl(h, d_in, w, hh, channels, in_step, p, d_out, out_step, &any, produced, frames);
     } else {
@@ -834,28 +839,24 @@ extern "C" mc_status mc_process_clip(mc_handle* h, const uint8_t* in, int frames
                                      size_t in_step, const mc_params* p, uint8_t* out, size_t out_step, uint8_t* produced) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    const bool have = in != nullptr && width > 0 && height > 0 && (channels == 1 || channels == 3);
-    if (!have || frames < 1 || (long long)frames * h->lanes > MC_MAX_LANES || !produced || !h->inflight.empty())
-        return clip_impl(h, nullptr, frames, 0, 0, channels, 0, p, nullptr, 0, produced);   // argument errors, identity
-    const size_t row = (size_t)width * channels;
-    if (in_step < row || (out && out_step < row)) { h->err = "step too small"; return MC_ERR_INVALID; }
-    const size_t vl = (size_t)frames * h->lanes, rows = vl * height, frame_bytes = row * height;
-    mc_status st;
-    if ((st = grow(h, &h->k_in, &h->k_in_b, rows * row)) != MC_OK) return st;
-    if ((st = grow(h, &h->k_out, &h->k_out_b, rows * row)) != MC_OK) return st;
-    if (in_step == row) CK(cudaMemcpyAsync(h->k_in, in, rows * row, cudaMemcpyHostToDevice, h->stream));
-    else CK(cudaMemcpy2DAsync(h->k_in, row, in, in_step, row, rows, cudaMemcpyHostToDevice, h->stream));
-    st = clip_impl(h, h->k_in, frames, width, height, channels, row, p, h->k_out, row, produced);
+    mc_status st = check_clip(h, frames, produced);
+    if (st != MC_OK) return st;
+    if (!(in != nullptr && width > 0 && height > 0 && (channels == 1 || channels == 3)))
+        return clip_impl(h, nullptr, frames, 0, 0, channels, 0, p, nullptr, 0, produced);   // the identity
+    const Planes src = bgr_planes(in, width, height, channels, in_step), dst = bgr_planes(out, width, height, channels, out_step);
+    if (in_step < src.row || (out && out_step < src.row)) { h->err = "step too small"; return MC_ERR_INVALID; }
+    const size_t vl = (size_t)frames * h->lanes;
+    CK(h->k_in.grow(src.lane_bytes() * vl));
+    CK(h->k_out.grow(src.lane_bytes() * vl));
+    const Planes d_in = src.packed(h->k_in.p), d_out = src.packed(h->k_out.p);
+    if ((st = copy_planes(h, d_in, src, 0, vl, cudaMemcpyHostToDevice, h->stream)) != MC_OK) return st;
+    st = clip_impl(h, d_in.base[0], frames, width, height, channels, d_in.pitch, p, d_out.base[0], d_out.pitch, produced);
     if (st != MC_OK) return st;
     // only the frames that produced are downloaded, one copy per run of consecutive ones ([t][lane] order); the bytes of
     // the others in `out` are left as they are
     if (out)
-        st = for_each_run(vl, [&](size_t i) { return produced[i] != 0; }, [&](size_t a, size_t b) -> mc_status {
-            const uint8_t* src = h->k_out + a * frame_bytes;
-            uint8_t* dst = out + a * height * out_step;
-            if (out_step == row) CK(cudaMemcpyAsync(dst, src, (b - a) * frame_bytes, cudaMemcpyDeviceToHost, h->stream));
-            else CK(cudaMemcpy2DAsync(dst, out_step, src, row, row, (b - a) * height, cudaMemcpyDeviceToHost, h->stream));
-            return MC_OK;
+        st = for_each_run(vl, [&](size_t i) { return produced[i] != 0; }, [&](size_t a, size_t b) {
+            return copy_planes(h, dst, d_out, a, b, cudaMemcpyDeviceToHost, h->stream);
         });
     if (st != MC_OK) return st;
     CK(cudaStreamSynchronize(h->stream));
@@ -880,20 +881,28 @@ Nv12Planes planes_of(const mc_nv12& f) { return Nv12Planes{f.y, f.uv, f.pitch, f
 // Row pitch of the BGR staging: 16-byte rows keep the conversions on their 64-bit path.
 size_t bgr_step_of(int w) { return (size_t)round_up(3 * w, 16); }
 
-// `in` -> h->n_in (BGR, bgr_step_of(w)) for `vlanes` virtual lanes, and h->n_out sized for the magnifier's BGR output
-// unless the caller writes it elsewhere (bgr_out false).  Mode None does not read its input: no launch.
-mc_status nv12_ingest(mc_handle* h, const mc_nv12& in, int w, int hh, int vlanes, const mc_params* p, bool bgr_out = true) {
-    const size_t bytes = bgr_step_of(w) * hh * vlanes;
-    mc_status st;
-    if ((st = grow(h, &h->n_in, &h->n_in_b, bytes)) != MC_OK) return st;
-    if (bgr_out && (st = grow(h, &h->n_out, &h->n_out_b, bytes)) != MC_OK) return st;
-    if (p->mode == MC_MODE_NONE) return MC_OK;
-    const bool prof = h->profile && h->prof.begin("nv12_to_bgr", 0, h->stream);
-    const cudaError_t e = launch_nv12_to_bgr(planes_of(in), w, hh, vlanes, h->n_in, bgr_step_of(w), h->stream);
+// One kernel launch of the handle's own (`launch()` issues it on the handle's stream): counted, and timed as `name` under
+// profile_kernels.
+template <class Launch>
+mc_status launch_counted(mc_handle* h, const char* name, Launch launch) {
+    const bool prof = h->opt.profile_kernels && h->prof.begin(name, 0, h->stream);
+    const cudaError_t e = launch();
     if (prof) h->prof.end(h->stream);
     CK(e);
     ++h->launches;
     return MC_OK;
+}
+
+// `in` -> h->n_in (BGR, bgr_step_of(w)) for `vlanes` virtual lanes, and h->n_out sized for the magnifier's BGR output
+// unless the caller writes it elsewhere (bgr_out false).  Mode None does not read its input: no launch.
+mc_status nv12_ingest(mc_handle* h, const mc_nv12& in, int w, int hh, int vlanes, const mc_params* p, bool bgr_out = true) {
+    const size_t bytes = bgr_step_of(w) * hh * vlanes;
+    CK(h->n_in.grow(bytes));
+    if (bgr_out) CK(h->n_out.grow(bytes));
+    if (p->mode == MC_MODE_NONE) return MC_OK;
+    return launch_counted(h, "nv12_to_bgr", [&] {
+        return launch_nv12_to_bgr(planes_of(in), w, hh, vlanes, h->n_in.p, bgr_step_of(w), h->stream);
+    });
 }
 
 // h->n_out -> `out` for the virtual lanes whose flag (host, vlanes bytes) is set.  When only some produced, the flags go
@@ -903,38 +912,24 @@ mc_status nv12_egress(mc_handle* h, const mc_nv12& out, int w, int hh, int vlane
     if (n == 0) return MC_OK;
     const uint8_t* d_flags = nullptr;
     if (n < vlanes) {
-        mc_status st;
-        if ((st = grow(h, &h->n_flags, &h->n_flags_b, (size_t)vlanes)) != MC_OK) return st;
-        CK(cudaMemcpyAsync(h->n_flags, flags, (size_t)vlanes, cudaMemcpyHostToDevice, h->stream));
-        d_flags = h->n_flags;
+        CK(h->n_flags.grow((size_t)vlanes));
+        CK(cudaMemcpyAsync(h->n_flags.p, flags, (size_t)vlanes, cudaMemcpyHostToDevice, h->stream));
+        d_flags = h->n_flags.p;
     }
-    const bool prof = h->profile && h->prof.begin("bgr_to_nv12", 0, h->stream);
-    const cudaError_t e = launch_bgr_to_nv12(h->n_out, bgr_step_of(w), w, hh, vlanes, d_flags, out.y, out.uv, out.pitch,
-                                             out.lane_stride, h->stream);
-    if (prof) h->prof.end(h->stream);
-    CK(e);
-    ++h->launches;
-    return MC_OK;
+    return launch_counted(h, "bgr_to_nv12", [&] {
+        return launch_bgr_to_nv12(h->n_out.p, bgr_step_of(w), w, hh, vlanes, d_flags, out.y, out.uv, out.pitch, out.lane_stride,
+                                  h->stream);
+    });
 }
 
-// Lanes [a, b) of both planes between host and device: one 2D copy for the run when both sides hold packed frames back
-// to back (the Cb,Cr rows right after the luma rows), otherwise two per lane.
-bool packed_nv12(const mc_nv12& f, int hh, size_t lanes) {
-    return f.uv == f.y + f.pitch * hh && (lanes == 1 || f.lane_stride == f.pitch * hh / 2 * 3);
-}
-mc_status copy_nv12(mc_handle* h, const mc_nv12& dst, const mc_nv12& src, int w, int hh, size_t a, size_t b, cudaMemcpyKind kind,
-                    cudaStream_t s) {
-    if (packed_nv12(dst, hh, b - a) && packed_nv12(src, hh, b - a)) {
-        CK(cudaMemcpy2DAsync(dst.y + a * dst.lane_stride, dst.pitch, src.y + a * src.lane_stride, src.pitch, (size_t)w,
-                             (b - a) * hh / 2 * 3, kind, s));
-        return MC_OK;
-    }
-    for (size_t l = a; l < b; ++l) {
-        CK(cudaMemcpy2DAsync(dst.y + l * dst.lane_stride, dst.pitch, src.y + l * src.lane_stride, src.pitch, (size_t)w, (size_t)hh, kind, s));
-        CK(cudaMemcpy2DAsync(dst.uv + l * dst.lane_stride, dst.pitch, src.uv + l * src.lane_stride, src.pitch, (size_t)w, (size_t)hh / 2,
-                             kind, s));
-    }
-    return MC_OK;
+// One frame call on NV12 device planes: nv12_ingest -> the magnifier on the BGR staging -> nv12_egress.
+mc_status nv12_frame(mc_handle* h, const mc_nv12& in, const mc_nv12& out, int w, int hh, const mc_params* p, int* produced,
+                     uint8_t* lane_produced) {
+    mc_status st = nv12_ingest(h, in, w, hh, h->lanes, p);
+    if (st != MC_OK) return st;
+    const size_t step = bgr_step_of(w);
+    if ((st = process_device_impl(h, h->n_in.p, w, hh, 3, step, p, h->n_out.p, step, produced, lane_produced)) != MC_OK) return st;
+    return nv12_egress(h, out, w, hh, h->lanes, lane_produced);
 }
 }  // namespace
 
@@ -943,82 +938,39 @@ extern "C" mc_status mc_process_nv12_device(mc_handle* h, const mc_nv12* in, int
     if (!h || !produced) return MC_ERR_INVALID;
     *produced = 0;
     CK(cudaSetDevice(h->device));
-    mc_status st = check_nv12(h, {in, out}, width, height, h->lanes, p);
+    const mc_status st = check_nv12(h, {in, out}, width, height, h->lanes, p);
     if (st != MC_OK) return st;
-    if ((st = nv12_ingest(h, *in, width, height, h->lanes, p)) != MC_OK) return st;
-    const size_t step = bgr_step_of(width);
-    st = process_device_impl(h, h->n_in, width, height, 3, step, p, h->n_out, step, produced, h->lane_produced.data());
-    if (st != MC_OK) return st;
-    return nv12_egress(h, *out, width, height, h->lanes, h->lane_produced.data());
+    return nv12_frame(h, *in, *out, width, height, p, produced, h->lane_produced.data());
 } catch (...) { return on_exception(h); }
 
 extern "C" mc_status mc_process_clip_nv12_device(mc_handle* h, const mc_nv12* in, int frames, int width, int height,
                                                  const mc_params* p, const mc_nv12* out, uint8_t* produced) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    if (frames < 1 || (long long)frames * h->lanes > MC_MAX_LANES || !produced || !h->inflight.empty())
-        return clip_impl(h, nullptr, frames, 0, 0, 3, 0, p, nullptr, 0, produced);   // the clip's argument errors
-    const int vlanes = frames * h->lanes;
-    mc_status st = check_nv12(h, {in, out}, width, height, vlanes, p);
+    mc_status st = check_clip(h, frames, produced);
     if (st != MC_OK) return st;
+    const int vlanes = frames * h->lanes;
+    if ((st = check_nv12(h, {in, out}, width, height, vlanes, p)) != MC_OK) return st;
     if ((st = nv12_ingest(h, *in, width, height, vlanes, p)) != MC_OK) return st;
     const size_t step = bgr_step_of(width);
-    st = clip_impl(h, h->n_in, frames, width, height, 3, step, p, h->n_out, step, produced);
+    st = clip_impl(h, h->n_in.p, frames, width, height, 3, step, p, h->n_out.p, step, produced);
     if (st != MC_OK) return st;
     return nv12_egress(h, *out, width, height, vlanes, produced);
 } catch (...) { return on_exception(h); }
 
-// mc_submit on NV12 planes: the slot buffers hold NV12 (slot_nv12), so PCIe moves 1.5 B/px each way; the conversions run
-// on the compute stream around the magnifier, through the handle's BGR staging (stream-ordered, shared by the slots).
+// mc_submit on NV12 planes: the slot buffers hold NV12, so PCIe moves 1.5 B/px each way; the conversions run on the
+// compute stream around the magnifier, through the handle's BGR staging (stream-ordered, shared by the slots).
 extern "C" mc_status mc_submit_nv12(mc_handle* h, const mc_nv12* in, int width, int height, const mc_params* p,
                                     const mc_nv12* out) try {
     if (!h || !p) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
     if ((int)h->inflight.size() >= h->depth) { h->err = "pipeline full: call mc_collect first"; return MC_ERR_INVALID; }
-    mc_status st = check_nv12(h, {in, out}, width, height, h->lanes, p);
+    const mc_status st = check_nv12(h, {in, out}, width, height, h->lanes, p);
     if (st != MC_OK) return st;
-    const size_t lanes = (size_t)h->lanes, lane_bytes = (size_t)width * height / 2 * 3;
-    if ((st = ensure_slots(h, lane_bytes * lanes)) != MC_OK) return st;
-    const int si = h->next_slot;
-    Slot& s = h->slots[(size_t)si];
-    s.w = width; s.h = height; s.c = 3; s.produced = 0;
-    s.user_out = nullptr; s.user_out_step = 0; s.direct_out = false; s.nv12 = true; s.user_nv12 = *out;
-    const mc_nv12 d_in = slot_nv12(s.d_in, width, height), d_out = slot_nv12(s.d_out, width, height);
-    if (is_pinned(in->y) && is_pinned(in->uv)) {
-        if ((st = copy_nv12(h, d_in, *in, width, height, 0, lanes, cudaMemcpyHostToDevice, h->s_in)) != MC_OK) return st;
-    } else {
-        const mc_nv12 staged = slot_nv12(s.h_in, width, height);
-        for (size_t l = 0; l < lanes; ++l) host_copy_nv12(staged, *in, width, height, l);
-        CK(cudaMemcpyAsync(s.d_in, s.h_in, lane_bytes * lanes, cudaMemcpyHostToDevice, h->s_in));
-    }
-    CK(cudaEventRecord(s.ev_in, h->s_in));
-    CK(cudaStreamWaitEvent(h->stream, s.ev_in, 0));
-    if ((st = nv12_ingest(h, d_in, width, height, h->lanes, p)) != MC_OK) return st;
-    const size_t step = bgr_step_of(width);
-    int produced = 0;
-    st = process_device_impl(h, h->n_in, width, height, 3, step, p, h->n_out, step, &produced, s.lane_produced.data());
-    if (st != MC_OK) return st;
-    if ((st = nv12_egress(h, d_out, width, height, h->lanes, s.lane_produced.data())) != MC_OK) return st;
-    s.produced = produced;
-    CK(cudaEventRecord(s.ev_k, h->stream));
-    if (produced) {
-        CK(cudaStreamWaitEvent(h->s_out, s.ev_k, 0));
-        // only the lanes that produced are downloaded, one run of consecutive lanes at a time
-        const bool direct = is_pinned(out->y) && is_pinned(out->uv);
-        st = for_each_run(lanes, [&](size_t l) { return s.lane_produced[l] != 0; }, [&](size_t a, size_t b) -> mc_status {
-            if (direct) return copy_nv12(h, *out, d_out, width, height, a, b, cudaMemcpyDeviceToHost, h->s_out);
-            CK(cudaMemcpyAsync(s.h_out + a * lane_bytes, s.d_out + a * lane_bytes, (b - a) * lane_bytes, cudaMemcpyDeviceToHost, h->s_out));
-            return MC_OK;
-        });
-        if (st != MC_OK) return st;
-        s.direct_out = direct;
-        CK(cudaEventRecord(s.ev_done, h->s_out));
-    } else {
-        CK(cudaEventRecord(s.ev_done, h->stream));
-    }
-    h->inflight.push_back(si);
-    h->next_slot = (si + 1) % h->depth;
-    return MC_OK;
+    return submit_impl(h, nv12_planes(*in, width, height), nv12_planes(*out, width, height),
+                       [&](const Planes& d_in, const Planes& d_out, int* produced, uint8_t* lane_produced) {
+                           return nv12_frame(h, nv12_of(d_in), nv12_of(d_out), width, height, p, produced, lane_produced);
+                       });
 } catch (...) { return on_exception(h); }
 
 // ---- the processing chain: runChainOnce (ChainBuilder.cpp:19-29) = Preprocess -> Grayscale -> Magnification ----------
@@ -1079,16 +1031,16 @@ mc_status area_tables(mc_handle* h, const ChainGeom& g, FrontArgs& a) {
         std::memcpy(b.data() + bx, yt.data(), by);
         std::memcpy(b.data() + bx + by, xo.data(), bxo);
         std::memcpy(b.data() + bx + by + bxo, yo.data(), total - bx - by - bxo);
-        mc_status st;
-        if ((st = grow(h, &h->f_tabs, &h->f_tabs_b, total)) != MC_OK) return st;
-        CK(cudaMemcpyAsync(h->f_tabs, b.data(), total, cudaMemcpyHostToDevice, h->stream));
+        CK(h->f_tabs.grow(total));
+        CK(cudaMemcpyAsync(h->f_tabs.p, b.data(), total, cudaMemcpyHostToDevice, h->stream));
         h->f_tab_ofs[0] = bx; h->f_tab_ofs[1] = bx + by; h->f_tab_ofs[2] = bx + by + bxo;
         std::copy(key, key + 4, h->f_tab_key);
     }
-    a.xtab = (const AreaTap*)h->f_tabs;
-    a.ytab = (const AreaTap*)(h->f_tabs + h->f_tab_ofs[0]);
-    a.xofs = (const int*)(h->f_tabs + h->f_tab_ofs[1]);
-    a.yofs = (const int*)(h->f_tabs + h->f_tab_ofs[2]);
+    const uint8_t* t = h->f_tabs.p;
+    a.xtab = (const AreaTap*)t;
+    a.ytab = (const AreaTap*)(t + h->f_tab_ofs[0]);
+    a.xofs = (const int*)(t + h->f_tab_ofs[1]);
+    a.yofs = (const int*)(t + h->f_tab_ofs[2]);
     return MC_OK;
 }
 
@@ -1106,10 +1058,10 @@ mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc
         h->err = e;
         return MC_ERR_INVALID;
     }
-    if (empty || frames < 1 || (long long)frames * h->lanes > MC_MAX_LANES || !produced || !h->inflight.empty())
-        return clip_impl(h, nullptr, frames, 0, 0, channels, 0, p, nullptr, 0, produced);   // the clip's argument errors; identity
+    mc_status st = check_clip(h, frames, produced);
+    if (st != MC_OK) return st;
+    if (empty) return clip_impl(h, nullptr, frames, 0, 0, channels, 0, p, nullptr, 0, produced);   // the identity
     const size_t lanes = (size_t)h->lanes, vl = (size_t)frames * lanes;
-    mc_status st;
     if (nv) {
         if ((st = check_nv12(h, {nv}, w, hh, (int)vl, p)) != MC_OK) return st;
     } else if (in_step < (size_t)w * channels) {
@@ -1142,33 +1094,29 @@ mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc
             a.dst = d_orig; a.dst_step = orig_step;
         } else if (g.pre && !g.gray) {   // the preprocessed frames are the magnifier's input
             a.dst_step = (size_t)g.dw * channels;
-            if ((st = grow(h, &h->f_pre, &h->f_pre_b, a.dst_step * g.dh * vl)) != MC_OK) return st;
-            a.dst = h->f_pre;
+            CK(h->f_pre.grow(a.dst_step * g.dh * vl));
+            a.dst = h->f_pre.p;
         }
         a.dst_lane_stride = a.dst_step * g.dh;
         if (g.gray) {
-            if ((st = grow(h, &h->f_gray, &h->f_gray_b, (size_t)g.dw * g.dh * vl)) != MC_OK) return st;
-            a.gray = h->f_gray;
+            CK(h->f_gray.grow((size_t)g.dw * g.dh * vl));
+            a.gray = h->f_gray.p;
         }
         if (g.kind == FRONT_AREA && (st = area_tables(h, g, a)) != MC_OK) return st;
         if (std::any_of(h->hold.begin(), h->hold.end(), [](uint8_t x) { return x != 0; })) {
             h->f_flags_host.resize(vl);   // lives on the handle: the copy is asynchronous
             for (size_t v = 0; v < vl; ++v) h->f_flags_host[v] = !h->hold[v % lanes];
-            if ((st = grow(h, &h->f_flags, &h->f_flags_b, vl)) != MC_OK) return st;
-            CK(cudaMemcpyAsync(h->f_flags, h->f_flags_host.data(), vl, cudaMemcpyHostToDevice, h->stream));
-            a.flags = h->f_flags;
+            CK(h->f_flags.grow(vl));
+            CK(cudaMemcpyAsync(h->f_flags.p, h->f_flags_host.data(), vl, cudaMemcpyHostToDevice, h->stream));
+            a.flags = h->f_flags.p;
         }
         const int src = nv ? FRONT_NV12 : channels == 3 ? FRONT_BGR : FRONT_GRAY;
-        const bool prof = h->profile && h->prof.begin("chain_front", 0, h->stream);
-        const cudaError_t e = launch_chain_front(a, src, (int)vl, h->stream);
-        if (prof) h->prof.end(h->stream);
-        CK(e);
-        ++h->launches;
+        if ((st = launch_counted(h, "chain_front", [&] { return launch_chain_front(a, src, (int)vl, h->stream); })) != MC_OK) return st;
         mag_in = g.gray ? a.gray : a.dst;
         mag_step = g.gray ? (size_t)g.dw : a.dst_step;
     } else if (nv && p->mode != MC_MODE_NONE) {   // a plain NV12 -> BGR conversion
         if ((st = nv12_ingest(h, *nv, w, hh, (int)vl, p, false)) != MC_OK) return st;
-        mag_in = h->n_in;
+        mag_in = h->n_in.p;
         mag_step = bgr_step_of(w);
     }
 
@@ -1232,28 +1180,27 @@ extern "C" mc_status mc_chain_process(mc_handle* h, const uint8_t* in, int width
     }
     const size_t row = have ? (size_t)width * channels : 0, out_frame = (size_t)g.dw * g.dh * g.cc;
     const size_t orig_frame = (size_t)g.dw * g.dh * channels;
-    mc_status st;
     if (have) {
         if (in_step < row) { h->err = "step too small"; return MC_ERR_INVALID; }
-        if ((st = grow(h, &h->c_raw, &h->c_raw_b, row * height)) != MC_OK) return st;
-        if ((st = grow(h, &h->c_out, &h->c_out_b, out_frame)) != MC_OK) return st;
-        if (g.pre && (st = grow(h, &h->c_orig, &h->c_orig_b, orig_frame)) != MC_OK) return st;
-        CK(cudaMemcpy2DAsync(h->c_raw, row, in, in_step, row, (size_t)height, cudaMemcpyHostToDevice, h->stream));
+        CK(h->c_raw.grow(row * height));
+        CK(h->c_out.grow(out_frame));
+        if (g.pre) CK(h->c_orig.grow(orig_frame));
+        CK(cudaMemcpy2DAsync(h->c_raw.p, row, in, in_step, row, (size_t)height, cudaMemcpyHostToDevice, h->stream));
     }
     uint8_t produced = 0;
-    st = chain_impl(h, have ? h->c_raw : nullptr, row, nullptr, 1, width, height, channels, p, grayscale, h->c_out,
-                    (size_t)g.dw * g.cc, g.pre ? h->c_orig : nullptr, (size_t)g.dw * channels, &produced, info);
+    const mc_status st = chain_impl(h, have ? h->c_raw.p : nullptr, row, nullptr, 1, width, height, channels, p, grayscale, h->c_out.p,
+                                    (size_t)g.dw * g.cc, g.pre ? h->c_orig.p : nullptr, (size_t)g.dw * channels, &produced, info);
     if (st != MC_OK || !have) return st;
     if (produced && info->cur_is_input) {   // no front stage: the magnified frame is the chain's result
         info->cur_is_input = 0; info->out_w = g.dw; info->out_h = g.dh; info->out_channels = g.cc;
     }
     if (!info->orig_is_input && original) {
         if (original_bytes < orig_frame) { h->err = "original buffer too small"; return MC_ERR_INVALID; }
-        CK(cudaMemcpyAsync(original, h->c_orig, orig_frame, cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaMemcpyAsync(original, h->c_orig.p, orig_frame, cudaMemcpyDeviceToHost, h->stream));
     }
     if (!info->cur_is_input && out) {
         if (out_bytes < out_frame) { h->err = "out buffer too small"; return MC_ERR_INVALID; }
-        CK(cudaMemcpyAsync(out, h->c_out, out_frame, cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaMemcpyAsync(out, h->c_out.p, out_frame, cudaMemcpyDeviceToHost, h->stream));
     }
     CK(cudaStreamSynchronize(h->stream));
     return MC_OK;

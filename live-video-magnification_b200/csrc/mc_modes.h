@@ -27,24 +27,32 @@ struct Profiler {
     void end(cudaStream_t s) { cudaEventRecord(recs.back().b, s); }
 };
 
+// The handle's options (mc_set_option; each field is named as its key).
+struct Options {
+    bool faithful_level0 = false;
+    bool keep_float_output = false;   // keep the pre-quantisation tap of the last frame (mc_get_float_output)
+    bool profile_kernels = false;     // bracket every launch with events (mc_profile_read)
+    bool use_tma = true;          // stage level-kernel tiles with cp.async.bulk.tensor
+    bool prefetch_state = true;   // level kernel requests its state tiles by TMA at kernel entry
+    int egress_strip = 16;        // Laplace egress as the register/shuffle strip kernel (0 = tile kernel, 16 / 20 / 24 = strip
+                                  // kernel compiled for that many resident warps per SM)
+    int ingest_warps = 1;         // warps per CTA of the fused ingest kernel (1, 2 or 4)
+    bool band_from_state = true;  // synthesis rebuilds gain*(hi-lo) from the state planes instead of reading a stored band
+                                  // (with prefetch_state level[1] 205 -> 177 us, egress +8 us)
+    int lane_groups = 0;          // Laplace: number of lane groups run as concurrent launch chains (0 = automatic)
+    bool analysis_only = false;   // Laplace / Phase: update the temporal state but skip synthesis + egress (*produced = 0); used
+                                  // by the state-carry pass of temporal sharding (SURVEY 8f-3, lvm_b200.shard.magnify_segment)
+    bool color_lane_lifecycle = false;   // a multi-lane Color handle accepts holds and single-lane restarts
+};
+
 struct ModeCtx {
     cudaStream_t stream;
     const DeviceTables* tables;
     uint64_t* launches;
     std::string* err;
-    bool faithful0;
+    Options opt;       // the handle's, with one lane group while kernels are profiled
     float* float_out;  // optional [lanes][h][w][C] pre-quantisation tap
     Profiler* prof;    // optional
-    bool use_tma;      // stage level-kernel tiles with cp.async.bulk.tensor (option "use_tma", default on)
-    bool prefetch_state;    // level kernel requests its state tiles by TMA at kernel entry (option "prefetch_state", default on)
-    int egress_strip;       // Laplace egress as the register/shuffle strip kernel (option "egress_strip": 0 = tile kernel,
-                            // 16 / 20 / 24 = strip kernel compiled for that many resident warps per SM)
-    int ingest_warps;       // warps per CTA of the fused ingest kernel (option "ingest_warps": 1, 2 or 4)
-    bool band_from_state;   // synthesis rebuilds gain*(hi-lo) from the state planes instead of reading a stored band
-                            // (option "band_from_state", default on: with prefetch_state level[1] 205 -> 177 us, egress +8 us)
-    int lane_groups;        // Laplace: number of lane groups run as concurrent launch chains (option "lane_groups"; 0 = automatic)
-    bool analysis_only;     // Laplace / Phase: update the temporal state but skip synthesis + egress (*produced = 0); used by the
-                            // state-carry pass of temporal sharding (SURVEY 8f-3, lvm_b200.shard.magnify_segment)
     // Lane lifecycle (mc_restart_lane / mc_hold_lane): the handle's LaneOp per lane for this frame, the device buffer the
     // mode uploads its per-lane ops to (stream-ordered: the previous frame's kernels have read it before the copy runs),
     // and the mode's answers: which lanes produced, and whether held lanes lost their state (reallocation, Phase cutoff change).
@@ -189,7 +197,7 @@ struct MotionMode {
     bool allocated = false;
     int levels = 0, channels = 0, w = 0, h = 0;
     bool faithful = false;
-    bool from_state = false;   // ModeCtx::band_from_state at allocation time
+    bool from_state = false;   // Options::band_from_state at allocation time
     std::vector<Level> lv;              // 0..levels
     std::vector<float*> G, hi, lo, M;   // per level (null where not kept)
     int16_t* lab16 = nullptr;           // Lab planes of the current frame (C == 3)
@@ -215,7 +223,7 @@ struct MotionMode {
     };
     std::vector<Group> groups;
     cudaEvent_t ev_fork = nullptr;
-    int groups_req = 0;                    // ModeCtx::lane_groups at allocation time
+    int groups_req = 0;                    // Options::lane_groups at allocation time
     std::vector<float> gains;              // per-level gains of the current frame (member: no per-frame allocation)
     LanePlan plan;                         // per-lane ops of the current frame
 

@@ -84,7 +84,7 @@ mc_status MotionMode::make_groups(const ModeCtx& ctx) {
     // lane groups: automatic = two chains once each has >= 8 streams.  The stages contend for the same L1 data pipe,
     // so co-residency buys little beyond filling each other's tails.
     drop_groups();
-    groups_req = ctx.lane_groups;
+    groups_req = ctx.opt.lane_groups;
     int ng = groups_req > 0 ? groups_req : std::min(2, lanes / 8);
     ng = std::max(1, std::min(ng, lanes));
     groups.assign((size_t)ng, Group{});
@@ -117,8 +117,8 @@ mc_status MotionMode::make_groups(const ModeCtx& ctx) {
 mc_status MotionMode::allocate(const ModeCtx& ctx, const FrameIO& io, int nlevels) {
     reset();
     levels = nlevels; channels = io.channels; w = io.w; h = io.h;
-    faithful = ctx.faithful0;
-    from_state = ctx.band_from_state;
+    faithful = ctx.opt.faithful_level0;
+    from_state = ctx.opt.band_from_state;
     const size_t planes = (size_t)lanes * channels;
     lv.resize((size_t)levels + 1);
     int cw = w, ch = h;
@@ -158,11 +158,11 @@ mc_status MotionMode::allocate(const ModeCtx& ctx, const FrameIO& io, int nlevel
 
 mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_params& p, int nlevels, int* produced, int frames) {
     *produced = 0;
-    if (!allocated || faithful != ctx.faithful0 || from_state != ctx.band_from_state) {
+    if (!allocated || faithful != ctx.opt.faithful_level0 || from_state != ctx.opt.band_from_state) {
         if (allocated) *ctx.held_lost = true;
         mc_status st = allocate(ctx, io_in, nlevels);
         if (st != MC_OK) return st;
-    } else if (groups_req != ctx.lane_groups) {
+    } else if (groups_req != ctx.opt.lane_groups) {
         mc_status st = make_groups(ctx);
         if (st != MC_OK) return st;
     }
@@ -206,7 +206,7 @@ mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc
     lab16_frame = frames == 1 && lab16;
     // state-carry pass (analysis_only): the temporal state is up to date, only first frames are produced; a clip's later
     // frames run for the lanes that are not held
-    plan.produced(ctx, !ctx.analysis_only || first, true, produced, frames, !ctx.analysis_only);
+    plan.produced(ctx, !ctx.opt.analysis_only || first, true, produced, frames, !ctx.opt.analysis_only);
     return MC_OK;
 }
 
@@ -220,7 +220,7 @@ bool MotionMode::fused_ingest() const { return channels == 3 && !faithful && lev
 int MotionMode::first_level() const { return fused_ingest() ? 1 : ((levels >= 2 || faithful) ? 0 : levels); }
 
 mc_status MotionMode::ingest(const ModeCtx& ctx, const FrameIO& io, int16_t* lab, float* g1) {
-    if (fused_ingest()) LAUNCH("ingest_lab", 0, launch_ingest_lab(io, *ctx.tables, lab, pitch16, plane16, g1, lv[1], ctx.stream, ctx.ingest_warps));
+    if (fused_ingest()) LAUNCH("ingest_lab", 0, launch_ingest_lab(io, *ctx.tables, lab, pitch16, plane16, g1, lv[1], ctx.stream, ctx.opt.ingest_warps));
     else if (channels == 3) LAUNCH("lab16", 0, launch_lab16(io, *ctx.tables, lab, pitch16, plane16, ctx.stream));
     return MC_OK;
 }
@@ -272,7 +272,7 @@ mc_status MotionMode::copy_residual(const ModeCtx& ctx, const float* g_res, int 
 mc_status MotionMode::egress_first_frames(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, const int16_t* lab, float* fout, bool first) {
     if (first || plan.n_first > 0)
         LAUNCH("egress", 0, launch_egress(io, *ctx.tables, lab, pitch16, plane16, BandSrc{}, lv[levels >= 1 ? 1 : 0], BandSrc{},
-                                          lv[levels >= 2 ? 2 : 0], (float)p.chromAttenuation, fout, ctx.stream, ctx.egress_strip, !first));
+                                          lv[levels >= 2 ? 2 : 0], (float)p.chromAttenuation, fout, ctx.stream, ctx.opt.egress_strip, !first));
     return MC_OK;
 }
 
@@ -282,7 +282,7 @@ mc_status MotionMode::egress_first_frames(const ModeCtx& ctx, const FrameIO& io,
 // bands (|band| <= 256), so |m_l| <= 512 * 2^64 and the collapse sums stay far below FLT_MAX.  The strip egress alone has
 // an L-only form; the tile egress always synthesises every channel.
 bool MotionMode::luma_only(const ModeCtx& ctx, const mc_params& p) const {
-    if (channels != 3 || !ctx.egress_strip || !ab_bounded) return false;
+    if (channels != 3 || !ctx.opt.egress_strip || !ab_bounded) return false;
     if ((float)p.chromAttenuation * (1.0f / 64.0f) != 0.0f) return false;   // the egress's chroma64, as the device forms it
     for (float g : gains)
         if (!(std::fabs(g) <= 0x1p64f)) return false;
@@ -307,7 +307,7 @@ mc_status MotionMode::synthesize(const ModeCtx& ctx, const FrameIO& io, const mc
         if (levels >= 3) c2 = cur(2);
     }
     LAUNCH("egress", 0, launch_egress(io, *ctx.tables, lab, pitch16, plane16, m1, lv[levels >= 1 ? 1 : 0], c2, lv[levels >= 2 ? 2 : 0],
-                                      (float)p.chromAttenuation, fout, ctx.stream, ctx.egress_strip, false, luma));
+                                      (float)p.chromAttenuation, fout, ctx.stream, ctx.opt.egress_strip, false, luma));
     return MC_OK;
 }
 
@@ -327,9 +327,9 @@ mc_status MotionMode::run_group(const ModeCtx& ctx, const FrameIO& io_all, const
     MCK_ST(ingest(ctx, io, lab, off(G[1], 1)));
     for (int l = first_level(); l < levels; ++l) {
         LevelArgs a = level_args(l, G, p0, lab, io, first, c_lo, c_hi);
-        if (l >= 1 && g.tmap_valid[(size_t)l] && ctx.use_tma) {
+        if (l >= 1 && g.tmap_valid[(size_t)l] && ctx.opt.use_tma) {
             a.tmap = &g.tmaps[(size_t)l];
-            if (ctx.prefetch_state) { a.tmap_hi = &g.tmaps_hi[(size_t)l]; a.tmap_lo = &g.tmaps_lo[(size_t)l]; }
+            if (ctx.opt.prefetch_state) { a.tmap_hi = &g.tmaps_hi[(size_t)l]; a.tmap_lo = &g.tmaps_lo[(size_t)l]; }
         }
         a.m = (first || from_state) ? nullptr : off(M[(size_t)l], l);
         a.m_luma = luma;
@@ -339,7 +339,7 @@ mc_status MotionMode::run_group(const ModeCtx& ctx, const FrameIO& io_all, const
         else LAUNCH("down", l, launch_down(a, ctx.stream));
     }
     MCK_ST(copy_residual(ctx, G[(size_t)levels], g.lane0, g.lanes));
-    if (ctx.analysis_only) return egress_first_frames(ctx, io, p, lab, fout, first);
+    if (ctx.opt.analysis_only) return egress_first_frames(ctx, io, p, lab, fout, first);
     auto band = [&](int l) {
         return from_state ? BandSrc{off(hi[(size_t)l], l), off(lo[(size_t)l], l), gains[(size_t)l]} : BandSrc{off(M[(size_t)l], l), nullptr, 1.0f};
     };
@@ -373,8 +373,8 @@ mc_status MotionMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_
     MCK_ST(ingest(ctx, io, clip.lab16, clip.G[1]));
     for (int l = first_level(); l < levels; ++l) {
         LevelArgs a = level_args(l, clip.G, 0, clip.lab16, io, first, c_lo, c_hi);
-        if (l >= 1 && clip.tmap_valid[(size_t)l] && ctx.use_tma) a.tmap = &clip.tmaps[(size_t)l];
-        a.m = ctx.analysis_only ? nullptr : clip.M[(size_t)l];
+        if (l >= 1 && clip.tmap_valid[(size_t)l] && ctx.opt.use_tma) a.tmap = &clip.tmaps[(size_t)l];
+        a.m = ctx.opt.analysis_only ? nullptr : clip.M[(size_t)l];
         a.m_luma = luma;
         if (a.band) {
             a.planes = lanes * channels; a.ops = io0.ops;   // state planes, per-lane ops of the clip's first frame
@@ -387,7 +387,7 @@ mc_status MotionMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_
     MCK_ST(copy_residual(ctx, clip.G[(size_t)levels], 0, lanes));   // frame 0 is the first `lanes` virtual lanes
     // state-carry pass: only the clip's first frame can produce; it is frame 0's egress of a frame call, so the float
     // tap is written in place
-    if (ctx.analysis_only) return egress_first_frames(ctx, io0, p, clip.lab16, ctx.float_out, first);
+    if (ctx.opt.analysis_only) return egress_first_frames(ctx, io0, p, clip.lab16, ctx.float_out, first);
     MCK_ST(synthesize(ctx, io, p, clip.lab16, ctx.float_out ? clip.fout : nullptr, true, luma,
                       [&](int l) { return BandSrc{clip.M[(size_t)l], nullptr, 1.0f}; }, [&](int l) { return clip.M[(size_t)l]; }));
     return clip.copy_last_tap(ctx, plan, frames, (size_t)w * h * channels);

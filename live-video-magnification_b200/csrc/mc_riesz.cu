@@ -699,7 +699,7 @@ mc_status RieszMode::build_pyramid(const ModeCtx& ctx, const FrameIO& io, int16_
     for (int i = 0; i < levels - 1; ++i) {
         const Level& l = lv[(size_t)i];
         dim3 grid(cdiv(l.w, R9_W), cdiv(l.h, R9_H), io.lanes);
-        const int tma = ctx.use_tma && valid[(size_t)i];
+        const int tma = ctx.opt.use_tma && valid[(size_t)i];
         KLAUNCH("riesz_analysis", i, k_riesz_analysis<<<grid, 256, 0, ctx.stream>>>(l, lv[(size_t)i + 1], octs[(size_t)i], bands[(size_t)i], octs[(size_t)i + 1],
                                                                                     *reinterpret_cast<const CUtensorMap*>(&tm[(size_t)i]), tma, io.ops));
     }
@@ -733,7 +733,7 @@ mc_status RieszMode::collapse_egress(const ModeCtx& ctx, const FrameIO& io, cons
     for (int i = levels - 2; i >= 0; --i) {
         const Level& l = lv[(size_t)i];
         dim3 grid(cdiv(l.w, R9_W), cdiv(l.h, R9_H), io.lanes);
-        const int tma = ctx.use_tma && valid[(size_t)i];
+        const int tma = ctx.opt.use_tma && valid[(size_t)i];
         KLAUNCH("riesz_collapse", i, k_riesz_collapse<<<grid, 256, 0, ctx.stream>>>(l, lv[(size_t)i + 1], bands[(size_t)i], result, out[(size_t)i],
                                                                                     *reinterpret_cast<const CUtensorMap*>(&tm[(size_t)i]), tma, io.ops));
         result = out[(size_t)i];
@@ -878,7 +878,7 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_
         std::swap(cur_rx[(size_t)i], old_rx[(size_t)i]);
         std::swap(cur_ry[(size_t)i], old_ry[(size_t)i]);
     }
-    if (ctx.analysis_only) {   // state-carry pass of temporal sharding: pyramids and filter registers are up to date
+    if (ctx.opt.analysis_only) {   // state-carry pass of temporal sharding: pyramids and filter registers are up to date
         *produced = 0;
         return MC_OK;
     }
@@ -958,11 +958,11 @@ mc_status RieszMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_p
         PhaseClipArgs a;
         a.l = lv[(size_t)i];
         a.band = clip.band[(size_t)i];
-        a.rx = ctx.analysis_only ? nullptr : clip.rx[(size_t)i];
-        a.ry = ctx.analysis_only ? nullptr : clip.ry[(size_t)i];
-        a.amp = ctx.analysis_only ? nullptr : clip.amp;
-        a.t_c = ctx.analysis_only ? nullptr : clip.t_c;
-        a.t_s = ctx.analysis_only ? nullptr : clip.t_s;
+        a.rx = ctx.opt.analysis_only ? nullptr : clip.rx[(size_t)i];
+        a.ry = ctx.opt.analysis_only ? nullptr : clip.ry[(size_t)i];
+        a.amp = ctx.opt.analysis_only ? nullptr : clip.amp;
+        a.t_c = ctx.opt.analysis_only ? nullptr : clip.t_c;
+        a.t_s = ctx.opt.analysis_only ? nullptr : clip.t_s;
         a.old_low = old_low[(size_t)i]; a.old_rx = old_rx[(size_t)i]; a.old_ry = old_ry[(size_t)i];
         a.ph_c = phase_c[(size_t)i]; a.ph_s = phase_s[(size_t)i];
         a.lo_r0c = lo_r0c[(size_t)i]; a.lo_r0s = lo_r0s[(size_t)i]; a.lo_r1c = lo_r1c[(size_t)i]; a.lo_r1s = lo_r1s[(size_t)i];
@@ -974,16 +974,16 @@ mc_status RieszMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_p
         a.ops = ops0;
         dim3 grid(cdiv(a.l.w, RT_W), cdiv(a.l.h, RT_H), lanes);
         const CUtensorMap& tm = *reinterpret_cast<const CUtensorMap*>(&clip.tm_band[(size_t)i]);
-        if (ctx.use_tma && clip.tm_valid[(size_t)i])
+        if (ctx.opt.use_tma && clip.tm_valid[(size_t)i])
             KLAUNCH("riesz_phase_clip", i, k_riesz_phase_clip<true><<<grid, 256, 0, ctx.stream>>>(a, frames, lanes, tm));
         else
             KLAUNCH("riesz_phase_clip", i, k_riesz_phase_clip<false><<<grid, 256, 0, ctx.stream>>>(a, frames, lanes, tm));
-        if (ctx.analysis_only) continue;
+        if (ctx.opt.analysis_only) continue;
         // the amplified band overwrites the Riesz pair's rx, point for point
         MCK_ST(amplify(ctx, p, i, vl, io.ops, clip.amp, clip.t_c, clip.t_s, clip.band[(size_t)i], clip.rx[(size_t)i], clip.ry[(size_t)i],
                        clip.rx[(size_t)i]));
     }
-    if (ctx.analysis_only) return MC_OK;   // state-carry pass: nothing is produced
+    if (ctx.opt.analysis_only) return MC_OK;   // state-carry pass: nothing is produced
     // level i's collapse result overwrites its band, which amplify was the last to read
     MCK_ST(collapse_egress(ctx, io, clip.lab16, clip.oct[(size_t)levels - 1], clip.rx, clip.band, clip.tm_amp, clip.tm_valid,
                            ctx.float_out ? clip.fout : nullptr));

@@ -258,12 +258,10 @@ def test_hold_survives_structural_change_and_reset():
         assert np.array_equal(out[k], sout), k
 
 
-@pytest.mark.parametrize("mode,ui,pinned", [(O.MODE_LAPLACE, LAPLACE_UI, False), (O.MODE_LAPLACE, LAPLACE_UI, True),
-                                            (O.MODE_PHASE, PHASE_UI, False)])
-def test_pipelined_restarts_and_holds_equal_blocking(mode, ui, pinned):
+def check_pipelined(mode, ui, pinned, w, h):
     """Restarts and holds are taken at submit time: three frames in flight give the blocking path's frames and flags."""
     cfg, _ = make_cfgs(mode, *ui)
-    w, h, c, lanes, n, depth = 120, 90, 3, 4, 9, 3
+    c, lanes, n, depth = 3, 4, 9, 3
     events = {1: [("hold", 3, 1)], 2: [("restart", 0)], 4: [("hold", 3, 0), ("restart", 2)],
               5: [("restart", 1), ("hold", 2, 1)], 7: [("hold", 2, 0)]}
 
@@ -311,6 +309,12 @@ def test_pipelined_restarts_and_holds_equal_blocking(mode, ui, pinned):
         b.close()
         for p in bufs:
             lib.mc_host_free(p)
+
+
+@pytest.mark.parametrize("mode,ui,pinned", [(O.MODE_LAPLACE, LAPLACE_UI, False), (O.MODE_LAPLACE, LAPLACE_UI, True),
+                                            (O.MODE_PHASE, PHASE_UI, False)])
+def test_pipelined_restarts_and_holds_equal_blocking(mode, ui, pinned):
+    check_pipelined(mode, ui, pinned, 120, 90)
 
 
 def test_color_multi_lane_refuses_and_keeps_its_window():

@@ -222,16 +222,13 @@ def _pinned(lib, shape, keep):
     return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), shape=shape)
 
 
-@pytest.mark.parametrize("mname", ["laplace", "phase"])
-@pytest.mark.parametrize("pinned", [False, True])
-@pytest.mark.parametrize("layout", ["packed", "uv_offset"])
-def test_submit_nv12_equals_device_calls(mname, pinned, layout):
+def check_submit_nv12(mname, pinned, layout, w, h):
     """Three frames in flight, restarts and holds taken at submit: mc_submit_nv12 / mc_collect give the device calls'
     planes and flags; both planes of lanes that did not produce keep the sentinel."""
     mode, ui = MODES[mname]
     cfg, _ = make_cfgs(mode, *ui)
-    w, h, lanes, n, depth = 130, 74, 4, 9, 3
-    lay = Layout(w, h) if layout == "packed" else Layout(w, h, pitch=136, uv_row=h + 6)
+    lanes, n, depth = 4, 9, 3
+    lay = Layout(w, h) if layout == "packed" else Layout(w, h, pitch=w + 6, uv_row=h + 6)
     events = {1: [("hold", 3, 1)], 2: [("restart", 0)], 4: [("hold", 3, 0), ("restart", 2)],
               5: [("restart", 1), ("hold", 2, 1)], 7: [("hold", 2, 0)]}
 
@@ -278,6 +275,13 @@ def test_submit_nv12_equals_device_calls(mname, pinned, layout):
         sub.close()
         for p in keep:
             lib.mc_host_free(p)
+
+
+@pytest.mark.parametrize("mname", ["laplace", "phase"])
+@pytest.mark.parametrize("pinned", [False, True])
+@pytest.mark.parametrize("layout", ["packed", "uv_offset"])
+def test_submit_nv12_equals_device_calls(mname, pinned, layout):
+    check_submit_nv12(mname, pinned, layout, 130, 74)
 
 
 def test_bad_arguments_leave_state_untouched():
