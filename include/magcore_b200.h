@@ -376,7 +376,16 @@ mc_status mc_set_option(mc_handle* h, const char* key, int value);
  *   "phase.c", "phase.s" (itsPhase — the two filters' copies are identical), "lo.r0.c", "lo.r0.s", "lo.r1.c",
  *   "lo.r1.s", "hi.r0.c", "hi.r0.s", "hi.r1.c", "hi.r1.s" (itsRegister0/1 of the low / high cutoff filters,
  *   TemporalFilter.cpp:299-317);
- * Color keeps its rolling window in a device ring buffer that is not exposed.
+ * Color, read-only (mc_set_state returns MC_ERR_INVALID), the buffers of the last frame call, `channels` channels:
+ *   "gauss", level 0..levels: the Gaussian pyramid (level 0 is the u8 frame as f32);
+ *   "window", level k = logical column 0..n-1 of the rolling window (column 0 the oldest), each lane's own ring slot,
+ *   as rows x cols of the smallest pyramid level;
+ *   "filtered", level k: the same column after the inverse DFT, before normalisation (both DFT scales applied);
+ *   "up", level 0..levels (+1 when the bilinear resize ran): level 0 is the normalised reconstructed column times the
+ *   amplification, the last level the colour image that is added to the input.
+ *   Lanes of one handle may have windows of different length: a column is served only while every lane has it, and
+ *   "filtered" / "up" only while every lane ran the filter in the last frame call that was not held for all lanes
+ *   (otherwise 0 rows).  All are absent before the first frame and after mc_reset or a change of mode or geometry.
  * Laplace and Phase, level 0, three channels, read-only: "lab16", the BGR->Lab conversion of the last frame call as
  *   the kernels hold it, the raw fixed-point values L*2^14/100, (a+128)*64, (b+128)*64 widened (exactly) to f32.  It
  *   exists only after a frame call on 3-channel input; before the first frame, after mc_reset and after a clip call it

@@ -628,6 +628,38 @@ mc_status ColorMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_par
     return MC_OK;
 }
 
-void ColorMode::find_state(const char*, int, StateRef& out) { out = StateRef{}; }
+// Read-only taps on the buffers of the last frame call (include/magcore_b200.h, at mc_get_state).  A column of "window" or
+// "filtered" is served only while every lane has it, "filtered" and "up" only while every lane ran the filter.
+void ColorMode::find_state(const char* name, int level, StateRef& out) {
+    out = StateRef{};
+    if (!allocated || level < 0) return;
+    int have = count[0], filt = table[0].n;   // columns every lane has / every lane filtered
+    for (int k = 1; k < lanes; ++k) {
+        have = std::min(have, count[(size_t)k]);
+        filt = std::min(filt, table[(size_t)k].n);
+    }
+    const std::string nm(name);
+    out.channels = channels; out.read_only = true;
+    auto planes_of = [&](float* p, const Level& l) {
+        out.ptr = p; out.rows = l.h; out.cols = l.w; out.pitch = l.pitch; out.plane_stride = l.plane;
+    };
+    if (nm == "gauss") {
+        if (level <= levels && *std::max_element(count.begin(), count.end()) > 0) planes_of(G[(size_t)level], lv[(size_t)level]);
+    } else if (nm == "up") {
+        if (filt >= 2 && level <= levels) planes_of(U[(size_t)level], ulv[(size_t)level]);
+        else if (filt >= 2 && level == levels + 1 && U[(size_t)level]) planes_of(U[(size_t)level], lv[0]);
+    } else if (nm == "window" || nm == "filtered") {
+        const bool win = nm == "window";
+        if (level >= (win ? have : filt)) return;
+        // a slot holds every lane's block of channels * pixels tightly packed signals, odd blocks of a multi-lane handle
+        // followed by one padding float (process()); logical column `level` of a lane is its slot (head + level) % mod
+        const Level& ls = lv[(size_t)levels];
+        const size_t lane_sig = (size_t)channels * small_rows, lstride = lane_sig + (lanes > 1 ? (lane_sig & 1) : 0);
+        out.ptr = win ? ring : work;
+        out.rows = ls.h; out.cols = ls.w; out.pitch = ls.w; out.plane_stride = (size_t)small_rows;
+        for (int k = 0; k < lanes; ++k)
+            out.lane_off.push_back((size_t)((head[(size_t)k] + level) % mod[(size_t)k]) * lanes * lstride + (size_t)k * lstride);
+    }
+}
 
 }  // namespace mc

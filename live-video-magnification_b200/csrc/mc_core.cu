@@ -713,7 +713,7 @@ static mc_status state_xfer(mc_handle* h, const char* name, int level, float* ho
     else if (h->t_mode == MC_MODE_COLOR) h->color.find_state(name, level, r);
     else if (h->t_mode == MC_MODE_PHASE) h->riesz.find_state(name, level, r);
     if (!r.found()) { h->err = std::string("no such state: ") + name; return MC_ERR_INVALID; }
-    if (r.ptr16 && !get) { h->err = std::string("read-only state: ") + name; return MC_ERR_INVALID; }
+    if ((r.ptr16 || r.read_only) && !get) { h->err = std::string("read-only state: ") + name; return MC_ERR_INVALID; }
     const size_t planes = (size_t)h->lanes * r.channels;
     if (n < planes * r.rows * r.cols) { h->err = "state buffer too small"; return MC_ERR_INVALID; }
     CK(cudaStreamSynchronize(h->stream));
@@ -730,7 +730,9 @@ static mc_status state_xfer(mc_handle* h, const char* name, int level, float* ho
         return MC_OK;
     }
     for (size_t pl = 0; pl < planes; ++pl) {
-        float* d = r.ptr + pl * r.plane_stride;
+        const size_t lane = pl / (size_t)r.channels;
+        float* d = r.lane_off.empty() ? r.ptr + pl * r.plane_stride
+                                      : r.ptr + r.lane_off[lane] + (pl - lane * (size_t)r.channels) * r.plane_stride;
         float* hp = host + pl * (size_t)r.rows * r.cols;
         if (get) CK(cudaMemcpy2D(hp, (size_t)r.cols * 4, d, (size_t)r.pitch * 4, (size_t)r.cols * 4, r.rows, cudaMemcpyDeviceToHost));
         else CK(cudaMemcpy2D(d, (size_t)r.pitch * 4, hp, (size_t)r.cols * 4, (size_t)r.cols * 4, r.rows, cudaMemcpyHostToDevice));

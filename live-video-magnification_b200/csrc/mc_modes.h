@@ -129,6 +129,10 @@ struct StateRef {  // a named state plane set for mc_get_state / mc_set_state
     const int16_t* ptr16 = nullptr;   // read-only int16 planes ("lab16"), widened to f32 on download
     int rows = 0, cols = 0, channels = 0, pitch = 0;
     size_t plane_stride = 0;
+    // floats from `ptr` to each lane's first plane, where the lanes are not channels * plane_stride apart (Color: the
+    // pad float of odd lane blocks, and a ring slot of each lane's own); empty: lane * channels * plane_stride
+    std::vector<size_t> lane_off;
+    bool read_only = false;           // a tap of scratch the kernels overwrite every frame: mc_set_state refuses it
     bool found() const { return ptr || ptr16; }
 };
 
