@@ -376,6 +376,16 @@ mc_status mc_set_option(mc_handle* h, const char* key, int value);
  *   "phase.c", "phase.s" (itsPhase — the two filters' copies are identical), "lo.r0.c", "lo.r0.s", "lo.r1.c",
  *   "lo.r1.s", "hi.r0.c", "hi.r0.s", "hi.r1.c", "hi.r1.s" (itsRegister0/1 of the low / high cutoff filters,
  *   TemporalFilter.cpp:299-317);
+ * Phase, read-only (mc_set_state returns MC_ERR_INVALID), the buffers of the last frame call, one channel:
+ *   "oct", level 0..levels-1: octave i of the analysis (level 0 the f32 L plane, level levels-1 the residual the collapse
+ *   starts from); "amp", "t_c", "t_s", band level 0..levels-2: the phase kernel's amplitude and (hiIIR - loIIR) *
+ *   amplitude; "amplified", band level 0..levels-2: the amplified band; "collapsed", band level 0..levels-2: the
+ *   collapse result of that level (level 0 is the L' the egress merges with a, b).  They follow "lab16": they exist only
+ *   after a frame call on 3-channel input, and are absent before the first frame, after mc_reset, after a clip call and
+ *   after a change of mode or geometry.  "amp" / "t_c" / "t_s" exist only when some lane ran the phase kernel (not on a
+ *   frame where every lane is on its first frame or held), "amplified" / "collapsed" only when the frame was amplified
+ *   (not under analysis_only).  A lane that did not run (first frame, held) keeps in them what an earlier frame left;
+ *   a held lane also keeps its "oct".
  * Color, read-only (mc_set_state returns MC_ERR_INVALID), the buffers of the last frame call, `channels` channels:
  *   "gauss", level 0..levels: the Gaussian pyramid (level 0 is the u8 frame as f32);
  *   "window", level k = logical column 0..n-1 of the rolling window (column 0 the oldest), each lane's own ring slot,

@@ -332,6 +332,10 @@ struct RieszMode {
     int pitch16 = 0;
     size_t plane16 = 0;
     bool lab16_frame = false;   // lab16 holds the last frame call's Lab (clips write their own scratch)
+    // How far the last frame call got, for the read-only taps (valid while lab16_frame): the octaves; + the phase kernel's
+    // amp / t_c / t_s (some lane ran it); + the amplified band and the collapse (amplify ran)
+    enum { TAPS_OCT = 1, TAPS_PHASE = 2, TAPS_SYNTH = 3 };
+    int frame_taps = 0;
     // TMA descriptors of the 9x9 kernels' input tiles (72 x 24 boxes): octave i (analysis), amplified band i (collapse)
     std::vector<TensorMapStorage> tm_oct, tm_band;
     std::vector<char> tm_valid;

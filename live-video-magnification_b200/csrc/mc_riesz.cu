@@ -61,6 +61,11 @@ __device__ __forceinline__ float f2d(float c, float v, float acc, bool tail) {
     return tail ? __fadd_rn(acc, __fmul_rn(c, v)) : fmaf(c, v, acc);
 }
 
+// filter2D also leaves out the kernel's zero coefficients: the four 0.0000 corner taps of c_hp take no part.  With
+// finite input that changes no bit; a NaN of the amplified band (blurred amplitude 0, where L is 0) then reaches the
+// 77 outputs it reaches in the reference, not 81.  The 9x9 loops are unrolled, so this is a compile-time test.
+__device__ __forceinline__ constexpr bool hp_tap(int ky, int kx) { return !((ky == 0 || ky == 8) && (kx == 0 || kx == 8)); }
+
 // 9x9 kernels are register-blocked: a thread owns a 1x4 strip, loads 12 tile values per kernel row with three
 // 128-bit shared-memory reads and issues 36 FMAs on them.  Rows are dealt to warps so that both rows of a
 // warp have the same parity (the sub-sampled low-pass / the zero-injected up-sampling only touch one parity),
@@ -131,6 +136,7 @@ __global__ void __launch_bounds__(256) k_riesz_analysis(Level l, Level ln, const
             const float v[12] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w, a2.x, a2.y, a2.z, a2.w};
 #pragma unroll
             for (int kx = 0; kx < 9; ++kx) {
+                if (!hp_tap(ky, kx)) continue;
                 const float c = c_hp[ky * 9 + kx];
 #pragma unroll
                 for (int p = 0; p < 4; ++p) acc[p] = fmaf(c, v[p + kx], acc[p]);
@@ -153,6 +159,7 @@ __global__ void __launch_bounds__(256) k_riesz_analysis(Level l, Level ln, const
             const float v[12] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w, a2.x, a2.y, a2.z, a2.w};
 #pragma unroll
             for (int kx = 0; kx < 9; ++kx) {
+                if (!hp_tap(ky, kx)) continue;
                 const float c = c_hp[ky * 9 + kx];
 #pragma unroll
                 for (int p = 0; p < 4; ++p) acc[p] = f2d(c, v[p + kx], acc[p], p >= tail_from);
@@ -611,6 +618,7 @@ __global__ void __launch_bounds__(256) k_riesz_collapse(Level l, Level lc, const
         if (!mixed) {
 #pragma unroll
             for (int kx = 0; kx < 9; ++kx) {
+                if (!hp_tap(ky, kx)) continue;
                 const float cf = c_hp[ky * 9 + kx];
 #pragma unroll
                 for (int p = 0; p < 4; ++p) hp[p] = fmaf(cf, v[p + kx], hp[p]);
@@ -618,6 +626,7 @@ __global__ void __launch_bounds__(256) k_riesz_collapse(Level l, Level lc, const
         } else {
 #pragma unroll
             for (int kx = 0; kx < 9; ++kx) {
+                if (!hp_tap(ky, kx)) continue;
                 const float cf = c_hp[ky * 9 + kx];
 #pragma unroll
                 for (int p = 0; p < 4; ++p) hp[p] = f2d(cf, v[p + kx], hp[p], p >= tail_from);
@@ -846,6 +855,7 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_
     MCK(plan.upload(ctx, &io.ops));
     MCK_ST(build_pyramid(ctx, io, lab16, oct, cur_low, tm_oct, tm_valid));
     lab16_frame = true;
+    frame_taps = TAPS_OCT;
     if (first) {
         // old = pyramid of the first frame with a zero Riesz pair; the frame itself is shown unmagnified (:239)
         for (int i = 0; i < levels - 1; ++i) std::swap(cur_low[(size_t)i], old_low[(size_t)i]);
@@ -872,6 +882,7 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_
         dim3 grid(cdiv(a.l.w, RT_W), cdiv(a.l.h, RT_H), lanes);
         KLAUNCH("riesz_phase", i, k_riesz_phase<<<grid, 256, 0, ctx.stream>>>(a));
     }
+    if (plan.n_run > 0) frame_taps = TAPS_PHASE;
     // *old = *cur (before amplification, :267): the buffers just written become `old`
     for (int i = 0; i < nb; ++i) {
         std::swap(cur_low[(size_t)i], old_low[(size_t)i]);
@@ -888,6 +899,7 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_
         MCK_ST(amplify(ctx, p, i, lanes, io.ops, amp[(size_t)i], t_c[(size_t)i], t_s[(size_t)i], old_low[(size_t)i], old_rx[(size_t)i],
                        old_ry[(size_t)i], low_amp[(size_t)i]));
     MCK_ST(collapse_egress(ctx, io, lab16, oct[(size_t)levels - 1], low_amp, res, tm_band, tm_valid, ctx.float_out));
+    frame_taps = TAPS_SYNTH;
     plan.produced(ctx, true, false, produced);
     return MC_OK;
 }
@@ -999,7 +1011,20 @@ void RieszMode::find_state(const char* name, int level, StateRef& out) {
         if (level == 0) lab16_state(lab16, lab16_frame, w, h, pitch16, plane16, out);
         return;
     }
-    if (!allocated || level < 0 || level >= levels - 1) return;
+    if (!allocated || level < 0) return;
+    // read-only taps on the buffers of the last frame call (include/magcore_b200.h, at mc_get_state), while lab16 is current
+    struct { const char* n; std::vector<float*>* v; int stage, nlev; } taps[] = {
+        {"oct", &oct, TAPS_OCT, levels}, {"amp", &amp, TAPS_PHASE, levels - 1}, {"t_c", &t_c, TAPS_PHASE, levels - 1},
+        {"t_s", &t_s, TAPS_PHASE, levels - 1}, {"amplified", &low_amp, TAPS_SYNTH, levels - 1}, {"collapsed", &res, TAPS_SYNTH, levels - 1}};
+    for (auto& t : taps)
+        if (!std::strcmp(name, t.n)) {
+            if (!lab16_frame || frame_taps < t.stage || level >= t.nlev) return;
+            const Level& l = lv[(size_t)level];
+            out.ptr = (*t.v)[(size_t)level]; out.rows = l.h; out.cols = l.w; out.channels = 1; out.pitch = l.pitch; out.plane_stride = l.plane;
+            out.read_only = true;
+            return;
+        }
+    if (level >= levels - 1) return;
     struct { const char* n; std::vector<float*>* v; } map[] = {
         {"old.lowpass", &old_low}, {"old.rx", &old_rx}, {"old.ry", &old_ry}, {"phase.c", &phase_c}, {"phase.s", &phase_s},
         {"lo.r0.c", &lo_r0c}, {"lo.r0.s", &lo_r0s}, {"lo.r1.c", &lo_r1c}, {"lo.r1.s", &lo_r1s},
