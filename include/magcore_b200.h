@@ -328,6 +328,51 @@ mc_status mc_chain_compose_nv12_device(mc_handle* h, const mc_nv12* in, int fram
                                        const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
                                        uint8_t* produced, mc_chain_info* info);
 
+/* --- packed 4:2:2 camera frames (V4L2 YUYV / UYVY) into the processing chain ---------------------------------------
+ * A YUYV frame is height rows of width / 2 groups of 4 bytes, Y0 Cb Y1 Cr (UYVY: Cb Y0 Cr Y1); both pixels of a group
+ * take its Cb,Cr.  The core converts it exactly as OpenCV's capture does, cvtColor(COLOR_YUV2BGR_YUYV / _UYVY) (BT.601
+ * limited range, the fixed point of the NV12 conversion), pixel by pixel inside the chain's front kernel, so no
+ * full-resolution BGR frame is stored unless the caller asks for it.
+ *   Equivalence: for any input X, a call equals the BGR chain call (mc_chain_process_device / _compose_device /
+ *     mc_chain_process, channels 3) on B = cv2.cvtColor(X, COLOR_YUV2BGR_YUYV or _UYVY), bit for bit: the processed
+ *     frames, the original tap, the produced flags, mc_lane_produced and the temporal state afterwards.  YUYV, NV12 and
+ *     BGR calls of the same geometry interleave on one handle without a structural reset (the tracker sees channels 3).
+ *   The conversion is a front stage that always runs: where the BGR call would leave its result to the input
+ *     (cur_is_input / orig_is_input), the YUYV call writes it, B or its BGR2GRAY under grayscale.  `info` has
+ *     cur_is_input = orig_is_input = 0, and the geometry of the front's output (width x height without a Preprocess
+ *     stage).  d_out is written for every virtual lane that is not held, and so is d_original when it is not NULL.
+ *   Compose: the original pane is the preprocessed frame when a Preprocess stage runs, otherwise B, read straight from
+ *     the YUYV frame.
+ *   Errors: MC_ERR_INVALID, before any kernel or copy runs and with no caller buffer or state changed, for a NULL `in` or
+ *     `data`, an order out of range, width odd or < 2, height < 1, pitch < 2 * width, lane_stride < pitch * height with
+ *     more than one virtual lane, and every argument error of the matching BGR call.  Held lanes, Color's multi-lane
+ *     refusals (MC_ERR_UNSUPPORTED) and the clip rules are those of the BGR calls.
+ *   Device scratch: the front's staging holds B (width x height x 3 per virtual lane) when neither d_original nor a
+ *     gray-only magnifier input takes its place. */
+typedef enum mc_yuv422_order { MC_YUV422_YUYV = 0, MC_YUV422_UYVY = 1 } mc_yuv422_order;
+typedef struct mc_yuv422 {
+    uint8_t* data;        /* frame of (virtual) lane 0: height rows of 2 * width bytes */
+    size_t pitch;         /* bytes per row (V4L2 bytesperline), >= 2 * width */
+    size_t lane_stride;   /* bytes from one virtual lane's frame to the next */
+    int32_t order;        /* mc_yuv422_order */
+} mc_yuv422;
+
+/* device frames, every lane, clips: the layout and rules of mc_chain_process_nv12_device (frame t of lane k is virtual
+ * lane t * lanes + k, at v * lane_stride of `data`) */
+mc_status mc_chain_process_yuv422_device(mc_handle* h, const mc_yuv422* in, int frames, int width, int height,
+                                         const mc_params* p, int grayscale, uint8_t* d_out, size_t out_step,
+                                         uint8_t* d_original, size_t original_step, uint8_t* produced, mc_chain_info* info);
+/* the same followed by compose (export from a YUYV recording): the rules of mc_chain_compose_nv12_device */
+mc_status mc_chain_compose_yuv422_device(mc_handle* h, const mc_yuv422* in, int frames, int width, int height,
+                                         const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                                         uint8_t* produced, mc_chain_info* info);
+/* the live camera form: one host frame (pinned or pageable), 1-lane handle, blocking; the rules of mc_chain_process.
+ * Only the 2 * width bytes of each row cross PCIe (2 B/px against 3 for BGR).  `out` and `original` (either may be
+ * NULL) are written tight; out_bytes / original_bytes smaller than info's frames are MC_ERR_INVALID before any copy. */
+mc_status mc_chain_process_yuv422(mc_handle* h, const mc_yuv422* in, int width, int height, const mc_params* p,
+                                  int grayscale, uint8_t* out, size_t out_bytes, uint8_t* original, size_t original_bytes,
+                                  mc_chain_info* info);
+
 /* Pinned host memory for frames (so FramePool buffers can be DMA'd directly). */
 void* mc_host_alloc(size_t bytes);
 void mc_host_free(void* p);

@@ -35,6 +35,14 @@ class McNv12(C.Structure):
     _fields_ = [("y", C.c_void_p), ("uv", C.c_void_p), ("pitch", C.c_size_t), ("lane_stride", C.c_size_t)]
 
 
+MC_YUV422_YUYV, MC_YUV422_UYVY = 0, 1
+
+
+class McYuv422(C.Structure):
+    """mc_yuv422: one packed 4:2:2 frame set (YUYV / UYVY camera frames; `data` is a host or device address as an integer)."""
+    _fields_ = [("data", C.c_void_p), ("pitch", C.c_size_t), ("lane_stride", C.c_size_t), ("order", C.c_int32)]
+
+
 MC_SPLIT_NONE, MC_SPLIT_LEFT_RIGHT, MC_SPLIT_TOP_BOTTOM = 0, 1, 2
 MC_CANVAS_BGR, MC_CANVAS_NV12 = 0, 1
 
@@ -50,6 +58,7 @@ _u8p, _f32p, _vp = C.POINTER(C.c_uint8), C.POINTER(C.c_float), C.c_void_p
 _PP = C.POINTER(McParams)
 _NV = C.POINTER(McNv12)
 _CV = C.POINTER(McCanvas)
+_YV = C.POINTER(McYuv422)
 SIGNATURES = {
     "mc_abi_version": (C.c_int, []),
     "mc_device_count": (C.c_int, []),
@@ -83,6 +92,12 @@ SIGNATURES = {
                                           _u8p, C.POINTER(McChainInfo)]),
     "mc_chain_compose_nv12_device": (C.c_int, [_vp, _NV, C.c_int, C.c_int, C.c_int, _PP, C.c_int, C.c_int, _CV, _u8p,
                                                C.POINTER(McChainInfo)]),
+    "mc_chain_process_yuv422_device": (C.c_int, [_vp, _YV, C.c_int, C.c_int, C.c_int, _PP, C.c_int, _vp, C.c_size_t, _vp,
+                                                 C.c_size_t, _u8p, C.POINTER(McChainInfo)]),
+    "mc_chain_compose_yuv422_device": (C.c_int, [_vp, _YV, C.c_int, C.c_int, C.c_int, _PP, C.c_int, C.c_int, _CV, _u8p,
+                                                 C.POINTER(McChainInfo)]),
+    "mc_chain_process_yuv422": (C.c_int, [_vp, _YV, C.c_int, C.c_int, _PP, C.c_int, _vp, C.c_size_t, _vp, C.c_size_t,
+                                          C.POINTER(McChainInfo)]),
     "mc_pipeline_depth": (C.c_int, [_vp]),
     "mc_submit": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t]),
     "mc_collect": (C.c_int, [_vp, C.POINTER(C.c_int)]),

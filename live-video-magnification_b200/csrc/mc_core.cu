@@ -1076,42 +1076,62 @@ const char* check_compose(const ComposeReq& c, const ChainGeom& g, size_t vl) {
     return nullptr;
 }
 
+const char* check_yuv422(const mc_yuv422& f, int w, int hh, size_t vl) {
+    if (!f.data) return "YUYV frame is null";
+    if (f.order != MC_YUV422_YUYV && f.order != MC_YUV422_UYVY) return "YUYV order out of range";
+    if (w < 2 || (w & 1) || hh < 1) return "YUYV width must be even and >= 2, height >= 1";
+    if (f.pitch < (size_t)2 * w) return "YUYV pitch < 2 * width";
+    if (vl > 1 && f.lane_stride < f.pitch * hh) return "YUYV lane_stride < pitch * height";
+    return nullptr;
+}
+
 // runChainOnce for every lane and `frames` consecutive frames: the source is d_in (u8 BGR or gray, in_step) or, when nv
-// is not null, NV12 planes (channels 3).  Everything is checked before the front kernel runs; then one front launch
+// is not null, NV12 planes, or, when yv is not null, a packed 4:2:2 frame (both channels 3).  A 4:2:2 source's conversion
+// is a front stage that always runs: the front writes its BGR frame (d_orig, or the magnifier's input in staging) where
+// a BGR source would leave the result to the input.  Everything is checked before the front kernel runs; then one front launch
 // writes the preprocessed frames (d_original, or staging) and the magnifier's input (the same frames or their gray),
 // the magnifier writes d_out, and the frames it did not produce get the front's output.  produced: frames * lanes flags.
 // With cmp, the call composes instead: d_out / d_orig are not the caller's, the magnifier writes h->x_mag, the
 // preprocessed frames stay in h->f_pre when the canvas shows them, and one compose launch reads every pane where it is.
-mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc_nv12* nv, int frames, int w, int hh,
-                     int channels, const mc_params* p, int grayscale, uint8_t* d_out, size_t out_step, uint8_t* d_orig,
-                     size_t orig_step, uint8_t* produced, mc_chain_info* info, const ComposeReq* cmp = nullptr) {
+mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc_nv12* nv, const mc_yuv422* yv, int frames,
+                     int w, int hh, int channels, const mc_params* p, int grayscale, uint8_t* d_out, size_t out_step,
+                     uint8_t* d_orig, size_t orig_step, uint8_t* produced, mc_chain_info* info,
+                     const ComposeReq* cmp = nullptr) {
     if (!p || !info) { h->err = "params or info is null"; return MC_ERR_INVALID; }
-    const bool empty = !nv && (d_in == nullptr || w <= 0 || hh <= 0);
+    const bool empty = !nv && !yv && (d_in == nullptr || w <= 0 || hh <= 0);
     ChainGeom g;
     if (const char* e = chain_geometry(p, empty ? 0 : w, empty ? 0 : hh, channels, grayscale, g, info)) {
         h->err = e;
         return MC_ERR_INVALID;
     }
+    const bool pre = g.pre || yv, front = g.front() || yv;   // what the front writes: see above
+    if (yv) {
+        info->orig_is_input = 0; info->orig_w = g.dw; info->orig_h = g.dh; info->orig_channels = 3;
+        info->cur_is_input = 0; info->out_w = g.dw; info->out_h = g.dh; info->out_channels = g.cc;
+    }
     mc_status st = check_clip(h, frames, produced);
     if (st != MC_OK) return st;
     const size_t lanes = (size_t)h->lanes, vl = (size_t)frames * lanes;
+    if (yv) {
+        if (const char* e = check_yuv422(*yv, w, hh, vl)) { h->err = e; return MC_ERR_INVALID; }
+    }
     if (cmp) {
         if (const char* e = check_compose(*cmp, g, vl)) { h->err = e; return MC_ERR_INVALID; }
     }
     if (empty) return clip_impl(h, nullptr, frames, 0, 0, channels, 0, p, nullptr, 0, produced);   // the identity
     if (nv) {
         if ((st = check_nv12(h, {nv}, w, hh, (int)vl, p)) != MC_OK) return st;
-    } else if (in_step < (size_t)w * channels) {
+    } else if (!yv && in_step < (size_t)w * channels) {
         h->err = "step too small";
         return MC_ERR_INVALID;
     }
     if (p->mode < 0 || p->mode > MC_MODE_NONE) { h->err = "bad mode"; return MC_ERR_INVALID; }
     const size_t out_row = (size_t)g.dw * g.cc;
-    if (!cmp && (g.front() || p->mode != MC_MODE_NONE)) {
+    if (!cmp && (front || p->mode != MC_MODE_NONE)) {
         if (!d_out) { h->err = "output pointer is null"; return MC_ERR_INVALID; }
         if (out_step < out_row) { h->err = "out_step too small"; return MC_ERR_INVALID; }
     }
-    if (!cmp && g.pre && d_orig && orig_step < (size_t)g.dw * channels) {
+    if (!cmp && pre && d_orig && orig_step < (size_t)g.dw * channels) {
         h->err = "original_step too small";
         return MC_ERR_INVALID;
     }
@@ -1132,19 +1152,20 @@ mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc
             d_orig = h->f_pre.p;
         }
     }
-    const bool tap = g.pre && d_orig;
+    const bool tap = pre && d_orig;
 
     // ---- the front: one launch over the virtual lanes; held lanes are skipped
     const uint8_t* mag_in = d_in;
     size_t mag_step = in_step;
-    if (g.front()) {
+    if (front) {
         FrontArgs a;
         if (nv) { a.src = nv->y; a.uv = nv->uv; a.step = nv->pitch; a.lane_stride = nv->lane_stride; }
+        else if (yv) { a.src = yv->data; a.step = yv->pitch; a.lane_stride = yv->lane_stride; }
         else { a.src = d_in; a.step = in_step; a.lane_stride = in_step * hh; }
         a.rx = g.rx; a.ry = g.ry; a.dw = g.dw; a.dh = g.dh; a.kind = g.kind; a.isx = g.isx; a.isy = g.isy;
         if (tap) {
             a.dst = d_orig; a.dst_step = orig_step;
-        } else if (g.pre && !g.gray) {   // the preprocessed frames are the magnifier's input
+        } else if (pre && !g.gray) {   // the preprocessed frames are the magnifier's input
             a.dst_step = (size_t)g.dw * channels;
             CK(h->f_pre.grow(a.dst_step * g.dh * vl));
             a.dst = h->f_pre.p;
@@ -1162,7 +1183,7 @@ mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc
             CK(cudaMemcpyAsync(h->f_flags.p, h->f_flags_host.data(), vl, cudaMemcpyHostToDevice, h->stream));
             a.flags = h->f_flags.p;
         }
-        const int src = nv ? FRONT_NV12 : channels == 3 ? FRONT_BGR : FRONT_GRAY;
+        const int src = nv ? FRONT_NV12 : yv ? FRONT_YUYV + yv->order : channels == 3 ? FRONT_BGR : FRONT_GRAY;
         if ((st = launch_counted(h, "chain_front", [&] { return launch_chain_front(a, src, (int)vl, h->stream); })) != MC_OK) return st;
         mag_in = g.gray ? a.gray : a.dst;
         mag_step = g.gray ? (size_t)g.dw : a.dst_step;
@@ -1180,11 +1201,12 @@ mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc
         a.w = g.dw & ~1; a.h = g.dh & ~1;
         if (a.w <= 0 || a.h <= 0) return MC_OK;   // a 0 x 0 canvas
         const int in_kind = channels == 3 ? FRONT_BGR : FRONT_GRAY, out_kind = g.cc == 3 ? FRONT_BGR : FRONT_GRAY;
-        const PaneSrc input = nv ? PaneSrc{nv->y, nv->uv, nv->pitch, nv->lane_stride, FRONT_NV12}
-                                 : PaneSrc{d_in, nullptr, in_step, in_step * hh, in_kind};
+        const PaneSrc input = nv   ? PaneSrc{nv->y, nv->uv, nv->pitch, nv->lane_stride, FRONT_NV12}
+                              : yv ? PaneSrc{yv->data, nullptr, yv->pitch, yv->lane_stride, FRONT_YUYV + yv->order}
+                                   : PaneSrc{d_in, nullptr, in_step, in_step * hh, in_kind};
         a.src[0] = tap ? PaneSrc{d_orig, nullptr, orig_step, orig_step * g.dh, in_kind} : input;
         a.src[1] = PaneSrc{d_out, nullptr, out_step, out_step * g.dh, out_kind};
-        a.src[2] = g.front() ? PaneSrc{mag_in, nullptr, mag_step, mag_step * g.dh, out_kind} : input;
+        a.src[2] = front ? PaneSrc{mag_in, nullptr, mag_step, mag_step * g.dh, out_kind} : input;
         // the pane choice of every virtual lane goes to the device on the handle's stream, as the front's flags do
         h->x_ops_host.resize(vl);   // lives on the handle: the copy is asynchronous
         for (size_t v = 0; v < vl; ++v)
@@ -1198,7 +1220,7 @@ mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc
         a.data = cv.data; a.uv = cv.uv; a.pitch = cv.pitch; a.lane_stride = cv.lane_stride;
         return launch_counted(h, "compose", [&] { return launch_compose(a, (int)vl, h->stream); });
     }
-    if (!g.front()) return MC_OK;
+    if (!front) return MC_OK;
     const size_t in_lane = mag_step * g.dh, out_lane = out_step * g.dh;
     return for_each_run(vl, [&](size_t v) { return !produced[v] && !h->hold[v % lanes]; }, [&](size_t a, size_t b) -> mc_status {
         CK(cudaMemcpy2DAsync(d_out + a * out_lane, out_step, mag_in + a * in_lane, mag_step, out_row, (b - a) * g.dh,
@@ -1221,7 +1243,7 @@ extern "C" mc_status mc_chain_process_device(mc_handle* h, const uint8_t* d_in, 
                                              mc_chain_info* info) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    return chain_impl(h, d_in, in_step, nullptr, frames, width, height, channels, p, grayscale, d_out, out_step, d_original,
+    return chain_impl(h, d_in, in_step, nullptr, nullptr, frames, width, height, channels, p, grayscale, d_out, out_step, d_original,
                       original_step, produced, info);
 } catch (...) { return on_exception(h); }
 
@@ -1232,7 +1254,7 @@ extern "C" mc_status mc_chain_process_nv12_device(mc_handle* h, const mc_nv12* i
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
     if (!in) { h->err = "NV12 plane is null"; return MC_ERR_INVALID; }
-    return chain_impl(h, nullptr, 0, in, frames, width, height, 3, p, grayscale, d_out, out_step, d_original, original_step,
+    return chain_impl(h, nullptr, 0, in, nullptr, frames, width, height, 3, p, grayscale, d_out, out_step, d_original, original_step,
                       produced, info);
 } catch (...) { return on_exception(h); }
 
@@ -1252,7 +1274,7 @@ extern "C" mc_status mc_chain_compose_device(mc_handle* h, const uint8_t* d_in, 
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
     const ComposeReq c{split, canvas};
-    return chain_impl(h, d_in, in_step, nullptr, frames, width, height, channels, p, grayscale, nullptr, 0, nullptr, 0, produced,
+    return chain_impl(h, d_in, in_step, nullptr, nullptr, frames, width, height, channels, p, grayscale, nullptr, 0, nullptr, 0, produced,
                       info, &c);
 } catch (...) { return on_exception(h); }
 
@@ -1263,7 +1285,29 @@ extern "C" mc_status mc_chain_compose_nv12_device(mc_handle* h, const mc_nv12* i
     CK(cudaSetDevice(h->device));
     if (!in) { h->err = "NV12 plane is null"; return MC_ERR_INVALID; }
     const ComposeReq c{split, canvas};
-    return chain_impl(h, nullptr, 0, in, frames, width, height, 3, p, grayscale, nullptr, 0, nullptr, 0, produced, info, &c);
+    return chain_impl(h, nullptr, 0, in, nullptr, frames, width, height, 3, p, grayscale, nullptr, 0, nullptr, 0, produced, info, &c);
+} catch (...) { return on_exception(h); }
+
+extern "C" mc_status mc_chain_process_yuv422_device(mc_handle* h, const mc_yuv422* in, int frames, int width, int height,
+                                                    const mc_params* p, int grayscale, uint8_t* d_out, size_t out_step,
+                                                    uint8_t* d_original, size_t original_step, uint8_t* produced,
+                                                    mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    if (!in) { h->err = "YUYV frame is null"; return MC_ERR_INVALID; }
+    return chain_impl(h, nullptr, 0, nullptr, in, frames, width, height, 3, p, grayscale, d_out, out_step, d_original,
+                      original_step, produced, info);
+} catch (...) { return on_exception(h); }
+
+extern "C" mc_status mc_chain_compose_yuv422_device(mc_handle* h, const mc_yuv422* in, int frames, int width, int height,
+                                                    const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                                                    uint8_t* produced, mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    if (!in) { h->err = "YUYV frame is null"; return MC_ERR_INVALID; }
+    const ComposeReq c{split, canvas};
+    return chain_impl(h, nullptr, 0, nullptr, in, frames, width, height, 3, p, grayscale, nullptr, 0, nullptr, 0, produced, info,
+                      &c);
 } catch (...) { return on_exception(h); }
 
 // The one-lane host form: the frame is uploaded, runs the device chain, and what it wrote comes back tight.
@@ -1293,7 +1337,7 @@ extern "C" mc_status mc_chain_process(mc_handle* h, const uint8_t* in, int width
         CK(cudaMemcpy2DAsync(h->c_raw.p, row, in, in_step, row, (size_t)height, cudaMemcpyHostToDevice, h->stream));
     }
     uint8_t produced = 0;
-    const mc_status st = chain_impl(h, have ? h->c_raw.p : nullptr, row, nullptr, 1, width, height, channels, p, grayscale, h->c_out.p,
+    const mc_status st = chain_impl(h, have ? h->c_raw.p : nullptr, row, nullptr, nullptr, 1, width, height, channels, p, grayscale, h->c_out.p,
                                     (size_t)g.dw * g.cc, g.pre ? h->c_orig.p : nullptr, (size_t)g.dw * channels, &produced, info);
     if (st != MC_OK || !have) return st;
     if (produced && info->cur_is_input) {   // no front stage: the magnified frame is the chain's result
@@ -1307,6 +1351,41 @@ extern "C" mc_status mc_chain_process(mc_handle* h, const uint8_t* in, int width
         if (out_bytes < out_frame) { h->err = "out buffer too small"; return MC_ERR_INVALID; }
         CK(cudaMemcpyAsync(out, h->c_out.p, out_frame, cudaMemcpyDeviceToHost, h->stream));
     }
+    CK(cudaStreamSynchronize(h->stream));
+    return MC_OK;
+} catch (...) { return on_exception(h); }
+
+// The live camera form: the 2 * width bytes of each row go up in one 2D copy, run the device chain, and both of its
+// frames (always written for a 4:2:2 source) come back tight.  Every argument is checked before the upload.
+extern "C" mc_status mc_chain_process_yuv422(mc_handle* h, const mc_yuv422* in, int width, int height, const mc_params* p,
+                                             int grayscale, uint8_t* out, size_t out_bytes, uint8_t* original,
+                                             size_t original_bytes, mc_chain_info* info) try {
+    if (!h || !p || !info) return MC_ERR_INVALID;
+    std::memset(info, 0, sizeof(*info));
+    info->cur_is_input = 1; info->orig_is_input = 1;
+    CK(cudaSetDevice(h->device));
+    if (h->lanes != 1) { h->err = "mc_chain_process_yuv422 needs a 1-lane handle"; return MC_ERR_INVALID; }
+    if (!h->inflight.empty()) { h->err = "mc_chain_process_yuv422 called with pipelined frames in flight"; return MC_ERR_INVALID; }
+    if (h->hold[0]) { h->err = "mc_chain_process_yuv422 called while lane 0 is held"; return MC_ERR_INVALID; }
+    if (!in) { h->err = "YUYV frame is null"; return MC_ERR_INVALID; }
+    if (const char* e = check_yuv422(*in, width, height, 1)) { h->err = e; return MC_ERR_INVALID; }
+    if (p->mode < 0 || p->mode > MC_MODE_NONE) { h->err = "bad mode"; return MC_ERR_INVALID; }
+    ChainGeom g;
+    if (const char* e = chain_geometry(p, width, height, 3, grayscale, g, info)) { h->err = e; return MC_ERR_INVALID; }
+    const size_t row = (size_t)2 * width, out_frame = (size_t)g.dw * g.dh * g.cc, orig_frame = (size_t)g.dw * g.dh * 3;
+    if (out && out_bytes < out_frame) { h->err = "out buffer too small"; return MC_ERR_INVALID; }
+    if (original && original_bytes < orig_frame) { h->err = "original buffer too small"; return MC_ERR_INVALID; }
+    CK(h->c_raw.grow(row * height));
+    CK(h->c_out.grow(out_frame));
+    if (original) CK(h->c_orig.grow(orig_frame));
+    CK(cudaMemcpy2DAsync(h->c_raw.p, row, in->data, in->pitch, row, (size_t)height, cudaMemcpyHostToDevice, h->stream));
+    const mc_yuv422 dev{h->c_raw.p, row, row * height, in->order};
+    uint8_t produced = 0;
+    const mc_status st = chain_impl(h, nullptr, 0, nullptr, &dev, 1, width, height, 3, p, grayscale, h->c_out.p,
+                                    (size_t)g.dw * g.cc, original ? h->c_orig.p : nullptr, (size_t)g.dw * 3, &produced, info);
+    if (st != MC_OK) return st;
+    if (original) CK(cudaMemcpyAsync(original, h->c_orig.p, orig_frame, cudaMemcpyDeviceToHost, h->stream));
+    if (out) CK(cudaMemcpyAsync(out, h->c_out.p, out_frame, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return MC_OK;
 } catch (...) { return on_exception(h); }

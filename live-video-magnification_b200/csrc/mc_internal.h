@@ -153,10 +153,11 @@ cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16
                           bool luma_only = false);
 
 // PreprocessProcessor + GrayscaleProcessor on the device (mc_preprocess.cu): one launch over `vlanes` virtual lanes.
-enum FrontSrc { FRONT_BGR = 0, FRONT_GRAY = 1, FRONT_NV12 = 2 };
+// FRONT_YUYV + mc_yuv422_order is the packed 4:2:2 source of that byte order.
+enum FrontSrc { FRONT_BGR = 0, FRONT_GRAY = 1, FRONT_NV12 = 2, FRONT_YUYV = 3, FRONT_UYVY = 4 };
 enum FrontKind { FRONT_COPY = 0, FRONT_AREA_FAST = 1, FRONT_AREA = 2 };   // crop only / integer INTER_AREA / general INTER_AREA
 struct FrontArgs {
-    const uint8_t* src = nullptr;   // lane 0's frame (BGR / gray) or luma plane (NV12)
+    const uint8_t* src = nullptr;   // lane 0's frame (BGR / gray / YUYV / UYVY) or luma plane (NV12)
     const uint8_t* uv = nullptr;    // NV12: lane 0's Cb,Cr plane
     size_t step = 0, lane_stride = 0;   // row pitch and virtual-lane stride of the source (both NV12 planes)
     int rx = 0, ry = 0;             // ROI origin in the source
@@ -167,6 +168,7 @@ struct FrontArgs {
     size_t dst_step = 0, dst_lane_stride = 0;
     uint8_t* gray = nullptr;        // their BGR2GRAY, tight [v][dh][dw], or null (3-channel sources only)
     const uint8_t* flags = nullptr; // per virtual lane, 0 = skip (held); null = every lane
+    int vec = 0;                    // YUYV / UYVY: every group can be read as one 32-bit word (set by launch_chain_front)
 };
 cudaError_t launch_chain_front(const FrontArgs& a, int src, int vlanes, cudaStream_t s);
 
@@ -190,7 +192,7 @@ struct PaneSrc {
     const uint8_t* p = nullptr;
     const uint8_t* uv = nullptr;
     size_t step = 0, lane_stride = 0;
-    int kind = FRONT_BGR;           // FrontSrc: BGR, gray (expanded as GRAY2BGR) or NV12 (converted as YUV2BGR_NV12)
+    int kind = FRONT_BGR;           // FrontSrc: BGR, gray (expanded as GRAY2BGR), NV12 or YUYV / UYVY (converted as cvtColor)
 };
 // Which frame is virtual lane v's `cur` pane
 enum ComposeOp : uint8_t { COMPOSE_SKIP = 0, COMPOSE_MAGNIFIED = 1, COMPOSE_FALLBACK = 2 };

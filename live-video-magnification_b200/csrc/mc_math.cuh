@@ -289,6 +289,13 @@ MC_HD void nv12_to_bgr_px(int y, int u, int v, uint8_t& b, uint8_t& g, uint8_t& 
     r = sat_u8((yy + 1673527 * v) >> 20);
 }
 
+// cv::cvtColor(COLOR_YUV2BGR_YUYV / _UYVY) of pixel j (0 or 1) of a packed 4:2:2 group: its 4 bytes, the first lowest
+// (YUYV: Y0 Cb Y1 Cr; UYVY: Cb Y0 Cr Y1).  Both pixels take the group's Cb, Cr, with the arithmetic of YUV2BGR_NV12.
+MC_HD void yuv422_to_bgr_px(uint32_t grp, int j, bool uyvy, uint8_t& b, uint8_t& g, uint8_t& r) {
+    const int c = uyvy ? 0 : 8;   // bit offset of Cb; Cr is 16 bits above it, Y_j at 16 j + 8 - c
+    nv12_to_bgr_px((int)(grp >> (16 * j + 8 - c) & 255), (int)(grp >> c & 255), (int)(grp >> (c + 16) & 255), b, g, r);
+}
+
 // cv::cvtColor(COLOR_BGR2YUV_I420) of one pixel: its Y, and the Cb, Cr that OpenCV stores for a 2x2 block whose
 // top-left pixel it is (the other three pixels of the block do not contribute).
 MC_HD void bgr_to_ycc_px(int b, int g, int r, uint8_t& y, uint8_t& cb, uint8_t& cr) {

@@ -1,8 +1,9 @@
 // Front of the reference chain fused onto the device (SURVEY.md 8f-1): PreprocessProcessor (normalised ROI crop +
 // INTER_AREA 1/2..1/8 downscale, reference src/processing/PreprocessProcessor.cpp:10-51) and GrayscaleProcessor
 // (BGR2GRAY, src/processing/GrayscaleProcessor.cpp:7-16), bit-exact with OpenCV's u8 paths (mc_math.cuh), in one kernel
-// over every virtual lane whose source is u8 BGR, u8 gray or NV12 planes (an NV12 pixel is converted as
-// cvtColor(YUV2BGR_NV12) converts it inside the tap walk, so no full-resolution BGR frame is ever stored); and the NV12
+// over every virtual lane whose source is u8 BGR, u8 gray, NV12 planes or a packed 4:2:2 camera frame (YUYV / UYVY; an
+// NV12 or 4:2:2 pixel is converted as cvtColor converts it inside the tap walk, so no full-resolution BGR frame needs to
+// be stored); and the NV12
 // conversions around the magnifier for the video decoder / encoder hand-off, and the export canvas built from the chain's
 // two taps (the exporter's compose, SURVEY.md 8f-2).
 #include "../../include/magcore_b200.h"
@@ -35,6 +36,24 @@ template <> struct FrontPx<FRONT_NV12> {   // cvtColor(YUV2BGR_NV12) of the pixe
         v[0] = b; v[1] = g; v[2] = r;
     }
 };
+// cvtColor(YUV2BGR_YUYV / _UYVY) of the pixel: its Y and its group's Cb,Cr, the group read as one 32-bit word when every
+// group is 4-byte aligned (vec), else byte by byte.  p is the ROI's first row; the group of a pixel follows from its
+// column in the frame (ox + sx), so a crop at an odd column still pairs the frame's pixels.
+template <bool UYVY> struct Yuv422Px {
+    const uint8_t* p; size_t pitch; int ox; bool vec;
+    __device__ void operator()(int sx, int sy, int (&v)[3]) const {
+        const int ax = ox + sx;
+        const uint8_t* q = p + (size_t)sy * pitch + (size_t)2 * (ax & ~1);
+        const uint32_t grp = vec ? __ldg(reinterpret_cast<const unsigned*>(q))
+                                 : (uint32_t)__ldg(q) | (uint32_t)__ldg(q + 1) << 8 | (uint32_t)__ldg(q + 2) << 16 |
+                                       (uint32_t)__ldg(q + 3) << 24;
+        uint8_t b, g, r;
+        yuv422_to_bgr_px(grp, ax & 1, UYVY, b, g, r);
+        v[0] = b; v[1] = g; v[2] = r;
+    }
+};
+template <> struct FrontPx<FRONT_YUYV> : Yuv422Px<false> {};
+template <> struct FrontPx<FRONT_UYVY> : Yuv422Px<true> {};
 
 // One thread per output pixel of one virtual lane (blockIdx.z): every channel of the preprocessed pixel and its gray
 // byte from one walk over the pixel's source taps.
@@ -47,6 +66,8 @@ __global__ void __launch_bounds__(256) k_chain_front(const FrontArgs a) {
     FrontPx<SRC> px;
     if constexpr (SRC == FRONT_NV12) {
         px = FrontPx<SRC>{a.src + v * a.lane_stride, a.uv + v * a.lane_stride, a.step, a.rx, a.ry};
+    } else if constexpr (SRC == FRONT_YUYV || SRC == FRONT_UYVY) {
+        px.p = a.src + v * a.lane_stride + (size_t)a.ry * a.step; px.pitch = a.step; px.ox = a.rx; px.vec = a.vec != 0;
     } else {
         px = FrontPx<SRC>{a.src + v * a.lane_stride + (size_t)a.ry * a.step + (size_t)CN * a.rx, a.step};
     }
@@ -65,11 +86,15 @@ __global__ void __launch_bounds__(256) k_chain_front(const FrontArgs a) {
 
 }  // namespace
 
-cudaError_t launch_chain_front(const FrontArgs& a, int src, int vlanes, cudaStream_t s) {
+cudaError_t launch_chain_front(const FrontArgs& args, int src, int vlanes, cudaStream_t s) {
+    FrontArgs a = args;
+    a.vec = (reinterpret_cast<uintptr_t>(a.src) & 3) == 0 && a.step % 4 == 0 && (vlanes == 1 || a.lane_stride % 4 == 0);
     const dim3 grid((unsigned)((a.dw + 255) / 256), (unsigned)a.dh, (unsigned)vlanes);
     switch (src) {
         case FRONT_BGR: k_chain_front<FRONT_BGR><<<grid, 256, 0, s>>>(a); break;
         case FRONT_GRAY: k_chain_front<FRONT_GRAY><<<grid, 256, 0, s>>>(a); break;
+        case FRONT_YUYV: k_chain_front<FRONT_YUYV><<<grid, 256, 0, s>>>(a); break;
+        case FRONT_UYVY: k_chain_front<FRONT_UYVY><<<grid, 256, 0, s>>>(a); break;
         default: k_chain_front<FRONT_NV12><<<grid, 256, 0, s>>>(a); break;
     }
     return cudaGetLastError();
@@ -199,7 +224,8 @@ __global__ void __launch_bounds__(kBlockX * kBlockY) k_bgr_to_nv12(const ToNv12A
     store(a.uv + lane * a.lane_stride + (size_t)r * a.pitch + x0, full && a.vec_out, n, c);
 }
 // Two rows (2r, 2r + 1) of n <= 8 pixels from column x0 of virtual lane v's frame in a pane source, as BGR bytes: gray
-// expanded as GRAY2BGR, NV12 converted as cvtColor(YUV2BGR_NV12) (x0 and n are even, so the Cb,Cr pairs are whole).
+// expanded as GRAY2BGR, NV12 and YUYV / UYVY converted as cvtColor does (x0 and n are even, so the Cb,Cr pairs and the
+// 4:2:2 groups are whole).
 __device__ __forceinline__ void load_pane(const PaneSrc& s, bool vec, size_t v, int x0, int r, int n, uint8_t (&o0)[24],
                                           uint8_t (&o1)[24]) {
     const uint8_t* row = s.p + v * s.lane_stride + (size_t)(2 * r) * s.step;
@@ -213,6 +239,24 @@ __device__ __forceinline__ void load_pane(const PaneSrc& s, bool vec, size_t v, 
             const int u = c[i & ~1], w = c[i | 1];
             nv12_to_bgr_px(y0[i], u, w, o0[3 * i], o0[3 * i + 1], o0[3 * i + 2]);
             nv12_to_bgr_px(y1[i], u, w, o1[3 * i], o1[3 * i + 1], o1[3 * i + 2]);
+        }
+    } else if (s.kind == FRONT_YUYV || s.kind == FRONT_UYVY) {   // 4 groups of 4 bytes per row, from byte 2 * x0
+        const bool uyvy = s.kind == FRONT_UYVY;
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            uint8_t t0[8], t1[8];
+            const int nk = min(8, max(0, 2 * n - 8 * k));
+            load8(row + (size_t)2 * x0 + 8 * k, vec, nk, t0);
+            load8(row + s.step + (size_t)2 * x0 + 8 * k, vec, nk, t1);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {   // pixel 4k + i: group 2k + i / 2
+                const int g = 4 * (i >> 1);
+                const uint32_t g0 = (uint32_t)t0[g] | (uint32_t)t0[g + 1] << 8 | (uint32_t)t0[g + 2] << 16 | (uint32_t)t0[g + 3] << 24;
+                const uint32_t g1 = (uint32_t)t1[g] | (uint32_t)t1[g + 1] << 8 | (uint32_t)t1[g + 2] << 16 | (uint32_t)t1[g + 3] << 24;
+                const int px = 3 * (4 * k + i);
+                yuv422_to_bgr_px(g0, i & 1, uyvy, o0[px], o0[px + 1], o0[px + 2]);
+                yuv422_to_bgr_px(g1, i & 1, uyvy, o1[px], o1[px + 1], o1[px + 2]);
+            }
         }
     } else if (s.kind == FRONT_GRAY) {
         uint8_t g0[8], g1[8];

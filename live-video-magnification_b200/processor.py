@@ -333,6 +333,16 @@ class MagnificationProcessor(IProcessor):
                                                            flags.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(info)))
         return flags.astype(bool), info
 
+    def chain_compose_yuv422_device(self, d_in: capi.McYuv422, frames: int, w: int, h: int, cfg: ProcessorConfig, split: int,
+                                    canvas: capi.McCanvas):
+        """mc_chain_compose_yuv422_device on packed YUYV / UYVY device frames -> (produced bool[frames, lanes], McChainInfo)."""
+        p, info = _to_mc(cfg), capi.McChainInfo()
+        flags = np.zeros((int(frames), self.lanes), np.uint8)
+        self._check(self._lib.mc_chain_compose_yuv422_device(self._h, C.byref(d_in), int(frames), w, h, C.byref(p),
+                                                             int(cfg.grayscale), int(split), C.byref(canvas),
+                                                             flags.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(info)))
+        return flags.astype(bool), info
+
     def sync(self):
         self._check(self._lib.mc_sync(self._h))
 
@@ -388,7 +398,8 @@ class ProcessingChainB200:
 
     ``run_chain_once(frame, cfg) -> (cur, original)`` returns the *same* frame object wherever the reference
     returns the same FrameRef (identity stages / passthrough); it needs ``lanes == 1``.  ``process_device`` and
-    ``process_nv12_device`` run the chain on device frames of every lane, for one frame or a clip."""
+    ``process_nv12_device`` / ``process_yuv422_device`` run the chain on device frames of every lane, for one frame or a
+    clip; ``run_chain_once`` of a ``Frame`` whose format is "YUYV" or "UYVY" takes a camera's packed 4:2:2 bytes."""
 
     def __init__(self, device: int = 0, lanes: int = 1):
         self.magnifier = MagnificationProcessor(device=device, lanes=lanes)
@@ -427,7 +438,41 @@ class ProcessingChainB200:
                                                      flags.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(info)))
         return flags.astype(bool), info
 
+    def process_yuv422_device(self, d_in: capi.McYuv422, frames: int, w: int, h: int, cfg: ProcessorConfig, d_out: int,
+                              out_step: int, d_original: int = 0, original_step: int = 0):
+        """mc_chain_process_yuv422_device on packed YUYV / UYVY device frames -> (produced bool[frames, lanes], McChainInfo)."""
+        m, p, info = self.magnifier, _to_mc(cfg), capi.McChainInfo()
+        flags = np.zeros((int(frames), self.lanes), np.uint8)
+        m._check(m._lib.mc_chain_process_yuv422_device(m._h, C.byref(d_in), int(frames), w, h, C.byref(p), int(cfg.grayscale),
+                                                       d_out, out_step, d_original or None, original_step,
+                                                       flags.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(info)))
+        return flags.astype(bool), info
+
+    def _run_chain_once_yuv422(self, frame: Frame, cfg: ProcessorConfig):
+        """run_chain_once of a camera frame in YUYV / UYVY (image: [h][w][2] or [h][2w] bytes) through mc_chain_process_yuv422:
+        the conversion always runs, so both results are fresh BGR (or gray) frames."""
+        m, p, info = self.magnifier, _to_mc(cfg), capi.McChainInfo()
+        img = frame.image
+        if img.dtype != np.uint8:
+            raise TypeError("image must be uint8")
+        img = img if img.flags["C_CONTIGUOUS"] else np.ascontiguousarray(img)
+        h, w = img.shape[0], img.size // (2 * img.shape[0])
+        order = capi.MC_YUV422_UYVY if frame.format == "UYVY" else capi.MC_YUV422_YUYV
+        out, orig = np.empty(h * w * 3, np.uint8), np.empty(h * w * 3, np.uint8)
+        m._check(m._lib.mc_chain_process_yuv422(m._h, C.byref(capi.McYuv422(img.ctypes.data, 2 * w, 2 * w * h, order)), w, h,
+                                                C.byref(p), int(cfg.grayscale), out.ctypes.data, out.size, orig.ctypes.data,
+                                                orig.size, C.byref(info)))
+        ow, oh, oc = info.out_w, info.out_h, info.out_channels
+        cur = out[:ow * oh * oc].reshape((oh, ow) if oc == 1 else (oh, ow, oc)).copy()
+        original = orig[:info.orig_w * info.orig_h * 3].reshape(info.orig_h, info.orig_w, 3).copy()
+        return (replace(frame, image=cur, width=ow, height=oh, format="BGR8" if oc == 3 else "Gray8"),
+                replace(frame, image=original, width=info.orig_w, height=info.orig_h, format="BGR8"))
+
     def run_chain_once(self, frame: Frame, cfg: ProcessorConfig):
+        """-> (cur, original).  A frame whose format is "YUYV" or "UYVY" (a camera's packed 4:2:2 bytes) is converted on the
+        device as cv2.cvtColor(COLOR_YUV2BGR_YUYV / _UYVY) would convert it first."""
+        if frame.format in ("YUYV", "UYVY") and frame.image is not None and frame.image.size:
+            return self._run_chain_once_yuv422(frame, cfg)
         m = self.magnifier
         p = _to_mc(cfg)
         info = capi.McChainInfo()

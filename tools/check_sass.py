@@ -120,9 +120,10 @@ def main():
         lines.append(f"     {k}: main loop {n} instructions ({n - rare} outside the warp-voted dark-end spline) "
                      f"per 2 output rows x 4 columns per lane")
     front = [k for k in body if k.startswith("void k_chain_front<")]
-    need(len(front) == 3 and all(count(k, r"\b(STL|LDL)\b") == 0 for k in front), "k_chain_front<BGR, gray, NV12>: no local memory (STL / LDL)")
+    need(len(front) == 5 and all(count(k, r"\b(STL|LDL)\b") == 0 for k in front),
+         "k_chain_front<BGR, gray, NV12, YUYV, UYVY>: no local memory (STL / LDL)")
     fspills = clip_spills("k_chain_front", "mc_preprocess")
-    need(len(fspills) == 3 and all(s == (0, 0) for s in fspills.values()), f"k_chain_front<*>: no spills (ptxas -v, {len(fspills)} instances)")
+    need(len(fspills) == 5 and all(s == (0, 0) for s in fspills.values()), f"k_chain_front<*>: no spills (ptxas -v, {len(fspills)} instances)")
     rz = [k for k in body if k.startswith("k_riesz_egress") or "k_riesz_egress(" in k]
     # the select is either an FSEL per channel or a saturate predicated on the NaN test over a preset 1.0
     nan_sel = lambda k: count(k, "FSEL") + count(k, r"@!P\d FADD\.SAT")
