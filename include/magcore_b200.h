@@ -162,12 +162,15 @@ mc_status mc_sync(mc_handle* h);
  *            the virtual lanes, and the phase kernel carries each pixel's prior pyramid, phases and Butterworth
  *            registers in registers across the clip.  A filter design that is not finite (every frame is a first frame)
  *            runs as frame calls.  analysis_only updates the state and produces nothing, as frame calls do.
- *   Color:   one frame call per frame (same results; the clip call works whatever the mode).
+ *   Color:   one launch set for the whole clip, apart from the window filter.  The ingest, the Gaussian chain and
+ *            everything after the filter (window min / max, column select, pyrUp chain, resize, output stretch) run
+ *            over the virtual lanes; the append to the window and its DFT pair run frame by frame, as in frame calls.
+ *            The read-only taps ("gauss", "window", "filtered", "up") after a clip are those of its last frame.
  * MC_ERR_INVALID, with the state untouched, when frames < 1, frames * lanes > MC_MAX_LANES, produced is NULL or frames of
  * mc_submit are in flight; the parameter checks of mc_process_device apply unchanged.  Mode None and an empty image
  * are the identity (all flags 0, state dropped).  A failed clip drops the state like a failed frame.  The clip path
  * keeps device scratch for the largest clip seen, released by mc_reset: ~29 MB (Laplace) or ~82 MB (Phase) per 1080p
- * colour frame at 6 levels. */
+ * colour frame at 6 levels, ~91 MB (Color, 64-frame window, 3 or 6 levels). */
 mc_status mc_process_clip_device(mc_handle* h, const uint8_t* d_in, int frames, int width, int height, int channels,
                                  size_t in_step, const mc_params* p, uint8_t* d_out, size_t out_step, uint8_t* produced);
 /* The same on host pointers, blocking (upload, kernels, download of the produced frames only).  Pinned or pageable. */
@@ -203,8 +206,8 @@ mc_status mc_chain_geometry(const mc_params* p, int width, int height, int chann
  *   Layout: virtual lane v = t * lanes + k is frame t of lane k.  It sits at v * height * in_step in d_in, at
  *     v * out_h * out_step in d_out and at v * orig_h * original_step in d_original (out_h / orig_h of `info`, or height
  *     where the stage is an identity).  produced: frames * lanes bytes, [t][lane].  frames == 1 is a frame call; frames
- *     > 1 follows the clip rules of mc_process_clip_device unchanged (lifecycle taken at the first frame, Laplace and
- *     Phase batched, Color a loop of frame calls).
+ *     > 1 follows the clip rules of mc_process_clip_device unchanged (lifecycle taken at the first frame, every mode
+ *     batched, Color's window filter frame by frame).
  *   Equivalence: every virtual lane gets, bit for bit, what mc_chain_process on a 1-lane handle gives when fed that
  *     lane's frames in order: the processed frame, the original tap, the info and the temporal state afterwards (held
  *     lanes and Color's lanes as in the lane lifecycle above).
@@ -440,7 +443,8 @@ mc_status mc_set_option(mc_handle* h, const char* key, int value);
  *   amplification, the last level the colour image that is added to the input.
  *   Lanes of one handle may have windows of different length: a column is served only while every lane has it, and
  *   "filtered" / "up" only while every lane ran the filter in the last frame call that was not held for all lanes
- *   (otherwise 0 rows).  All are absent before the first frame and after mc_reset or a change of mode or geometry.
+ *   (otherwise 0 rows).  A held lane's "gauss" is the pyramid of whatever its input slot held (in a chain call with
+ *   a front stage, which skips held lanes, bytes an earlier call left in the front's staging).  All are absent before the first frame and after mc_reset or a change of mode or geometry.
  * Laplace and Phase, level 0, three channels, read-only: "lab16", the BGR->Lab conversion of the last frame call as
  *   the kernels hold it, the raw fixed-point values L*2^14/100, (a+128)*64, (b+128)*64 widened (exactly) to f32.  It
  *   exists only after a frame call on 3-channel input; before the first frame, after mc_reset and after a clip call it

@@ -5,6 +5,7 @@
 #include <cfloat>
 #include <cmath>
 #include <algorithm>
+#include <cassert>
 #include <cstring>
 
 #include "mc_modes.h"
@@ -117,17 +118,20 @@ __device__ __forceinline__ void block_minmax_commit(float mn, float mx, unsigned
 }
 
 // min/max of one stream's part of the filtered window: nchunks contiguous runs of `chunk` floats, chunk_stride apart
-// (TemporalFilter.cpp:55); 128-bit loads when the runs are 16-byte aligned
+// (TemporalFilter.cpp:55); 128-bit loads when the runs are 16-byte aligned.  blockIdx.y is the (virtual) lane v: frame
+// v / lanes, whose window starts win_stride floats after the previous frame's, lane v % lanes of it.
 __global__ void __launch_bounds__(256) k_minmax(const float* __restrict__ base, size_t chunk, int nchunks, size_t chunk_stride,
-                                                unsigned* __restrict__ mm, int vec_ok, int pad, const ColorLane* __restrict__ tab) {
-    const int lane = blockIdx.y;
+                                                unsigned* __restrict__ mm, int vec_ok, int pad, const ColorLane* __restrict__ tab,
+                                                int lanes, size_t win_stride) {
+    const int v = blockIdx.y;
+    const int f = v / lanes, lane = v - f * lanes;
     if (tab) {
-        nchunks = tab[lane].n;
+        nchunks = tab[v].n;
         if (nchunks == 0) return;
     }
     float mn = INFINITY, mx = -INFINITY;
     for (int t = 0; t < nchunks; ++t) {
-        const float* __restrict__ p = base + (size_t)t * chunk_stride + (size_t)lane * (chunk + pad);
+        const float* __restrict__ p = base + (size_t)f * win_stride + (size_t)t * chunk_stride + (size_t)lane * (chunk + pad);
         if (vec_ok) {
             const float4* __restrict__ p4 = reinterpret_cast<const float4*>(p);
             for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < chunk / 4; i += (size_t)gridDim.x * blockDim.x) {
@@ -143,12 +147,14 @@ __global__ void __launch_bounds__(256) k_minmax(const float* __restrict__ base, 
             }
         }
     }
-    block_minmax_commit(mn, mx, mm + 2 * lane);
+    block_minmax_commit(mn, mx, mm + 2 * v);
 }
 
-// the reconstructed column: physical slot `phys` of the filtered window, or each lane's own with a lane table
+// the reconstructed column: physical slot `phys` of the filtered window, or each lane's own with a lane table.  Virtual
+// lane v reads the window of frame v / lanes, win_stride = S + tstep floats after the previous frame's (tstep 0: one frame).
 __global__ void k_select(const float* __restrict__ work, size_t S, int pad, int phys, const unsigned* __restrict__ mm, int C, int w, int h,
-                         float alpha, float* __restrict__ dst, int pitch, size_t plane, int planes, const ColorLane* __restrict__ tab) {
+                         float alpha, float* __restrict__ dst, int pitch, size_t plane, int planes, const ColorLane* __restrict__ tab,
+                         int lanes, size_t tstep) {
     const size_t n = (size_t)planes * h * w;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
         const int pl = (int)(i / ((size_t)h * w));
@@ -159,7 +165,8 @@ __global__ void k_select(const float* __restrict__ work, size_t S, int pad, int 
         if (tab || pad) {
             const int slot = tab ? tab[lane].sel : phys;
             if (slot < 0) continue;
-            o = (size_t)slot * S + i + (size_t)lane * pad;
+            // i + lane * pad is lane * (lane block + pad) into the frame's slot; frame f's window adds f * tstep
+            o = (size_t)slot * S + i + (size_t)lane * pad + (size_t)(lane / lanes) * tstep;
         }
         const double smin = (double)ord2f(mm[2 * lane]), smax = (double)ord2f(mm[2 * lane + 1]);
         const double scale = (smax - smin > DBL_EPSILON) ? 1.0 / (smax - smin) : 0.0;   // cv::normalize NORM_MINMAX
@@ -269,11 +276,12 @@ __global__ void __launch_bounds__(256) k_sum_minmax(const float* __restrict__ a,
 }
 
 
-// out8u = convertTo(input + colorImg, 255/(max-min), -min*255/(max-min))  (MagnifyCore.hpp:202-203)
+// out8u = convertTo(input + colorImg, 255/(max-min), -min*255/(max-min))  (MagnifyCore.hpp:202-203).  The float tap takes
+// (virtual) lanes fout_v0 and up: a clip's last frame.
 template <int C>
 __global__ void k_color_egress(const float* __restrict__ a, const float* __restrict__ b, Level l,
                                const unsigned* __restrict__ mm, uint8_t* __restrict__ out, size_t step,
-                               size_t lane_stride, float* __restrict__ fout, const ColorLane* __restrict__ tab) {
+                               size_t lane_stride, float* __restrict__ fout, int fout_v0, const ColorLane* __restrict__ tab) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, lane = blockIdx.z;
     if (x >= l.w || idle_lane(tab, lane)) return;
     const double mn = (double)ord2f(mm[2 * lane]), mx = (double)ord2f(mm[2 * lane + 1]);
@@ -284,7 +292,7 @@ __global__ void k_color_egress(const float* __restrict__ a, const float* __restr
         const size_t o = (size_t)(lane * C + c) * l.plane + (size_t)y * l.pitch + x;
         const float v = a[o] + b[o];
         q[c] = scaled_to_u8(v, sa, sb);
-        if (fout) fout[(((size_t)lane * l.h + y) * l.w + x) * C + c] = v;
+        if (fout && lane >= fout_v0) fout[(((size_t)(lane - fout_v0) * l.h + y) * l.w + x) * C + c] = v;
     }
 }
 
@@ -311,6 +319,38 @@ void ColorMode::reset() {
     allocated = false;
     count.clear(); head.clear(); mod.clear(); table.clear();
     ring_cap = 0;
+    clip.arena.release();
+    clip = Clip{};
+    tap_frame = -1;
+}
+
+// Grows the clip scratch to `vl` virtual lanes and `work_floats` floats of filtered windows.  The float tap is written in
+// place by the last frame's egress, so the scratch holds none.
+mc_status ColorMode::alloc_clip(const ModeCtx& ctx, int vl, size_t work_floats) {
+    ModeCtx c = ctx;
+    c.float_out = nullptr;
+    MCK_ST(ClipScratch::grow(clip, c, vl, 0, 0, [&]() -> mc_status {
+        const size_t vplanes = (size_t)vl * channels;
+        clip.G.assign((size_t)levels + 1, nullptr);
+        for (int l = 0; l <= levels; ++l) MCK(clip.arena.alloc(&clip.G[(size_t)l], vplanes * lv[(size_t)l].plane));
+        clip.U.assign((size_t)levels + 2, nullptr);
+        for (int i = 0; i <= levels; ++i) MCK(clip.arena.alloc(&clip.U[(size_t)i], vplanes * ulv[(size_t)i].plane));
+        if (U[(size_t)levels + 1]) MCK(clip.arena.alloc(&clip.U[(size_t)levels + 1], vplanes * lv[0].plane));
+        void* v = nullptr;
+        MCK(clip.arena.alloc_bytes(&v, sizeof(unsigned) * 4 * (size_t)vl));
+        clip.minmax = (unsigned*)v;
+        MCK(clip.arena.alloc_bytes(&v, sizeof(ColorLane) * (size_t)vl));
+        clip.d_table = (ColorLane*)v;
+        return MC_OK;
+    }));
+    if (work_floats > clip.work_floats) {   // the ring grew since the scratch was made
+        if (clip.work) clip.arena.free_block(clip.work);
+        clip.work = nullptr;
+        clip.work_floats = 0;
+        MCK(clip.arena.alloc(&clip.work, work_floats));
+        clip.work_floats = work_floats;
+    }
+    return MC_OK;
 }
 
 #define CUFFT_CK(call)                                                            \
@@ -364,7 +404,192 @@ mc_status ColorMode::fft_plan(const ModeCtx& ctx, int n, bool one_lane, FftPlans
     return MC_OK;
 }
 
-mc_status ColorMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int nlevels, int* produced) {
+// Append to the rolling window; once full drop the oldest column (SpatialFilter.cpp:63-84).  Then the filter's operands:
+// a lane's signal is physical slots [0, n) (warming: head 0; full: n == mod), so n alone picks its DFT.  A frame call
+// runs this once, a clip once per frame.
+ColorMode::Step ColorMode::step(const mc_params& p, int want_cap, ColorLane* rows) {
+    const double lo = p.coLow == 0.0 ? p.coLow + 0.01 : p.coLow, hi = p.coHigh;   // TemporalFilter.cpp:26-27
+    Step s;
+    for (int k = 0; k < lanes; ++k) {
+        ColorLane& L = rows[k];
+        int& cnt = count[(size_t)k];
+        int& hd = head[(size_t)k];
+        L.append = -1; L.n = 0; L.sel = -1; L.sc = 0.f; L.fl = L.fh = 0.0;
+        if (plan.op[(size_t)k] == LANE_HOLD) continue;
+        L.append = (hd + cnt) % mod[(size_t)k];
+        ++cnt;
+        if (cnt > want_cap && want_cap > 0) {
+            hd = (hd + 1) % mod[(size_t)k];
+            --cnt;
+        }
+        if (cnt < 2) continue;  // MagnifyCore.hpp:180 (passthrough)
+        L.n = cnt;
+        L.sel = (hd + std::min(1, cnt - 1)) % mod[(size_t)k];   // the reconstructed column is logical min(1, n-1) (:189-192)
+        // createIdealBandpassFilter (TemporalFilter.cpp:59-80): real 0/1 mask over packed indices x, read back by
+        // mulSpectrums as the complex number m[2k-1] + i m[2k] per bin (SURVEY A.4).
+        const float width = (float)cnt;
+        L.fl = 2 * lo * width / p.framerate;
+        L.fh = 2 * hi * width / p.framerate;
+        L.sc = 1.0f / ((float)cnt * (float)cnt);
+        if (s.n_filter && cnt != s.n_filter) s.one_length = false;
+        s.n_filter = s.n_filter ? s.n_filter : cnt;
+        s.n_max = std::max(s.n_max, cnt);
+    }
+    // Uniform lanes (every lane appends to the same slot and filters the same columns: always so for a handle whose
+    // lanes run in lock-step) take the kernels' scalar path; otherwise the kernels read the table.
+    s.uniform = plan.n_hold == 0;
+    for (int k = 1; k < lanes && s.uniform; ++k)
+        s.uniform = rows[k].append == rows[0].append && rows[k].n == rows[0].n && rows[k].sel == rows[0].sel;
+    return s;
+}
+
+// u8 frames of `vl` (virtual) lanes -> f32 planes g[0], and the Gaussian chain g[1 .. levels] (SpatialFilter.cpp:13-23)
+mc_status ColorMode::ingest(const ModeCtx& ctx, const FrameIO& io, int vl, const std::vector<float*>& g) {
+    dim3 grid(cdiv(w, 256), h, (unsigned)vl);
+    const bool pp = ctx.prof && ctx.prof->begin("u8_to_planes", 0, ctx.stream);
+    if (channels == 3) k_u8_to_planes<3><<<grid, 256, 0, ctx.stream>>>(io.in, io.in_step, io.in_lane_stride, w, h, g[0], lv[0].pitch, lv[0].plane);
+    else k_u8_to_planes<1><<<grid, 256, 0, ctx.stream>>>(io.in, io.in_step, io.in_lane_stride, w, h, g[0], lv[0].pitch, lv[0].plane);
+    if (pp) ctx.prof->end(ctx.stream);
+    MCK(cudaGetLastError());
+    ++*ctx.launches;
+    for (int l = 0; l < levels; ++l) {
+        LevelArgs a;
+        a.in_kind = 0; a.g = g[(size_t)l]; a.in_plane = lv[(size_t)l].plane; a.in_row = lv[(size_t)l].pitch;
+        a.channels = channels; a.lf = lv[(size_t)l]; a.lc = lv[(size_t)l + 1]; a.g_next = g[(size_t)l + 1];
+        a.planes = vl * channels; a.band = 0;
+        LAUNCH("gauss_down", l, launch_down(a, ctx.stream));
+    }
+    return MC_OK;
+}
+
+// The temporal part of one frame on the handle's ring: the append of its top Gaussian level `top` (rows: the frame's lane
+// table, d_rows its device copy), then the ideal band-pass (TemporalFilter.cpp:24-57) on the physical column order into
+// the window `win`, with the DFT length of each lane's window: one transform over all lanes when every filtering lane
+// has the same length, else one per lane.
+mc_status ColorMode::filter(const ModeCtx& ctx, const Step& s, const ColorLane* rows, const ColorLane* d_rows, const float* top,
+                            float* win) {
+    const Level& ls = lv[(size_t)levels];
+    const int C = channels, planes = lanes * C;
+    const size_t lane_sig = (size_t)C * small_rows;
+    const int pad = lanes > 1 ? (int)(lane_sig & 1) : 0;
+    const size_t lstride = lane_sig + pad, S = (size_t)lanes * lstride;
+    const ColorLane* tab = s.uniform ? nullptr : d_rows;
+    {
+        const bool pp = ctx.prof && ctx.prof->begin("ring_append", 0, ctx.stream);
+        k_ring_append<<<gs_blocks(S), 256, 0, ctx.stream>>>(top, ls.w, ls.h, ls.pitch, ls.plane, ring, S, pad, rows[0].append, planes, C, tab);
+        if (pp) ctx.prof->end(ctx.stream);
+        MCK(cudaGetLastError());
+        ++*ctx.launches;
+    }
+    if (s.n_filter == 0) return MC_OK;
+    if (plan_signals != S) {
+        for (auto& kv : plans) { cufftDestroy(kv.second.r2c); cufftDestroy(kv.second.c2r); }
+        plans.clear();
+        plan_signals = S;
+    }
+    auto exec = [&](bool r2c) -> mc_status {
+        for (int k = 0; k < (s.one_length ? 1 : lanes); ++k) {
+            const int n = s.one_length ? s.n_filter : rows[k].n;
+            if (n == 0) continue;
+            FftPlans* pl = nullptr;
+            MCK_ST(fft_plan(ctx, n, !s.one_length, &pl));
+            const size_t o = s.one_length ? 0 : (size_t)k * lstride;
+            const bool pp = ctx.prof && ctx.prof->begin(r2c ? "cufft_r2c" : "cufft_c2r", 0, ctx.stream);
+            if (r2c) CUFFT_CK(cufftExecR2C(pl->r2c, ring + o, spec + o));
+            else CUFFT_CK(cufftExecC2R(pl->c2r, spec + o, win + o));
+            if (pp) ctx.prof->end(ctx.stream);
+            ++*ctx.launches;
+        }
+        return MC_OK;
+    };
+    MCK_ST(exec(true));
+    {
+        const ColorLane& L = rows[0];   // the scalars of uniform lanes
+        const bool pp = ctx.prof && ctx.prof->begin("mask_mul", 0, ctx.stream);
+        k_mask_mul<<<gs_blocks(S * (size_t)(s.n_max / 2 + 1)), 256, 0, ctx.stream>>>((float2*)spec, S, s.n_max / 2 + 1, L.n, L.fl, L.fh, L.sc,
+                                                                                      tab, lstride);
+        if (pp) ctx.prof->end(ctx.stream);
+        MCK(cudaGetLastError());
+        ++*ctx.launches;
+    }
+    return exec(false);
+}
+
+// Everything after the filter, over `vl` (virtual) lanes: frame v / lanes of virtual lane v reads its filtered window at
+// win + (v / lanes) * win_stride.  row0: the scalars of uniform lanes (tab null); mm: 4 * vl slots.
+mc_status ColorMode::reconstruct(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int vl, const ColorLane& row0,
+                                 const ColorLane* tab, const std::vector<float*>& g, const std::vector<float*>& u, const float* win,
+                                 size_t win_stride, unsigned* mm, int fout_v0) {
+    const Level& ls = lv[(size_t)levels];
+    const int C = channels, vplanes = vl * C;
+    const size_t lane_sig = (size_t)C * small_rows;
+    const int pad = lanes > 1 ? (int)(lane_sig & 1) : 0;
+    const size_t S = (size_t)lanes * (lane_sig + pad);
+    k_mm_init<<<cdiv(4 * vl, 256), 256, 0, ctx.stream>>>(mm, 4 * vl);
+    MCK(cudaGetLastError());
+    ++*ctx.launches;
+    {
+        // global min/max per stream over all pixels, frames and channels (TemporalFilter.cpp:55)
+        const size_t chunk = lane_sig;
+        const int vec_ok = chunk % 4 == 0 && S % 4 == 0 && win_stride % 4 == 0 && (reinterpret_cast<uintptr_t>(win) & 15) == 0;
+        dim3 grid((unsigned)std::max<size_t>(1, std::min<size_t>(chunk / 1024 + 1, (size_t)(592 / vl + 1))), (unsigned)vl);
+        const bool pp = ctx.prof && ctx.prof->begin("minmax_window", 0, ctx.stream);
+        k_minmax<<<grid, 256, 0, ctx.stream>>>(win, chunk, row0.n, S, mm, vec_ok, pad, tab, lanes, win_stride);
+        if (pp) ctx.prof->end(ctx.stream);
+        MCK(cudaGetLastError());
+        ++*ctx.launches;
+    }
+    {
+        const bool pp = ctx.prof && ctx.prof->begin("select", 0, ctx.stream);
+        k_select<<<gs_blocks((size_t)(vl / lanes) * S), 256, 0, ctx.stream>>>(win, S, pad, row0.sel, mm, C, ls.w, ls.h, (float)p.amplification,
+                                                                              u[0], ulv[0].pitch, ulv[0].plane, vplanes, tab, lanes,
+                                                                              win_stride - S);
+        if (pp) ctx.prof->end(ctx.stream);
+        MCK(cudaGetLastError());
+        ++*ctx.launches;
+    }
+    // pyrUp chain with default 2x sizes, then bilinear resize to the frame size (SpatialFilter.cpp:40-50)
+    for (int i = 0; i < levels; ++i) {
+        const Level& s0 = ulv[(size_t)i];
+        const Level& d0 = ulv[(size_t)i + 1];
+        dim3 grid(cdiv(d0.w, 64), cdiv(d0.h, 32), (unsigned)vplanes);
+        const bool pp = ctx.prof && ctx.prof->begin("pyrup2x", i, ctx.stream);
+        k_pyrup2x<<<grid, 256, 0, ctx.stream>>>(s0, d0, u[(size_t)i], u[(size_t)i + 1], tab, C);
+        if (pp) ctx.prof->end(ctx.stream);
+        MCK(cudaGetLastError());
+        ++*ctx.launches;
+    }
+    const float* color_img = u[(size_t)levels];
+    if (u[(size_t)levels + 1]) {
+        dim3 grid(cdiv(w, 256), h, (unsigned)vplanes);
+        const bool pp = ctx.prof && ctx.prof->begin("resize", 0, ctx.stream);
+        k_resize_linear<<<grid, 256, 0, ctx.stream>>>(ulv[(size_t)levels], lv[0], u[(size_t)levels], u[(size_t)levels + 1], tab, C);
+        if (pp) ctx.prof->end(ctx.stream);
+        MCK(cudaGetLastError());
+        ++*ctx.launches;
+        color_img = u[(size_t)levels + 1];
+    }
+    {
+        dim3 grid((unsigned)std::max(1, std::min(C * h, 1184 / vl + 1)), (unsigned)vl);
+        const bool pp = ctx.prof && ctx.prof->begin("minmax_out", 0, ctx.stream);
+        k_sum_minmax<<<grid, 256, 0, ctx.stream>>>(g[0], color_img, lv[0], C, mm + 2 * vl, tab);
+        if (pp) ctx.prof->end(ctx.stream);
+        MCK(cudaGetLastError());
+        ++*ctx.launches;
+    }
+    {
+        dim3 grid(cdiv(w, 256), h, (unsigned)vl);
+        const bool pp = ctx.prof && ctx.prof->begin("color_egress", 0, ctx.stream);
+        if (C == 3) k_color_egress<3><<<grid, 256, 0, ctx.stream>>>(g[0], color_img, lv[0], mm + 2 * vl, io.out, io.out_step, io.out_lane_stride, ctx.float_out, fout_v0, tab);
+        else k_color_egress<1><<<grid, 256, 0, ctx.stream>>>(g[0], color_img, lv[0], mm + 2 * vl, io.out, io.out_step, io.out_lane_stride, ctx.float_out, fout_v0, tab);
+        if (pp) ctx.prof->end(ctx.stream);
+        MCK(cudaGetLastError());
+        ++*ctx.launches;
+    }
+    return MC_OK;
+}
+
+mc_status ColorMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int nlevels, int* produced, int frames) {
     *produced = 0;
     const int want_cap = optimal_buffer_size((int)p.framerate);  // MagnifyCore.hpp:176
     const int C = io.channels;
@@ -438,45 +663,29 @@ mc_status ColorMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_par
     const bool grow = ring == nullptr || ring_cap < need;
     const bool relayout = (grow || rotate) && has_data;
 
-    // append to the rolling window; once full drop the oldest column (SpatialFilter.cpp:63-84).  Then the filter's
-    // operands: a lane's signal is physical slots [0, n) (warming: head 0; full: n == mod), so n alone picks its DFT.
-    const double lo = p.coLow == 0.0 ? p.coLow + 0.01 : p.coLow, hi = p.coHigh;   // TemporalFilter.cpp:26-27
-    int n_filter = 0, n_max = 0;
-    bool one_length = true;
-    for (int k = 0; k < lanes; ++k) {
-        ColorLane& L = table[(size_t)k];
-        int& cnt = count[(size_t)k];
-        int& hd = head[(size_t)k];
-        L.append = -1; L.n = 0; L.sel = -1; L.sc = 0.f; L.fl = L.fh = 0.0;
-        if (plan.op[(size_t)k] == LANE_HOLD) continue;
-        L.append = (hd + cnt) % mod[(size_t)k];
-        ++cnt;
-        if (cnt > want_cap && want_cap > 0) {
-            hd = (hd + 1) % mod[(size_t)k];
-            --cnt;
-        }
-        if (cnt < 2) continue;  // MagnifyCore.hpp:180 (passthrough)
-        L.n = cnt;
-        L.sel = (hd + std::min(1, cnt - 1)) % mod[(size_t)k];   // the reconstructed column is logical min(1, n-1) (:189-192)
-        // createIdealBandpassFilter (TemporalFilter.cpp:59-80): real 0/1 mask over packed indices x, read back by
-        // mulSpectrums as the complex number m[2k-1] + i m[2k] per bin (SURVEY A.4).
-        const float width = (float)cnt;
-        L.fl = 2 * lo * width / p.framerate;
-        L.fh = 2 * hi * width / p.framerate;
-        L.sc = 1.0f / ((float)cnt * (float)cnt);
-        if (n_filter && cnt != n_filter) one_length = false;
-        n_filter = n_filter ? n_filter : cnt;
-        n_max = std::max(n_max, cnt);
+    // The append and filter rules, frame by frame: a frame call's rows are `table`, a clip's the rows of every virtual
+    // lane.  The clip's restarts and ring geometry are those of its first frame; with constant params a lane's logical
+    // ring size cannot change after that (its window grows to the cap or, above a lowered cap, keeps its length).
+    const int vl = frames * lanes;
+    const size_t win_stride = ((size_t)need * S + 63) / 64 * 64;   // a clip's filtered windows, 256-byte aligned
+    ColorLane* rows = table.data();
+    Step s1;
+    if (frames > 1) {
+        MCK_ST(alloc_clip(ctx, vl, (size_t)frames * win_stride));
+        clip.table.assign((size_t)vl, ColorLane{});
+        clip.steps.assign((size_t)frames, Step{});
+        std::copy(table.begin(), table.end(), clip.table.begin());   // frame 0's relayout fields
+        rows = clip.table.data();
     }
-    // Uniform lanes (every lane appends to the same slot and filters the same columns: always so for a handle whose
-    // lanes run in lock-step) take the kernels' scalar path; otherwise the kernels read the table.
-    bool uniform = plan.n_hold == 0;
-    for (int k = 1; k < lanes && uniform; ++k)
-        uniform = table[(size_t)k].append == table[0].append && table[(size_t)k].n == table[0].n && table[(size_t)k].sel == table[0].sel;
-    const ColorLane* tab = uniform ? nullptr : d_table;
+    for (int t = 0; t < frames; ++t) {
+        for (int k = 0; t > 0 && k < lanes; ++k)
+            assert(plan.op[(size_t)k] == LANE_HOLD || std::max(std::max(want_cap, count[(size_t)k]), 2) == mod[(size_t)k]);
+        (frames > 1 ? clip.steps[(size_t)t] : s1) = step(p, want_cap, rows + (size_t)t * lanes);
+    }
+    ColorLane* dtab = frames > 1 ? clip.d_table : d_table;
     // pageable source: staged before the call returns; stream-ordered after the previous frame's kernels read the table
-    if (relayout || !uniform)
-        MCK(cudaMemcpyAsync(d_table, table.data(), sizeof(ColorLane) * (size_t)lanes, cudaMemcpyHostToDevice, ctx.stream));
+    if (frames > 1 || relayout || !s1.uniform)
+        MCK(cudaMemcpyAsync(dtab, rows, sizeof(ColorLane) * (size_t)vl, cudaMemcpyHostToDevice, ctx.stream));
 
     if (grow || rotate) {
         float* dst = work;
@@ -489,7 +698,7 @@ mc_status ColorMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_par
         }
         if (relayout) {
             const bool pp = ctx.prof && ctx.prof->begin("ring_relayout", 0, ctx.stream);
-            k_ring_relayout<<<dim3(gs_blocks(lane_sig), (unsigned)lanes), 256, 0, ctx.stream>>>(ring, dst, S, lane_sig, lstride, d_table);
+            k_ring_relayout<<<dim3(gs_blocks(lane_sig), (unsigned)lanes), 256, 0, ctx.stream>>>(ring, dst, S, lane_sig, lstride, dtab);
             if (pp) ctx.prof->end(ctx.stream);
             MCK(cudaGetLastError());
             ++*ctx.launches;
@@ -505,130 +714,38 @@ mc_status ColorMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_par
         }
     }
 
-    // ingest + Gaussian chain (SpatialFilter.cpp:13-23)
-    {
-        dim3 grid(cdiv(w, 256), h, lanes);
-        if (C == 3) { const bool pp = ctx.prof && ctx.prof->begin("u8_to_planes", 0, ctx.stream); k_u8_to_planes<3><<<grid, 256, 0, ctx.stream>>>(io.in, io.in_step, io.in_lane_stride, w, h, G[0], lv[0].pitch, lv[0].plane); if (pp) ctx.prof->end(ctx.stream); }
-        else { const bool pp = ctx.prof && ctx.prof->begin("u8_to_planes", 0, ctx.stream); k_u8_to_planes<1><<<grid, 256, 0, ctx.stream>>>(io.in, io.in_step, io.in_lane_stride, w, h, G[0], lv[0].pitch, lv[0].plane); if (pp) ctx.prof->end(ctx.stream); }
-        MCK(cudaGetLastError());
-        ++*ctx.launches;
-    }
-    for (int l = 0; l < levels; ++l) {
-        LevelArgs a;
-        a.in_kind = 0; a.g = G[(size_t)l]; a.in_plane = lv[(size_t)l].plane; a.in_row = lv[(size_t)l].pitch;
-        a.channels = C; a.lf = lv[(size_t)l]; a.lc = lv[(size_t)l + 1]; a.g_next = G[(size_t)l + 1];
-        a.planes = planes; a.band = 0;
-        LAUNCH("gauss_down", l, launch_down(a, ctx.stream));
-    }
-    const Level& ls = lv[(size_t)levels];
-    {
-        const bool pp = ctx.prof && ctx.prof->begin("ring_append", 0, ctx.stream);
-        k_ring_append<<<gs_blocks(S), 256, 0, ctx.stream>>>(G[(size_t)levels], ls.w, ls.h, ls.pitch, ls.plane, ring, S, pad, table[0].append, planes, C, tab);
-        if (pp) ctx.prof->end(ctx.stream);
-        MCK(cudaGetLastError());
-        ++*ctx.launches;
-    }
-    if (n_filter == 0) return MC_OK;
-
-    // ideal temporal band-pass (TemporalFilter.cpp:24-57) on the physical column order, with the DFT length of each
-    // lane's window: one transform over all lanes when every filtering lane has the same length, else one per lane
-    if (plan_signals != S) {
-        for (auto& kv : plans) { cufftDestroy(kv.second.r2c); cufftDestroy(kv.second.c2r); }
-        plans.clear();
-        plan_signals = S;
-    }
-    auto exec = [&](bool r2c) -> mc_status {
-        for (int k = 0; k < (one_length ? 1 : lanes); ++k) {
-            const int n = one_length ? n_filter : table[(size_t)k].n;
-            if (n == 0) continue;
-            FftPlans* pl = nullptr;
-            MCK_ST(fft_plan(ctx, n, !one_length, &pl));
-            const size_t o = one_length ? 0 : (size_t)k * lstride;
-            const bool pp = ctx.prof && ctx.prof->begin(r2c ? "cufft_r2c" : "cufft_c2r", 0, ctx.stream);
-            if (r2c) CUFFT_CK(cufftExecR2C(pl->r2c, ring + o, spec + o));
-            else CUFFT_CK(cufftExecC2R(pl->c2r, spec + o, work + o));
-            if (pp) ctx.prof->end(ctx.stream);
-            ++*ctx.launches;
-        }
+    if (frames == 1) {
+        tap_frame = -1;
+        MCK_ST(ingest(ctx, io, lanes, G));
+        MCK_ST(filter(ctx, s1, rows, d_table, G[(size_t)levels], work));
+        if (s1.n_filter == 0) return MC_OK;
+        MCK_ST(reconstruct(ctx, io, p, lanes, table[0], s1.uniform ? nullptr : d_table, G, U, work, S, (unsigned*)minmax, 0));
+        for (int k = 0; k < lanes; ++k) ctx.lane_produced[(size_t)k] = table[(size_t)k].n > 0 ? 1 : 0;
+        *produced = 1;
         return MC_OK;
-    };
-    MCK_ST(exec(true));
-    {
-        const ColorLane& L = table[0];   // the scalars of uniform lanes
-        const bool pp = ctx.prof && ctx.prof->begin("mask_mul", 0, ctx.stream);
-        k_mask_mul<<<gs_blocks(S * (size_t)(n_max / 2 + 1)), 256, 0, ctx.stream>>>((float2*)spec, S, n_max / 2 + 1, L.n, L.fl, L.fh, L.sc,
-                                                                                    tab, lstride);
-        if (pp) ctx.prof->end(ctx.stream);
-        MCK(cudaGetLastError());
-        ++*ctx.launches;
     }
-    MCK_ST(exec(false));
-    unsigned* mm = (unsigned*)minmax;
-    k_mm_init<<<cdiv(4 * lanes, 256), 256, 0, ctx.stream>>>(mm, 4 * lanes);
-    MCK(cudaGetLastError());
-    ++*ctx.launches;
-    {
-        // global min/max per stream over all pixels, frames and channels (TemporalFilter.cpp:55)
-        const size_t chunk = lane_sig;
-        const int vec_ok = chunk % 4 == 0 && S % 4 == 0 && (reinterpret_cast<uintptr_t>(work) & 15) == 0;
-        dim3 grid((unsigned)std::max<size_t>(1, std::min<size_t>(chunk / 1024 + 1, (size_t)(592 / lanes + 1))), lanes);
-        const bool pp = ctx.prof && ctx.prof->begin("minmax_window", 0, ctx.stream);
-        k_minmax<<<grid, 256, 0, ctx.stream>>>(work, chunk, table[0].n, S, mm, vec_ok, pad, tab);
-        if (pp) ctx.prof->end(ctx.stream);
-        MCK(cudaGetLastError());
-        ++*ctx.launches;
+
+    // A clip: the per-frame kernels once over every virtual lane, the temporal part frame by frame on the ring exactly as
+    // frame calls run it (same plans, operands and layout), each frame's filtered window kept for the kernels after it.
+    tap_frame = frames - 1;
+    clip.win_stride = win_stride;
+    MCK_ST(ingest(ctx, io, vl, clip.G));
+    const Level& ls = lv[(size_t)levels];
+    bool any = false;
+    for (int t = 0; t < frames; ++t) {
+        const Step& s = clip.steps[(size_t)t];
+        MCK_ST(filter(ctx, s, rows + (size_t)t * lanes, dtab + (size_t)t * lanes, clip.G[(size_t)levels] + (size_t)t * planes * ls.plane,
+                      clip.work + (size_t)t * win_stride));
+        any |= s.n_filter > 0;
     }
-    {
-        const bool pp = ctx.prof && ctx.prof->begin("select", 0, ctx.stream);
-        k_select<<<gs_blocks(S), 256, 0, ctx.stream>>>(work, S, pad, table[0].sel, mm, C, ls.w, ls.h, (float)p.amplification, U[0], ulv[0].pitch, ulv[0].plane, planes, tab);
-        if (pp) ctx.prof->end(ctx.stream);
-        MCK(cudaGetLastError());
-        ++*ctx.launches;
-    }
-    // pyrUp chain with default 2x sizes, then bilinear resize to the frame size (SpatialFilter.cpp:40-50)
-    for (int i = 0; i < levels; ++i) {
-        const Level& s0 = ulv[(size_t)i];
-        const Level& d0 = ulv[(size_t)i + 1];
-        dim3 grid(cdiv(d0.w, 64), cdiv(d0.h, 32), planes);
-        const bool pp = ctx.prof && ctx.prof->begin("pyrup2x", i, ctx.stream);
-        k_pyrup2x<<<grid, 256, 0, ctx.stream>>>(s0, d0, U[(size_t)i], U[(size_t)i + 1], tab, C);
-        if (pp) ctx.prof->end(ctx.stream);
-        MCK(cudaGetLastError());
-        ++*ctx.launches;
-    }
-    const float* color_img = U[(size_t)levels];
-    if (U[(size_t)levels + 1]) {
-        dim3 grid(cdiv(w, 256), h, planes);
-        const bool pp = ctx.prof && ctx.prof->begin("resize", 0, ctx.stream);
-        k_resize_linear<<<grid, 256, 0, ctx.stream>>>(ulv[(size_t)levels], lv[0], U[(size_t)levels], U[(size_t)levels + 1], tab, C);
-        if (pp) ctx.prof->end(ctx.stream);
-        MCK(cudaGetLastError());
-        ++*ctx.launches;
-        color_img = U[(size_t)levels + 1];
-    }
-    {
-        dim3 grid((unsigned)std::max(1, std::min(C * h, 1184 / lanes + 1)), lanes);
-        const bool pp = ctx.prof && ctx.prof->begin("minmax_out", 0, ctx.stream);
-        k_sum_minmax<<<grid, 256, 0, ctx.stream>>>(G[0], color_img, lv[0], C, mm + 2 * lanes, tab);
-        if (pp) ctx.prof->end(ctx.stream);
-        MCK(cudaGetLastError());
-        ++*ctx.launches;
-    }
-    {
-        dim3 grid(cdiv(w, 256), h, lanes);
-        const bool pp = ctx.prof && ctx.prof->begin("color_egress", 0, ctx.stream);
-        if (C == 3) k_color_egress<3><<<grid, 256, 0, ctx.stream>>>(G[0], color_img, lv[0], mm + 2 * lanes, io.out, io.out_step, io.out_lane_stride, ctx.float_out, tab);
-        else k_color_egress<1><<<grid, 256, 0, ctx.stream>>>(G[0], color_img, lv[0], mm + 2 * lanes, io.out, io.out_step, io.out_lane_stride, ctx.float_out, tab);
-        if (pp) ctx.prof->end(ctx.stream);
-        MCK(cudaGetLastError());
-        ++*ctx.launches;
-    }
-    for (int k = 0; k < lanes; ++k) ctx.lane_produced[(size_t)k] = table[(size_t)k].n > 0 ? 1 : 0;
-    *produced = 1;
+    if (any) MCK_ST(reconstruct(ctx, io, p, vl, rows[0], dtab, clip.G, clip.U, clip.work, win_stride, clip.minmax, vl - lanes));
+    for (int v = 0; v < vl; ++v) ctx.lane_produced[(size_t)v] = rows[v].n > 0 ? 1 : 0;
+    *produced = any ? 1 : 0;
+    std::copy(rows + (size_t)(vl - lanes), rows + vl, table.begin());   // the taps read the last frame's rows
     return MC_OK;
 }
 
-// Read-only taps on the buffers of the last frame call (include/magcore_b200.h, at mc_get_state).  A column of "window" or
+// Read-only taps on the buffers of the last frame call or of a clip's last frame (include/magcore_b200.h, at mc_get_state).  A column of "window" or
 // "filtered" is served only while every lane has it, "filtered" and "up" only while every lane ran the filter.
 void ColorMode::find_state(const char* name, int level, StateRef& out) {
     out = StateRef{};
@@ -640,14 +757,18 @@ void ColorMode::find_state(const char* name, int level, StateRef& out) {
     }
     const std::string nm(name);
     out.channels = channels; out.read_only = true;
+    // after a clip the per-frame planes are its last frame's in the clip scratch
+    auto frame_planes = [&](const std::vector<float*>& own, const std::vector<float*>& clipped, int l, const Level& lvl) {
+        return tap_frame < 0 ? own[(size_t)l] : clipped[(size_t)l] + (size_t)tap_frame * lanes * channels * lvl.plane;
+    };
     auto planes_of = [&](float* p, const Level& l) {
         out.ptr = p; out.rows = l.h; out.cols = l.w; out.pitch = l.pitch; out.plane_stride = l.plane;
     };
     if (nm == "gauss") {
-        if (level <= levels && *std::max_element(count.begin(), count.end()) > 0) planes_of(G[(size_t)level], lv[(size_t)level]);
+        if (level <= levels && *std::max_element(count.begin(), count.end()) > 0) planes_of(frame_planes(G, clip.G, level, lv[(size_t)level]), lv[(size_t)level]);
     } else if (nm == "up") {
-        if (filt >= 2 && level <= levels) planes_of(U[(size_t)level], ulv[(size_t)level]);
-        else if (filt >= 2 && level == levels + 1 && U[(size_t)level]) planes_of(U[(size_t)level], lv[0]);
+        if (filt >= 2 && level <= levels) planes_of(frame_planes(U, clip.U, level, ulv[(size_t)level]), ulv[(size_t)level]);
+        else if (filt >= 2 && level == levels + 1 && U[(size_t)level]) planes_of(frame_planes(U, clip.U, level, lv[0]), lv[0]);
     } else if (nm == "window" || nm == "filtered") {
         const bool win = nm == "window";
         if (level >= (win ? have : filt)) return;
@@ -655,7 +776,7 @@ void ColorMode::find_state(const char* name, int level, StateRef& out) {
         // followed by one padding float (process()); logical column `level` of a lane is its slot (head + level) % mod
         const Level& ls = lv[(size_t)levels];
         const size_t lane_sig = (size_t)channels * small_rows, lstride = lane_sig + (lanes > 1 ? (lane_sig & 1) : 0);
-        out.ptr = win ? ring : work;
+        out.ptr = win ? ring : tap_frame < 0 ? work : clip.work + (size_t)tap_frame * clip.win_stride;
         out.rows = ls.h; out.cols = ls.w; out.pitch = ls.w; out.plane_stride = (size_t)small_rows;
         for (int k = 0; k < lanes; ++k)
             out.lane_off.push_back((size_t)((head[(size_t)k] + level) % mod[(size_t)k]) * lanes * lstride + (size_t)k * lstride);

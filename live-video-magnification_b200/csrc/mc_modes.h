@@ -304,13 +304,45 @@ struct ColorMode {
     size_t fft_work_bytes = 0;
     DeviceArena arena;
     LanePlan plan;                   // per-lane ops of the current frame
+    int tap_frame = -1;              // the taps' frame in the clip scratch (the last clip's last frame); -1: the frame planes
+
+    // What one frame's rows of the lane table ask of the filter
+    struct Step {
+        int n_filter = 0, n_max = 0;   // the first and the largest DFT length of a filtering lane (0: no lane filters)
+        bool one_length = true;        // every filtering lane has the same length: one transform over all lanes
+        bool uniform = true;           // every lane appends to the same slot and filters the same columns (scalar path)
+    };
+
+    // Scratch of the clip path: the per-frame planes of `cap` virtual lanes (frame t of lane k is virtual lane
+    // t * lanes + k), one filtered window per frame, and the lane table of every virtual lane.  The window ring stays the
+    // mode's own, so clip and frame calls interleave.
+    struct Clip : ClipScratch {
+        std::vector<float*> G, U;         // the Gaussian chain and the up chain (+ resized plane) of every virtual lane
+        float* work = nullptr;            // frame t's filtered window at work + t * win_stride
+        size_t work_floats = 0, win_stride = 0;
+        unsigned* minmax = nullptr;       // per virtual lane: window min / max, then output min / max
+        ColorLane* d_table = nullptr;
+        std::vector<ColorLane> table;     // host rows, [t][lane]
+        std::vector<Step> steps;          // per frame
+    } clip;
 
     void reset();
-    mc_status process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced);
+    // frames > 1: `frames` consecutive frames of every lane ([t][lane] in io's lane stride); ctx.lane_produced then
+    // holds frames * lanes flags
+    mc_status process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced, int frames = 1);
     void find_state(const char* name, int level, StateRef& out);
 
 private:
     mc_status fft_plan(const ModeCtx& ctx, int n, bool one_lane, FftPlans** out);
+    mc_status alloc_clip(const ModeCtx& ctx, int vlanes, size_t work_floats);
+    // the append and filter rules of one frame: writes its `lanes` rows of a lane table, moves count / head
+    Step step(const mc_params& p, int want_cap, ColorLane* rows);
+    // the launch sets shared by the frame and the clip path, over `vl` (virtual) lanes
+    mc_status ingest(const ModeCtx& ctx, const FrameIO& io, int vl, const std::vector<float*>& g);
+    mc_status filter(const ModeCtx& ctx, const Step& s, const ColorLane* rows, const ColorLane* d_rows, const float* top, float* win);
+    mc_status reconstruct(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int vl, const ColorLane& row0, const ColorLane* tab,
+                          const std::vector<float*>& g, const std::vector<float*>& u, const float* win, size_t win_stride,
+                          unsigned* mm, int fout_v0);
 };
 
 struct RieszMode {

@@ -16,7 +16,11 @@ UI amplification 50, wavelength 50, 0.4-3 Hz @30fps, timed the same way.  Report
 times, the phase kernels' bytes per frame counted from shapes, and the clip scratch per frame.  A Phase handle's first
 frame passes through, so only the handle's first frame is allowed not to produce.
 
-    python tools/bench_clip.py [--mode laplace|phase] [--seconds 1.0] [--rounds 3] [--out result.json]
+With --mode color / color6 the workload is tools/mode_bench.py's `color` / `color6` config: Color 1920x1080x3, 3 / 6
+levels, UI amplification 100, 0.8-1.2 Hz @30fps (a 64-frame window).  Every handle is first fed past 64 frames, so the
+timed frames run with a full window.  Reported as for Phase, with the Color clip scratch per frame counted from shapes.
+
+    python tools/bench_clip.py [--mode laplace|phase|color|color6] [--seconds 1.0] [--rounds 3] [--out result.json]
 """
 import argparse
 import ctypes as C
@@ -85,6 +89,26 @@ def phase_clip_scratch_bytes():
     return 4 * floats + 2 * 3 * H * ((W + 63) // 64 * 64)
 
 
+COLOR_WORKLOAD = "Color 1920x1080x3 BGR, {} levels, UI amplification 100, 0.8-1.2 Hz @30fps (window 64)"
+
+
+def color_clip_scratch_bytes(levels, window=64):
+    """Device scratch of a Color clip per frame of one lane (ColorMode::Clip): the Gaussian chain (levels 0 .. L) and the
+    up chain (L + 1 planes, + the resized plane when the chain misses the frame size) as pitched f32 planes, the frame's
+    filtered window (`window` columns of the smallest level), its 4 min / max slots and its 40-byte lane table row."""
+    sizes = [(W, H)]
+    for _ in range(levels):
+        sizes.append(((sizes[-1][0] + 1) // 2, (sizes[-1][1] + 1) // 2))
+    plane = lambda w, h: h * ((w + 31) // 32 * 32)
+    sw, sh = sizes[-1]
+    up = [(sw << i, sh << i) for i in range(levels + 1)]
+    floats = CH * (sum(plane(w, h) for w, h in sizes) + sum(plane(w, h) for w, h in up))
+    if up[-1] != (W, H):
+        floats += CH * plane(W, H)
+    floats += window * CH * sw * sh
+    return 4 * floats + 16 + 40
+
+
 def card():
     try:
         r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -100,9 +124,11 @@ def main():
     ap.add_argument("--seconds", type=float, default=1.0, help="least length of one timed window")
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--out", default=None, help="also write the JSON result here")
-    ap.add_argument("--mode", choices=["laplace", "phase"], default="laplace")
+    ap.add_argument("--mode", choices=["laplace", "phase", "color", "color6"], default="laplace")
     args = ap.parse_args()
-    phase = args.mode == "phase"
+    color = args.mode.startswith("color")
+    color_levels = 6 if args.mode == "color6" else 3
+    phase = args.mode == "phase" or color   # reported the same way
 
     import torch
     import lvm_b200 as L
@@ -111,7 +137,9 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_clip.py needs an H100: the magnification core has no CPU fallback")
     p = capi.McParams()
-    if phase:
+    if color:
+        capi.lib().mc_params_from_ui(C.byref(p), capi.MODE_COLOR, 100, 0.0, 0.8, 1.2, 0, color_levels, 30.0)
+    elif phase:
         capi.lib().mc_params_from_ui(C.byref(p), capi.MODE_PHASE, *PHASE_UI)
     else:
         capi.lib().mc_params_from_ui(C.byref(p), capi.MODE_LAPLACE, UI["amplification"], UI["wavelength"], UI["low"], UI["high"],
@@ -128,7 +156,7 @@ def main():
             self.stream = torch.cuda.ExternalStream(self.proc.stream)
             self.out = torch.empty_like(d_in)
             self.fps = []
-            self.fresh = phase   # Phase: the handle's first frame passes through
+            self.fresh = phase   # Phase and Color: the handle's first frame passes through
 
         def step(self):
             """the N-frame sequence once"""
@@ -157,10 +185,12 @@ def main():
             return e0.elapsed_time(e1) * 1e-3
 
     methods = [Method("frame", 1)] + [Method("clip", t) for t in TS] + [Method("lanes", 1, lanes=t) for t in TS]
-    # warm-up of every shape, then the number of passes that makes the slowest window >= --seconds
+    # warm-up of every shape (Color: past its 64-frame window), then the number of passes that makes the slowest window
+    # >= --seconds
     steps = 1
     for m in methods:
-        m.step()
+        for _ in range(3 if color else 1):
+            m.step()
         torch.cuda.synchronize()
         steps = max(steps, math.ceil(args.seconds / m.time(1)))
     for _ in range(args.rounds):
@@ -177,7 +207,7 @@ def main():
         pr = L.MagnificationProcessor(0)
         pr.set_option("profile_kernels", 1)
         o = torch.empty_like(d_in)
-        for _ in range(2):
+        for _ in range(3 if color else 2):
             for i in range(0, N, t_frames):
                 if t_frames == 1:
                     pr.process_device(base + i * frame_bytes, W, H, CH, row, p, o.data_ptr() + i * frame_bytes, row)
@@ -194,6 +224,15 @@ def main():
             rates[key] = {"fps": round(statistics.median(m.fps), 1), "fps_rounds": [round(x, 1) for x in m.fps]}
         px, frame_b, _ = phase_counted_bytes(1)
         result = {
+            "workload": COLOR_WORKLOAD.format(color_levels) + ", one stream, frames in HBM",
+            "card": card(),
+            "unit": "frames/s (device-resident, CUDA events on the handle's stream, median of rounds)",
+            "window_s_min": args.seconds, "passes_per_window": steps, "frames_per_pass": N,
+            "rates": rates,
+            "bit_equal_to_frame_calls": equal,
+            "clip_scratch_MB_per_frame": round(color_clip_scratch_bytes(color_levels) / 1e6, 1),
+            "kernel_us_per_frame": kernels,
+        } if color else {
             "workload": PHASE_WORKLOAD + ", one stream, frames in HBM",
             "card": card(),
             "unit": "frames/s (device-resident, CUDA events on the handle's stream, median of rounds)",

@@ -124,6 +124,10 @@ def main():
          "k_chain_front<BGR, gray, NV12, YUYV, UYVY>: no local memory (STL / LDL)")
     fspills = clip_spills("k_chain_front", "mc_preprocess")
     need(len(fspills) == 5 and all(s == (0, 0) for s in fspills.values()), f"k_chain_front<*>: no spills (ptxas -v, {len(fspills)} instances)")
+    # the Color kernels that read virtual lanes (frame calls and clips): k_minmax, k_select, k_color_egress<1, 3>
+    cspills = {k: s for name in ("k_minmax", "k_select", "k_color_egress") for k, s in clip_spills(name, "mc_color").items()}
+    need(len(cspills) == 4 and all(s == (0, 0) for s in cspills.values()),
+         f"k_minmax, k_select, k_color_egress<*>: no spills (ptxas -v, {len(cspills)} instances)")
     rz = [k for k in body if k.startswith("k_riesz_egress") or "k_riesz_egress(" in k]
     # the select is either an FSEL per channel or a saturate predicated on the NaN test over a preset 1.0
     nan_sel = lambda k: count(k, "FSEL") + count(k, r"@!P\d FADD\.SAT")
