@@ -390,19 +390,16 @@ void* mc_stream(mc_handle* h);
  *   "pipeline_depth"  (default 3)
  *   "keep_float_output" (default 0): keep the pre-quantisation float image (tests)
  *   "profile_kernels" (default 0): see mc_profile_read
- *   "use_tma" (default 1): stage the fused level kernel's tiles with TMA (cp.async.bulk.tensor); 0 selects
- *        the 128-bit LDG staging path (same results; kept for A/B measurements)
- *   "prefetch_state" (default 1; needs use_tma): the fused level kernel requests the tile's two state planes as TMA
- *        bulk copies at kernel entry, together with its input window, instead of loading them in its last phase
- *        (same results; 0 kept for A/B measurements)
+ *   "use_tma" (default 1): stage the fused level kernel's tiles with TMA (cp.async.bulk.tensor): its input window and
+ *        the tile's two state planes are requested at kernel entry; 0 selects the 128-bit LDG staging path that also
+ *        runs when a tensor map cannot be encoded (same results)
  *   "lane_groups" (default 0 = automatic: min(2, lanes / 8), at least 1): Laplace — the lanes of the handle run as
  *        that many concurrent launch chains on separate CUDA streams, forked from and joined into mc_stream(); the
  *        L1-bound ingest, issue-bound egress and HBM-bound level kernels of different groups then share the SMs
  *        instead of running back to back (same results; profile_kernels forces 1)
- *   "egress_strip" (default 16): Laplace egress runs as the shuffle strip kernel (one warp per 128-column strip,
- *        sliding windows in per-lane shared-memory rings; the value 16 / 20 / 24 picks the register cap = resident
- *        warps per SM, 1 means the default); 0 selects the shared-memory tile kernel (bit-identical results; kept for A/B)
- *   "ingest_warps" (default 1): warps per CTA (1, 2 or 4) of the fused BGR->Lab ingest kernel (same results; A/B)
+ *   "egress_strip" (default 1): Laplace egress runs as the shuffle strip kernel (one warp per 128-column strip,
+ *        sliding windows in per-lane shared-memory rings); 0 selects the shared-memory tile kernel, the reference the
+ *        strip kernel is tested against (bit-identical results); any non-zero value selects the strip kernel
  *   "analysis_only" (default 0): Laplace and Phase — frames after the first update the temporal state (EMA planes;
  *        Riesz pyramids, phase accumulators and Butterworth registers) but skip synthesis and egress and report
  *        *produced = 0; the cheap first pass of temporal sharding (SURVEY 8f-3)

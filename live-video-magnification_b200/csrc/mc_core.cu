@@ -611,10 +611,8 @@ mc_status mc_set_option(mc_handle* h, const char* key, int value) try {
     if (!std::strcmp(key, "keep_float_output")) { o.keep_float_output = value != 0; return MC_OK; }
     if (!std::strcmp(key, "profile_kernels")) { o.profile_kernels = value != 0; return MC_OK; }
     if (!std::strcmp(key, "use_tma")) { o.use_tma = value != 0; return MC_OK; }
-    if (!std::strcmp(key, "prefetch_state")) { o.prefetch_state = value != 0; return MC_OK; }
     if (!std::strcmp(key, "lane_groups")) { o.lane_groups = value < 0 ? 0 : value; return MC_OK; }
-    if (!std::strcmp(key, "egress_strip")) { o.egress_strip = value == 1 ? 16 : value; return MC_OK; }
-    if (!std::strcmp(key, "ingest_warps")) { o.ingest_warps = value; return MC_OK; }
+    if (!std::strcmp(key, "egress_strip")) { o.egress_strip = value != 0; return MC_OK; }
     if (!std::strcmp(key, "band_from_state")) { o.band_from_state = value != 0; return MC_OK; }
     if (!std::strcmp(key, "analysis_only")) { o.analysis_only = value != 0; return MC_OK; }
     if (!std::strcmp(key, "color_lane_lifecycle")) { o.color_lane_lifecycle = value != 0; return MC_OK; }

@@ -88,7 +88,7 @@ cudaError_t launch_lab16(const FrameIO& io, const DeviceTables& tb, int16_t* lab
 
 // fused ingest of the production path: u8 BGR -> Lab16 planes + G1 = pyrDown(Lab) (MagnifyCore.hpp:87-96, level 0)
 cudaError_t launch_ingest_lab(const FrameIO& io, const DeviceTables& tb, int16_t* lab, int pitch16, size_t plane16,
-                              float* g1, const Level& l1, cudaStream_t s, int warps_per_cta = 1);
+                              float* g1, const Level& l1, cudaStream_t s);
 
 struct LevelArgs {
     int in_kind = 0;           // 0: f32 planes, 1: Lab int16 planes, 2: u8 gray frame
@@ -149,7 +149,7 @@ cudaError_t launch_collapse(const Level& lf, const Level& lc, const BandSrc& fin
 // factor; the caller guarantees that the a / b motion it skips is finite).
 cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16_t* lab, int pitch16, size_t plane16,
                           const BandSrc& m1, const Level& l1, const BandSrc& c2, const Level& l2, float chroma,
-                          float* float_out_or_null, cudaStream_t s, int strip = 20, bool first_only = false,
+                          float* float_out_or_null, cudaStream_t s, bool strip = true, bool first_only = false,
                           bool luma_only = false);
 
 // PreprocessProcessor + GrayscaleProcessor on the device (mc_preprocess.cu): one launch over `vlanes` virtual lanes.

@@ -281,23 +281,25 @@ __device__ __forceinline__ void level_filter(const LevelKArgs& a, const float (*
     }
 }
 
-// PREFETCH (with USE_TMA): the tile's two state planes are requested as bulk-tensor copies at kernel entry, together
-// with the input window, and only waited for in the last phase — the fused kernel is latency-bound, so what matters is how many bytes each CTA keeps in flight.
-template <int KIND, bool USE_TMA, bool PREFETCH>
+// With USE_TMA the tile's two state planes are requested as bulk-tensor copies at kernel entry, together with the input
+// window, and only waited for in the last phase — the fused kernel is latency-bound, so what matters is how many bytes
+// each CTA keeps in flight (measured on a B200, 32 lanes: level[1] 235 -> 205 us against loading them in the last
+// phase).  The LDG path reads the state from global memory.
+template <int KIND, bool USE_TMA>
 __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_constant__ CUtensorMap tmap,
                                                const __grid_constant__ CUtensorMap tmap_hi,
                                                const __grid_constant__ CUtensorMap tmap_lo) {
     __shared__ __align__(128) float sG[GH][GW];
     __shared__ __align__(16) float sH[GH][DP];
     __shared__ __align__(16) float sD[DH][DP];
-    __shared__ __align__(128) float sS[PREFETCH ? 2 : 1][PREFETCH ? TH : 1][PREFETCH ? TW : 4];   // hi / lo tiles
+    __shared__ __align__(128) float sS[USE_TMA ? 2 : 1][USE_TMA ? TH : 1][USE_TMA ? TW : 4];   // hi / lo tiles
     __shared__ __align__(8) uint64_t tma_bar;
     __shared__ __align__(8) uint64_t st_bar;
     const int plane = blockIdx.z;
     const int op = lane_op(a.ops, plane / a.channels);
     if (op == LANE_HOLD) return;                     // held lane: state and G_{l+1} are left as they are
     const bool first = a.first || op == LANE_FIRST;  // this lane's first frame: hi = lo = band
-    const bool prefetch = PREFETCH && a.band && !first;
+    const bool prefetch = USE_TMA && a.band && !first;
     const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH;
     const int wf = a.lf.w, hf = a.lf.h, wc = a.lc.w, hc = a.lc.h;
     const bool interior = x0 >= 4 && x0 + TW + 4 <= wf && y0 >= 4 && y0 + TH + 3 <= hf && (KIND != IN_U8 || a.in_vec_ok);
@@ -308,7 +310,7 @@ __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_
         // BORDER_REFLECT_101 copies taken from inside the window.
         if (threadIdx.x == 0) {
             mbar_init(&tma_bar, 1);
-            if (PREFETCH) mbar_init(&st_bar, 1);
+            mbar_init(&st_bar, 1);
         }
         __syncthreads();
         if (threadIdx.x == 0) {
@@ -317,7 +319,7 @@ __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_
             if (prefetch) {
                 mbar_expect_tx(&st_bar, 2 * TH * TW * sizeof(float));
                 tma_load_3d(&sS[0][0][0], &tmap_hi, x0, y0, plane, &st_bar);
-                tma_load_3d(&sS[PREFETCH ? 1 : 0][0][0], &tmap_lo, x0, y0, plane, &st_bar);
+                tma_load_3d(&sS[USE_TMA ? 1 : 0][0][0], &tmap_lo, x0, y0, plane, &st_bar);
             }
         }
         mbar_wait(&tma_bar, 0);
@@ -354,8 +356,8 @@ __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_
         } else {
             float4 h4, l4;
             if (prefetch) {
-                h4 = *reinterpret_cast<const float4*>(&sS[0][PREFETCH ? 2 * ty + ry : 0][PREFETCH ? 4 * tx : 0]);
-                l4 = *reinterpret_cast<const float4*>(&sS[PREFETCH ? 1 : 0][PREFETCH ? 2 * ty + ry : 0][PREFETCH ? 4 * tx : 0]);
+                h4 = *reinterpret_cast<const float4*>(&sS[0][USE_TMA ? 2 * ty + ry : 0][USE_TMA ? 4 * tx : 0]);
+                l4 = *reinterpret_cast<const float4*>(&sS[USE_TMA ? 1 : 0][USE_TMA ? 2 * ty + ry : 0][USE_TMA ? 4 * tx : 0]);
             } else {
                 h4 = *reinterpret_cast<const float4*>(hi + o);
                 l4 = *reinterpret_cast<const float4*>(lo + o);
@@ -650,13 +652,14 @@ __device__ __forceinline__ void ig_row(const IngestArgs& a, const IgRaw raw, int
     o = ds_rowpass(r); hB[0] = o.h0; hB[1] = o.h1;
 }
 
-template <int WARPS>
-__global__ void __launch_bounds__(32 * WARPS) k_ingest_lab(const IngestArgs a) {
+__global__ void __launch_bounds__(32) k_ingest_lab(const IngestArgs a) {
     const int lane_id = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int lane = blockIdx.z;                                       // stream
     if (lane_op(a.ops, lane) == LANE_HOLD) return;
     const int gx = blockIdx.x * DS_COLS - 4 + lane_id * 4;
-    const int k0 = (blockIdx.y * WARPS + warp) * IG_ROWS;
+    // warp is 0 at one warp per CTA; without that term ptxas allocates the kernel differently (80 registers instead of
+    // 96), a variant that has not been measured
+    const int k0 = (blockIdx.y + warp) * IG_ROWS;
     const int wc = a.l1.w, hc = a.l1.h;
     if (k0 >= hc) return;
     const int k_end = min(k0 + IG_ROWS, hc);
@@ -1197,8 +1200,11 @@ __device__ __forceinline__ void strip_store(const StripPx<C>& o, uint8_t* q, flo
 // the rings are touched, and a, b go from Lab16 to the pixel stage unchanged.  This is the full synthesis bit for bit
 // when the a / b motion is finite and the chroma factor is zero: u * 0 = +-0, and a + (+-0) = a for a = v/64 - 128, which
 // is never -0 (the driver's condition, DESIGN §4).
-template <int C, int NS, int MINB, bool FOUT>
-__global__ void __launch_bounds__(32, MINB) k_egress_strip(const EgressArgs a) {
+//
+// The min-blocks bound (resident warps per SM) caps the registers: colour frames at 16 (<= 128 registers), the fastest of
+// the caps 16 / 20 / 24 measured on an H100 (DESIGN §5); gray frames at 24 (<= 80), which they fit without spilling.
+template <int C, int NS, bool FOUT>
+__global__ void __launch_bounds__(32, C == 3 ? 16 : 24) k_egress_strip(const EgressArgs a) {
     static_assert(NS == C || NS == 1, "L-only or full synthesis");
     const unsigned full = 0xffffffffu;
     const int lane_id = threadIdx.x;
@@ -1518,18 +1524,15 @@ cudaError_t launch_lab16(const FrameIO& io, const DeviceTables& tb, int16_t* lab
 }
 
 cudaError_t launch_ingest_lab(const FrameIO& io, const DeviceTables& tb, int16_t* lab, int pitch16, size_t plane16,
-                              float* g1, const Level& l1, cudaStream_t s, int warps) {
+                              float* g1, const Level& l1, cudaStream_t s) {
     IngestArgs a;
     a.in = io.in; a.in_step = io.in_step; a.in_lane_stride = io.in_lane_stride;
     a.w = io.w; a.h = io.h;
     a.aligned = (reinterpret_cast<uintptr_t>(io.in) % 4 == 0) && (io.in_step % 4 == 0) && (io.in_lane_stride % 4 == 0);
     a.lut = tb.lab_lut; a.lab = lab; a.pitch16 = pitch16; a.plane16 = plane16; a.g1 = g1; a.l1 = l1;
     a.ops = io.ops;
-    if (warps != 2 && warps != 4) warps = 1;
-    dim3 grid(cdiv(io.w, DS_COLS), cdiv(l1.h, IG_ROWS * warps), io.lanes);
-    if (warps == 4) k_ingest_lab<4><<<grid, 128, 0, s>>>(a);
-    else if (warps == 2) k_ingest_lab<2><<<grid, 64, 0, s>>>(a);
-    else k_ingest_lab<1><<<grid, 32, 0, s>>>(a);
+    dim3 grid(cdiv(io.w, DS_COLS), cdiv(l1.h, IG_ROWS), io.lanes);
+    k_ingest_lab<<<grid, 32, 0, s>>>(a);
     return cudaGetLastError();
 }
 
@@ -1565,12 +1568,11 @@ cudaError_t launch_level(const LevelArgs& a, cudaStream_t s) {
     static const CUtensorMap dummy{};
     const CUtensorMap* tg = reinterpret_cast<const CUtensorMap*>(a.tmap);
     if (a.in_kind == IN_F32 && tg && a.tmap_hi && a.tmap_lo)
-        k_level<IN_F32, true, true><<<grid, 256, 0, s>>>(k, *tg, *reinterpret_cast<const CUtensorMap*>(a.tmap_hi),
-                                                          *reinterpret_cast<const CUtensorMap*>(a.tmap_lo));
-    else if (a.in_kind == IN_F32 && tg) k_level<IN_F32, true, false><<<grid, 256, 0, s>>>(k, *tg, dummy, dummy);
-    else if (a.in_kind == IN_F32) k_level<IN_F32, false, false><<<grid, 256, 0, s>>>(k, dummy, dummy, dummy);
-    else if (a.in_kind == IN_LAB16) k_level<IN_LAB16, false, false><<<grid, 256, 0, s>>>(k, dummy, dummy, dummy);
-    else k_level<IN_U8, false, false><<<grid, 256, 0, s>>>(k, dummy, dummy, dummy);
+        k_level<IN_F32, true><<<grid, 256, 0, s>>>(k, *tg, *reinterpret_cast<const CUtensorMap*>(a.tmap_hi),
+                                                    *reinterpret_cast<const CUtensorMap*>(a.tmap_lo));
+    else if (a.in_kind == IN_F32) k_level<IN_F32, false><<<grid, 256, 0, s>>>(k, dummy, dummy, dummy);
+    else if (a.in_kind == IN_LAB16) k_level<IN_LAB16, false><<<grid, 256, 0, s>>>(k, dummy, dummy, dummy);
+    else k_level<IN_U8, false><<<grid, 256, 0, s>>>(k, dummy, dummy, dummy);
     return cudaGetLastError();
 }
 
@@ -1595,25 +1597,15 @@ cudaError_t launch_collapse(const Level& lf, const Level& lc, const BandSrc& fin
     return cudaGetLastError();
 }
 
-// the float tap (keep_float_output, a test hook) has one instance per synthesis: its extra stores do not fit the
-// tighter register caps without spilling, and the cap does not change a result
-template <int C, int NS, int MINB>
+template <int C, int NS>
 static void launch_egress_strip(const EgressArgs& a, dim3 grid, cudaStream_t s) {
-    if (a.fout) k_egress_strip<C, NS, C == 3 ? 16 : MINB, true><<<grid, 32, 0, s>>>(a);
-    else k_egress_strip<C, NS, MINB, false><<<grid, 32, 0, s>>>(a);
-}
-
-// colour frames: the register cap (resident warps per SM) 16 -> <= 128 registers, 20 -> 96, 24 -> 80
-template <int NS>
-static void launch_egress_strip3(const EgressArgs& a, int cap, dim3 grid, cudaStream_t s) {
-    if (cap == 16) launch_egress_strip<3, NS, 16>(a, grid, s);
-    else if (cap == 24) launch_egress_strip<3, NS, 24>(a, grid, s);
-    else launch_egress_strip<3, NS, 20>(a, grid, s);
+    if (a.fout) k_egress_strip<C, NS, true><<<grid, 32, 0, s>>>(a);
+    else k_egress_strip<C, NS, false><<<grid, 32, 0, s>>>(a);
 }
 
 cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16_t* lab, int pitch16, size_t plane16,
                           const BandSrc& m1, const Level& l1, const BandSrc& c2, const Level& l2, float chroma,
-                          float* fout, cudaStream_t s, int strip, bool first_only, bool luma_only) {
+                          float* fout, cudaStream_t s, bool strip, bool first_only, bool luma_only) {
     EgressArgs a;
     a.in = io.in; a.in_step = io.in_step; a.in_lane_stride = io.in_lane_stride;
     a.lab = lab; a.pitch16 = pitch16; a.plane16 = plane16;
@@ -1624,9 +1616,9 @@ cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16
     a.ops = io.ops; a.first_only = first_only ? 1 : 0;
     if (strip) {
         dim3 grid(cdiv(io.w, DS_COLS), cdiv(io.h, EG_ROWS), io.lanes);
-        if (io.channels != 3) launch_egress_strip<1, 1, 24>(a, grid, s);
-        else if (luma_only) launch_egress_strip3<1>(a, strip, grid, s);
-        else launch_egress_strip3<3>(a, strip, grid, s);
+        if (io.channels != 3) launch_egress_strip<1, 1>(a, grid, s);
+        else if (luma_only) launch_egress_strip<3, 1>(a, grid, s);
+        else launch_egress_strip<3, 3>(a, grid, s);
     } else {
         dim3 grid(cdiv(io.w, TW), cdiv(io.h, TH), io.lanes);
         if (io.channels == 3) k_egress<3><<<grid, 256, 0, s>>>(a);

@@ -33,12 +33,9 @@ struct Options {
     bool keep_float_output = false;   // keep the pre-quantisation tap of the last frame (mc_get_float_output)
     bool profile_kernels = false;     // bracket every launch with events (mc_profile_read)
     bool use_tma = true;          // stage level-kernel tiles with cp.async.bulk.tensor
-    bool prefetch_state = true;   // level kernel requests its state tiles by TMA at kernel entry
-    int egress_strip = 16;        // Laplace egress as the register/shuffle strip kernel (0 = tile kernel, 16 / 20 / 24 = strip
-                                  // kernel compiled for that many resident warps per SM)
-    int ingest_warps = 1;         // warps per CTA of the fused ingest kernel (1, 2 or 4)
+    bool egress_strip = true;     // Laplace egress as the register/shuffle strip kernel (false: the shared-memory tile kernel)
     bool band_from_state = true;  // synthesis rebuilds gain*(hi-lo) from the state planes instead of reading a stored band
-                                  // (with prefetch_state level[1] 205 -> 177 us, egress +8 us)
+                                  // (B200, with the state prefetch: level[1] 205 -> 177 us, egress +8 us)
     int lane_groups = 0;          // Laplace: number of lane groups run as concurrent launch chains (0 = automatic)
     bool analysis_only = false;   // Laplace / Phase: update the temporal state but skip synthesis + egress (*produced = 0); used
                                   // by the state-carry pass of temporal sharding (SURVEY 8f-3, lvm_b200.shard.magnify_segment)

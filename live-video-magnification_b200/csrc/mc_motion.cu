@@ -220,7 +220,7 @@ bool MotionMode::fused_ingest() const { return channels == 3 && !faithful && lev
 int MotionMode::first_level() const { return fused_ingest() ? 1 : ((levels >= 2 || faithful) ? 0 : levels); }
 
 mc_status MotionMode::ingest(const ModeCtx& ctx, const FrameIO& io, int16_t* lab, float* g1) {
-    if (fused_ingest()) LAUNCH("ingest_lab", 0, launch_ingest_lab(io, *ctx.tables, lab, pitch16, plane16, g1, lv[1], ctx.stream, ctx.opt.ingest_warps));
+    if (fused_ingest()) LAUNCH("ingest_lab", 0, launch_ingest_lab(io, *ctx.tables, lab, pitch16, plane16, g1, lv[1], ctx.stream));
     else if (channels == 3) LAUNCH("lab16", 0, launch_lab16(io, *ctx.tables, lab, pitch16, plane16, ctx.stream));
     return MC_OK;
 }
@@ -329,7 +329,8 @@ mc_status MotionMode::run_group(const ModeCtx& ctx, const FrameIO& io_all, const
         LevelArgs a = level_args(l, G, p0, lab, io, first, c_lo, c_hi);
         if (l >= 1 && g.tmap_valid[(size_t)l] && ctx.opt.use_tma) {
             a.tmap = &g.tmaps[(size_t)l];
-            if (ctx.opt.prefetch_state) { a.tmap_hi = &g.tmaps_hi[(size_t)l]; a.tmap_lo = &g.tmaps_lo[(size_t)l]; }
+            a.tmap_hi = &g.tmaps_hi[(size_t)l];
+            a.tmap_lo = &g.tmaps_lo[(size_t)l];
         }
         a.m = (first || from_state) ? nullptr : off(M[(size_t)l], l);
         a.m_luma = luma;

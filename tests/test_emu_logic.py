@@ -159,7 +159,8 @@ def test_round2_kernel_forms_agree_on_emulation(emu):
     """Round-2 kernel forms, logic only (the H100 runs the same checks in test_gpu_laplace.py / test_gpu_riesz.py):
     (1) the shuffle-strip egress equals the shared-memory tile egress bit for bit over several strips and chunks, both band
     sources, float taps included; (2) lanes run as two launch chains (option lane_groups) equal one chain; (3) the 9x9 Riesz
-    kernels give the same bits with TMA-staged and with LDG-staged tiles."""
+    kernels give the same bits with TMA-staged and with LDG-staged tiles; (4) the retired kernel-form options
+    prefetch_state and ingest_warps are rejected like any unknown key."""
     w, h, lv = 250, 131, 3
     cfg, _ = make_cfgs(O.MODE_LAPLACE, 20, 50.0, 0.4, 3.0, 30, lv)
     for bfs in (1, 0):
@@ -193,6 +194,10 @@ def test_round2_kernel_forms_agree_on_emulation(emu):
         pa, oa = a.process_image(f, cfgp)
         pb, ob = b.process_image(f, cfgp)
         assert pa == pb and (not pa or np.array_equal(oa, ob)), t
+    for key, value in (("prefetch_state", 0), ("ingest_warps", 2)):
+        with pytest.raises(L.MagcoreError) as e:
+            a.set_option(key, value)
+        assert e.value.status == capi.MC_ERR_INVALID, key
     a.close(); b.close()
 
 

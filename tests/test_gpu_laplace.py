@@ -329,30 +329,14 @@ def test_band_from_state_option_equals_stored_band():
             assert np.array_equal(oa, ob), (w, h, t)
 
 
-def test_prefetch_state_option_equals_default():
-    """Option prefetch_state (the level kernel requests its hi / lo tiles by TMA at kernel entry and reads them from
-    shared memory in the last phase) must not change a single bit of the output or of the state, ragged borders
-    included."""
-    for (w, h, c, lv) in [(640, 480, 3, 4), (333, 251, 1, 5), (131, 75, 3, 3)]:
-        cfg, _ = make_cfgs(O.MODE_LAPLACE, 20, 50.0, 0.4, 3.0, 30, lv)
-        a, b = L.MagnificationProcessor(0), L.MagnificationProcessor(0)
-        b.set_option("prefetch_state", 0)
-        for t in range(5):
-            f = synth_frame(t, w, h, c)
-            _, oa = a.process_image(f, cfg)
-            _, ob = b.process_image(f, cfg)
-            assert np.array_equal(oa, ob), (w, h, t)
-        for lvl in range(1, lv):
-            for name in ("lowpassHi", "lowpassLo"):
-                assert np.array_equal(a.get_state(name, lvl), b.get_state(name, lvl)), (w, h, lvl, name)
-
-
-@pytest.mark.parametrize("opts", [{"prefetch_state": 0}, {"band_from_state": 0}, {"prefetch_state": 0, "band_from_state": 0},
-                                  {"use_tma": 0}, {"ingest_warps": 2, "band_from_state": 0}, {"ingest_warps": 4},
-                                  {"egress_strip": 0}, {"egress_strip": 0, "band_from_state": 0}])
+@pytest.mark.parametrize("opts", [{"band_from_state": 0}, {"use_tma": 0}, {"egress_strip": 0}, {"egress_strip": 0, "band_from_state": 0},
+                                  {"use_tma": 0, "band_from_state": 0}, {"use_tma": 0, "egress_strip": 0},
+                                  {"use_tma": 0, "egress_strip": 0, "band_from_state": 0}, {"keep_float_output": 1}],
+                         ids=lambda opts: ",".join(f"{k}={v}" for k, v in opts.items()))
 def test_option_combinations_agree_with_default(opts):
-    """The A/B options compose: any combination gives the default path's frames bit for bit, over the first frame,
-    ragged borders and a parameter change."""
+    """The A/B options compose: every combination of band_from_state, use_tma and egress_strip, and the strip egress's
+    float-tap instance, give the default path's frames bit for bit, over the first frame, ragged borders and a
+    parameter change."""
     w, h, levels = 333, 251, 5
     a, b = L.MagnificationProcessor(0), L.MagnificationProcessor(0)
     for k, v in opts.items():
@@ -408,19 +392,4 @@ def test_lane_groups_equal_single_chain(lanes, groups):
         for name in ("lowpassHi", "lowpassLo"):
             assert np.array_equal(a.get_state(name, lvl), b.get_state(name, lvl)), (lvl, name)
 
-
-def test_ingest_warps_option_equals_default():
-    """Option ingest_warps (CTA shape of the fused BGR->Lab ingest kernel) must not change a bit: outputs and state,
-    interior and ragged strips (widths around the 120-column strip size), odd heights."""
-    for (w, h, lv) in [(640, 480, 4), (333, 251, 5), (121, 75, 3), (119, 64, 3), (240, 67, 2)]:
-        cfg, _ = make_cfgs(O.MODE_LAPLACE, 20, 50.0, 0.4, 3.0, 30, lv)
-        a, b = L.MagnificationProcessor(0), L.MagnificationProcessor(0)
-        b.set_option("ingest_warps", 4)
-        for t in range(3):
-            f = synth_frame(t, w, h, 3)
-            _, oa = a.process_image(f, cfg)
-            _, ob = b.process_image(f, cfg)
-            assert np.array_equal(oa, ob), (w, h, t)
-        for lvl in range(1, min(lv, L.calculateMaxLevels(w, h))):
-            assert np.array_equal(a.get_state("lowpassHi", lvl), b.get_state("lowpassHi", lvl)), (w, h, lvl)
 

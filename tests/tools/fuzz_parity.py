@@ -142,10 +142,9 @@ def main():
         proc = L.MagnificationProcessor(0)
         opts = []
         if args.options:
-            opts = [k for k in ("prefetch_state", "ingest_warps", "band_from_state", "faithful_level0", "use_tma")
-                    if rng.random() < 0.4]
+            opts = [k for k in ("band_from_state", "faithful_level0", "use_tma") if rng.random() < 0.4]
             for k in opts:
-                proc.set_option(k, {"faithful_level0": 1, "ingest_warps": 4}.get(k, 0))
+                proc.set_option(k, {"faithful_level0": 1}.get(k, 0))
         if R is not None:
             ref, rcfg = R.Processor(), livim_ref.to_ref_config(R, ocfg)
         else:

@@ -5,7 +5,7 @@ the blocking host API.  Prints one JSON line.
 
     python tests/tools/quick_gpu_probe.py                 # parity + one table (PROBE_LANES, default 8)
     python tests/tools/quick_gpu_probe.py --ab 8,32       # A/B of the kernel options at those lane counts:
-                                                    # the option sets in PROBE_VARIANTS (JSON list), default: ingest_warps 2 / 4, prefetch_state 0, band_from_state 0
+                                                    # the option sets in PROBE_VARIANTS (JSON list), default: band_from_state 0
 """
 import json
 import os
@@ -86,9 +86,7 @@ def main():
         lane_list = [int(x) for x in sys.argv[sys.argv.index("--ab") + 1].split(",")]
         # every variant in its own process: a kernel fault poisons the CUDA context of the process it happens in
         import subprocess
-        variants = json.loads(os.environ.get("PROBE_VARIANTS", "null")) or (
-            {}, {"ingest_warps": 2}, {"ingest_warps": 4}, {"prefetch_state": 0}, {"band_from_state": 0},
-            {"prefetch_state": 0, "band_from_state": 0})
+        variants = json.loads(os.environ.get("PROBE_VARIANTS", "null")) or ({}, {"band_from_state": 0})
         out["ab"] = []
         for n in lane_list:
             for o in variants:

@@ -87,10 +87,9 @@ def main():
         ok = ok and cond
 
     lines.append("")
-    tma = [k for k in body if k.startswith("void k_level<0, true")]
-    need(bool(tma) and all(count(k, "UTMALDG") >= 1 and count(k, "SYNCS") >= 2 for k in tma), "k_level<f32, TMA, *>: cp.async.bulk.tensor (UTMALDG) + mbarrier (SYNCS)")
-    pre = [k for k in tma if k.startswith("void k_level<0, true, true")]
-    need(bool(pre) and all(count(k, "UTMALDG") == 3 for k in pre), "k_level<f32, TMA, PREFETCH>: three bulk-tensor copies (input window + both state tiles)")
+    tma = [k for k in body if k.startswith("void k_level<0, true>")]
+    need(len(tma) == 1 and count(tma[0], "UTMALDG") == 3 and count(tma[0], "SYNCS") >= 2,
+         "k_level<f32, TMA>: three cp.async.bulk.tensor copies (UTMALDG: input window + both state tiles) + mbarrier (SYNCS)")
     clip = [k for k in body if k.startswith("void k_level_clip<0, true>")]
     need(len(clip) == 1 and count(clip[0], "UTMALDG") >= 1 and count(clip[0], "SYNCS") >= 2,
          "k_level_clip<f32, TMA>: double-buffered cp.async.bulk.tensor (UTMALDG) + mbarrier (SYNCS)")
@@ -104,8 +103,8 @@ def main():
          f"k_riesz_phase_clip<*>: no local-memory spills (ptxas -v, {len(pspills)} instances)")
     r9 = [k for k in body if k.startswith("k_riesz_analysis(") or k.startswith("k_riesz_collapse(")]
     need(len(r9) == 2 and all(count(k, "UTMALDG") == 1 and count(k, "SYNCS") >= 2 for k in r9), "k_riesz_analysis / k_riesz_collapse: 9x9 input tile by one bulk-tensor copy")
-    ing = [k for k in body if k.startswith("void k_ingest_lab<")]
-    need(bool(ing) and all(count(k, r"LDG\.E\.128") >= 8 and count(k, r"LDG\.E\.128") == count(k, r"LDG\.E\.64") for k in ing),
+    ing = [k for k in body if k.startswith("k_ingest_lab(")]
+    need(len(ing) == 1 and count(ing[0], r"LDG\.E\.128") >= 8 and count(ing[0], r"LDG\.E\.128") == count(ing[0], r"LDG\.E\.64"),
          "k_ingest_lab: each LUT gather is one LDG.E.128 + one LDG.E.64 (the 24 used bytes of a 32-byte cell)")
     strip = [k for k in body if k.startswith("void k_egress_strip<3")]
     need(bool(strip) and all(count(k, r"CCTL\.E\.PF1") >= 8 and count(k, r"BAR\.SYNC") == 0 for k in strip), "k_egress_strip<3,*>: L1 prefetches, no barrier")
@@ -114,7 +113,7 @@ def main():
     need(len(espills) == len(strip) + 2 and all(s == (0, 0) for s in espills.values()),
          f"k_egress_strip<*>: no spills (ptxas -v, {len(espills)} instances)")
     luma = [k for k in strip if k.startswith("void k_egress_strip<3, 1,")]
-    need(len(luma) == 4, f"k_egress_strip<3, 1, *>: L-only synthesis at every register cap and with the float tap ({len(luma)} instances)")
+    need(len(luma) == 2, f"k_egress_strip<3, 1, *>: L-only synthesis with and without the float tap ({len(luma)} instances)")
     for k in strip:
         n, rare = loop_counts(body[k])
         lines.append(f"     {k}: main loop {n} instructions ({n - rare} outside the warp-voted dark-end spline) "
