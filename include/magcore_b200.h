@@ -415,8 +415,14 @@ mc_status mc_set_option(mc_handle* h, const char* key, int value);
  * Names: Laplace "lowpassHi" / "lowpassLo" (MotionState, MagnifyCore.hpp:24-29), level 0..levels (levels 0 and
  *   `levels` exist only with option faithful_level0); Laplace "band", the frame path's band planes of a level: the
  *   amplified band gain * (hi - lo) the level kernel stores (levels 1..levels-1 with band_from_state 0), overwritten by
- *   the collapse sum cur_l at levels 2..levels-2.  When a frame synthesises L only (zero chroma, see DESIGN.md
- *   §4) their a / b planes are left as they are;
+ *   the collapse sum cur_l at levels 2..levels-2 (so on a frame that synthesised, "band" at levels 2..levels-2 is
+ *   cur_l, not the band).  When a frame synthesises L only (zero chroma, see DESIGN.md §4) their a / b planes are
+ *   left as they are;
+ * Laplace, read-only (mc_set_state returns MC_ERR_INVALID): "gauss", level 1..levels, the Gaussian pyramid G_l of the
+ *   last frame call, `channels` channels.  It follows "lab16": it exists only after a frame call, and is absent before
+ *   the first frame, after mc_reset, after a clip call (clips build their own pyramid) and after a change of mode or
+ *   geometry; for gray input it exists as well.  It is absent when levels is 1 without faithful_level0, where no
+ *   kernel builds G_1.  A held lane keeps in it what an earlier frame left;
  * Phase, per band level 0..levels-2, one channel: "old.lowpass", "old.rx", "old.ry" (RieszState::old),
  *   "phase.c", "phase.s" (itsPhase — the two filters' copies are identical), "lo.r0.c", "lo.r0.s", "lo.r1.c",
  *   "lo.r1.s", "hi.r0.c", "hi.r0.s", "hi.r1.c", "hi.r1.s" (itsRegister0/1 of the low / high cutoff filters,

@@ -385,9 +385,15 @@ MC_HD uint8_t resize_area_sample(const uint8_t* __restrict__ src, size_t step, i
     return (uint8_t)v[0];
 }
 
-// iirFilter (TemporalFilter.cpp:9-22): cv::addWeighted rounds once from a double sum (SURVEY A.5).
+// iirFilter (TemporalFilter.cpp:9-22): cv::addWeighted rounds once from a double sum (SURVEY A.5).  The form is pinned
+// to the one nvcc contracts it to in every level kernel: x * c rounded (DMUL), then state * (1 - c) fused into the add
+// (DFMA), so that the host and emulation builds give the device's bits (tests/test_gpu_laplace_stages.py checks them).
 MC_HD float ema(float state, float x, double one_minus_c, double c) {
-    return (float)((double)state * one_minus_c + (double)x * c);
+#if defined(__CUDA_ARCH__) && !defined(MC_CUDA_EMU)
+    return (float)__fma_rn((double)state, one_minus_c, __dmul_rn((double)x, c));
+#else
+    return (float)std::fma((double)state, one_minus_c, (double)x * c);
+#endif
 }
 
 }  // namespace mc

@@ -205,6 +205,7 @@ struct MotionMode {
     int pitch16 = 0;
     size_t plane16 = 0;
     bool lab16_frame = false;           // lab16 holds the last frame call's Lab (clips write their own scratch)
+    bool gauss_frame = false;           // G holds the last frame call's pyramid (clips write clip.G)
     // Every EMA step of the state since the state of all lanes was last dropped used cutoffs in [0, 1], so the a / b
     // state is bounded by the bands (a condition of L-only synthesis, DESIGN §4)
     bool ab_bounded = true;

@@ -73,6 +73,7 @@ void MotionMode::reset() {
     lv.clear(); G.clear(); hi.clear(); lo.clear(); M.clear();
     lab16 = nullptr;
     lab16_frame = false;
+    gauss_frame = false;
     allocated = false;
     empty = true;
     ab_bounded = true;
@@ -184,6 +185,7 @@ mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc
     const bool luma = luma_only(ctx, p);
 
     lab16_frame = false;   // a clip converts into its own scratch; a frame call rewrites lab16 below
+    gauss_frame = false;   // likewise its pyramid (clip.G)
     if (frames > 1) {
         MCK_ST(run_clip(ctx, io, p, frames, first, c_lo, c_hi, luma));
     } else if (groups.size() == 1) {
@@ -204,6 +206,7 @@ mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc
     }
     empty = false;
     lab16_frame = frames == 1 && lab16;
+    gauss_frame = frames == 1;
     // state-carry pass (analysis_only): the temporal state is up to date, only first frames are produced; a clip's later
     // frames run for the lanes that are not held
     plan.produced(ctx, !ctx.opt.analysis_only || first, true, produced, frames, !ctx.opt.analysis_only);
@@ -401,6 +404,15 @@ void MotionMode::find_state(const char* name, int level, StateRef& out) {
         return;
     }
     if (!allocated || empty || level < 0 || level > levels) return;
+    if (!std::strcmp(name, "gauss")) {
+        // read-only tap of G_1 .. G_levels of the last frame call (include/magcore_b200.h, at mc_get_state); with one
+        // level and no faithful level 0 no kernel writes G_1 (the level loop is empty, the ingest is k_lab16)
+        if (!gauss_frame || level < 1 || first_level() >= levels) return;
+        const Level& l = lv[(size_t)level];
+        out.ptr = G[(size_t)level]; out.rows = l.h; out.cols = l.w; out.channels = channels; out.pitch = l.pitch;
+        out.plane_stride = l.plane; out.read_only = true;
+        return;
+    }
     float* p = nullptr;
     if (!std::strcmp(name, "lowpassHi")) p = hi[(size_t)level];
     else if (!std::strcmp(name, "lowpassLo")) p = lo[(size_t)level];
