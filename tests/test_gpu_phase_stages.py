@@ -331,7 +331,8 @@ def check_frame(hd, frames, out, ops, before, prev, lv, prm, rebuild, stats):
         A = (lab[k, 1] * F32(1.0 / 64.0) - F32(128.0)).astype(F32)
         B = (lab[k, 2] * F32(1.0 / 64.0) - F32(128.0)).astype(F32)
         ref = cv2.cvtColor(cv2.merge([collapsed[0], A, B]), cv2.COLOR_Lab2BGR)
-        assert float(np.abs(fout[k] - ref).max()) <= 8e-6, k               # cv2 makes a NaN L' white: 1.0
+        if prm.get("egress_cv2", True):
+            assert float(np.abs(fout[k] - ref).max()) <= 8e-6, k           # cv2 makes a NaN L' white: 1.0
         assert (fout[k][np.isnan(collapsed[0])] == WHITE).all(), k
         assert np.array_equal(out[k], O._f32_to_u8(fout[k], 255.0, 1.0 / 255.0)), k
 
