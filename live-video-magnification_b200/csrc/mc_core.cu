@@ -533,13 +533,17 @@ mc_status mc_create_lanes(int device, int lanes, mc_handle** out) try {
     if ((e = cudaStreamCreateWithFlags(&h->s_out, cudaStreamNonBlocking)) != cudaSuccess) return fail("stream", e);
     std::vector<LabLutCell> lut;
     build_lab_lut_cells(lut);
-    if (lut.empty()) { g_create_error = "embedded Lab LUT missing"; mc_destroy(h); return MC_ERR_INVALID; }
+    std::vector<LabLutPack> pack;
+    if (!lut.empty()) build_lab_lut_packs(lut, pack);
+    if (pack.empty()) { g_create_error = "embedded Lab LUT missing"; mc_destroy(h); return MC_ERR_INVALID; }
     std::vector<float4> gam;
     build_inv_gamma_spline(gam);
     build_lab_inv_coeffs(h->tables.inv_coeffs);
     if ((e = cudaMalloc((void**)&h->tables.lab_lut, lut.size() * sizeof(LabLutCell))) != cudaSuccess) return fail("cudaMalloc lut", e);
     if ((e = cudaMalloc((void**)&h->tables.inv_gamma, gam.size() * sizeof(float4))) != cudaSuccess) return fail("cudaMalloc gamma", e);
     if ((e = cudaMemcpy(h->tables.lab_lut, lut.data(), lut.size() * sizeof(LabLutCell), cudaMemcpyHostToDevice)) != cudaSuccess) return fail("copy lut", e);
+    if ((e = cudaMalloc((void**)&h->tables.lab_pack, pack.size() * sizeof(LabLutPack))) != cudaSuccess) return fail("cudaMalloc packed lut", e);
+    if ((e = cudaMemcpy(h->tables.lab_pack, pack.data(), pack.size() * sizeof(LabLutPack), cudaMemcpyHostToDevice)) != cudaSuccess) return fail("copy packed lut", e);
     if ((e = cudaMemcpy(h->tables.inv_gamma, gam.data(), gam.size() * sizeof(float4), cudaMemcpyHostToDevice)) != cudaSuccess) return fail("copy gamma", e);
     h->motion.lanes = h->color.lanes = h->riesz.lanes = lanes;
     h->has_state.assign((size_t)lanes, 0);
@@ -562,6 +566,7 @@ void mc_destroy(mc_handle* h) try {
     if (h->s_out) cudaStreamSynchronize(h->s_out);
     reset_modes(h);
     if (h->tables.lab_lut) cudaFree(h->tables.lab_lut);
+    if (h->tables.lab_pack) cudaFree(h->tables.lab_pack);
     if (h->tables.inv_gamma) cudaFree(h->tables.inv_gamma);
     if (h->d_ops) cudaFree(h->d_ops);
     if (h->stream) cudaStreamDestroy(h->stream);

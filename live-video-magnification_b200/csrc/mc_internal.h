@@ -29,12 +29,14 @@ inline Level make_level(int w, int h) {
 // Device constant tables shared by every handle on a device (built once per device).
 struct DeviceTables {
     LabLutCell* lab_lut = nullptr;   // [34][33][33] cells (mc_math.cuh)
+    LabLutPack* lab_pack = nullptr;  // the same cells packed into 16 B (mc_math.cuh)
     float4* inv_gamma = nullptr;      // [1024] spline coefficients {f, b, c, d}
     LabInvCoeffs inv_coeffs{};
 };
 
 // mc_tables.cpp ------------------------------------------------------------------------------
 void build_lab_lut_cells(std::vector<LabLutCell>& out);          // from the embedded int16 table
+void build_lab_lut_packs(const std::vector<LabLutCell>& cells, std::vector<LabLutPack>& out);   // empty if a field overflows
 void build_inv_gamma_spline(std::vector<float4>& out);             // OpenCV sRGBInvGammaTab
 void build_lab_inv_coeffs(LabInvCoeffs& out);
 int calculate_max_levels(int w, int h);

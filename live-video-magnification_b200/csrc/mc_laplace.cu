@@ -583,7 +583,7 @@ __global__ void __launch_bounds__(32 * DS_WARPS) k_down_strip(const DownArgs a) 
 // ingest_lab: u8 BGR -> Lab (exact OpenCV LUT) -> { Lab16 planes for egress, G1 = pyrDown(Lab) } in one
 // pass.  Same strip structure as down_strip (row pass by shuffles, column pass as a register window),
 // with the three Lab channels carried together.  The kernel is bound by the divergent LUT gathers (L1 tag
-// lookups) and by issue slots, not by HBM: each pixel costs two 256-bit gathers (LabLutCell) and ~80 instructions;
+// lookups) and by issue slots, not by HBM: each pixel costs two 128-bit gathers (LabLutPack, one per b slab);
 // the next row's 12 input bytes per lane are requested before the current row is converted.
 // ------------------------------------------------------------------------------------------------
 constexpr int IG_ROWS = 32;   // coarse rows per warp (halo rows re-convert 4 of 68 fine rows)
@@ -591,7 +591,7 @@ constexpr int IG_ROWS = 32;   // coarse rows per warp (halo rows re-convert 4 of
 struct IngestArgs {
     const uint8_t* in; size_t in_step, in_lane_stride;
     int w, h, aligned;
-    const LabLutCell* lut;
+    const LabLutPack* lut;
     int16_t* lab; int pitch16; size_t plane16;
     float* g1; Level l1;
     const uint8_t* ops;   // LaneOp per lane or null
@@ -619,6 +619,37 @@ __device__ __forceinline__ IgRaw ig_load(const IngestArgs& a, const uint8_t* fra
     return r;
 }
 
+// One b slab of ig_lab: adds w0 * (r-interpolation of row g) + w1 * (that of row g+1) of each channel.  With the
+// cell's v, dr, dg, e (mc_math.cuh), (16 - xr) v(g, r) + xr v(g, r+1) = 16 v + xr dr and
+// (16 - xr) v(g+1, r) + xr v(g+1, r+1) = 16 (v + dg) + xr e.  The a and b values lack their offsets; ig_lab adds them.
+__device__ __forceinline__ void ig_slab(const uint4 p, int xr, int w0, int w1, int& sL, int& sA, int& sB) {
+    const int Lv = (int)(p.x & 0x7fffu), Ldr = (int)((p.x >> 15) & 0x1ffu), bdr = (int)(p.x >> 24);
+    const int av = (int)(p.y & 0x3fffu), adr = (int)((p.y >> 14) & 0x1ffu), adg = -(int)(p.y >> 23);
+    const int bv = (int)(p.z & 0x3fffu), bdg = (int)((p.z >> 14) & 0x1ffu), ae = (int)(p.z >> 23);
+    const int Ldg = (int)(p.w & 0x3ffu), Le = (int)((p.w >> 10) & 0x1ffu), be = (int)(p.w >> 19);
+    sL += w0 * (16 * Lv + xr * Ldr) + w1 * (16 * (Lv + Ldg) + xr * Le);
+    sA += w0 * (16 * av + xr * adr) + w1 * (16 * (av + adg) + xr * ae);
+    sB += w0 * (16 * bv + xr * bdr) + w1 * (16 * (bv + bdg) + xr * be);
+}
+
+// lab_fixed_from_q from the packed cells: one 128-bit gather per b slab, the same integer sum.  The offsets of the
+// a and b values enter once: the four weights add up to 256, so they contribute 256 * 16 * offset.
+__device__ __forceinline__ void ig_lab(int qb, int qg, int qr, const LabLutPack* __restrict__ lut, int& sL, int& sA, int& sB) {
+    const int tb = qb >> 4, tg = qg >> 4, tr = qr >> 4;
+    const int xb = qb & 15, xg = qg & 15, xr = qr & 15;
+    const LabLutPack* c0 = lut + ((tb * kLabLutDim + tg) * kLabLutDim + tr);
+    const uint4 p0 = __ldg(reinterpret_cast<const uint4*>(c0)), p1 = __ldg(reinterpret_cast<const uint4*>(c0 + kLabLutSlab));
+    const int w01 = (16 - xb) * xg, w00 = ((16 - xb) << 4) - w01, w11 = xb * xg, w10 = (xb << 4) - w11;
+    sL = 2048;
+    sA = 2048 + 4096 * kPackA0;
+    sB = 2048 + 4096 * kPackB0;
+    ig_slab(p0, xr, w00, w01, sL, sA, sB);
+    ig_slab(p1, xr, w10, w11, sL, sA, sB);
+    sL >>= 12;
+    sA >>= 12;
+    sB >>= 12;
+}
+
 // converts the lane's 4 pixels of fine row `row`, optionally stores Lab16, returns the row pass of the three channels
 __device__ __forceinline__ void ig_row(const IngestArgs& a, const IgRaw raw, int row, int gx, bool own, int16_t* lab_lane,
                                        float (&hL)[2], float (&hA)[2], float (&hB)[2]) {
@@ -632,7 +663,7 @@ __device__ __forceinline__ void ig_row(const IngestArgs& a, const IgRaw raw, int
     int sL[4], sA[4], sB[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
-        lab_fixed_from_q(lab_q_of_u8((int)px[3 * i]), lab_q_of_u8((int)px[3 * i + 1]), lab_q_of_u8((int)px[3 * i + 2]), a.lut, sL[i], sA[i], sB[i]);
+        ig_lab(lab_q_of_u8((int)px[3 * i]), lab_q_of_u8((int)px[3 * i + 1]), lab_q_of_u8((int)px[3 * i + 2]), a.lut, sL[i], sA[i], sB[i]);
     if (own) {   // this warp owns the row and the lane owns the columns: emit the Lab16 planes
         int16_t* o = lab_lane + (size_t)row * a.pitch16 + gx;
         *reinterpret_cast<short4*>(o) = make_short4((short)sL[0], (short)sL[1], (short)sL[2], (short)sL[3]);
@@ -1529,7 +1560,7 @@ cudaError_t launch_ingest_lab(const FrameIO& io, const DeviceTables& tb, int16_t
     a.in = io.in; a.in_step = io.in_step; a.in_lane_stride = io.in_lane_stride;
     a.w = io.w; a.h = io.h;
     a.aligned = (reinterpret_cast<uintptr_t>(io.in) % 4 == 0) && (io.in_step % 4 == 0) && (io.in_lane_stride % 4 == 0);
-    a.lut = tb.lab_lut; a.lab = lab; a.pitch16 = pitch16; a.plane16 = plane16; a.g1 = g1; a.l1 = l1;
+    a.lut = tb.lab_pack; a.lab = lab; a.pitch16 = pitch16; a.plane16 = plane16; a.g1 = g1; a.l1 = l1;
     a.ops = io.ops;
     dim3 grid(cdiv(io.w, DS_COLS), cdiv(l1.h, IG_ROWS), io.lanes);
     k_ingest_lab<<<grid, 32, 0, s>>>(a);

@@ -26,6 +26,16 @@ struct alignas(32) LabLutCell { int16_t v[16]; };  // {L00,L01, a00,a01, b00,b01
 constexpr int kLabLutSlab = kLabLutDim * kLabLutDim;   // cells per b slab
 constexpr int kLabLutCells = (kLabLutDim + 1) * kLabLutSlab;
 
+// The same cells, losslessly packed into 16 B for the fused ingest (k_ingest_lab): one 128-bit gather per b slab
+// instead of a 128-bit + a 64-bit one from the same sector.  Per channel the cell holds the value v at (g, r), the
+// r step dr = v(g, r+1) - v(g, r), the g step dg = v(g+1, r) - v(g, r) and the r step of row g+1,
+// e = v(g+1, r+1) - v(g+1, r), as bit fields that never straddle a word:
+//   w0 = L.v | L.dr << 15 | b.dr << 24           w1 = (a.v - kPackA0) | a.dr << 14 | -a.dg << 23
+//   w2 = (b.v - kPackB0) | b.dg << 14 | a.e << 23  w3 = L.dg | L.e << 10 | b.e << 19
+// build_lab_lut_packs checks that every field of OpenCV's table fits its width (fields are unsigned; a.dg is <= 0).
+struct alignas(16) LabLutPack { uint32_t w[4]; };
+constexpr int kPackA0 = 2676, kPackB0 = 1289;   // smallest a and b entries of the table
+
 MC_HD int reflect101(int i, int n) {
     if (i < 0) i = -i;
     if (i >= n) i = 2 * n - 2 - i;

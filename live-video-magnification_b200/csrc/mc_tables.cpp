@@ -38,6 +38,34 @@ void build_lab_lut_cells(std::vector<LabLutCell>& out) {
             }
 }
 
+void build_lab_lut_packs(const std::vector<LabLutCell>& cells, std::vector<LabLutPack>& out) {
+    out.assign(cells.size(), LabLutPack{});
+    for (size_t i = 0; i < cells.size(); ++i) {
+        const int16_t* c = cells[i].v;   // {L00,L01, a00,a01, b00,b01, L10,L11, a10,a11, b10,b11}
+        const int v[3] = {c[0], c[2] - kPackA0, c[4] - kPackB0};
+        int dr[3], dg[3], e[3];
+        for (int ch = 0; ch < 3; ++ch) {
+            dr[ch] = c[2 * ch + 1] - c[2 * ch];
+            dg[ch] = c[6 + 2 * ch] - c[2 * ch];
+            e[ch] = c[6 + 2 * ch + 1] - c[6 + 2 * ch];
+        }
+        dg[1] = -dg[1];
+        // {value, bit width} of every field in the order of the layout (mc_math.cuh)
+        const int f[12][2] = {{v[0], 15}, {dr[0], 9}, {dr[2], 8}, {v[1], 14}, {dr[1], 9}, {dg[1], 9},
+                              {v[2], 14}, {dg[2], 9}, {e[1], 9}, {dg[0], 10}, {e[0], 9}, {e[2], 8}};
+        for (int k = 0; k < 12; ++k)
+            if (f[k][0] < 0 || f[k][0] >= (1 << f[k][1])) {
+                out.clear();
+                return;
+            }
+        LabLutPack& p = out[i];
+        p.w[0] = (uint32_t)f[0][0] | (uint32_t)f[1][0] << 15 | (uint32_t)f[2][0] << 24;
+        p.w[1] = (uint32_t)f[3][0] | (uint32_t)f[4][0] << 14 | (uint32_t)f[5][0] << 23;
+        p.w[2] = (uint32_t)f[6][0] | (uint32_t)f[7][0] << 14 | (uint32_t)f[8][0] << 23;
+        p.w[3] = (uint32_t)f[9][0] | (uint32_t)f[10][0] << 10 | (uint32_t)f[11][0] << 19;
+    }
+}
+
 // OpenCV's sRGBInvGammaTab: natural cubic spline (splineBuild) through the inverse sRGB transfer
 // function sampled at i/1024; f32 arithmetic as OpenCV's softfloat build does it.
 void build_inv_gamma_spline(std::vector<float4>& out) {

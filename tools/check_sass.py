@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Static checks of the built library's SASS (cuobjdump works without a GPU) and the evidence file the docs cite:
-which kernels use the TMA path (UTMALDG + mbarrier SYNCS), that each ingest LUT gather is one 128-bit + one 64-bit load,
+which kernels use the TMA path (UTMALDG + mbarrier SYNCS), that each ingest LUT gather is one 128-bit load,
 that the strip egress
 prefetches into L1 and has no local memory, spill or barrier (it also prints the length of its main loop), and that the Phase egress clips NaN to 1.0 with an explicit select (OpenCV's max(min(v,1),0)) instead
 of a .SAT folded into the producing FFMA (round-1 hardware failure).  Usage: python tools/check_sass.py [out.txt]"""
@@ -23,7 +23,7 @@ def kernels():
             cur = subprocess.run(["c++filt", m.group(1)], capture_output=True, text=True).stdout.strip() or m.group(1)
             cur = re.sub(r"mc::\(anonymous namespace\)::", "", cur)
             body[cur] = []
-        elif cur and re.match(r"\s+/\*[0-9a-f]{4}\*/", line):
+        elif cur and re.match(r"\s+/\*[0-9a-f]{4,}\*/", line):
             body[cur].append(re.sub(r"\s*/\*.*?\*/\s*", " ", line).strip())
     return body
 
@@ -104,8 +104,8 @@ def main():
     r9 = [k for k in body if k.startswith("k_riesz_analysis(") or k.startswith("k_riesz_collapse(")]
     need(len(r9) == 2 and all(count(k, "UTMALDG") == 1 and count(k, "SYNCS") >= 2 for k in r9), "k_riesz_analysis / k_riesz_collapse: 9x9 input tile by one bulk-tensor copy")
     ing = [k for k in body if k.startswith("k_ingest_lab(")]
-    need(len(ing) == 1 and count(ing[0], r"LDG\.E\.128") >= 8 and count(ing[0], r"LDG\.E\.128") == count(ing[0], r"LDG\.E\.64"),
-         "k_ingest_lab: each LUT gather is one LDG.E.128 + one LDG.E.64 (the 24 used bytes of a 32-byte cell)")
+    need(len(ing) == 1 and count(ing[0], r"LDG\.E\.128") >= 8 and count(ing[0], r"LDG\.E\.64") == 0,
+         "k_ingest_lab: each LUT gather is one LDG.E.128 (a 16-byte packed cell), no LDG.E.64")
     strip = [k for k in body if k.startswith("void k_egress_strip<3")]
     need(bool(strip) and all(count(k, r"CCTL\.E\.PF1") >= 8 and count(k, r"BAR\.SYNC") == 0 for k in strip), "k_egress_strip<3,*>: L1 prefetches, no barrier")
     need(bool(strip) and all(count(k, r"\b(STL|LDL)\b") == 0 for k in strip), "k_egress_strip<3,*>: no local memory (STL / LDL)")
