@@ -284,7 +284,7 @@ mc_status mc_chain_process_nv12_device(mc_handle* h, const mc_nv12* in, int fram
 
 /* --- the export canvas on the device (SURVEY.md 8f-2) -------------------------------------------------------------
  * The frame the reference's exporter writes to the file, compose(original, cur, split) of src/export/Exporter.cpp:25-34,
- * 53-88 without text labels: both taps are expanded to BGR (a gray frame as GRAY2BGR) and cropped, from the top-left
+ * 53-88 (its labels through mc_set_overlay, below): both taps are expanded to BGR (a gray frame as GRAY2BGR) and cropped, from the top-left
  * corner, to their common even size w x h (W & ~1, H & ~1 of the chain's output, which H.264 / FFV1 need); then
  *   MC_SPLIT_NONE        the processed pane alone: w x h
  *   MC_SPLIT_LEFT_RIGHT  the original pane left of the processed one: 2w x h
@@ -320,7 +320,8 @@ mc_status mc_compose_geometry(const mc_params* p, int width, int height, int cha
  *   converted in registers, and no full-resolution BGR frame is stored for them.
  *   Errors, returned before any kernel runs and with no canvas or state changed: MC_ERR_INVALID for a split out of
  *   range, a NULL canvas or canvas plane, a pitch smaller than a canvas row, lane_stride < pitch * canvas height with
- *   more than one virtual lane, and the chain call's own argument errors (d_out / d_original are not arguments here).
+ *   more than one virtual lane, a canvas that is not 0 x 0 and not the geometry of the overlay set (mc_set_overlay),
+ *   and the chain call's own argument errors (d_out / d_original are not arguments here).
  *   Device scratch: besides the chain's, the magnifier's output for the largest frame set seen (out_w * out_h *
  *   out_channels bytes per virtual lane), a byte per virtual lane for the pane choice, and, with a split and a
  *   Preprocess stage, the preprocessed frames in the front's staging. */
@@ -330,6 +331,44 @@ mc_status mc_chain_compose_device(mc_handle* h, const uint8_t* d_in, int frames,
 mc_status mc_chain_compose_nv12_device(mc_handle* h, const mc_nv12* in, int frames, int width, int height,
                                        const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
                                        uint8_t* produced, mc_chain_info* info);
+
+/* --- labels on the export canvas (ExportRequest::textOverlay, Exporter.cpp:36-50) ------------------------------------
+ * The exporter's "Original" / "Processed" labels darken a box (addWeighted(box, 0.35, black, 0.65, 0)) and draw white
+ * anti-aliased text over it.  Both steps are pointwise and treat the three channels alike, so a labelled canvas is
+ *     out[y][x][c] = map[index(x, y)][in[y][x][c]]
+ * inside a few rectangles and the canvas itself outside them: one u8 -> u8 tone map per labelled pixel.  The caller
+ * builds these maps once per export geometry by drawing the labels with its own OpenCV onto the 256 flat grey canvases
+ * (live-video-magnification_b200/labels.py is the executable specification; INTEGRATION.md §2b), and the compose
+ * kernel applies them to every canvas it writes.  The core draws no text itself.
+ *   Configuration, not temporal state: the overlay belongs to the handle and is kept across mc_reset, structural
+ *     resets and failed frames, until it is replaced or cleared.
+ *   Stream order: mc_set_overlay copies the overlay to device memory in stream order on mc_stream().  Compose calls
+ *     enqueued before it use the previous overlay, calls after it the new one.  The caller's buffers may be freed as
+ *     soon as it returns.
+ *   Every compose call (BGR, NV12 and YUYV sources; BGR and NV12 canvases; frames, clips and lanes) maps each canvas it
+ *     writes: a canvas pixel inside a rect becomes map[index][v] in each of its channels, before the NV12 conversion (a
+ *     2x2 block whose top-left pixel is labelled takes its Cb,Cr from the labelled value).  Held lanes and 0 x 0
+ *     canvases stay untouched, as without an overlay.  Chain calls that do not compose ignore it.
+ *   Errors, MC_ERR_INVALID: mc_set_overlay with canvas_w or canvas_h < 1, rects or maps out of range, a NULL map or
+ *     index, a rect that is empty or not inside the canvas, two rects that overlap, or an index >= maps; the previous
+ *     overlay is kept.  A compose call while an overlay is set whose canvas (mc_compose_geometry) is neither 0 x 0 nor
+ *     canvas_w x canvas_h, returned before any kernel runs with no canvas or state changed: a stale overlay is never
+ *     dropped or misplaced silently.
+ *   Device memory: maps * 256 bytes plus 2 bytes per rect pixel, kept for the largest overlay set. */
+#define MC_OVERLAY_MAX_RECTS 2
+typedef struct mc_overlay_rect {
+    int32_t x, y, w, h;          /* on the canvas, inside it */
+    const uint16_t* index;       /* host: h rows of w entries, the tone map of each pixel */
+} mc_overlay_rect;
+typedef struct mc_overlay {
+    int32_t canvas_w, canvas_h;                 /* the canvas geometry it was built for */
+    int32_t rects;                              /* 0 .. MC_OVERLAY_MAX_RECTS, pairwise disjoint */
+    mc_overlay_rect rect[MC_OVERLAY_MAX_RECTS];
+    int32_t maps;                               /* 1 .. 65536 */
+    const uint8_t* map;                         /* host: maps x 256 bytes, map[m][v] */
+} mc_overlay;
+/* Sets the handle's overlay (see above); ov == NULL clears it. */
+mc_status mc_set_overlay(mc_handle* h, const mc_overlay* ov);
 
 /* --- packed 4:2:2 camera frames (V4L2 YUYV / UYVY) into the processing chain ---------------------------------------
  * A YUYV frame is height rows of width / 2 groups of 4 bytes, Y0 Cb Y1 Cr (UYVY: Cb Y0 Cr Y1); both pixels of a group

@@ -53,6 +53,20 @@ class McCanvas(C.Structure):
                 ("lane_stride", C.c_size_t)]
 
 
+MC_OVERLAY_MAX_RECTS = 2
+
+
+class McOverlayRect(C.Structure):
+    """mc_overlay_rect: a canvas rect and its h x w u16 map indices (a host address as an integer)."""
+    _fields_ = [("x", C.c_int32), ("y", C.c_int32), ("w", C.c_int32), ("h", C.c_int32), ("index", C.c_void_p)]
+
+
+class McOverlay(C.Structure):
+    """mc_overlay: the export canvas's labels as per-pixel u8 tone maps (labels.py builds one)."""
+    _fields_ = [("canvas_w", C.c_int32), ("canvas_h", C.c_int32), ("rects", C.c_int32),
+                ("rect", McOverlayRect * MC_OVERLAY_MAX_RECTS), ("maps", C.c_int32), ("map", C.c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol include/magcore_b200.h declares
 _u8p, _f32p, _vp = C.POINTER(C.c_uint8), C.POINTER(C.c_float), C.c_void_p
 _PP = C.POINTER(McParams)
@@ -98,6 +112,7 @@ SIGNATURES = {
                                                  C.POINTER(McChainInfo)]),
     "mc_chain_process_yuv422": (C.c_int, [_vp, _YV, C.c_int, C.c_int, _PP, C.c_int, _vp, C.c_size_t, _vp, C.c_size_t,
                                           C.POINTER(McChainInfo)]),
+    "mc_set_overlay": (C.c_int, [_vp, C.POINTER(McOverlay)]),
     "mc_pipeline_depth": (C.c_int, [_vp]),
     "mc_submit": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t]),
     "mc_collect": (C.c_int, [_vp, C.POINTER(C.c_int)]),

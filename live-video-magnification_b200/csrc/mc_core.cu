@@ -114,6 +114,16 @@ struct mc_handle {
     // chain compose calls: the magnifier's output and the ComposeOp of every virtual lane, with its host copy
     DeviceBuffer<> x_mag, x_ops;
     std::vector<uint8_t> x_ops_host;
+    // the export canvas's overlay (mc_set_overlay): configuration, kept across resets.  ov_dev holds the maps, then each
+    // rect's index plane at byte offset ofs[i]
+    struct Overlay {
+        bool set = false;
+        int cw = 0, ch = 0, rects = 0;
+        OverlayRect rect[kOverlayRects];
+        size_t ofs[kOverlayRects] = {};
+    } ov;
+    DeviceBuffer<> ov_dev;
+    std::vector<uint8_t> ov_host;
 
     // mc_process_clip device staging: the clip's frames in and out
     DeviceBuffer<> k_in, k_out;
@@ -1067,13 +1077,14 @@ struct ComposeReq {
     const mc_canvas* canvas;
 };
 
-const char* check_compose(const ComposeReq& c, const ChainGeom& g, size_t vl) {
+const char* check_compose(const ComposeReq& c, const ChainGeom& g, size_t vl, const mc_handle::Overlay& ov) {
     if (c.split < MC_SPLIT_NONE || c.split > MC_SPLIT_TOP_BOTTOM) return "split out of range";
     const mc_canvas* cv = c.canvas;
     if (!cv || (cv->format != MC_CANVAS_BGR && cv->format != MC_CANVAS_NV12)) return "canvas is null or of an unknown format";
     if (!cv->data || (cv->format == MC_CANVAS_NV12 && !cv->uv)) return "canvas plane is null";
     int cw, ch;
     canvas_size(g, c.split, cw, ch);
+    if (ov.set && cw > 0 && (cw != ov.cw || ch != ov.ch)) return "canvas geometry differs from the overlay's";
     if (cv->pitch < (size_t)cw * (cv->format == MC_CANVAS_BGR ? 3 : 1)) return "canvas pitch < canvas row";
     if (vl > 1 && cv->lane_stride < cv->pitch * ch) return "canvas lane_stride < pitch * canvas height";
     return nullptr;
@@ -1119,7 +1130,7 @@ mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc
         if (const char* e = check_yuv422(*yv, w, hh, vl)) { h->err = e; return MC_ERR_INVALID; }
     }
     if (cmp) {
-        if (const char* e = check_compose(*cmp, g, vl)) { h->err = e; return MC_ERR_INVALID; }
+        if (const char* e = check_compose(*cmp, g, vl, h->ov)) { h->err = e; return MC_ERR_INVALID; }
     }
     if (empty) return clip_impl(h, nullptr, frames, 0, 0, channels, 0, p, nullptr, 0, produced);   // the identity
     if (nv) {
@@ -1221,6 +1232,14 @@ mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc
         const mc_canvas& cv = *cmp->canvas;
         a.nv12 = cv.format == MC_CANVAS_NV12;
         a.data = cv.data; a.uv = cv.uv; a.pitch = cv.pitch; a.lane_stride = cv.lane_stride;
+        if (h->ov.set) {
+            a.ov_rects = h->ov.rects;
+            a.ov_map = h->ov_dev.p;
+            for (int i = 0; i < h->ov.rects; ++i) {
+                a.ov[i] = h->ov.rect[i];
+                a.ov[i].index = reinterpret_cast<const uint16_t*>(h->ov_dev.p + h->ov.ofs[i]);
+            }
+        }
         return launch_counted(h, "compose", [&] { return launch_compose(a, (int)vl, h->stream); });
     }
     if (!front) return MC_OK;
@@ -1270,6 +1289,57 @@ extern "C" mc_status mc_compose_geometry(const mc_params* p, int width, int heig
     canvas_size(g, split, *canvas_w, *canvas_h);
     return MC_OK;
 } catch (...) { return on_exception(nullptr); }
+
+namespace {
+const char* check_overlay(const mc_overlay& o) {
+    static_assert(kOverlayRects == MC_OVERLAY_MAX_RECTS, "the kernel's rect count is the ABI's");
+    if (o.canvas_w < 1 || o.canvas_h < 1) return "overlay canvas size < 1";
+    if (o.rects < 0 || o.rects > MC_OVERLAY_MAX_RECTS) return "overlay rects out of range";
+    if (o.maps < 1 || o.maps > 65536 || !o.map) return "overlay maps out of range or map is null";
+    for (int i = 0; i < o.rects; ++i) {
+        const mc_overlay_rect& r = o.rect[i];
+        if (!r.index) return "overlay index is null";
+        if (r.w < 1 || r.h < 1 || r.x < 0 || r.y < 0 || r.x > o.canvas_w - r.w || r.y > o.canvas_h - r.h)
+            return "overlay rect is empty or not inside the canvas";
+        for (int j = 0; j < i; ++j) {
+            const mc_overlay_rect& q = o.rect[j];
+            if (r.x < q.x + q.w && q.x < r.x + r.w && r.y < q.y + q.h && q.y < r.y + r.h) return "overlay rects overlap";
+        }
+        const size_t n = (size_t)r.w * r.h;
+        if (std::any_of(r.index, r.index + n, [&](uint16_t m) { return m >= o.maps; })) return "overlay index >= maps";
+    }
+    return nullptr;
+}
+}  // namespace
+
+extern "C" mc_status mc_set_overlay(mc_handle* h, const mc_overlay* o) try {
+    if (!h) return MC_ERR_INVALID;
+    if (!o) { h->ov.set = false; return MC_OK; }
+    if (const char* e = check_overlay(*o)) { h->err = e; return MC_ERR_INVALID; }
+    CK(cudaSetDevice(h->device));
+    // one host image of maps and index planes, uploaded in one copy on the handle's stream: compose launches enqueued
+    // before it still read the previous overlay.  The source is pageable, so it is staged before the call returns.
+    mc_handle::Overlay ov;
+    ov.cw = o->canvas_w; ov.ch = o->canvas_h; ov.rects = o->rects;
+    size_t total = (size_t)o->maps * 256;
+    for (int i = 0; i < o->rects; ++i) {
+        const mc_overlay_rect& r = o->rect[i];
+        ov.rect[i] = OverlayRect{r.x, r.y, r.w, r.h, nullptr};
+        ov.ofs[i] = total;
+        total += (size_t)r.w * r.h * sizeof(uint16_t);
+    }
+    std::vector<uint8_t>& b = h->ov_host;
+    b.resize(total);
+    std::memcpy(b.data(), o->map, (size_t)o->maps * 256);
+    for (int i = 0; i < o->rects; ++i)
+        std::memcpy(b.data() + ov.ofs[i], o->rect[i].index, (size_t)o->rect[i].w * o->rect[i].h * sizeof(uint16_t));
+    h->ov.set = false;   // a CUDA error from here on leaves no overlay (and says so)
+    CK(h->ov_dev.grow(total));   // frees a smaller old copy first: cudaFree waits for the launches that read it
+    CK(cudaMemcpyAsync(h->ov_dev.p, b.data(), total, cudaMemcpyHostToDevice, h->stream));
+    ov.set = true;
+    h->ov = ov;
+    return MC_OK;
+} catch (...) { return on_exception(h); }
 
 extern "C" mc_status mc_chain_compose_device(mc_handle* h, const uint8_t* d_in, int frames, int width, int height, int channels,
                                              size_t in_step, const mc_params* p, int grayscale, int split, const mc_canvas* canvas,

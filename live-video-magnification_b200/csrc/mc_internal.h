@@ -188,7 +188,8 @@ cudaError_t launch_nv12_to_bgr(const Nv12Planes& in, int w, int h, int lanes, ui
 cudaError_t launch_bgr_to_nv12(const uint8_t* bgr, size_t bgr_step, int w, int h, int lanes, const uint8_t* flags,
                                uint8_t* y, uint8_t* uv, size_t pitch, size_t lane_stride, cudaStream_t s);
 
-// The export canvas (mc_preprocess.cu): Exporter.cpp's compose(original, cur, split) without labels, over virtual lanes.
+// The export canvas (mc_preprocess.cu): Exporter.cpp's compose(original, cur, split) over virtual lanes, its labels as
+// the handle's overlay (mc_set_overlay): per-pixel u8 tone maps inside at most kOverlayRects disjoint canvas rects.
 // A pane source holds virtual lane v's frame at p + v * lane_stride (NV12: its Cb,Cr plane at uv + v * lane_stride).
 struct PaneSrc {
     const uint8_t* p = nullptr;
@@ -198,6 +199,11 @@ struct PaneSrc {
 };
 // Which frame is virtual lane v's `cur` pane
 enum ComposeOp : uint8_t { COMPOSE_SKIP = 0, COMPOSE_MAGNIFIED = 1, COMPOSE_FALLBACK = 2 };
+constexpr int kOverlayRects = 2;    // MC_OVERLAY_MAX_RECTS
+struct OverlayRect {
+    int x = 0, y = 0, w = 0, h = 0;   // on the canvas
+    const uint16_t* index = nullptr;  // device: h rows of w map indices
+};
 struct ComposeArgs {
     PaneSrc src[3];                 // the original pane, the magnifier's output, the fallback `cur` (front output or input)
     const uint8_t* ops = nullptr;   // ComposeOp per virtual lane; null: every lane MAGNIFIED
@@ -207,6 +213,9 @@ struct ComposeArgs {
     uint8_t* data = nullptr;        // BGR canvas or NV12 luma plane of virtual lane 0
     uint8_t* uv = nullptr;          // NV12: Cb,Cr plane of virtual lane 0
     size_t pitch = 0, lane_stride = 0;
+    int ov_rects = 0;               // the overlay: 0 .. kOverlayRects rects; 0 leaves every canvas as composed
+    OverlayRect ov[kOverlayRects];
+    const uint8_t* ov_map = nullptr;   // device: the tone maps, 256 bytes each
     int vec_src = 0, vec_out = 0, pane_blocks = 0;   // set by launch_compose
 };
 cudaError_t launch_compose(ComposeArgs a, int vlanes, cudaStream_t s);

@@ -102,7 +102,8 @@ cudaError_t launch_chain_front(const FrontArgs& args, int src, int vlanes, cudaS
 
 // ---- NV12 frames in and out of the magnifier (the hand-off format of hardware video decoders and encoders): the
 // conversions to and from the packed BGR frames the modes work on, bit-exact with OpenCV's u8 fixed point
-// (nv12_to_bgr_px / bgr_to_ycc_px in mc_math.cuh); and the export canvas of Exporter.cpp:25-34, 53-88 (without labels),
+// (nv12_to_bgr_px / bgr_to_ycc_px in mc_math.cuh); and the export canvas of Exporter.cpp:25-34, 53-88 (labels as the
+// handle's overlay of per-pixel tone maps),
 // whose panes are BGR, gray (GRAY2BGR) or NV12 sources and whose canvas is BGR or NV12.  All three kernels are
 // bandwidth-bound: 1.5 B/px of NV12 and 3 B/px of BGR per pixel.  A thread owns a 2-row x 8-column block: one 64-bit load
 // or store per luma or gray row, one for the 4 Cb,Cr pairs of the block, and three per BGR row (24 bytes); rows or
@@ -277,10 +278,46 @@ __device__ __forceinline__ void load_pane(const PaneSrc& s, bool vec, size_t v, 
     }
 }
 
+// The overlay on canvas row y, columns cx .. cx + 7 held in p (BGR): each pixel inside a rect becomes map[index][v] per
+// channel.  One index load per labelled pixel, one palette byte per channel.  Columns past the pane's last one are
+// mapped too when a rect covers them (their index is inside that rect's plane) but never stored.
+__device__ __forceinline__ void overlay_row(const ComposeArgs& a, int cx, int y, uint8_t (&p)[24]) {
+#pragma unroll
+    for (int i = 0; i < kOverlayRects; ++i) {
+        const OverlayRect& o = a.ov[i];
+        const int dy = y - o.y;
+        if (i >= a.ov_rects || (unsigned)dy >= (unsigned)o.h || cx + 8 <= o.x || o.x + o.w <= cx) continue;
+        const uint16_t* row = o.index + (size_t)dy * o.w;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const int dx = cx + k - o.x;
+            if ((unsigned)dx < (unsigned)o.w) {
+                const uint8_t* t = a.ov_map + (size_t)__ldg(row + dx) * 256;
+#pragma unroll
+                for (int c = 0; c < 3; ++c) p[3 * k + c] = __ldg(t + p[3 * k + c]);
+            }
+        }
+    }
+}
+
+// Whether the canvas box [x0, x0 + w) x [y0, y0 + h) meets a rect of the overlay.
+__device__ __forceinline__ bool overlay_meets(const ComposeArgs& a, int x0, int y0, int w, int h) {
+    bool hit = false;
+#pragma unroll
+    for (int i = 0; i < kOverlayRects; ++i) {
+        const OverlayRect& o = a.ov[i];
+        hit |= i < a.ov_rects && o.x < x0 + w && x0 < o.x + o.w && o.y < y0 + h && y0 < o.y + o.h;
+    }
+    return hit;
+}
+
 // One 2-row x 8-column block of one pane of virtual lane blockIdx.z's canvas.  blockIdx.y runs over the row blocks of
-// pane 0, then those of pane 1, so a CTA stays inside one pane and reads one source.
+// pane 0, then those of pane 1, so a CTA stays inside one pane and reads one source.  A CTA whose canvas box meets an
+// overlay rect maps its pixels in registers before they are stored or converted; the others take one uniform branch.
+// Each row is mapped just before it is stored or converted, and 8 CTAs per SM (64 registers) keep the occupancy of the
+// kernel without an overlay path, with no spills (-Xptxas -v).
 template <bool NV12_OUT>
-__global__ void __launch_bounds__(kBlockX * kBlockY) k_compose(const ComposeArgs a) {
+__global__ void __launch_bounds__(kBlockX * kBlockY, 8) k_compose(const ComposeArgs a) {
     const size_t v = blockIdx.z;
     const int op = a.ops ? a.ops[v] : COMPOSE_MAGNIFIED;
     if (op == COMPOSE_SKIP) return;
@@ -296,22 +333,30 @@ __global__ void __launch_bounds__(kBlockX * kBlockY) k_compose(const ComposeArgs
     load_pane(s, full && (a.vec_src >> i & 1), v, x0, r, n, p0, p1);
     const int cx = x0 + (a.split == MC_SPLIT_LEFT_RIGHT ? pane * a.w : 0);
     const int cy = 2 * r + (a.split == MC_SPLIT_TOP_BOTTOM ? pane * a.h : 0);
+    const bool ov = a.ov_rects && overlay_meets(a, cx - 8 * (int)threadIdx.x, cy - 2 * (int)threadIdx.y, 8 * kBlockX, 2 * kBlockY);
+    if (ov) overlay_row(a, cx, cy, p0);
     const bool vec = full && a.vec_out && cx % 8 == 0;
     uint8_t* row = a.data + v * a.lane_stride + (size_t)cy * a.pitch;
     if constexpr (NV12_OUT) {
         uint8_t y0[8], y1[8], c[8];
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
-            uint8_t cb, cr, cb1, cr1;
+            uint8_t cb, cr;
             bgr_to_ycc_px(p0[3 * k], p0[3 * k + 1], p0[3 * k + 2], y0[k], cb, cr);
-            bgr_to_ycc_px(p1[3 * k], p1[3 * k + 1], p1[3 * k + 2], y1[k], cb1, cr1);   // chroma unused: dead code
             if ((k & 1) == 0) { c[k] = cb; c[k + 1] = cr; }
+        }
+        if (ov) overlay_row(a, cx, cy + 1, p1);   // row 0 is converted first: fewer bytes live while row 1 is mapped
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            uint8_t cb1, cr1;
+            bgr_to_ycc_px(p1[3 * k], p1[3 * k + 1], p1[3 * k + 2], y1[k], cb1, cr1);   // chroma unused: dead code
         }
         store(row + cx, vec, n, y0);
         store(row + a.pitch + cx, vec, n, y1);
         store(a.uv + v * a.lane_stride + (size_t)(cy / 2) * a.pitch + cx, vec, n, c);
     } else {
         store(row + (size_t)3 * cx, vec, 3 * n, p0);
+        if (ov) overlay_row(a, cx, cy + 1, p1);
         store(row + a.pitch + (size_t)3 * cx, vec, 3 * n, p1);
     }
 }

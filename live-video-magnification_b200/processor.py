@@ -343,6 +343,16 @@ class MagnificationProcessor(IProcessor):
                                                              flags.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(info)))
         return flags.astype(bool), info
 
+    def set_overlay(self, ov) -> None:
+        """mc_set_overlay: every later compose call maps its canvases through `ov` (a labels.Overlay or a
+        capi.McOverlay), until it is replaced or cleared.  The core copies it; `ov` may be dropped afterwards."""
+        st = ov.struct if hasattr(ov, "struct") else ov
+        self._check(self._lib.mc_set_overlay(self._h, C.byref(st)))
+
+    def clear_overlay(self) -> None:
+        """mc_set_overlay(NULL): later compose calls write the canvases without labels."""
+        self._check(self._lib.mc_set_overlay(self._h, None))
+
     def sync(self):
         self._check(self._lib.mc_sync(self._h))
 

@@ -11,7 +11,12 @@ Then, in a pass of its own, the compose kernel's device time (profile_kernels) a
 data-sheet 3.35 TB/s: per canvas it reads 1.5 B/px of NV12 input and 3 B/px of BGR output and writes 1.5 B/px of NV12
 over two panes.  Prints the card's name, power limit and SM clocks read in the same run, and one JSON line.
 
-    python tools/bench_compose.py [--frames 16] [--lanes 16] [--window 2.0] [--repeats 3]"""
+--labels measures the exporter's burnt-in labels instead (mc_set_overlay with lvm_b200.labels.export_labels): on
+`--lanes` lanes only, two handles take the same fused calls, one with the labels' overlay and one without, alternated
+window by window (median of `--repeats`), then their compose kernel times (profile_kernels) in alternating rounds.  The
+labels touch about 25.6 k of the canvas's 4.15 M pixels, so the difference is expected inside the run-to-run spread.
+
+    python tools/bench_compose.py [--frames 16] [--lanes 16] [--window 2.0] [--repeats 3] [--labels]"""
 import argparse
 import ctypes as C
 import json
@@ -33,6 +38,7 @@ def main():
     ap.add_argument("--lanes", type=int, default=16)
     ap.add_argument("--window", type=float, default=2.0)
     ap.add_argument("--repeats", type=int, default=3)
+    ap.add_argument("--labels", action="store_true", help="labels on against labels off (see above)")
     args = ap.parse_args()
 
     import cv2
@@ -61,6 +67,8 @@ def main():
         uv = np.stack([i420[n:n + n // 4], i420[n + n // 4:]], -1).reshape(H // 2, W)
         return np.concatenate([i420[:n].reshape(H, W), uv])
 
+    if args.labels:
+        return labels_main(args, cfg, nv12, cw, ch, lane_nv, canvas_nv, before)
     results = {}
     for lanes in (1, args.lanes):
         v = T * lanes
@@ -129,6 +137,76 @@ def main():
     result = {
         "workload": f"Laplace {W}x{H} NV12 in, {UI['levels']} levels, LeftRight into a {cw}x{ch} NV12 canvas, clips of {T}",
         **results, "window_s": args.window, "repeats": args.repeats, "card_before": before, "card_after": after,
+    }
+    print(f"card: {before.get('name')}, power limit {before.get('power.limit')}, SM clock {before.get('clocks.sm')} "
+          f"(max {before.get('clocks.max.sm')})", flush=True)
+    print(json.dumps(result), flush=True)
+
+
+def labels_main(args, cfg, nv12, cw, ch, lane_nv, canvas_nv, before):
+    import numpy as np
+    import torch
+    import lvm_b200 as L
+    from lvm_b200 import capi
+    from lvm_b200.labels import export_labels
+    from bench import H, UI, W, make_clip
+
+    T, lanes, split = args.frames, args.lanes, capi.MC_SPLIT_LEFT_RIGHT
+    v = T * lanes
+    ov = export_labels(cw, ch, split)
+    clip = make_clip(2, lanes)
+    nv = np.stack([np.stack([nv12(f) for f in fs]) for fs in clip])
+    d_nv = torch.from_numpy(nv[np.arange(v) // lanes % 2, np.arange(v) % lanes]).cuda()
+    planes_in = capi.McNv12(d_nv.data_ptr(), d_nv.data_ptr() + W * H, W, lane_nv)
+    chains, canvases = {}, {}
+    for k in ("labels", "plain"):
+        d = torch.empty((v, canvas_nv), dtype=torch.uint8, device="cuda")
+        canvases[k] = (d, capi.McCanvas(capi.MC_CANVAS_NV12, d.data_ptr(), d.data_ptr() + cw * ch, cw, canvas_nv))
+        chains[k] = L.ProcessingChainB200(0, lanes=lanes)
+    chains["labels"].magnifier.set_overlay(ov)
+
+    def call(k):
+        return lambda i: (chains[k].magnifier.chain_compose_nv12_device(planes_in, T, W, H, cfg, split, canvases[k][1]),
+                          chains[k].magnifier.sync())
+
+    paths = {k: call(k) for k in chains}
+    for fn in paths.values():
+        fn(0)
+        fn(1)
+    # the two handles ran the same frames: their canvases differ only inside the labels' rects
+    diff = (canvases["labels"][0] != canvases["plain"][0]).reshape(v, -1)[:, :cw * ch].reshape(v, ch, cw)
+    outside = diff.clone()
+    for x, y, w, h in ov.boxes():
+        outside[:, y:y + h, x:x + w] = False
+    assert not bool(outside.any()) and bool(diff.any())
+    rates = {k: [] for k in paths}
+    for _ in range(args.repeats):
+        for k, fn in paths.items():
+            n, dt = timed(fn, args.window)
+            rates[k].append(n * v / dt)
+    kernel_us = {k: [] for k in paths}
+    n_prof = 10
+    for _ in range(args.repeats):
+        for k in paths:
+            m = chains[k].magnifier
+            m.set_option("profile_kernels", 1)
+            m.profile_read()
+            for _i in range(n_prof):
+                m.chain_compose_nv12_device(planes_in, T, W, H, cfg, split, canvases[k][1])
+            launches, total_ms = m.profile_read()[("compose", 0)]
+            m.set_option("profile_kernels", 0)
+            assert launches == n_prof
+            kernel_us[k].append(total_ms * 1e3 / launches)
+    result = {
+        "workload": f"Laplace {W}x{H} NV12 in, {UI['levels']} levels, {lanes} lanes, LeftRight into a {cw}x{ch} NV12 canvas, "
+                    f"clips of {T}, labels on / off",
+        "virtual_lanes": v,
+        "label_rects": ov.boxes(), "label_pixels": sum(w * h for *_, w, h in ov.boxes()), "label_maps": len(ov.palette),
+        "frames_per_s": {k: [round(r, 1) for r in rs] for k, rs in rates.items()},
+        "frames_per_s_median": {k: round(statistics.median(rs), 1) for k, rs in rates.items()},
+        "compose_us_per_launch": {k: [round(t, 2) for t in ts] for k, ts in kernel_us.items()},
+        "compose_us_per_launch_median": {k: round(statistics.median(ts), 2) for k, ts in kernel_us.items()},
+        "window_s": args.window, "repeats": args.repeats, "card_before": before, "card_after": card(),
     }
     print(f"card: {before.get('name')}, power limit {before.get('power.limit')}, SM clock {before.get('clocks.sm')} "
           f"(max {before.get('clocks.max.sm')})", flush=True)
