@@ -218,7 +218,7 @@ mc_status mc_chain_geometry(const mc_params* p, int width, int height, int chann
  *     both buffers untouched.  mc_lane_produced reports the last frame's flags.
  *   Errors, returned before any kernel runs and with no caller buffer or state changed: MC_ERR_INVALID for steps smaller
  *     than a row, a NULL d_out when the call would write to it (a front stage is on or the mode is not None), frames < 1,
- *     frames * lanes > MC_MAX_LANES, NULL produced / info / params, or frames of mc_submit in flight; MC_ERR_UNSUPPORTED
+ *     frames * lanes > MC_MAX_LANES, NULL produced / info / params, or pipelined frames in flight; MC_ERR_UNSUPPORTED
  *     for Color's multi-lane refusals (without option "color_lane_lifecycle").  Mode None and an empty image are the
  *     identity for the magnifier: the front stages still run when they are on.
  *   Device scratch: the front keeps staging for its output (the preprocessed frames when d_original is NULL, the gray
@@ -238,6 +238,32 @@ int mc_pipeline_depth(mc_handle* h);
 mc_status mc_submit(mc_handle* h, const uint8_t* in, int width, int height, int channels,
                     size_t in_step, const mc_params* p, uint8_t* out, size_t out_step);
 mc_status mc_collect(mc_handle* h, int* produced);
+
+/* The processing chain on host frames, pipelined: mc_chain_process_device with frames == 1 on host memory, submitted
+ * and collected as mc_submit is.  One call submits one frame of every lane; mc_collect collects it, in strict FIFO
+ * order with mc_submit, mc_submit_nv12 and the other chain submits on the handle.  `*produced` of mc_collect is "at
+ * least one lane magnified", and mc_lane_produced then gives the lanes' flags (a chain submit does not change what
+ * mc_lane_produced reports before its frame is collected).
+ *   Layout: lane k of `in` at k * height * in_step (BGR or gray; NV12 and 4:2:2 frames: at k * lane_stride); lane k of
+ *     `out` at k * out_h * out_step and of `original` at k * orig_h * original_step (out_h / orig_h of `info`, or height
+ *     where the stage is an identity).  Each buffer may be pinned or pageable, independently of the others, and must stay
+ *     valid until its frame is collected.
+ *   What is written: that of mc_chain_process_device.  For each lane that is not held, `out` when the lane's flag is 1
+ *     or info.cur_is_input == 0, and `original` when info.orig_is_input == 0 and original is not NULL.  Held lanes, row
+ *     padding and the other lanes' bytes stay untouched.  For any sequence of submits and lifecycle, parameter or
+ *     structural changes, the bytes written, the flags, mc_lane_produced and the temporal state equal, bit for bit, those
+ *     of mc_chain_process_device (or its _nv12 / _yuv422 form) on the same frames uploaded by the caller; restarts,
+ *     holds and parameters are taken at submit.
+ *   info: filled by the submit, final when it returns; mc_chain_geometry's (for a 4:2:2 source both frames are written),
+ *     with magnified 0: the collected *produced carries that fact.
+ *   Errors, returned before any copy or kernel is enqueued, with the handle's state and the frames in flight unchanged:
+ *     MC_ERR_INVALID for a full pipeline, slot buffers that would have to grow while frames are in flight ("pipeline
+ *     geometry changed"), and every argument error of the matching device chain call (a NULL `out` where the call would
+ *     write it included); MC_ERR_UNSUPPORTED for Color's multi-lane refusals.  Clips are not submitted.
+ * mc_chain_submit_nv12 and mc_chain_submit_yuv422 follow the NV12 and 4:2:2 sections below. */
+mc_status mc_chain_submit(mc_handle* h, const uint8_t* in, int width, int height, int channels, size_t in_step,
+                          const mc_params* p, int grayscale, uint8_t* out, size_t out_step, uint8_t* original,
+                          size_t original_step, mc_chain_info* info);
 
 /* --- NV12 frames: the hand-off format of hardware video decoders and encoders ---------------------------------------
  * NV12 is 4:2:0 YCbCr in two planes: a luma plane (height rows of width bytes) and a plane of interleaved Cb,Cr pairs
@@ -271,6 +297,9 @@ mc_status mc_process_clip_nv12_device(mc_handle* h, const mc_nv12* in, int frame
  * each way); pageable planes go through NV12-sized pinned staging.  There is no blocking host NV12 call: submit and
  * collect. */
 mc_status mc_submit_nv12(mc_handle* h, const mc_nv12* in, int width, int height, const mc_params* p, const mc_nv12* out);
+/* mc_chain_submit on NV12 host planes (the checks of mc_chain_process_nv12_device): 1.5 B/px cross PCIe upwards. */
+mc_status mc_chain_submit_nv12(mc_handle* h, const mc_nv12* in, int width, int height, const mc_params* p, int grayscale,
+                               uint8_t* out, size_t out_step, uint8_t* original, size_t original_step, mc_chain_info* info);
 /* mc_chain_process_device on NV12 device planes: see the chain section above. */
 /* The same on NV12 device planes (laid out as in mc_process_clip_nv12_device; channels is 3).  For any NV12
  * input X it equals mc_chain_process_device on cv2.cvtColor(X, COLOR_YUV2BGR_NV12): the same bytes written, flags, info
@@ -414,6 +443,10 @@ mc_status mc_chain_compose_yuv422_device(mc_handle* h, const mc_yuv422* in, int 
 mc_status mc_chain_process_yuv422(mc_handle* h, const mc_yuv422* in, int width, int height, const mc_params* p,
                                   int grayscale, uint8_t* out, size_t out_bytes, uint8_t* original, size_t original_bytes,
                                   mc_chain_info* info);
+/* mc_chain_submit on packed 4:2:2 host frames (the checks of mc_chain_process_yuv422_device): 2 B/px cross PCIe upwards,
+ * and both frames come back, as every chain call on a 4:2:2 source writes them. */
+mc_status mc_chain_submit_yuv422(mc_handle* h, const mc_yuv422* in, int width, int height, const mc_params* p, int grayscale,
+                                 uint8_t* out, size_t out_step, uint8_t* original, size_t original_step, mc_chain_info* info);
 
 /* Pinned host memory for frames (so FramePool buffers can be DMA'd directly). */
 void* mc_host_alloc(size_t bytes);

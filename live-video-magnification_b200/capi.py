@@ -116,6 +116,12 @@ SIGNATURES = {
     "mc_pipeline_depth": (C.c_int, [_vp]),
     "mc_submit": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t]),
     "mc_collect": (C.c_int, [_vp, C.POINTER(C.c_int)]),
+    "mc_chain_submit": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, C.c_int, _vp, C.c_size_t, _vp, C.c_size_t,
+                                  C.POINTER(McChainInfo)]),
+    "mc_chain_submit_nv12": (C.c_int, [_vp, _NV, C.c_int, C.c_int, _PP, C.c_int, _vp, C.c_size_t, _vp, C.c_size_t,
+                                       C.POINTER(McChainInfo)]),
+    "mc_chain_submit_yuv422": (C.c_int, [_vp, _YV, C.c_int, C.c_int, _PP, C.c_int, _vp, C.c_size_t, _vp, C.c_size_t,
+                                         C.POINTER(McChainInfo)]),
     "mc_process_nv12_device": (C.c_int, [_vp, _NV, C.c_int, C.c_int, _PP, _NV, C.POINTER(C.c_int)]),
     "mc_process_clip_nv12_device": (C.c_int, [_vp, _NV, C.c_int, C.c_int, C.c_int, _PP, _NV, _u8p]),
     "mc_submit_nv12": (C.c_int, [_vp, _NV, C.c_int, C.c_int, _PP, _NV]),

@@ -65,14 +65,24 @@ Planes nv12_planes(const mc_nv12& f, int w, int hh) {
 }
 mc_nv12 nv12_of(const Planes& f) { return mc_nv12{f.base[0], f.base[1], f.pitch, f.lane_stride}; }
 
+Planes yuv422_planes(const mc_yuv422& f, int w, int hh) {
+    return Planes{{f.data, nullptr}, {(size_t)hh, 0}, (size_t)2 * w, f.pitch, f.lane_stride};
+}
+
+// A slot's output frame sets: the processed frames and, for chain submits, the original tap.  Set k sits at
+// out_ofs(k) in the slot's device output and in its pinned output staging.
+constexpr int kOutSets = 2;
+
 struct Slot {  // one in-flight frame of the pinned pipeline; frees what it holds
-    uint8_t *h_in = nullptr, *h_out = nullptr;   // pinned staging (lanes frames, packed)
+    uint8_t *h_in = nullptr, *h_out = nullptr;   // pinned staging (lanes frames, packed): input bytes, output bytes
     DeviceBuffer<> d_in, d_out;                  // device frames (packed)
     cudaEvent_t ev_in = nullptr, ev_k = nullptr, ev_done = nullptr;
     int produced = 0;
-    std::vector<uint8_t> lane_produced;          // per lane: its bytes of `out` are written
-    Planes out;                                  // the caller's destination (base null: none)
-    bool direct_out = false;                     // D2H went straight into `out` (pinned)
+    std::vector<uint8_t> lane_produced;          // per lane: the magnifier produced
+    Planes out[kOutSets];                        // the caller's destinations (base null: none)
+    size_t out_ofs[kOutSets] = {};
+    std::vector<uint8_t> written[kOutSets];      // per set and lane: its bytes of out[k] are written
+    bool direct_out[kOutSets] = {};              // D2H went straight into out[k] (pinned)
     ~Slot() {
         for (uint8_t* p : {h_in, h_out}) if (p) cudaFreeHost(p);
         for (cudaEvent_t e : {ev_in, ev_k, ev_done}) if (e) cudaEventDestroy(e);
@@ -109,8 +119,6 @@ struct mc_handle {
     int f_tab_key[4] = {-1, -1, -1, -1};
     size_t f_tab_ofs[3] = {0, 0, 0};   // byte offsets of the y taps, x offsets, y offsets
     std::vector<uint8_t> f_tabs_host, f_flags_host;
-    // mc_chain_process: device copies of its host frame, processed frame and original tap
-    DeviceBuffer<> c_raw, c_out, c_orig;
     // chain compose calls: the magnifier's output and the ComposeOp of every virtual lane, with its host copy
     DeviceBuffer<> x_mag, x_ops;
     std::vector<uint8_t> x_ops_host;
@@ -228,20 +236,28 @@ void free_slots(mc_handle* h) {
     h->next_slot = 0;
 }
 
-mc_status ensure_slots(mc_handle* h, size_t bytes) {
-    if ((int)h->slots.size() == h->depth && h->slots[0].d_in.n >= bytes) return MC_OK;
+// Slots for `in_bytes` of input and `out_bytes` of output per frame set.  They are reallocated, never below their current
+// sizes, only while nothing is in flight.
+mc_status ensure_slots(mc_handle* h, size_t in_bytes, size_t out_bytes) {
+    const bool have = (int)h->slots.size() == h->depth;
+    if (have && h->slots[0].d_in.n >= in_bytes && h->slots[0].d_out.n >= out_bytes) return MC_OK;
     if (!h->inflight.empty()) {
         h->err = "pipeline geometry changed with frames in flight";
         return MC_ERR_INVALID;
+    }
+    if (have) {
+        in_bytes = std::max(in_bytes, h->slots[0].d_in.n);
+        out_bytes = std::max(out_bytes, h->slots[0].d_out.n);
     }
     free_slots(h);
     h->slots = std::vector<Slot>((size_t)h->depth);
     for (auto& s : h->slots) {
         s.lane_produced.assign((size_t)h->lanes, 0);
-        CK(cudaHostAlloc((void**)&s.h_in, bytes, cudaHostAllocDefault));
-        CK(cudaHostAlloc((void**)&s.h_out, bytes, cudaHostAllocDefault));
-        CK(s.d_in.grow(bytes));
-        CK(s.d_out.grow(bytes));
+        for (auto& w : s.written) w.assign((size_t)h->lanes, 0);
+        CK(cudaHostAlloc((void**)&s.h_in, in_bytes, cudaHostAllocDefault));
+        CK(cudaHostAlloc((void**)&s.h_out, out_bytes, cudaHostAllocDefault));
+        CK(s.d_in.grow(in_bytes));
+        CK(s.d_out.grow(out_bytes));
         CK(cudaEventCreateWithFlags(&s.ev_in, cudaEventDisableTiming));
         CK(cudaEventCreateWithFlags(&s.ev_k, cudaEventDisableTiming));
         CK(cudaEventCreateWithFlags(&s.ev_done, cudaEventDisableTiming));
@@ -379,22 +395,35 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
 }
 
 // One frame set into the pipeline.  `in` is uploaded on the input stream into the next slot's packed device copy:
-// directly when it is pinned, through the slot's pinned staging when not.  `run(d_in, d_out, produced, lane_produced)`
-// then fills the slot's packed output on the handle's stream (with no buffers when `in` is empty: the identity).  Only
-// the lanes that produced are downloaded on the output stream, one copy per run of consecutive ones, into `out` when it
-// is pinned and into the staging, which mc_collect copies out, when not; the other lanes' bytes of `out` stay as they
-// are.  The slot's d_in is not overwritten before its kernels ran: the next upload into it follows mc_collect of this
-// frame, which waits on ev_done.
+// directly when it is pinned, through the slot's pinned staging when not.  `run(d_in, d_out, produced, lane_produced,
+// written)` then fills the slot's packed output sets d_out[k] (the shapes of out[k], which may differ from `in`'s) on the
+// handle's stream (with no buffers when `in` is empty: the identity), and says per set which lanes it wrote.  Only those
+// lanes are downloaded on the output stream, one copy per run of consecutive ones, into out[k] when it is pinned and into
+// the staging, which mc_collect copies out, when not; the other lanes' bytes of out[k] stay as they are.  The slot's d_in
+// is not overwritten before its kernels ran: the next upload into it follows mc_collect of this frame, which waits on
+// ev_done.  The slots' output holds at least out_reserve bytes.
 template <class Run>
-mc_status submit_impl(mc_handle* h, const Planes& in, const Planes& out, Run run) {
+mc_status submit_impl(mc_handle* h, const Planes& in, const Planes (&out)[kOutSets], Run run, size_t out_reserve = 0) {
     const size_t lanes = (size_t)h->lanes, bytes = in.lane_bytes() * lanes;
-    mc_status st = ensure_slots(h, std::max<size_t>(bytes, 1));
+    size_t ofs[kOutSets], out_bytes = 0;
+    for (int k = 0; k < kOutSets; ++k) {
+        if (out[k].base[0] && out[k].pitch < out[k].row) { h->err = "out_step too small"; return MC_ERR_INVALID; }
+        ofs[k] = out_bytes;
+        out_bytes += (out[k].lane_bytes() * lanes + 255) / 256 * 256;   // each set 256-byte aligned
+    }
+    mc_status st = ensure_slots(h, std::max<size_t>(bytes, 1), std::max<size_t>({out_bytes, out_reserve, 1}));
     if (st != MC_OK) return st;
-    if (out.base[0] && out.pitch < out.row) { h->err = "out_step too small"; return MC_ERR_INVALID; }
     const int si = h->next_slot;
     Slot& s = h->slots[(size_t)si];
-    s.produced = 0; s.out = out; s.direct_out = false;
-    const Planes none, d_in = bytes ? in.packed(s.d_in.p) : none, d_out = bytes ? in.packed(s.d_out.p) : none;
+    s.produced = 0;
+    const Planes none;
+    Planes d_out[kOutSets];
+    for (int k = 0; k < kOutSets; ++k) {
+        s.out[k] = out[k]; s.out_ofs[k] = ofs[k]; s.direct_out[k] = false;
+        std::fill(s.written[k].begin(), s.written[k].end(), (uint8_t)0);
+        d_out[k] = out[k].lane_bytes() ? out[k].packed(s.d_out.p + ofs[k]) : none;
+    }
+    const Planes d_in = bytes ? in.packed(s.d_in.p) : none;
     if (bytes) {
         const bool pinned = is_pinned(in);
         const Planes src = pinned ? in : in.packed(s.h_in);
@@ -405,16 +434,20 @@ mc_status submit_impl(mc_handle* h, const Planes& in, const Planes& out, Run run
         CK(cudaStreamWaitEvent(h->stream, s.ev_in, 0));
     }
     int produced = 0;
-    if ((st = run(d_in, d_out, &produced, s.lane_produced.data())) != MC_OK) return st;
+    if ((st = run(d_in, d_out, &produced, s.lane_produced.data(), s.written)) != MC_OK) return st;
     s.produced = produced;
-    if (produced) {
+    bool download = false;
+    for (int k = 0; k < kOutSets; ++k)
+        download |= out[k].base[0] && std::any_of(s.written[k].begin(), s.written[k].end(), [](uint8_t x) { return x != 0; });
+    if (download) {
         CK(cudaEventRecord(s.ev_k, h->stream));
         CK(cudaStreamWaitEvent(h->s_out, s.ev_k, 0));
-        if (out.base[0]) {
-            s.direct_out = is_pinned(out);
-            const Planes dst = s.direct_out ? out : out.packed(s.h_out);
-            st = for_each_run(lanes, [&](size_t l) { return s.lane_produced[l] != 0; }, [&](size_t a, size_t b) {
-                return copy_planes(h, dst, d_out, a, b, cudaMemcpyDeviceToHost, h->s_out);
+        for (int k = 0; k < kOutSets; ++k) {
+            if (!out[k].base[0]) continue;
+            s.direct_out[k] = is_pinned(out[k]);
+            const Planes dst = s.direct_out[k] ? out[k] : out[k].packed(s.h_out + ofs[k]);
+            st = for_each_run(lanes, [&](size_t l) { return s.written[k][l] != 0; }, [&](size_t a, size_t b) {
+                return copy_planes(h, dst, d_out[k], a, b, cudaMemcpyDeviceToHost, h->s_out);
             });
             if (st != MC_OK) return st;
         }
@@ -672,10 +705,12 @@ mc_status mc_submit(mc_handle* h, const uint8_t* in, int width, int height, int 
     if (have && in_step < (size_t)width * channels) { h->err = "step too small"; return MC_ERR_INVALID; }
     const Planes none;
     return submit_impl(h, have ? bgr_planes(in, width, height, channels, in_step) : none,
-                       have ? bgr_planes(out, width, height, channels, out_step) : none,
-                       [&](const Planes& d_in, const Planes& d_out, int* produced, uint8_t* lane_produced) {
-                           return process_device_impl(h, d_in.base[0], width, height, channels, d_in.pitch, p, d_out.base[0],
-                                                      d_out.pitch, produced, lane_produced);
+                       {have ? bgr_planes(out, width, height, channels, out_step) : none, none},
+                       [&](const Planes& d_in, const Planes* d_out, int* produced, uint8_t* lane_produced, std::vector<uint8_t>* written) {
+                           const mc_status st = process_device_impl(h, d_in.base[0], width, height, channels, d_in.pitch, p,
+                                                                    d_out[0].base[0], d_out[0].pitch, produced, lane_produced);
+                           std::copy(lane_produced, lane_produced + h->lanes, written[0].begin());
+                           return st;
                        });
 } catch (...) { return on_exception(h); }
 
@@ -689,10 +724,11 @@ mc_status mc_collect(mc_handle* h, int* produced) try {
     CK(cudaEventSynchronize(s.ev_done));
     *produced = s.produced;
     h->lane_produced = s.lane_produced;
-    if (s.produced && !s.direct_out && s.out.base[0]) {
-        const Planes staged = s.out.packed(s.h_out);
+    for (int k = 0; k < kOutSets; ++k) {
+        if (s.direct_out[k] || !s.out[k].base[0]) continue;
+        const Planes staged = s.out[k].packed(s.h_out + s.out_ofs[k]);
         for (size_t l = 0; l < (size_t)h->lanes; ++l)
-            if (s.lane_produced[l]) host_copy(s.out, staged, l);
+            if (s.written[k][l]) host_copy(s.out[k], staged, l);
     }
     return MC_OK;
 } catch (...) { return on_exception(h); }
@@ -823,14 +859,14 @@ mc_status check_clip(mc_handle* h, int frames, const uint8_t* produced) {
     return MC_OK;
 }
 
-// d_in null: the identity (no frame produces; a handle that was magnifying drops its state)
-mc_status clip_impl(mc_handle* h, const uint8_t* d_in, int frames, int w, int hh, int channels, size_t in_step, const mc_params* p,
-                    uint8_t* d_out, size_t out_step, uint8_t* produced) {
-    mc_status st = check_clip(h, frames, produced);
-    if (st != MC_OK) return st;
+// The magnifier over `frames` consecutive frames of every lane, once the clip's arguments are checked.  d_in null: the
+// identity (no frame produces; a handle that was magnifying drops its state)
+mc_status clip_run(mc_handle* h, const uint8_t* d_in, int frames, int w, int hh, int channels, size_t in_step, const mc_params* p,
+                   uint8_t* d_out, size_t out_step, uint8_t* produced) {
     const size_t lanes = (size_t)h->lanes;
     std::fill(produced, produced + (size_t)frames * lanes, (uint8_t)0);
     int any = 0;
+    mc_status st = MC_OK;
     if (p && (p->mode == MC_MODE_LAPLACE || p->mode == MC_MODE_PHASE || p->mode == MC_MODE_COLOR) && frames > 1) {
         st = process_device_impl(h, d_in, w, hh, channels, in_step, p, d_out, out_step, &any, produced, frames);
     } else {
@@ -841,7 +877,16 @@ mc_status clip_impl(mc_handle* h, const uint8_t* d_in, int frames, int w, int hh
                                      d_out ? d_out + (size_t)t * out_frame : nullptr, out_step, &any, produced + (size_t)t * lanes);
     }
     if (st != MC_OK) std::fill(produced, produced + (size_t)frames * lanes, (uint8_t)0);   // the state was dropped
-    std::memcpy(h->lane_produced.data(), produced + (size_t)(frames - 1) * lanes, lanes);
+    return st;
+}
+
+// A device clip call: checked, run, and its last frame's flags are mc_lane_produced's.
+mc_status clip_impl(mc_handle* h, const uint8_t* d_in, int frames, int w, int hh, int channels, size_t in_step, const mc_params* p,
+                    uint8_t* d_out, size_t out_step, uint8_t* produced) {
+    mc_status st = check_clip(h, frames, produced);
+    if (st != MC_OK) return st;
+    st = clip_run(h, d_in, frames, w, hh, channels, in_step, p, d_out, out_step, produced);
+    std::memcpy(h->lane_produced.data(), produced + (size_t)(frames - 1) * h->lanes, (size_t)h->lanes);
     return st;
 }
 }  // namespace
@@ -985,9 +1030,12 @@ extern "C" mc_status mc_submit_nv12(mc_handle* h, const mc_nv12* in, int width, 
     if ((int)h->inflight.size() >= h->depth) { h->err = "pipeline full: call mc_collect first"; return MC_ERR_INVALID; }
     const mc_status st = check_nv12(h, {in, out}, width, height, h->lanes, p);
     if (st != MC_OK) return st;
-    return submit_impl(h, nv12_planes(*in, width, height), nv12_planes(*out, width, height),
-                       [&](const Planes& d_in, const Planes& d_out, int* produced, uint8_t* lane_produced) {
-                           return nv12_frame(h, nv12_of(d_in), nv12_of(d_out), width, height, p, produced, lane_produced);
+    return submit_impl(h, nv12_planes(*in, width, height), {nv12_planes(*out, width, height), Planes{}},
+                       [&](const Planes& d_in, const Planes* d_out, int* produced, uint8_t* lane_produced, std::vector<uint8_t>* written) {
+                           const mc_status st = nv12_frame(h, nv12_of(d_in), nv12_of(d_out[0]), width, height, p, produced,
+                                                           lane_produced);
+                           std::copy(lane_produced, lane_produced + h->lanes, written[0].begin());
+                           return st;
                        });
 } catch (...) { return on_exception(h); }
 
@@ -1099,32 +1147,29 @@ const char* check_yuv422(const mc_yuv422& f, int w, int hh, size_t vl) {
     return nullptr;
 }
 
-// runChainOnce for every lane and `frames` consecutive frames: the source is d_in (u8 BGR or gray, in_step) or, when nv
-// is not null, NV12 planes, or, when yv is not null, a packed 4:2:2 frame (both channels 3).  A 4:2:2 source's conversion
-// is a front stage that always runs: the front writes its BGR frame (d_orig, or the magnifier's input in staging) where
-// a BGR source would leave the result to the input.  Everything is checked before the front kernel runs; then one front launch
-// writes the preprocessed frames (d_original, or staging) and the magnifier's input (the same frames or their gray),
-// the magnifier writes d_out, and the frames it did not produce get the front's output.  produced: frames * lanes flags.
-// With cmp, the call composes instead: d_out / d_orig are not the caller's, the magnifier writes h->x_mag, the
-// preprocessed frames stay in h->f_pre when the canvas shows them, and one compose launch reads every pane where it is.
-mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc_nv12* nv, const mc_yuv422* yv, int frames,
-                     int w, int hh, int channels, const mc_params* p, int grayscale, uint8_t* d_out, size_t out_step,
-                     uint8_t* d_orig, size_t orig_step, uint8_t* produced, mc_chain_info* info,
-                     const ComposeReq* cmp = nullptr) {
+bool chain_empty(const uint8_t* in, const mc_nv12* nv, const mc_yuv422* yv, int w, int hh) {
+    return !nv && !yv && (in == nullptr || w <= 0 || hh <= 0);
+}
+
+// The argument errors of a chain call on `frames` consecutive frames of every lane, before anything changes, and its
+// geometry g and info.  Only the pointers' nullness is read, so host and device frame sets are checked alike: in (u8 BGR
+// or gray, in_step), or NV12 planes nv, or a packed 4:2:2 frame yv; out_given / orig_given: the processed frames' and
+// the original tap's destinations are not NULL.  A 4:2:2 source's conversion is a front stage that always runs: the
+// front writes its BGR frame where a BGR source would leave the result to the input, and info says so.
+mc_status chain_check(mc_handle* h, const uint8_t* in, size_t in_step, const mc_nv12* nv, const mc_yuv422* yv, int frames, int w,
+                      int hh, int channels, const mc_params* p, int grayscale, bool out_given, size_t out_step, bool orig_given,
+                      size_t orig_step, mc_chain_info* info, const ComposeReq* cmp, ChainGeom& g) {
     if (!p || !info) { h->err = "params or info is null"; return MC_ERR_INVALID; }
-    const bool empty = !nv && !yv && (d_in == nullptr || w <= 0 || hh <= 0);
-    ChainGeom g;
+    const bool empty = chain_empty(in, nv, yv, w, hh);
     if (const char* e = chain_geometry(p, empty ? 0 : w, empty ? 0 : hh, channels, grayscale, g, info)) {
         h->err = e;
         return MC_ERR_INVALID;
     }
-    const bool pre = g.pre || yv, front = g.front() || yv;   // what the front writes: see above
+    const bool pre = g.pre || yv, front = g.front() || yv;
     if (yv) {
         info->orig_is_input = 0; info->orig_w = g.dw; info->orig_h = g.dh; info->orig_channels = 3;
         info->cur_is_input = 0; info->out_w = g.dw; info->out_h = g.dh; info->out_channels = g.cc;
     }
-    mc_status st = check_clip(h, frames, produced);
-    if (st != MC_OK) return st;
     const size_t lanes = (size_t)h->lanes, vl = (size_t)frames * lanes;
     if (yv) {
         if (const char* e = check_yuv422(*yv, w, hh, vl)) { h->err = e; return MC_ERR_INVALID; }
@@ -1132,7 +1177,8 @@ mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc
     if (cmp) {
         if (const char* e = check_compose(*cmp, g, vl, h->ov)) { h->err = e; return MC_ERR_INVALID; }
     }
-    if (empty) return clip_impl(h, nullptr, frames, 0, 0, channels, 0, p, nullptr, 0, produced);   // the identity
+    if (empty) return MC_OK;   // the identity
+    mc_status st;
     if (nv) {
         if ((st = check_nv12(h, {nv}, w, hh, (int)vl, p)) != MC_OK) return st;
     } else if (!yv && in_step < (size_t)w * channels) {
@@ -1140,12 +1186,11 @@ mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc
         return MC_ERR_INVALID;
     }
     if (p->mode < 0 || p->mode > MC_MODE_NONE) { h->err = "bad mode"; return MC_ERR_INVALID; }
-    const size_t out_row = (size_t)g.dw * g.cc;
     if (!cmp && (front || p->mode != MC_MODE_NONE)) {
-        if (!d_out) { h->err = "output pointer is null"; return MC_ERR_INVALID; }
-        if (out_step < out_row) { h->err = "out_step too small"; return MC_ERR_INVALID; }
+        if (!out_given) { h->err = "output pointer is null"; return MC_ERR_INVALID; }
+        if (out_step < (size_t)g.dw * g.cc) { h->err = "out_step too small"; return MC_ERR_INVALID; }
     }
-    if (!cmp && pre && d_orig && orig_step < (size_t)g.dw * channels) {
+    if (!cmp && pre && orig_given && orig_step < (size_t)g.dw * channels) {
         h->err = "original_step too small";
         return MC_ERR_INVALID;
     }
@@ -1154,6 +1199,24 @@ mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc
         const int levels = std::min(std::max((int)p->levels, 1), max_levels);
         if ((st = color_lane_check(h, p, levels, g.cc, g.dw, g.dh)) != MC_OK) return st;
     }
+    return MC_OK;
+}
+
+// runChainOnce for every lane and `frames` consecutive frames, on device frame sets that passed chain_check (which gave
+// g).  One front launch writes the preprocessed frames (d_orig, or staging) and the magnifier's input (the same frames or
+// their gray), the magnifier writes d_out, and the frames it did not produce get the front's output.  produced: frames *
+// lanes flags.  With cmp, the call composes instead: d_out / d_orig are not the caller's, the magnifier writes h->x_mag,
+// the preprocessed frames stay in h->f_pre when the canvas shows them, and one compose launch reads every pane where it is.
+// Everything it uses of the handle's chain scratch (f_pre, f_gray, f_flags, f_tabs, n_in, x_mag, x_ops and the host
+// copies) is written and read on the handle's stream only, so pipelined frames may share it in submit order.
+mc_status chain_run(mc_handle* h, const ChainGeom& g, const uint8_t* d_in, size_t in_step, const mc_nv12* nv, const mc_yuv422* yv,
+                    int frames, int w, int hh, int channels, const mc_params* p, uint8_t* d_out, size_t out_step, uint8_t* d_orig,
+                    size_t orig_step, uint8_t* produced, const ComposeReq* cmp = nullptr) {
+    const size_t lanes = (size_t)h->lanes, vl = (size_t)frames * lanes;
+    if (chain_empty(d_in, nv, yv, w, hh)) return clip_run(h, nullptr, frames, 0, 0, channels, 0, p, nullptr, 0, produced);
+    const bool pre = g.pre || yv, front = g.front() || yv;
+    const size_t out_row = (size_t)g.dw * g.cc;
+    mc_status st;
     if (cmp) {
         if (p->mode != MC_MODE_NONE) {
             CK(h->x_mag.grow(out_row * g.dh * vl));
@@ -1167,7 +1230,6 @@ mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc
         }
     }
     const bool tap = pre && d_orig;
-
     // ---- the front: one launch over the virtual lanes; held lanes are skipped
     const uint8_t* mag_in = d_in;
     size_t mag_step = in_step;
@@ -1208,8 +1270,7 @@ mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc
     }
 
     // ---- the magnifier, straight into d_out; then the canvases, or the front's output for the frames it did not produce
-    if ((st = clip_impl(h, mag_in, frames, g.dw, g.dh, g.cc, mag_step, p, d_out, out_step, produced)) != MC_OK) return st;
-    info->magnified = std::any_of(produced, produced + vl, [](uint8_t x) { return x != 0; });
+    if ((st = clip_run(h, mag_in, frames, g.dw, g.dh, g.cc, mag_step, p, d_out, out_step, produced)) != MC_OK) return st;
     if (cmp) {
         ComposeArgs a;
         a.w = g.dw & ~1; a.h = g.dh & ~1;
@@ -1249,6 +1310,26 @@ mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc
                              cudaMemcpyDeviceToDevice, h->stream));
         return MC_OK;
     });
+}
+
+// A device chain call: checked (with the pipelined frames' refusal), run, and its last frame's flags are
+// mc_lane_produced's.
+mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc_nv12* nv, const mc_yuv422* yv, int frames,
+                     int w, int hh, int channels, const mc_params* p, int grayscale, uint8_t* d_out, size_t out_step,
+                     uint8_t* d_orig, size_t orig_step, uint8_t* produced, mc_chain_info* info,
+                     const ComposeReq* cmp = nullptr) {
+    mc_status st = check_clip(h, frames, produced);
+    if (st != MC_OK) return st;
+    ChainGeom g;
+    if ((st = chain_check(h, d_in, in_step, nv, yv, frames, w, hh, channels, p, grayscale, d_out != nullptr, out_step,
+                          d_orig != nullptr, orig_step, info, cmp, g)) != MC_OK)
+        return st;
+    st = chain_run(h, g, d_in, in_step, nv, yv, frames, w, hh, channels, p, d_out, out_step, d_orig, orig_step, produced, cmp);
+    if (st != MC_OK) return st;
+    const size_t lanes = (size_t)h->lanes, vl = (size_t)frames * lanes;
+    std::memcpy(h->lane_produced.data(), produced + vl - lanes, lanes);
+    info->magnified = std::any_of(produced, produced + vl, [](uint8_t x) { return x != 0; });
+    return MC_OK;
 }
 }  // namespace
 
@@ -1383,49 +1464,92 @@ extern "C" mc_status mc_chain_compose_yuv422_device(mc_handle* h, const mc_yuv42
                       &c);
 } catch (...) { return on_exception(h); }
 
+namespace {
+// The body of the chain submits and of the blocking host chain calls: chain_check on the host frame set, then one slot of
+// the pipeline whose run is chain_run on the slot's buffers.  The processed frames go to `out` (lane k at k * out_h *
+// out_step) and the original tap to `original` (lane k at k * orig_h * original_step).  out_optional: a NULL `out` is
+// not an error; the processed frames are then not downloaded.
+mc_status chain_submit(mc_handle* h, const uint8_t* in, size_t in_step, const mc_nv12* nv, const mc_yuv422* yv, int w, int hh,
+                       int channels, const mc_params* p, int grayscale, uint8_t* out, size_t out_step, uint8_t* original,
+                       size_t original_step, mc_chain_info* info, bool out_optional = false) {
+    if ((int)h->inflight.size() >= h->depth) { h->err = "pipeline full: call mc_collect first"; return MC_ERR_INVALID; }
+    ChainGeom g;
+    mc_status st = chain_check(h, in, in_step, nv, yv, 1, w, hh, channels, p, grayscale, out || out_optional, out_step,
+                               original != nullptr, original_step, info, nullptr, g);
+    if (st != MC_OK) return st;
+    const bool empty = chain_empty(in, nv, yv, w, hh), front = g.front() || yv, tap = (g.pre || yv) && original;
+    Planes src, dst[kOutSets];
+    if (!empty) {
+        src = nv ? nv12_planes(*nv, w, hh) : yv ? yuv422_planes(*yv, w, hh) : bgr_planes(in, w, hh, channels, in_step);
+        dst[0] = bgr_planes(out, g.dw, g.dh, g.cc, out_step);
+        if (tap) dst[1] = bgr_planes(original, g.dw, g.dh, channels, original_step);
+    }
+    // Room for the largest outputs of this frame size (no crop or downscale, no gray), so that a ROI, downscale or grayscale
+    // change with frames in flight does not have to grow the slots.
+    const size_t full = empty ? 0 : ((size_t)w * hh * (yv ? 3 : channels) * h->lanes + 255) / 256 * 256;
+    const int order = yv ? yv->order : 0;
+    return submit_impl(h, src, dst, [&](const Planes& d_in, const Planes* d_out, int* produced, uint8_t* lane_produced,
+                                        std::vector<uint8_t>* written) {
+        const mc_nv12 dnv = nv12_of(d_in);
+        const mc_yuv422 dyv{d_in.base[0], d_in.pitch, d_in.lane_stride, order};
+        const mc_status rs = chain_run(h, g, d_in.base[0], d_in.pitch, nv ? &dnv : nullptr, yv ? &dyv : nullptr, 1, w, hh, channels,
+                                       p, d_out[0].base[0], d_out[0].pitch, d_out[1].base[0], d_out[1].pitch, lane_produced);
+        if (rs != MC_OK) return rs;
+        *produced = std::any_of(lane_produced, lane_produced + h->lanes, [](uint8_t x) { return x != 0; });
+        for (size_t l = 0; l < (size_t)h->lanes; ++l) {   // what chain_run wrote: see mc_chain_process_device
+            written[0][l] = lane_produced[l] || (front && !h->hold[l]);
+            written[1][l] = tap && !h->hold[l];
+        }
+        return MC_OK;
+    }, original ? 2 * full : full);
+}
+
+// The blocking 1-lane host calls: chain_submit + mc_collect into tight buffers.  yuv: the source is the 4:2:2 frame yv,
+// whose conversion always runs, so a buffer too small for its frame is refused before anything runs.  A BGR or gray
+// frame's buffer that turns out too small for what the chain wrote is not downloaded, and the call returns
+// MC_ERR_INVALID once the frame ran.
+mc_status chain_host_call(mc_handle* h, const char* name, const uint8_t* in, size_t in_step, bool yuv, const mc_yuv422* yv, int w,
+                          int hh, int channels, const mc_params* p, int grayscale, uint8_t* out, size_t out_bytes, uint8_t* original,
+                          size_t original_bytes, mc_chain_info* info) {
+    std::memset(info, 0, sizeof(*info));
+    info->cur_is_input = 1; info->orig_is_input = 1;
+    if (h->lanes != 1) { h->err = std::string(name) + " needs a 1-lane handle"; return MC_ERR_INVALID; }
+    if (!h->inflight.empty()) { h->err = std::string(name) + " called with pipelined frames in flight"; return MC_ERR_INVALID; }
+    if (h->hold[0]) { h->err = std::string(name) + " called while lane 0 is held"; return MC_ERR_INVALID; }
+    if (yuv && !yv) { h->err = "YUYV frame is null"; return MC_ERR_INVALID; }
+    ChainGeom g;
+    const bool have = !chain_empty(in, nullptr, yv, w, hh);
+    if (const char* e = chain_geometry(p, have ? w : 0, have ? hh : 0, channels, grayscale, g, info)) {
+        h->err = e;
+        return MC_ERR_INVALID;
+    }
+    const size_t out_frame = (size_t)g.dw * g.dh * g.cc, orig_frame = (size_t)g.dw * g.dh * channels;
+    const bool out_fits = out && out_bytes >= out_frame, orig_fits = original && original_bytes >= orig_frame;
+    if (yuv && out && !out_fits) { h->err = "out buffer too small"; return MC_ERR_INVALID; }
+    if (yuv && original && !orig_fits) { h->err = "original buffer too small"; return MC_ERR_INVALID; }
+    mc_status st = chain_submit(h, in, in_step, nullptr, yv, w, hh, channels, p, grayscale, out_fits ? out : nullptr,
+                                (size_t)g.dw * g.cc, orig_fits ? original : nullptr, (size_t)g.dw * channels, info, true);
+    if (st != MC_OK) return st;
+    int produced = 0;
+    if ((st = mc_collect(h, &produced)) != MC_OK) return st;
+    info->magnified = produced != 0;
+    if (produced && info->cur_is_input) {   // no front stage: the magnified frame is the chain's result
+        info->cur_is_input = 0; info->out_w = g.dw; info->out_h = g.dh; info->out_channels = g.cc;
+    }
+    if (!info->orig_is_input && original && !orig_fits) { h->err = "original buffer too small"; return MC_ERR_INVALID; }
+    if (!info->cur_is_input && out && !out_fits) { h->err = "out buffer too small"; return MC_ERR_INVALID; }
+    return MC_OK;
+}
+}  // namespace
+
 // The one-lane host form: the frame is uploaded, runs the device chain, and what it wrote comes back tight.
 extern "C" mc_status mc_chain_process(mc_handle* h, const uint8_t* in, int width, int height, int channels, size_t in_step,
                                       const mc_params* p, int grayscale, uint8_t* out, size_t out_bytes, uint8_t* original,
                                       size_t original_bytes, mc_chain_info* info) try {
     if (!h || !p || !info) return MC_ERR_INVALID;
-    std::memset(info, 0, sizeof(*info));
-    info->cur_is_input = 1; info->orig_is_input = 1;
     CK(cudaSetDevice(h->device));
-    if (h->lanes != 1) { h->err = "mc_chain_process needs a 1-lane handle"; return MC_ERR_INVALID; }
-    if (!h->inflight.empty()) { h->err = "mc_chain_process called with pipelined frames in flight"; return MC_ERR_INVALID; }
-    if (h->hold[0]) { h->err = "mc_chain_process called while lane 0 is held"; return MC_ERR_INVALID; }
-    const bool have = in != nullptr && width > 0 && height > 0;
-    ChainGeom g;
-    if (const char* e = chain_geometry(p, have ? width : 0, have ? height : 0, channels, grayscale, g, info)) {
-        h->err = e;
-        return MC_ERR_INVALID;
-    }
-    const size_t row = have ? (size_t)width * channels : 0, out_frame = (size_t)g.dw * g.dh * g.cc;
-    const size_t orig_frame = (size_t)g.dw * g.dh * channels;
-    if (have) {
-        if (in_step < row) { h->err = "step too small"; return MC_ERR_INVALID; }
-        CK(h->c_raw.grow(row * height));
-        CK(h->c_out.grow(out_frame));
-        if (g.pre) CK(h->c_orig.grow(orig_frame));
-        CK(cudaMemcpy2DAsync(h->c_raw.p, row, in, in_step, row, (size_t)height, cudaMemcpyHostToDevice, h->stream));
-    }
-    uint8_t produced = 0;
-    const mc_status st = chain_impl(h, have ? h->c_raw.p : nullptr, row, nullptr, nullptr, 1, width, height, channels, p, grayscale, h->c_out.p,
-                                    (size_t)g.dw * g.cc, g.pre ? h->c_orig.p : nullptr, (size_t)g.dw * channels, &produced, info);
-    if (st != MC_OK || !have) return st;
-    if (produced && info->cur_is_input) {   // no front stage: the magnified frame is the chain's result
-        info->cur_is_input = 0; info->out_w = g.dw; info->out_h = g.dh; info->out_channels = g.cc;
-    }
-    if (!info->orig_is_input && original) {
-        if (original_bytes < orig_frame) { h->err = "original buffer too small"; return MC_ERR_INVALID; }
-        CK(cudaMemcpyAsync(original, h->c_orig.p, orig_frame, cudaMemcpyDeviceToHost, h->stream));
-    }
-    if (!info->cur_is_input && out) {
-        if (out_bytes < out_frame) { h->err = "out buffer too small"; return MC_ERR_INVALID; }
-        CK(cudaMemcpyAsync(out, h->c_out.p, out_frame, cudaMemcpyDeviceToHost, h->stream));
-    }
-    CK(cudaStreamSynchronize(h->stream));
-    return MC_OK;
+    return chain_host_call(h, "mc_chain_process", in, in_step, false, nullptr, width, height, channels, p, grayscale, out, out_bytes,
+                           original, original_bytes, info);
 } catch (...) { return on_exception(h); }
 
 // The live camera form: the 2 * width bytes of each row go up in one 2D copy, run the device chain, and both of its
@@ -1434,33 +1558,38 @@ extern "C" mc_status mc_chain_process_yuv422(mc_handle* h, const mc_yuv422* in, 
                                              int grayscale, uint8_t* out, size_t out_bytes, uint8_t* original,
                                              size_t original_bytes, mc_chain_info* info) try {
     if (!h || !p || !info) return MC_ERR_INVALID;
-    std::memset(info, 0, sizeof(*info));
-    info->cur_is_input = 1; info->orig_is_input = 1;
     CK(cudaSetDevice(h->device));
-    if (h->lanes != 1) { h->err = "mc_chain_process_yuv422 needs a 1-lane handle"; return MC_ERR_INVALID; }
-    if (!h->inflight.empty()) { h->err = "mc_chain_process_yuv422 called with pipelined frames in flight"; return MC_ERR_INVALID; }
-    if (h->hold[0]) { h->err = "mc_chain_process_yuv422 called while lane 0 is held"; return MC_ERR_INVALID; }
+    return chain_host_call(h, "mc_chain_process_yuv422", nullptr, 0, true, in, width, height, 3, p, grayscale, out, out_bytes,
+                           original, original_bytes, info);
+} catch (...) { return on_exception(h); }
+
+// The pipelined host chain: one frame of every lane per submit, collected by mc_collect in submit order with mc_submit and
+// mc_submit_nv12 frames.
+extern "C" mc_status mc_chain_submit(mc_handle* h, const uint8_t* in, int width, int height, int channels, size_t in_step,
+                                     const mc_params* p, int grayscale, uint8_t* out, size_t out_step, uint8_t* original,
+                                     size_t original_step, mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    return chain_submit(h, in, in_step, nullptr, nullptr, width, height, channels, p, grayscale, out, out_step, original,
+                        original_step, info);
+} catch (...) { return on_exception(h); }
+
+extern "C" mc_status mc_chain_submit_nv12(mc_handle* h, const mc_nv12* in, int width, int height, const mc_params* p, int grayscale,
+                                          uint8_t* out, size_t out_step, uint8_t* original, size_t original_step,
+                                          mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    if (!in) { h->err = "NV12 plane is null"; return MC_ERR_INVALID; }
+    return chain_submit(h, nullptr, 0, in, nullptr, width, height, 3, p, grayscale, out, out_step, original, original_step, info);
+} catch (...) { return on_exception(h); }
+
+extern "C" mc_status mc_chain_submit_yuv422(mc_handle* h, const mc_yuv422* in, int width, int height, const mc_params* p,
+                                            int grayscale, uint8_t* out, size_t out_step, uint8_t* original, size_t original_step,
+                                            mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
     if (!in) { h->err = "YUYV frame is null"; return MC_ERR_INVALID; }
-    if (const char* e = check_yuv422(*in, width, height, 1)) { h->err = e; return MC_ERR_INVALID; }
-    if (p->mode < 0 || p->mode > MC_MODE_NONE) { h->err = "bad mode"; return MC_ERR_INVALID; }
-    ChainGeom g;
-    if (const char* e = chain_geometry(p, width, height, 3, grayscale, g, info)) { h->err = e; return MC_ERR_INVALID; }
-    const size_t row = (size_t)2 * width, out_frame = (size_t)g.dw * g.dh * g.cc, orig_frame = (size_t)g.dw * g.dh * 3;
-    if (out && out_bytes < out_frame) { h->err = "out buffer too small"; return MC_ERR_INVALID; }
-    if (original && original_bytes < orig_frame) { h->err = "original buffer too small"; return MC_ERR_INVALID; }
-    CK(h->c_raw.grow(row * height));
-    CK(h->c_out.grow(out_frame));
-    if (original) CK(h->c_orig.grow(orig_frame));
-    CK(cudaMemcpy2DAsync(h->c_raw.p, row, in->data, in->pitch, row, (size_t)height, cudaMemcpyHostToDevice, h->stream));
-    const mc_yuv422 dev{h->c_raw.p, row, row * height, in->order};
-    uint8_t produced = 0;
-    const mc_status st = chain_impl(h, nullptr, 0, nullptr, &dev, 1, width, height, 3, p, grayscale, h->c_out.p,
-                                    (size_t)g.dw * g.cc, original ? h->c_orig.p : nullptr, (size_t)g.dw * 3, &produced, info);
-    if (st != MC_OK) return st;
-    if (original) CK(cudaMemcpyAsync(original, h->c_orig.p, orig_frame, cudaMemcpyDeviceToHost, h->stream));
-    if (out) CK(cudaMemcpyAsync(out, h->c_out.p, out_frame, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    return MC_OK;
+    return chain_submit(h, nullptr, 0, nullptr, in, width, height, 3, p, grayscale, out, out_step, original, original_step, info);
 } catch (...) { return on_exception(h); }
 
 /* test hooks, not declared in the public header: the two conversion kernels alone on device buffers (default stream,

@@ -409,7 +409,8 @@ class ProcessingChainB200:
     ``run_chain_once(frame, cfg) -> (cur, original)`` returns the *same* frame object wherever the reference
     returns the same FrameRef (identity stages / passthrough); it needs ``lanes == 1``.  ``process_device`` and
     ``process_nv12_device`` / ``process_yuv422_device`` run the chain on device frames of every lane, for one frame or a
-    clip; ``run_chain_once`` of a ``Frame`` whose format is "YUYV" or "UYVY" takes a camera's packed 4:2:2 bytes."""
+    clip; ``submit`` / ``submit_nv12`` / ``submit_yuv422`` pipeline host frames of every lane, and ``collect`` returns them
+    in order; ``run_chain_once`` of a ``Frame`` whose format is "YUYV" or "UYVY" takes a camera's packed 4:2:2 bytes."""
 
     def __init__(self, device: int = 0, lanes: int = 1):
         self.magnifier = MagnificationProcessor(device=device, lanes=lanes)
@@ -457,6 +458,39 @@ class ProcessingChainB200:
                                                        d_out, out_step, d_original or None, original_step,
                                                        flags.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(info)))
         return flags.astype(bool), info
+
+    # -- pipelined host frames of every lane (mc_chain_submit*, collected by collect()) -------------------------------------
+    def submit(self, in_ptr: int, w: int, h: int, c: int, in_step: int, cfg: ProcessorConfig, out_ptr: int, out_step: int,
+               original_ptr: int = 0, original_step: int = 0) -> "capi.McChainInfo":
+        """mc_chain_submit: one BGR or gray host frame of every lane (lane k at k * h * in_step; pinned or pageable) into the
+        chain -> its McChainInfo (magnified 0).  Lane k of the processed frames goes to k * out_h * out_step of out_ptr, of
+        the original tap to k * orig_h * original_step of original_ptr (0: not wanted).  The buffers must stay valid until
+        the frame is collected."""
+        m, p, info = self.magnifier, _to_mc(cfg), capi.McChainInfo()
+        m._check(m._lib.mc_chain_submit(m._h, in_ptr or None, w, h, c, in_step, C.byref(p), int(cfg.grayscale), out_ptr or None,
+                                        out_step, original_ptr or None, original_step, C.byref(info)))
+        return info
+
+    def submit_nv12(self, in_planes: capi.McNv12, w: int, h: int, cfg: ProcessorConfig, out_ptr: int, out_step: int,
+                    original_ptr: int = 0, original_step: int = 0) -> "capi.McChainInfo":
+        """mc_chain_submit_nv12: submit() on NV12 host planes (lane k at k * lane_stride)."""
+        m, p, info = self.magnifier, _to_mc(cfg), capi.McChainInfo()
+        m._check(m._lib.mc_chain_submit_nv12(m._h, C.byref(in_planes), w, h, C.byref(p), int(cfg.grayscale), out_ptr or None,
+                                             out_step, original_ptr or None, original_step, C.byref(info)))
+        return info
+
+    def submit_yuv422(self, in_frame: capi.McYuv422, w: int, h: int, cfg: ProcessorConfig, out_ptr: int, out_step: int,
+                      original_ptr: int = 0, original_step: int = 0) -> "capi.McChainInfo":
+        """mc_chain_submit_yuv422: submit() on packed YUYV / UYVY host frames (lane k at k * lane_stride)."""
+        m, p, info = self.magnifier, _to_mc(cfg), capi.McChainInfo()
+        m._check(m._lib.mc_chain_submit_yuv422(m._h, C.byref(in_frame), w, h, C.byref(p), int(cfg.grayscale), out_ptr or None,
+                                               out_step, original_ptr or None, original_step, C.byref(info)))
+        return info
+
+    def collect(self) -> np.ndarray:
+        """mc_collect of the oldest frame in flight -> bool[lanes]: which lanes magnified it."""
+        self.magnifier.collect()
+        return self.magnifier.lane_produced()
 
     def _run_chain_once_yuv422(self, frame: Frame, cfg: ProcessorConfig):
         """run_chain_once of a camera frame in YUYV / UYVY (image: [h][w][2] or [h][2w] bytes) through mc_chain_process_yuv422:
