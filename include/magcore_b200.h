@@ -125,6 +125,38 @@ mc_status mc_restart_lane(mc_handle* h, int lane);
  * range.  mc_chain_process returns MC_ERR_INVALID while lane 0 is held. */
 mc_status mc_hold_lane(mc_handle* h, int lane, int hold);
 
+/* --- per-lane parameters: each lane of a multi-lane handle with its own magnification parameters -------------------- */
+/* The non-structural fields of mc_params, in the same (algorithm) units. */
+typedef struct mc_lane_params {
+    double amplification, coWavelength, coLow, coHigh, chromAttenuation, framerate;
+} mc_lane_params;
+/* lp != NULL: from the next frame call or submit on, `lane` uses these six fields in place of those of the call's
+ * params; mode, levels and preprocess still come from the call.  lp == NULL: the lane follows the call's params again.
+ * Effective params "differ" when their fields differ bit for bit (+0 / -0 can step the state into different bits).
+ *   Equivalence: lane k's effective params at a frame are the call's mc_params with the six fields replaced by lane k's
+ *     override, if it has one.  Lane k then gives, bit for bit, what a 1-lane handle gives when fed lane k's frames with
+ *     those params, under the restarts and holds it saw: the output bytes, the produced flag, mc_lane_produced and the
+ *     temporal state afterwards.
+ *   Where it applies: every call that runs the magnifier — frame calls, clips (the override is taken at the clip's first
+ *     frame, like restarts and holds), chain, compose, NV12 and YUYV / UYVY calls, and every submit.  For pipelined
+ *     submits the override is taken at submit: frames already in flight keep the params they were submitted with.
+ *   Lifetime: an override is configuration, not temporal state.  It survives mc_reset, structural resets and failed
+ *     frames, as holds and the overlay do, until it is replaced or cleared.
+ *   Laplace: each lane's gains, EMA coefficients and chroma attenuation come from its own params.
+ *   Phase: each lane keeps its own filter design (itsFrequency / itsFramerate), with the framerate fixed when the lane's
+ *     design is made from scratch: when the handle's state is built (every lane's first frame at once, as after
+ *     mc_reset) or when the lane's design was not finite.  A cutoff change on one lane re-designs only that lane's
+ *     filters at its framerate, zeroes only its registers and rebuilds only its `old`; a held lane whose cutoffs change
+ *     drops its state and restarts on release.  A lane restarted alone (mc_restart_lane) keeps its design's framerate:
+ *     after a framerate change its 1-lane twin, restarted with mc_reset, re-designs at the new rate, so the two differ
+ *     from there on; this is the behaviour lanes without an override have always had.  A clip with a NaN cutoff runs as
+ *     frame calls.
+ *   Color: each lane's window cap comes from its own framerate, and its mask and amplification from its own params.  A
+ *     Color handle with lanes > 1 whose lanes' effective params differ needs option "color_lane_lifecycle"; without it
+ *     the frame call returns MC_ERR_UNSUPPORTED and changes nothing.
+ * MC_ERR_INVALID for a NULL handle or a lane out of range. */
+mc_status mc_set_lane_params(mc_handle* h, int lane, const mc_lane_params* lp);
+
 /* Per-lane produced flags (n == lanes) of the frame most recently returned by mc_process / mc_process_device /
  * mc_chain_process, or collected by mc_collect.  The `*produced` of those calls is "at least one lane produced", and
  * a lane's bytes of `out` are written only when its flag is 1.  MC_ERR_INVALID if n != lanes. */

@@ -24,6 +24,12 @@ class McParams(C.Structure):
     ]
 
 
+class McLaneParams(C.Structure):
+    """mc_lane_params: the six non-structural fields of mc_params (mc_set_lane_params)."""
+    _fields_ = [("amplification", C.c_double), ("coWavelength", C.c_double), ("coLow", C.c_double),
+                ("coHigh", C.c_double), ("chromAttenuation", C.c_double), ("framerate", C.c_double)]
+
+
 class McChainInfo(C.Structure):
     _fields_ = [("cur_is_input", C.c_int32), ("out_w", C.c_int32), ("out_h", C.c_int32), ("out_channels", C.c_int32),
                 ("orig_is_input", C.c_int32), ("orig_w", C.c_int32), ("orig_h", C.c_int32), ("orig_channels", C.c_int32),
@@ -89,6 +95,7 @@ SIGNATURES = {
     "mc_restart_lane": (C.c_int, [_vp, C.c_int]),
     "mc_hold_lane": (C.c_int, [_vp, C.c_int, C.c_int]),
     "mc_lane_produced": (C.c_int, [_vp, _u8p, C.c_int]),
+    "mc_set_lane_params": (C.c_int, [_vp, C.c_int, C.POINTER(McLaneParams)]),
     "mc_process": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t, C.POINTER(C.c_int)]),
     "mc_process_device": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t, C.POINTER(C.c_int)]),
     "mc_sync": (C.c_int, [_vp]),

@@ -168,11 +168,12 @@ __global__ void k_select(const float* __restrict__ work, size_t S, int pad, int 
             // i + lane * pad is lane * (lane block + pad) into the frame's slot; frame f's window adds f * tstep
             o = (size_t)slot * S + i + (size_t)lane * pad + (size_t)(lane / lanes) * tstep;
         }
+        const float amp = tab ? tab[lane].amp : alpha;
         const double smin = (double)ord2f(mm[2 * lane]), smax = (double)ord2f(mm[2 * lane + 1]);
         const double scale = (smax - smin > DBL_EPSILON) ? 1.0 / (smax - smin) : 0.0;   // cv::normalize NORM_MINMAX
         const double shift = 0.0 - smin * scale;
         const float v = fmaf(work[o], (float)scale, (float)shift);
-        dst[(size_t)pl * plane + (size_t)y * pitch + x] = v * alpha;
+        dst[(size_t)pl * plane + (size_t)y * pitch + x] = v * amp;
     }
 }
 
@@ -407,14 +408,16 @@ mc_status ColorMode::fft_plan(const ModeCtx& ctx, int n, bool one_lane, FftPlans
 // Append to the rolling window; once full drop the oldest column (SpatialFilter.cpp:63-84).  Then the filter's operands:
 // a lane's signal is physical slots [0, n) (warming: head 0; full: n == mod), so n alone picks its DFT.  A frame call
 // runs this once, a clip once per frame.
-ColorMode::Step ColorMode::step(const mc_params& p, int want_cap, ColorLane* rows) {
-    const double lo = p.coLow == 0.0 ? p.coLow + 0.01 : p.coLow, hi = p.coHigh;   // TemporalFilter.cpp:26-27
+ColorMode::Step ColorMode::step(const mc_params& p0, const mc_params* lp, const std::vector<int>& want_caps, ColorLane* rows) {
     Step s;
     for (int k = 0; k < lanes; ++k) {
+        const mc_params& p = lp ? lp[k] : p0;
+        const double lo = p.coLow == 0.0 ? p.coLow + 0.01 : p.coLow, hi = p.coHigh;   // TemporalFilter.cpp:26-27
+        const int want_cap = want_caps[(size_t)k];
         ColorLane& L = rows[k];
         int& cnt = count[(size_t)k];
         int& hd = head[(size_t)k];
-        L.append = -1; L.n = 0; L.sel = -1; L.sc = 0.f; L.fl = L.fh = 0.0;
+        L.append = -1; L.n = 0; L.sel = -1; L.sc = 0.f; L.fl = L.fh = 0.0; L.amp = (float)p.amplification;
         if (plan.op[(size_t)k] == LANE_HOLD) continue;
         L.append = (hd + cnt) % mod[(size_t)k];
         ++cnt;
@@ -436,8 +439,9 @@ ColorMode::Step ColorMode::step(const mc_params& p, int want_cap, ColorLane* row
         s.n_max = std::max(s.n_max, cnt);
     }
     // Uniform lanes (every lane appends to the same slot and filters the same columns: always so for a handle whose
-    // lanes run in lock-step) take the kernels' scalar path; otherwise the kernels read the table.
-    s.uniform = plan.n_hold == 0;
+    // lanes run in lock-step) take the kernels' scalar path; otherwise the kernels read the table.  Lanes with parameters
+    // of their own (mask range, amplification) always read the table.
+    s.uniform = plan.n_hold == 0 && !lp;
     for (int k = 1; k < lanes && s.uniform; ++k)
         s.uniform = rows[k].append == rows[0].append && rows[k].n == rows[0].n && rows[k].sel == rows[0].sel;
     return s;
@@ -591,7 +595,9 @@ mc_status ColorMode::reconstruct(const ModeCtx& ctx, const FrameIO& io, const mc
 
 mc_status ColorMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int nlevels, int* produced, int frames) {
     *produced = 0;
-    const int want_cap = optimal_buffer_size((int)p.framerate);  // MagnifyCore.hpp:176
+    want_cap.resize((size_t)lanes);
+    for (int k = 0; k < lanes; ++k)   // MagnifyCore.hpp:176, from each lane's own frame rate
+        want_cap[(size_t)k] = optimal_buffer_size((int)(ctx.lane_params ? ctx.lane_params[k] : p).framerate);
     const int C = io.channels;
     const int planes = lanes * C;
     if (!allocated) {
@@ -649,7 +655,7 @@ mc_status ColorMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_par
     for (int k = 0; k < lanes; ++k) {
         ColorLane& L = table[(size_t)k];
         if (plan.op[(size_t)k] == LANE_FIRST) count[(size_t)k] = head[(size_t)k] = 0;   // the lane's window restarts empty
-        const int want_mod = std::max(std::max(want_cap, count[(size_t)k]), 2);
+        const int want_mod = std::max(std::max(want_cap[(size_t)k], count[(size_t)k]), 2);
         L.src_head = 0; L.src_mod = std::max(mod[(size_t)k], 1); L.copy_n = count[(size_t)k];
         if (plan.op[(size_t)k] != LANE_HOLD && want_mod != mod[(size_t)k]) {
             L.src_head = head[(size_t)k];
@@ -679,8 +685,8 @@ mc_status ColorMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_par
     }
     for (int t = 0; t < frames; ++t) {
         for (int k = 0; t > 0 && k < lanes; ++k)
-            assert(plan.op[(size_t)k] == LANE_HOLD || std::max(std::max(want_cap, count[(size_t)k]), 2) == mod[(size_t)k]);
-        (frames > 1 ? clip.steps[(size_t)t] : s1) = step(p, want_cap, rows + (size_t)t * lanes);
+            assert(plan.op[(size_t)k] == LANE_HOLD || std::max(std::max(want_cap[(size_t)k], count[(size_t)k]), 2) == mod[(size_t)k]);
+        (frames > 1 ? clip.steps[(size_t)t] : s1) = step(p, ctx.lane_params, want_cap, rows + (size_t)t * lanes);
     }
     ColorLane* dtab = frames > 1 ? clip.d_table : d_table;
     // pageable source: staged before the call returns; stream-ordered after the previous frame's kernels read the table

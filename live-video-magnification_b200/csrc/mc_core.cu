@@ -150,6 +150,13 @@ struct mc_handle {
     std::vector<uint8_t> has_state, hold, ops;
     std::vector<uint8_t> lane_produced;   // of the frame most recently returned / collected
     uint8_t* d_ops = nullptr;             // device copy of a mixed frame's ops (the mode uploads it on the handle's stream)
+    // Per-lane parameters (mc_set_lane_params): configuration, kept across resets.  lane_eff holds each lane's effective
+    // parameters of the current frame call.
+    std::vector<mc_lane_params> lane_lp;
+    std::vector<uint8_t> lane_lp_set;
+    int n_lane_lp = 0;
+    std::vector<mc_params> lane_eff;
+    std::vector<uint8_t> lane_lost;   // per frame call: lanes whose state the mode dropped
 };
 
 namespace {
@@ -316,6 +323,31 @@ mc_status color_lane_check(mc_handle* h, const mc_params* p, int levels, int cha
     return MC_OK;
 }
 
+// Each lane's effective parameters: the call's, with the six fields of the lane's override (mc_set_lane_params).  *q gets
+// lane 0's; returns the `lanes` of them when they differ and null when every lane's are *q.  "Differ" is bitwise: +0 and
+// -0 (or two NaNs) can step the temporal state into different bits, so only identical fields share the scalar path.
+bool same_lane_fields(const mc_params& a, const mc_params& b) {
+    static_assert(offsetof(mc_params, framerate) - offsetof(mc_params, amplification) == 5 * sizeof(double), "six adjacent doubles");
+    return std::memcmp(&a.amplification, &b.amplification, 6 * sizeof(double)) == 0;
+}
+const mc_params* effective_params(mc_handle* h, const mc_params& p, mc_params* q) {
+    *q = p;
+    if (h->n_lane_lp == 0) return nullptr;
+    h->lane_eff.assign((size_t)h->lanes, p);
+    bool same = true;
+    for (size_t l = 0; l < (size_t)h->lanes; ++l) {
+        mc_params& e = h->lane_eff[l];
+        if (h->lane_lp_set[l]) {
+            const mc_lane_params& o = h->lane_lp[l];
+            e.amplification = o.amplification; e.coWavelength = o.coWavelength; e.coLow = o.coLow; e.coHigh = o.coHigh;
+            e.chromAttenuation = o.chromAttenuation; e.framerate = o.framerate;
+        }
+        same = same && same_lane_fields(e, h->lane_eff[0]);
+    }
+    *q = h->lane_eff[0];
+    return same ? nullptr : h->lane_eff.data();
+}
+
 // The body of MagnificationProcessor::process on device-resident frames.
 // lane_produced: `lanes` per-lane flags (written).  frames > 1: a clip of that many consecutive
 // frames of every lane, [t][lane] in the lane stride, with frames * lanes flags.
@@ -342,6 +374,13 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
     const int max_levels = calculate_max_levels(w, hh);  // :32-33
     if (max_levels < 1) return MC_OK;
     const int levels = std::min(std::max((int)p->levels, 1), max_levels);  // :34
+    mc_params q;
+    const mc_params* lane_params = effective_params(h, *p, &q);
+    if (lane_params && p->mode == MC_MODE_COLOR && !h->opt.color_lane_lifecycle) {
+        h->err = "Color lanes with different parameters (mc_set_lane_params) need option color_lane_lifecycle";
+        return MC_ERR_UNSUPPORTED;
+    }
+    p = &q;
     if (p->mode == MC_MODE_COLOR) {
         // A held 1-lane handle skips the call: its window stays as it is.
         if (h->lanes == 1 && h->hold[0]) return MC_OK;
@@ -365,12 +404,14 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
     if (h->opt.keep_float_output) CK(h->float_out.grow((size_t)h->lanes * w * hh * channels));
 
     bool held_lost = false;
+    h->lane_lost.assign((size_t)h->lanes, 0);
     Options opt = h->opt;
     if (opt.profile_kernels) opt.lane_groups = 1;   // one launch chain: the events time one kernel at a time
     const ModeCtx ctx{.stream = h->stream, .tables = &h->tables, .launches = &h->launches, .err = &h->err, .opt = opt,
                       .float_out = opt.keep_float_output ? h->float_out.p : nullptr,
                       .prof = opt.profile_kernels ? &h->prof : nullptr,
-                      .lane_ops = h->ops.data(), .d_lane_ops = h->d_ops, .lane_produced = lane_produced, .held_lost = &held_lost};
+                      .lane_ops = h->ops.data(), .d_lane_ops = h->d_ops, .lane_produced = lane_produced, .held_lost = &held_lost,
+                      .lane_params = lane_params, .lane_lost = h->lane_lost.data()};
     mc_status st = MC_OK;
     switch (p->mode) {
         case MC_MODE_LAPLACE: st = h->motion.process(ctx, io, *p, levels, produced, frames); break;
@@ -389,7 +430,7 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
     }
     for (int l = 0; l < h->lanes; ++l) {
         if (h->ops[(size_t)l] != LANE_HOLD) h->has_state[(size_t)l] = 1;
-        else if (held_lost) h->has_state[(size_t)l] = 0;
+        else if (held_lost || h->lane_lost[(size_t)l]) h->has_state[(size_t)l] = 0;
     }
     return st;
 }
@@ -593,6 +634,8 @@ mc_status mc_create_lanes(int device, int lanes, mc_handle** out) try {
     h->hold.assign((size_t)lanes, 0);
     h->ops.assign((size_t)lanes, 0);
     h->lane_produced.assign((size_t)lanes, 0);
+    h->lane_lp.assign((size_t)lanes, mc_lane_params{});
+    h->lane_lp_set.assign((size_t)lanes, 0);
     if ((e = cudaMalloc((void**)&h->d_ops, (size_t)lanes)) != cudaSuccess) return fail("cudaMalloc lane ops", e);
     *out = h;
     return MC_OK;
@@ -642,6 +685,15 @@ mc_status mc_hold_lane(mc_handle* h, int lane, int hold) try {
     if (!h) return MC_ERR_INVALID;
     if (lane < 0 || lane >= h->lanes) { h->err = "lane out of range"; return MC_ERR_INVALID; }
     h->hold[(size_t)lane] = hold != 0;
+    return MC_OK;
+} catch (...) { return on_exception(h); }
+
+mc_status mc_set_lane_params(mc_handle* h, int lane, const mc_lane_params* lp) try {
+    if (!h) return MC_ERR_INVALID;
+    if (lane < 0 || lane >= h->lanes) { h->err = "lane out of range"; return MC_ERR_INVALID; }
+    h->n_lane_lp += (lp != nullptr) - (h->lane_lp_set[(size_t)lane] != 0);
+    h->lane_lp_set[(size_t)lane] = lp != nullptr;
+    if (lp) h->lane_lp[(size_t)lane] = *lp;   // taken into the next frame call; frames in flight are not affected
     return MC_OK;
 } catch (...) { return on_exception(h); }
 

@@ -112,6 +112,10 @@ struct LevelArgs {
     const void* tmap = nullptr;   // CUtensorMap of the f32 input planes (TMA-staged tile) or null
     const void* tmap_hi = nullptr, *tmap_lo = nullptr;   // CUtensorMaps of the state planes: prefetch their tiles too
     const uint8_t* ops = nullptr;   // device LaneOp per lane (plane / channels) or null: HOLD skips, FIRST acts as `first`
+    // lanes whose parameters differ (mc_set_lane_params): per lane (plane / channels) {c_hi, 1 - c_hi, c_lo, 1 - c_lo} and
+    // the gain, in place of the four coefficients and `gain` above; null: every lane uses those
+    const double* lane_ema = nullptr;
+    const float* lane_gain = nullptr;
 };
 // 128-byte opaque CUtensorMap storage + encoder for the level kernel's (72 x 39 x 1) box
 struct alignas(64) TensorMapStorage { unsigned char bytes[128]; };
@@ -136,6 +140,7 @@ struct BandSrc {
     const float* a = nullptr;
     const float* b = nullptr;
     float gain = 1.0f;
+    const float* lane_gain = nullptr;   // with b: the gain of each lane (mc_set_lane_params), in place of `gain`; or null
 };
 
 // out_l = pyrUp(coarse) + fine (SpatialFilter.cpp:52-61); `out` may be the stored fine plane itself (in place)
@@ -149,10 +154,11 @@ cudaError_t launch_collapse(const Level& lf, const Level& lc, const BandSrc& fin
 // io.ops: HOLD lanes are skipped, and with first_only also RUN lanes (analysis_only: only FIRST lanes are converted).
 // luma_only (strip kernel, C == 3): only the L planes of m1 and c2 are read, a and b are the input's (a zero chroma
 // factor; the caller guarantees that the a / b motion it skips is finite).
+// lane_chroma (mc_set_lane_params): lane v's chroma is lane_chroma[v % chroma_lanes] in place of `chroma`; or null.
 cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16_t* lab, int pitch16, size_t plane16,
                           const BandSrc& m1, const Level& l1, const BandSrc& c2, const Level& l2, float chroma,
                           float* float_out_or_null, cudaStream_t s, bool strip = true, bool first_only = false,
-                          bool luma_only = false);
+                          bool luma_only = false, const float* lane_chroma = nullptr, int chroma_lanes = 1);
 
 // PreprocessProcessor + GrayscaleProcessor on the device (mc_preprocess.cu): one launch over `vlanes` virtual lanes.
 // FRONT_YUYV + mc_yuv422_order is the packed 4:2:2 source of that byte order.

@@ -152,7 +152,17 @@ struct LevelKArgs {
     int m_luma;               // store m for channel 0 only
     int in_vec_ok;            // u8 rows are 4-byte aligned
     const uint8_t* ops;       // LaneOp per lane or null
+    const double* lane_ema;   // per lane {c_hi, omc_hi, c_lo, omc_lo} (mc_set_lane_params) or null: the four above
+    const float* lane_gain;   // per lane gain, with lane_ema
 };
+
+// The temporal filter's coefficients of one lane: the launch's, or the lane's row of the per-lane table
+struct Ema { double c_hi, omc_hi, c_lo, omc_lo; float gain; };
+__device__ __forceinline__ Ema lane_ema(const LevelKArgs& a, int lane) {
+    if (!a.lane_ema) return Ema{a.c_hi, a.omc_hi, a.c_lo, a.omc_lo, a.gain};
+    const double* e = a.lane_ema + 4 * (size_t)lane;
+    return Ema{__ldg(e), __ldg(e + 1), __ldg(e + 2), __ldg(e + 3), __ldg(a.lane_gain + lane)};
+}
 
 // ---- the level kernels' stencil stages, shared by k_level (one frame) and k_level_clip (a clip of frames) ----------
 
@@ -263,7 +273,7 @@ __device__ __forceinline__ void level_up(const float (*sD)[DP], int tx, int ty, 
 // The band of fine row 2ty+ry at the thread's 4 pixels and the temporal filter on it: a lane's first frame sets
 // hi = lo = band and m = gain * (band - band) = +-0 (MagnifyCore.hpp:98-103); otherwise both EMAs step
 // (TemporalFilter.cpp:9-22) and m = gain * (hi - lo).
-__device__ __forceinline__ void level_filter(const LevelKArgs& a, const float (*sG)[GW], const float (&up)[2][4], int tx, int ty,
+__device__ __forceinline__ void level_filter(const Ema& a, const float (*sG)[GW], const float (&up)[2][4], int tx, int ty,
                                              int ry, bool first, float (&h)[4], float (&l)[4], float (&m)[4]) {
     const float4 gv = *reinterpret_cast<const float4*>(&sG[2 * ty + ry + 4][4 * tx + 4]);
     const float band[4] = {gv.x - up[ry][0], gv.y - up[ry][1], gv.z - up[ry][2], gv.w - up[ry][3]};
@@ -300,6 +310,7 @@ __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_
     if (op == LANE_HOLD) return;                     // held lane: state and G_{l+1} are left as they are
     const bool first = a.first || op == LANE_FIRST;  // this lane's first frame: hi = lo = band
     const bool prefetch = USE_TMA && a.band && !first;
+    const Ema ema = lane_ema(a, plane / a.channels);
     const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH;
     const int wf = a.lf.w, hf = a.lf.h, wc = a.lc.w, hc = a.lc.h;
     const bool interior = x0 >= 4 && x0 + TW + 4 <= wf && y0 >= 4 && y0 + TH + 3 <= hf && (KIND != IN_U8 || a.in_vec_ok);
@@ -352,7 +363,7 @@ __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_
         float nh[4], nl[4], mm[4];
         if (first) {
             // a lane's first frame among running lanes: its stored amplified band is gain * (hi - lo) = +-0
-            level_filter(a, sG, up, tx, ty, ry, true, nh, nl, mm);
+            level_filter(ema, sG, up, tx, ty, ry, true, nh, nl, mm);
         } else {
             float4 h4, l4;
             if (prefetch) {
@@ -364,7 +375,7 @@ __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_
             }
             nh[0] = h4.x; nh[1] = h4.y; nh[2] = h4.z; nh[3] = h4.w;
             nl[0] = l4.x; nl[1] = l4.y; nl[2] = l4.z; nl[3] = l4.w;
-            level_filter(a, sG, up, tx, ty, ry, false, nh, nl, mm);
+            level_filter(ema, sG, up, tx, ty, ry, false, nh, nl, mm);
         }
         *reinterpret_cast<float4*>(hi + o) = make_float4(nh[0], nh[1], nh[2], nh[3]);
         *reinterpret_cast<float4*>(lo + o) = make_float4(nl[0], nl[1], nl[2], nl[3]);
@@ -379,7 +390,7 @@ __global__ void __launch_bounds__(256) k_level(const LevelKArgs a, const __grid_
 // input window of virtual plane t * frame_planes + plane and writes G_{l+1}(t) and the amplified band M_l(t) of that
 // virtual plane.  With USE_TMA the window of frame t+1 is requested into the second buffer while frame t is computed.
 // ------------------------------------------------------------------------------------------------
-template <int KIND, bool USE_TMA>
+template <int KIND, bool USE_TMA, bool LANE_EMA>
 __global__ void __launch_bounds__(256) k_level_clip(const LevelKArgs a, const int frames, const int frame_planes,
                                                     const __grid_constant__ CUtensorMap tmap) {
     __shared__ __align__(128) float sG0[GH][GW];
@@ -391,6 +402,9 @@ __global__ void __launch_bounds__(256) k_level_clip(const LevelKArgs a, const in
     const int op = lane_op(a.ops, plane / a.channels);
     if (op == LANE_HOLD) return;                     // held lane: skipped for the whole clip
     const bool first = a.first || op == LANE_FIRST;  // the lane's first frame is the clip's first frame
+    // a lane's coefficients stay in registers for the whole clip: lanes with their own (LANE_EMA) take a separate
+    // instance, so that the common case keeps reading them from the parameter bank (48 instead of 64 registers)
+    const Ema ema = LANE_EMA ? lane_ema(a, plane / a.channels) : Ema{a.c_hi, a.omc_hi, a.c_lo, a.omc_lo, a.gain};
     const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH;
     const int wf = a.lf.w, hf = a.lf.h, wc = a.lc.w, hc = a.lc.h;
     const bool interior = x0 >= 4 && x0 + TW + 4 <= wf && y0 >= 4 && y0 + TH + 3 <= hf && (KIND != IN_U8 || a.in_vec_ok);
@@ -452,7 +466,7 @@ __global__ void __launch_bounds__(256) k_level_clip(const LevelKArgs a, const in
             const int gy = y0 + 2 * ty + ry;
             if (gy >= hf || gx >= wf) continue;
             float mm[4];
-            level_filter(a, sG, up, tx, ty, ry, first && t == 0, sh[ry], sl[ry], mm);
+            level_filter(ema, sG, up, tx, ty, ry, first && t == 0, sh[ry], sl[ry], mm);
             if (m) *reinterpret_cast<float4*>(m + (size_t)gy * a.lf.pitch + gx) = make_float4(mm[0], mm[1], mm[2], mm[3]);
         }
         // sG, sH and sD are refilled by the next frame; a border tile's generic writes to sG precede a later TMA write
@@ -762,9 +776,12 @@ __global__ void __launch_bounds__(32) k_ingest_lab(const IngestArgs a) {
 // thread block 4 x 2 (same register pyrUp as the level kernel), 128-bit accesses.  Grid z runs over every
 // plane_stride-th plane: 1 for every plane, `channels` for the L planes only (L-only synthesis).
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float band_at(const BandSrc& b, size_t off) {
+// the gain of lane `lane`'s band (used with b.b only)
+__device__ __forceinline__ float band_gain(const BandSrc& b, int lane) { return b.lane_gain ? __ldg(b.lane_gain + lane) : b.gain; }
+
+__device__ __forceinline__ float band_at(const BandSrc& b, size_t off, float gain) {
     const float v = __ldg(b.a + off);
-    return b.b ? band_of(v, __ldg(b.b + off), b.gain) : v;
+    return b.b ? band_of(v, __ldg(b.b + off), gain) : v;
 }
 
 __global__ void __launch_bounds__(256) k_collapse(Level lf, Level lc, BandSrc fine, BandSrc coarse, float* out,
@@ -774,10 +791,11 @@ __global__ void __launch_bounds__(256) k_collapse(Level lf, Level lc, BandSrc fi
     if (lane_op(ops, plane / channels) == LANE_HOLD) return;
     const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH;
     const size_t cbase = (size_t)plane * lc.plane;
+    const float g_fine = band_gain(fine, plane / channels), g_coarse = band_gain(coarse, plane / channels);
     for (int i = threadIdx.x; i < DH * DW; i += 256) {
         const int k = i / DW, j = i - k * DW;
         const int iy = upsrc(y0 / 2 - 1 + k, lc.h), ix = upsrc(x0 / 2 - 1 + j, lc.w);
-        sD[k][j] = band_at(coarse, cbase + (size_t)iy * lc.pitch + ix);
+        sD[k][j] = band_at(coarse, cbase + (size_t)iy * lc.pitch + ix, g_coarse);
     }
     __syncthreads();
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
@@ -802,7 +820,7 @@ __global__ void __launch_bounds__(256) k_collapse(Level lf, Level lc, BandSrc fi
         float4 v = *reinterpret_cast<const float4*>(fine.a + o);   // plain load: `out` may be this very plane
         if (fine.b) {
             const float4 u = __ldg(reinterpret_cast<const float4*>(fine.b + o));
-            v.x = band_of(v.x, u.x, fine.gain); v.y = band_of(v.y, u.y, fine.gain); v.z = band_of(v.z, u.z, fine.gain); v.w = band_of(v.w, u.w, fine.gain);
+            v.x = band_of(v.x, u.x, g_fine); v.y = band_of(v.y, u.y, g_fine); v.z = band_of(v.z, u.z, g_fine); v.w = band_of(v.w, u.w, g_fine);
         }
         if (ry == 0) {
             v.x = __fmaf_rn(up3(e[0][0], e[1][0], e[2][0]), kInv64, v.x);   // * 2^-6 is exact: one rounding, in the add
@@ -836,10 +854,16 @@ struct EgressArgs {
     BandSrc m1; Level l1;           // band 1 = gain_1 * (hi_1 - lo_1) rebuilt from the state planes; a == null: no motion
     BandSrc c2; Level l2;           // collapsed level 2 (or band 2 from state when it is the top band); a == null: cur_1 = m_1
     float chroma;
+    const float* lane_chroma;       // lane v's chroma is lane_chroma[v % chroma_lanes] (mc_set_lane_params); or null: chroma
+    int chroma_lanes;
     float* fout;
     const uint8_t* ops;             // LaneOp per lane or null: HOLD lanes are skipped
     int first_only;                 // skip RUN lanes too (analysis_only frames convert only the lanes' first frames)
 };
+
+__device__ __forceinline__ float egress_chroma64(const EgressArgs& a, int lane) {
+    return (a.lane_chroma ? __ldg(a.lane_chroma + lane % a.chroma_lanes) : a.chroma) * kInv64;
+}
 
 __device__ __forceinline__ bool egress_skips(const EgressArgs& a, int lane) {
     const int op = lane_op(a.ops, lane);
@@ -932,12 +956,12 @@ __device__ __forceinline__ void lab_to_bgr_egress(float L, float a, float b, con
 // `up` holds the pyrUp tap sums BEFORE their 1/64 scale: the scale is exact, so it is folded into the add (L) and
 // into the chroma factor (a, b) without changing a bit.  q / f: the row's output pointers at column gx (f may be null).
 template <int C>
-__device__ __forceinline__ void egress_convert(const EgressArgs& a, uint8_t* q, float* f, int gx, const EgressIn<C>& in, const float (&up)[C][4]);
+__device__ __forceinline__ void egress_convert(const EgressArgs& a, int lane, uint8_t* q, float* f, int gx, const EgressIn<C>& in, const float (&up)[C][4]);
 template <>
-__device__ __forceinline__ void egress_convert<3>(const EgressArgs& a, uint8_t* q, float* f, int gx, const EgressIn<3>& in, const float (&up)[3][4]) {
+__device__ __forceinline__ void egress_convert<3>(const EgressArgs& a, int lane, uint8_t* q, float* f, int gx, const EgressIn<3>& in, const float (&up)[3][4]) {
     uint8_t o8[12];
     float of[12];
-    const float chroma64 = a.chroma * kInv64;
+    const float chroma64 = egress_chroma64(a, lane);
     const short vL[4] = {in.L.x, in.L.y, in.L.z, in.L.w}, vA[4] = {in.A.x, in.A.y, in.A.z, in.A.w}, vB[4] = {in.B.x, in.B.y, in.B.z, in.B.w};
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -967,7 +991,7 @@ __device__ __forceinline__ void egress_convert<3>(const EgressArgs& a, uint8_t* 
     }
 }
 template <>
-__device__ __forceinline__ void egress_convert<1>(const EgressArgs& a, uint8_t* q, float* f, int gx, const EgressIn<1>& in, const float (&up)[1][4]) {
+__device__ __forceinline__ void egress_convert<1>(const EgressArgs& a, int, uint8_t* q, float* f, int gx, const EgressIn<1>& in, const float (&up)[1][4]) {
     uint8_t o8[4];
     float of[4];
 #pragma unroll
@@ -996,7 +1020,7 @@ __device__ __forceinline__ void egress_pixels(const EgressArgs& a, int lane, int
     const EgressIn<C> in = egress_load<C>(a, lane, gy, gx);
     uint8_t* q = a.out + (size_t)lane * a.out_lane_stride + (size_t)gy * a.out_step + (size_t)gx * C;
     float* f = a.fout ? a.fout + (((size_t)lane * a.h0 + gy) * a.w0 + gx) * C : nullptr;
-    egress_convert<C>(a, q, f, gx, in, up);
+    egress_convert<C>(a, lane, q, f, gx, in, up);
 }
 
 template <int C>
@@ -1017,6 +1041,7 @@ __global__ void __launch_bounds__(256) k_egress(const EgressArgs a) {
         // the instructions.  Window index of level-2 pixel i is i - (x0/4 - 2); pyrUp's border rule is applied
         // when the level-2 window is loaded (entries hold s[upsrc(i)]).
         const bool has2 = a.c2.a != nullptr;
+        const float g2 = band_gain(a.c2, lane);
         const int bx2 = x0 / 4 - 2, by2 = y0 / 4 - 2;
         if (has2) {
             {
@@ -1025,7 +1050,7 @@ __global__ void __launch_bounds__(256) k_egress(const EgressArgs a) {
                     const int k = i / E2W, j = i - k * E2W;
                     const int o2 = upsrc(by2 + k, a.l2.h) * a.l2.pitch + upsrc(bx2 + j, a.l2.w);
 #pragma unroll
-                    for (int ch = 0; ch < C; ++ch) sC2[ch][k][j] = band_at(a.c2, base2 + (size_t)ch * a.l2.plane + o2);
+                    for (int ch = 0; ch < C; ++ch) sC2[ch][k][j] = band_at(a.c2, base2 + (size_t)ch * a.l2.plane + o2, g2);
                 }
                 __syncthreads();
             }
@@ -1050,7 +1075,7 @@ __global__ void __launch_bounds__(256) k_egress(const EgressArgs a) {
             ph[ch] = a.m1.a + (size_t)(lane * C + ch) * a.l1.plane;
             pl[ch] = a.m1.b ? a.m1.b + (size_t)(lane * C + ch) * a.l1.plane : nullptr;
         }
-        const float g1 = a.m1.gain;
+        const float g1 = band_gain(a.m1, lane);
         const bool from_state = a.m1.b != nullptr;
         for (int i = threadIdx.x; i < DH * DW; i += 256) {
             const int k = i / DW, j = i - k * DW;
@@ -1258,7 +1283,7 @@ __global__ void __launch_bounds__(32, C == 3 ? 16 : 24) k_egress_strip(const Egr
     const int w1 = a.l1.w, h1 = a.l1.h, w2 = a.l2.w, h2 = a.l2.h;
     const int x1a = gx >> 1, x2 = gx >> 2;                           // lane 0 of strip 0: -2, -1
     const bool has2 = a.c2.a != nullptr, from_state = a.m1.b != nullptr, st2 = a.c2.b != nullptr;
-    const float g1 = a.m1.gain, g2 = a.c2.gain;
+    const float g1 = band_gain(a.m1, lane), g2 = band_gain(a.c2, lane);
     // clamped columns for the loads of lanes outside the level (their values are never used)
     const int x1l = x1a < 0 ? 0 : (x1a >= w1 ? ((w1 - 1) & ~1) : x1a);
     const int x2l = x2 < 0 ? 0 : (x2 >= w2 ? w2 - 1 : x2);
@@ -1411,7 +1436,7 @@ __global__ void __launch_bounds__(32, C == 3 ? 16 : 24) k_egress_strip(const Egr
     const bool words = px_owner && gx + 4 <= a.w0 &&
                        ((reinterpret_cast<uintptr_t>(a.out + (size_t)lane * a.out_lane_stride) | a.out_step) & 3) == 0;
     const bool bytes = px_owner && !words;
-    const float chroma64 = a.chroma * kInv64;
+    const float chroma64 = egress_chroma64(a, lane);
     int sm = slot(j0 - 1), s0 = slot(j0), sp = slot(j0 + 1);           // ring slots of cur_1 rows j-1, j, j+1
     for (int j = j0; j < j_end; ++j) {
         const int jn = j + 1;
@@ -1575,21 +1600,28 @@ static LevelKArgs level_kargs(const LevelArgs& a) {
     k.first = a.first; k.band = a.band;
     k.c_hi = a.c_hi; k.omc_hi = a.one_minus_c_hi; k.c_lo = a.c_lo; k.omc_lo = a.one_minus_c_lo;
     k.gain = a.gain;
+    k.lane_ema = a.lane_ema; k.lane_gain = a.lane_gain;
     k.m_luma = a.m_luma;
     k.ops = a.ops;
     k.in_vec_ok = a.in_kind == IN_U8 ? ((reinterpret_cast<uintptr_t>(a.g) % 4 == 0) && (a.in_row % 4 == 0) && (a.in_plane % 4 == 0)) : 1;
     return k;
 }
 
+template <bool LANE_EMA>
+static void launch_level_clip_as(const LevelKArgs& k, dim3 grid, int in_kind, const CUtensorMap* tg, int frames, int planes, cudaStream_t s) {
+    static const CUtensorMap dummy{};
+    if (in_kind == IN_F32 && tg) k_level_clip<IN_F32, true, LANE_EMA><<<grid, 256, 0, s>>>(k, frames, planes, *tg);
+    else if (in_kind == IN_F32) k_level_clip<IN_F32, false, LANE_EMA><<<grid, 256, 0, s>>>(k, frames, planes, dummy);
+    else if (in_kind == IN_LAB16) k_level_clip<IN_LAB16, false, LANE_EMA><<<grid, 256, 0, s>>>(k, frames, planes, dummy);
+    else k_level_clip<IN_U8, false, LANE_EMA><<<grid, 256, 0, s>>>(k, frames, planes, dummy);
+}
+
 cudaError_t launch_level_clip(const LevelArgs& a, int frames, cudaStream_t s) {
     const LevelKArgs k = level_kargs(a);
     dim3 grid(cdiv(a.lf.w, TW), cdiv(a.lf.h, TH), a.planes);
-    static const CUtensorMap dummy{};
     const CUtensorMap* tg = reinterpret_cast<const CUtensorMap*>(a.tmap);
-    if (a.in_kind == IN_F32 && tg) k_level_clip<IN_F32, true><<<grid, 256, 0, s>>>(k, frames, a.planes, *tg);
-    else if (a.in_kind == IN_F32) k_level_clip<IN_F32, false><<<grid, 256, 0, s>>>(k, frames, a.planes, dummy);
-    else if (a.in_kind == IN_LAB16) k_level_clip<IN_LAB16, false><<<grid, 256, 0, s>>>(k, frames, a.planes, dummy);
-    else k_level_clip<IN_U8, false><<<grid, 256, 0, s>>>(k, frames, a.planes, dummy);
+    if (a.lane_ema) launch_level_clip_as<true>(k, grid, a.in_kind, tg, frames, a.planes, s);
+    else launch_level_clip_as<false>(k, grid, a.in_kind, tg, frames, a.planes, s);
     return cudaGetLastError();
 }
 
@@ -1636,7 +1668,8 @@ static void launch_egress_strip(const EgressArgs& a, dim3 grid, cudaStream_t s) 
 
 cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16_t* lab, int pitch16, size_t plane16,
                           const BandSrc& m1, const Level& l1, const BandSrc& c2, const Level& l2, float chroma,
-                          float* fout, cudaStream_t s, bool strip, bool first_only, bool luma_only) {
+                          float* fout, cudaStream_t s, bool strip, bool first_only, bool luma_only, const float* lane_chroma,
+                          int chroma_lanes) {
     EgressArgs a;
     a.in = io.in; a.in_step = io.in_step; a.in_lane_stride = io.in_lane_stride;
     a.lab = lab; a.pitch16 = pitch16; a.plane16 = plane16;
@@ -1644,6 +1677,7 @@ cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16
     a.w0 = io.w; a.h0 = io.h;
     a.gtab = tb.inv_gamma; a.coeffs = tb.inv_coeffs;
     a.m1 = m1; a.l1 = l1; a.c2 = c2; a.l2 = l2; a.chroma = chroma; a.fout = fout;
+    a.lane_chroma = lane_chroma; a.chroma_lanes = chroma_lanes;
     a.ops = io.ops; a.first_only = first_only ? 1 : 0;
     if (strip) {
         dim3 grid(cdiv(io.w, DS_COLS), cdiv(io.h, EG_ROWS), io.lanes);

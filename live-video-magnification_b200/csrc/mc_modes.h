@@ -57,6 +57,11 @@ struct ModeCtx {
     uint8_t* d_lane_ops = nullptr;       // device, `lanes` bytes
     uint8_t* lane_produced = nullptr;    // host, `lanes` entries, [t][lane] for a clip of t frames (written)
     bool* held_lost = nullptr;           // (written)
+    // Per-lane parameters (mc_set_lane_params): each lane's effective parameters, `lanes` entries, when they are not all
+    // the same; null when every lane runs with the call's (then the mode's `p` already carries them).
+    const mc_params* lane_params = nullptr;
+    uint8_t* lane_lost = nullptr;        // host, `lanes` entries (written): lanes whose state the mode dropped (a held one
+                                         // restarts on release)
 };
 
 // The per-lane ops of one frame as a mode runs it: the handle's ops, with every lane that is not held turned into FIRST
@@ -228,6 +233,15 @@ struct MotionMode {
     int groups_req = 0;                    // Options::lane_groups at allocation time
     std::vector<float> gains;              // per-level gains of the current frame (member: no per-frame allocation)
     LanePlan plan;                         // per-lane ops of the current frame
+    // The per-lane table of a frame whose lanes' parameters differ (ModeCtx::lane_params), on the device: per lane
+    // {c_hi, 1 - c_hi, c_lo, 1 - c_lo}, per lane chroma, per level and lane the gain ([level][lane]).  Null members: every
+    // lane uses the scalars.  coef_host is the device copy's contents.
+    void* d_coef = nullptr;
+    std::vector<uint8_t> coef_host;
+    std::vector<double> coef_key;          // the lanes' six fields the table was built from (levels, w, h are the mode's)
+    bool coef_in01 = true, coef_luma = true;   // the table's lanes' cutoff and L-only conditions
+    const double* lane_ema = nullptr;
+    const float *lane_chroma = nullptr, *lane_gain = nullptr;
 
     // Scratch of the clip path; the temporal state stays in hi / lo above.
     struct Clip : ClipScratch {
@@ -246,7 +260,9 @@ private:
     mc_status allocate(const ModeCtx& ctx, const FrameIO& io, int levels);
     mc_status make_groups(const ModeCtx& ctx);
     void drop_groups();
-    bool luma_only(const ModeCtx& ctx, const mc_params& p) const;
+    bool luma_only(const ModeCtx& ctx) const;
+    mc_status lane_table(const ModeCtx& ctx, bool* cutoffs_in_01, bool* luma_ok);
+    const float* gain_of(int l, int lane0) const { return lane_gain ? lane_gain + (size_t)l * lanes + lane0 : nullptr; }
     mc_status run_group(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, Group& g, bool first, double c_lo, double c_hi,
                         bool luma);
     mc_status run_clip(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int frames, bool first, double c_lo, double c_hi,
@@ -258,9 +274,12 @@ private:
     LevelArgs level_args(int l, const std::vector<float*>& g, size_t p0, const int16_t* lab, const FrameIO& io, bool first,
                          double c_lo, double c_hi) const;
     mc_status copy_residual(const ModeCtx& ctx, const float* g_res, int lane0, int n);
-    mc_status egress_first_frames(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, const int16_t* lab, float* fout, bool first);
+    mc_status egress_first_frames(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int lane0, const int16_t* lab, float* fout,
+                                  bool first);
+    mc_status egress(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int lane0, const int16_t* lab, const BandSrc& m1,
+                     const BandSrc& c2, float* fout, bool first_only, bool luma);
     template <class Band, class Out>
-    mc_status synthesize(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, const int16_t* lab, float* fout, bool motion,
+    mc_status synthesize(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int lane0, const int16_t* lab, float* fout, bool motion,
                          bool luma, Band band, Out out);
 };
 
@@ -272,6 +291,16 @@ struct ColorLane {
     int sel;                         // physical slot of the reconstructed column (logical min(1, n - 1))
     float sc;                        // DFT scale of both transforms, 1 / n^2
     double fl, fh;                   // the CCS mask's packed index range for this n
+    float amp;                       // the lane's amplification (read by k_select when lanes differ)
+};
+
+// A 2nd-order Butterworth section as the Phase kernels read it: numerator b0..b2, denominator a1, a2 (a0 = 1)
+struct Butter { double b0, b1, b2, a1, a2; };
+// One lane's row of the Phase kernels' per-lane table (uploaded when the lanes' designs or amplifications differ)
+struct RieszLane {
+    Butter lo, hi;                   // the lane's two filters
+    float alpha, thresh;             // amplification and its clip (k_riesz_amplify)
+    int rebuild_old;                 // the lane's cutoffs changed this frame: its prior is this frame's pyramid
 };
 
 struct ColorMode {
@@ -303,6 +332,7 @@ struct ColorMode {
     DeviceArena arena;
     LanePlan plan;                   // per-lane ops of the current frame
     int tap_frame = -1;              // the taps' frame in the clip scratch (the last clip's last frame); -1: the frame planes
+    std::vector<int> want_cap;       // per lane: the window cap its frame rate asks for (MagnifyCore.hpp:176)
 
     // What one frame's rows of the lane table ask of the filter
     struct Step {
@@ -334,7 +364,8 @@ private:
     mc_status fft_plan(const ModeCtx& ctx, int n, bool one_lane, FftPlans** out);
     mc_status alloc_clip(const ModeCtx& ctx, int vlanes, size_t work_floats);
     // the append and filter rules of one frame: writes its `lanes` rows of a lane table, moves count / head
-    Step step(const mc_params& p, int want_cap, ColorLane* rows);
+    // (lp: each lane's params, or null when every lane has p's; want_cap: each lane's window cap)
+    Step step(const mc_params& p, const mc_params* lp, const std::vector<int>& want_cap, ColorLane* rows);
     // the launch sets shared by the frame and the clip path, over `vl` (virtual) lanes
     mc_status ingest(const ModeCtx& ctx, const FrameIO& io, int vl, const std::vector<float*>& g);
     mc_status filter(const ModeCtx& ctx, const Step& s, const ColorLane* rows, const ColorLane* d_rows, const float* top, float* win);
@@ -347,8 +378,18 @@ struct RieszMode {
     int lanes = 1;
     bool allocated = false;     // st.cur != null
     int levels = 0, w = 0, h = 0;
-    double lo_freq = 0, hi_freq = 0, framerate = 0;   // itsFrequency / itsFramerate of the two filters
-    double loA[3] = {1, 0, 0}, loB[3] = {0, 0, 0}, hiA[3] = {1, 0, 0}, hiB[3] = {0, 0, 0};
+    // Per lane: itsFrequency / itsFramerate of the two filters and their design.  The framerate is fixed when the lane's
+    // design is made from scratch (the handle's state is built, or the lane's design was not finite), as the reference
+    // fixes it at construction; a cutoff change re-designs at that framerate.
+    struct Design {
+        double lo_freq = 0, hi_freq = 0, framerate = 0;
+        double loA[3] = {1, 0, 0}, loB[3] = {0, 0, 0}, hiA[3] = {1, 0, 0}, hiB[3] = {0, 0, 0};
+        bool finite() const { return !std::isnan(loA[0]) && !std::isnan(hiA[0]); }
+    };
+    std::vector<Design> design;
+    std::vector<RieszLane> rows, rows_dev;   // this frame's per-lane table and the contents of its device copy
+    RieszLane* d_rows = nullptr;
+    std::vector<uint8_t> lane_ops;           // the handle's ops with lanes of a non-finite design turned FIRST
     std::vector<Level> lv;      // octave sizes, 0..levels-1 (band levels 0..levels-2 + low-pass residual)
     DeviceArena arena;
     // per level planes (one plane per lane: only L is processed)
@@ -392,13 +433,15 @@ struct RieszMode {
 
 private:
     mc_status allocate(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels);
-    mc_status apply_cutoffs(const ModeCtx& ctx, const mc_params& p, bool* rebuild_old);
+    mc_status apply_cutoffs(const ModeCtx& ctx, const mc_params& p, std::vector<uint8_t>& rebuild);
+    // the per-lane table of this frame (null when every lane's row is lane 0's: the scalars of row 0), uploaded on change
+    mc_status lane_table(const ModeCtx& ctx, const mc_params& p, const std::vector<uint8_t>& rebuild, const RieszLane** d);
     mc_status frame_loop(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced, int frames);
     mc_status run_clip(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int frames, bool first, int* produced);
     // the kernels shared by the frame and the clip path, over io.lanes lanes with io.ops
     mc_status build_pyramid(const ModeCtx& ctx, const FrameIO& io, int16_t* lab, const std::vector<float*>& octs,
                             const std::vector<float*>& bands, const std::vector<TensorMapStorage>& tm, const std::vector<char>& valid);
-    mc_status amplify(const ModeCtx& ctx, const mc_params& p, int i, int n, const uint8_t* ops, const float* a, const float* tc,
+    mc_status amplify(const ModeCtx& ctx, const RieszLane* tab, int i, int n, const uint8_t* ops, const float* a, const float* tc,
                       const float* ts, const float* low, const float* rx, const float* ry, float* out);
     mc_status collapse_egress(const ModeCtx& ctx, const FrameIO& io, const int16_t* lab, const float* residual,
                               const std::vector<float*>& bands, const std::vector<float*>& out, const std::vector<TensorMapStorage>& tm,

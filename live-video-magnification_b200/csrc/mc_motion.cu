@@ -72,6 +72,10 @@ void MotionMode::reset() {
     clip = Clip{};
     lv.clear(); G.clear(); hi.clear(); lo.clear(); M.clear();
     lab16 = nullptr;
+    d_coef = nullptr;
+    coef_host.clear();
+    coef_key.clear();
+    lane_ema = nullptr; lane_chroma = lane_gain = nullptr;
     lab16_frame = false;
     gauss_frame = false;
     allocated = false;
@@ -113,6 +117,20 @@ mc_status MotionMode::make_groups(const ModeCtx& ctx) {
     }
     if (ng > 1) MCK(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
     return MC_OK;
+}
+
+// TemporalFilter.cpp:11-12
+static void ema_cutoffs(const mc_params& p, double& c_lo, double& c_hi) {
+    c_lo = p.coLow == 0 ? 0.01 : p.coLow;
+    c_hi = p.coHigh;
+}
+static bool cutoffs_in_01(double c_lo, double c_hi) { return c_lo >= 0 && c_lo <= 1 && c_hi >= 0 && c_hi <= 1; }   // NaN is not
+// The parameters' part of the L-only condition (see luma_only): a zero chroma factor and bounded gains
+static bool luma_params(const mc_params& p, const std::vector<float>& g) {
+    if ((float)p.chromAttenuation * (1.0f / 64.0f) != 0.0f) return false;   // the egress's chroma64, as the device forms it
+    for (float v : g)
+        if (!(std::fabs(v) <= 0x1p64f)) return false;
+    return true;
 }
 
 mc_status MotionMode::allocate(const ModeCtx& ctx, const FrameIO& io, int nlevels) {
@@ -178,11 +196,13 @@ mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc
     FrameIO io = io_in;
     MCK(plan.upload(ctx, &io.ops));
     motion_gains(p.amplification, p.coWavelength, levels, w, h, gains);
-    double c_lo = p.coLow, c_hi = p.coHigh;
-    if (c_lo == 0) c_lo = 0.01;  // TemporalFilter.cpp:11-12
-    // a frame of a lane with state steps the EMAs (a clip's later frames always do); NaN is outside [0, 1]
-    if ((plan.n_run > 0 || frames > 1) && !(c_lo >= 0 && c_lo <= 1 && c_hi >= 0 && c_hi <= 1)) ab_bounded = false;
-    const bool luma = luma_only(ctx, p);
+    double c_lo, c_hi;
+    ema_cutoffs(p, c_lo, c_hi);
+    bool in01 = cutoffs_in_01(c_lo, c_hi), luma_ok = luma_params(p, gains);
+    MCK_ST(lane_table(ctx, &in01, &luma_ok));
+    // a frame of a lane with state steps the EMAs (a clip's later frames always do)
+    if ((plan.n_run > 0 || frames > 1) && !in01) ab_bounded = false;
+    const bool luma = luma_ok && luma_only(ctx);
 
     lab16_frame = false;   // a clip converts into its own scratch; a frame call rewrites lab16 below
     gauss_frame = false;   // likewise its pyramid (clip.G)
@@ -210,6 +230,49 @@ mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc
     // state-carry pass (analysis_only): the temporal state is up to date, only first frames are produced; a clip's later
     // frames run for the lanes that are not held
     plan.produced(ctx, !ctx.opt.analysis_only || first, true, produced, frames, !ctx.opt.analysis_only);
+    return MC_OK;
+}
+
+// Lanes with parameters of their own (ctx.lane_params): builds the per-lane table and uploads it on the handle's stream
+// when its contents changed (the kernels of earlier frames precede the copy in stream order).  ANDs every lane's
+// cutoff and L-only conditions into *in01 / *luma_ok, which a shared decision needs to hold for every lane.
+mc_status MotionMode::lane_table(const ModeCtx& ctx, bool* in01, bool* luma_ok) {
+    lane_ema = nullptr; lane_chroma = lane_gain = nullptr;
+    if (!ctx.lane_params) return MC_OK;
+    const size_t n = (size_t)lanes, bytes = n * 4 * sizeof(double) + n * sizeof(float) + (size_t)(levels + 1) * n * sizeof(float);
+    // The table follows from the lanes' six fields alone (levels, w and h are fixed until the next allocation, which
+    // clears the key), so it is rebuilt and uploaded only when they change.
+    bool same = d_coef && coef_key.size() == 6 * n;
+    for (size_t k = 0; same && k < n; ++k) same = std::memcmp(&ctx.lane_params[k].amplification, &coef_key[6 * k], 6 * sizeof(double)) == 0;
+    if (!same) {
+        coef_key.resize(6 * n);
+        coef_host.assign(bytes, 0);
+        double* ema = reinterpret_cast<double*>(coef_host.data());
+        float* chroma = reinterpret_cast<float*>(ema + 4 * n);
+        float* gain = chroma + n;
+        std::vector<float> g;
+        coef_in01 = coef_luma = true;
+        for (size_t k = 0; k < n; ++k) {
+            const mc_params& q = ctx.lane_params[k];
+            std::memcpy(&coef_key[6 * k], &q.amplification, 6 * sizeof(double));
+            double c_lo, c_hi;
+            ema_cutoffs(q, c_lo, c_hi);
+            ema[4 * k] = c_hi; ema[4 * k + 1] = 1 - c_hi; ema[4 * k + 2] = c_lo; ema[4 * k + 3] = 1 - c_lo;
+            chroma[k] = (float)q.chromAttenuation;
+            motion_gains(q.amplification, q.coWavelength, levels, w, h, g);
+            for (int l = 0; l <= levels; ++l) gain[(size_t)l * n + k] = g[(size_t)l];
+            coef_in01 = coef_in01 && cutoffs_in_01(c_lo, c_hi);
+            coef_luma = coef_luma && luma_params(q, g);
+        }
+        if (!d_coef) MCK(arena.alloc_bytes(&d_coef, bytes));
+        // pageable source: staged before the call returns; stream-ordered after the kernels that read the old contents
+        MCK(cudaMemcpyAsync(d_coef, coef_host.data(), bytes, cudaMemcpyHostToDevice, ctx.stream));
+    }
+    *in01 = *in01 && coef_in01;
+    *luma_ok = *luma_ok && coef_luma;
+    lane_ema = static_cast<const double*>(d_coef);
+    lane_chroma = reinterpret_cast<const float*>(lane_ema + 4 * n);
+    lane_gain = lane_chroma + n;
     return MC_OK;
 }
 
@@ -254,6 +317,9 @@ LevelArgs MotionMode::level_args(int l, const std::vector<float*>& g, size_t p0,
     a.band = (l >= 1 || faithful) ? 1 : 0;
     a.c_hi = c_hi; a.one_minus_c_hi = 1 - c_hi; a.c_lo = c_lo; a.one_minus_c_lo = 1 - c_lo;
     a.gain = gains[(size_t)l];
+    const size_t lane0 = p0 / (size_t)channels;
+    a.lane_ema = lane_ema ? lane_ema + 4 * lane0 : nullptr;
+    a.lane_gain = gain_of(l, (int)lane0);
     return a;
 }
 
@@ -272,10 +338,18 @@ mc_status MotionMode::copy_residual(const ModeCtx& ctx, const float* g_res, int 
 
 // analysis_only (state-carry pass): lanes on their first frame are still converted (no motion), running lanes produce
 // nothing.
-mc_status MotionMode::egress_first_frames(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, const int16_t* lab, float* fout, bool first) {
-    if (first || plan.n_first > 0)
-        LAUNCH("egress", 0, launch_egress(io, *ctx.tables, lab, pitch16, plane16, BandSrc{}, lv[levels >= 1 ? 1 : 0], BandSrc{},
-                                          lv[levels >= 2 ? 2 : 0], (float)p.chromAttenuation, fout, ctx.stream, ctx.opt.egress_strip, !first));
+mc_status MotionMode::egress_first_frames(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int lane0, const int16_t* lab, float* fout,
+                                          bool first) {
+    if (first || plan.n_first > 0) MCK_ST(egress(ctx, io, p, lane0, lab, BandSrc{}, BandSrc{}, fout, !first, false));
+    return MC_OK;
+}
+
+// The egress launch over io's lanes, the first of them the handle's lane lane0 (a clip's virtual lane v is lane v % lanes)
+mc_status MotionMode::egress(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int lane0, const int16_t* lab, const BandSrc& m1,
+                             const BandSrc& c2, float* fout, bool first_only, bool luma) {
+    LAUNCH("egress", 0, launch_egress(io, *ctx.tables, lab, pitch16, plane16, m1, lv[levels >= 1 ? 1 : 0], c2, lv[levels >= 2 ? 2 : 0],
+                                      (float)p.chromAttenuation, fout, ctx.stream, ctx.opt.egress_strip, first_only, luma,
+                                      lane_chroma ? lane_chroma + lane0 : nullptr, std::min(io.lanes, lanes)));
     return MC_OK;
 }
 
@@ -283,21 +357,16 @@ mc_status MotionMode::egress_first_frames(const ModeCtx& ctx, const FrameIO& io,
 // zero and u is finite the sum is a, b bit for bit, so only the L planes need to be synthesised.  u is finite when every
 // gain is finite with |g| <= 2^64 and the a / b state is bounded: EMAs with cutoffs in [0, 1] are convex combinations of
 // bands (|band| <= 256), so |m_l| <= 512 * 2^64 and the collapse sums stay far below FLT_MAX.  The strip egress alone has
-// an L-only form; the tile egress always synthesises every channel.
-bool MotionMode::luma_only(const ModeCtx& ctx, const mc_params& p) const {
-    if (channels != 3 || !ctx.opt.egress_strip || !ab_bounded) return false;
-    if ((float)p.chromAttenuation * (1.0f / 64.0f) != 0.0f) return false;   // the egress's chroma64, as the device forms it
-    for (float g : gains)
-        if (!(std::fabs(g) <= 0x1p64f)) return false;
-    return true;
-}
+// an L-only form; the tile egress always synthesises every channel.  The parameters' part (luma_params) is checked by the
+// caller, for every lane.
+bool MotionMode::luma_only(const ModeCtx& ctx) const { return channels == 3 && ctx.opt.egress_strip && ab_bounded; }
 
 // Synthesis: residual and finest band are zero (MagnifyCore.hpp:130-131), so the collapse starts from band levels-1
 // (cur_{levels-1} = 0 + m_{levels-1}) and writes cur_l to out(l) down to level 2; levels 1 and 0 are folded into egress.
 // band(l) is where level l's amplified band is found.  Without motion (first frames) egress converts the input as it is.
 // luma: L-only synthesis, the collapses run over each lane's L plane only.
 template <class Band, class Out>
-mc_status MotionMode::synthesize(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, const int16_t* lab, float* fout, bool motion,
+mc_status MotionMode::synthesize(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int lane0, const int16_t* lab, float* fout, bool motion,
                                  bool luma, Band band, Out out) {
     BandSrc m1, c2;
     if (motion && levels >= 2) {
@@ -309,9 +378,7 @@ mc_status MotionMode::synthesize(const ModeCtx& ctx, const FrameIO& io, const mc
         m1 = band(1);
         if (levels >= 3) c2 = cur(2);
     }
-    LAUNCH("egress", 0, launch_egress(io, *ctx.tables, lab, pitch16, plane16, m1, lv[levels >= 1 ? 1 : 0], c2, lv[levels >= 2 ? 2 : 0],
-                                      (float)p.chromAttenuation, fout, ctx.stream, ctx.opt.egress_strip, false, luma));
-    return MC_OK;
+    return egress(ctx, io, p, lane0, lab, m1, c2, fout, false, luma);
 }
 
 // One group's launch set for one frame: lanes [g.lane0, g.lane0 + g.lanes) on ctx.stream.
@@ -343,11 +410,12 @@ mc_status MotionMode::run_group(const ModeCtx& ctx, const FrameIO& io_all, const
         else LAUNCH("down", l, launch_down(a, ctx.stream));
     }
     MCK_ST(copy_residual(ctx, G[(size_t)levels], g.lane0, g.lanes));
-    if (ctx.opt.analysis_only) return egress_first_frames(ctx, io, p, lab, fout, first);
+    if (ctx.opt.analysis_only) return egress_first_frames(ctx, io, p, g.lane0, lab, fout, first);
     auto band = [&](int l) {
-        return from_state ? BandSrc{off(hi[(size_t)l], l), off(lo[(size_t)l], l), gains[(size_t)l]} : BandSrc{off(M[(size_t)l], l), nullptr, 1.0f};
+        return from_state ? BandSrc{off(hi[(size_t)l], l), off(lo[(size_t)l], l), gains[(size_t)l], gain_of(l, g.lane0)}
+                          : BandSrc{off(M[(size_t)l], l), nullptr, 1.0f};
     };
-    return synthesize(ctx, io, p, lab, fout, !first, luma, band, [&](int l) { return off(M[(size_t)l], l); });
+    return synthesize(ctx, io, p, g.lane0, lab, fout, !first, luma, band, [&](int l) { return off(M[(size_t)l], l); });
 }
 
 // One clip: the launch set of run_group over V = frames * lanes virtual lanes, with the level kernels replaced by
@@ -391,8 +459,8 @@ mc_status MotionMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_
     MCK_ST(copy_residual(ctx, clip.G[(size_t)levels], 0, lanes));   // frame 0 is the first `lanes` virtual lanes
     // state-carry pass: only the clip's first frame can produce; it is frame 0's egress of a frame call, so the float
     // tap is written in place
-    if (ctx.opt.analysis_only) return egress_first_frames(ctx, io0, p, clip.lab16, ctx.float_out, first);
-    MCK_ST(synthesize(ctx, io, p, clip.lab16, ctx.float_out ? clip.fout : nullptr, true, luma,
+    if (ctx.opt.analysis_only) return egress_first_frames(ctx, io0, p, 0, clip.lab16, ctx.float_out, first);
+    MCK_ST(synthesize(ctx, io, p, 0, clip.lab16, ctx.float_out ? clip.fout : nullptr, true, luma,
                       [&](int l) { return BandSrc{clip.M[(size_t)l], nullptr, 1.0f}; }, [&](int l) { return clip.M[(size_t)l]; }));
     return clip.copy_last_tap(ctx, plan, frames, (size_t)w * h * channels);
 }

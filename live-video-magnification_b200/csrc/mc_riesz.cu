@@ -182,8 +182,6 @@ __global__ void __launch_bounds__(256) k_riesz_analysis(Level l, Level ln, const
     }
 }
 
-struct Butter { double b0, b1, b2, a1, a2; };
-
 struct PhaseArgs {
     Level l;
     const float* low;                      // this frame's band (hp)
@@ -195,6 +193,7 @@ struct PhaseArgs {
     Butter lo, hi;
     float* cur_low;                        // == low, written only for held lanes
     const uint8_t* ops;                    // LaneOp per lane or null
+    const RieszLane* lane;                 // per lane: filters and rebuild_old in place of lo / hi / plow == null; or null
 };
 
 __device__ __forceinline__ float muld(float x, double s) { return (float)((double)x * s); }  // cv::multiply(Mat, double)
@@ -255,6 +254,9 @@ __global__ void __launch_bounds__(256) k_riesz_phase(const PhaseArgs a) {
     const Level l = a.l;
     const size_t pb = (size_t)plane * l.plane;
     const int op = lane_op(a.ops, plane);
+    // the lane's filters, and its prior (null: this frame's, after a cutoff change of this lane)
+    const Butter blo = a.lane ? a.lane[plane].lo : a.lo, bhi = a.lane ? a.lane[plane].hi : a.hi;
+    const float* const plow_p = a.lane && a.lane[plane].rebuild_old ? nullptr : a.plow;
     if (op != LANE_RUN) {
         for (int i = threadIdx.x; i < RT_H * RT_W; i += 256) {
             const int gy = y0 + i / RT_W, gx = x0 + i % RT_W;
@@ -262,7 +264,7 @@ __global__ void __launch_bounds__(256) k_riesz_phase(const PhaseArgs a) {
             const size_t o = pb + (size_t)gy * l.pitch + gx;
             if (op == LANE_HOLD) {
                 // the cur <-> old swap after this kernel must hand the held lane its `old` pyramid back unchanged
-                if (a.plow) { a.cur_low[o] = a.plow[o]; a.rx[o] = a.prx[o]; a.ry[o] = a.pry[o]; }
+                if (plow_p) { a.cur_low[o] = plow_p[o]; a.rx[o] = a.prx[o]; a.ry[o] = a.pry[o]; }
             } else {
                 // the lane's first frame (RieszPyramid.cpp:196-213, MagnifyCore.hpp:226-240): `old` becomes this frame's
                 // band with a zero Riesz pair, the phases and both filters' registers start at zero
@@ -290,9 +292,9 @@ __global__ void __launch_bounds__(256) k_riesz_phase(const PhaseArgs a) {
         riesz_pair(s, y, x, tail, rx, ry);
         a.rx[o] = rx;
         a.ry[o] = ry;
-        const float plow = a.plow ? a.plow[o] : low;
-        const float prx = a.plow ? a.prx[o] : rx;
-        const float pry = a.plow ? a.pry[o] : ry;
+        const float plow = plow_p ? plow_p[o] : low;
+        const float prx = plow_p ? a.prx[o] : rx;
+        const float pry = plow_p ? a.pry[o] : ry;
         float pd_c, pd_s, amp;
         phase_difference(low, rx, ry, plow, prx, pry, pd_c, pd_s, amp);
         // temporal band-pass of the accumulated phase (MagnifyCore.hpp:259-264)
@@ -301,16 +303,16 @@ __global__ void __launch_bounds__(256) k_riesz_phase(const PhaseArgs a) {
         a.ph_s[o] = ph_s;
         float r0, r1;
         r0 = a.lo_r0c[o]; r1 = a.lo_r1c[o];
-        const float lo_c = iir_step(ph_c, r0, r1, a.lo);
+        const float lo_c = iir_step(ph_c, r0, r1, blo);
         a.lo_r0c[o] = r0; a.lo_r1c[o] = r1;
         r0 = a.lo_r0s[o]; r1 = a.lo_r1s[o];
-        const float lo_s = iir_step(ph_s, r0, r1, a.lo);
+        const float lo_s = iir_step(ph_s, r0, r1, blo);
         a.lo_r0s[o] = r0; a.lo_r1s[o] = r1;
         r0 = a.hi_r0c[o]; r1 = a.hi_r1c[o];
-        const float hi_c = iir_step(ph_c, r0, r1, a.hi);
+        const float hi_c = iir_step(ph_c, r0, r1, bhi);
         a.hi_r0c[o] = r0; a.hi_r1c[o] = r1;
         r0 = a.hi_r0s[o]; r1 = a.hi_r1s[o];
-        const float hi_s = iir_step(ph_s, r0, r1, a.hi);
+        const float hi_s = iir_step(ph_s, r0, r1, bhi);
         a.hi_r0s[o] = r0; a.hi_r1s[o] = r1;
         a.amp[o] = amp;
         a.t_c[o] = normalize_change(hi_c, lo_c, amp);
@@ -341,9 +343,12 @@ struct PhaseClipArgs {
     int first;                             // every lane's first frame is the clip's first frame
     int rebuild_old;                       // cutoff change: frame 0's prior is frame 0 itself
     const uint8_t* ops;                    // LaneOp per lane at the clip's first frame, or null
+    const RieszLane* lane;                 // per lane: filters and rebuild_old in place of lo / hi / rebuild_old (LANE)
 };
 
-template <bool USE_TMA>
+// LANE: the lanes' filters come from the per-lane table.  The filters stay in registers for the whole clip, so the table
+// reader is an instance of its own and the common case keeps reading them from the parameter bank.
+template <bool USE_TMA, bool LANE>
 __global__ void __launch_bounds__(256) k_riesz_phase_clip(const PhaseClipArgs a, const int frames, const int lanes,
                                                           const __grid_constant__ CUtensorMap tm) {
     __shared__ __align__(128) float s0[RT_SH][RT_SW];
@@ -353,6 +358,8 @@ __global__ void __launch_bounds__(256) k_riesz_phase_clip(const PhaseClipArgs a,
     const int op = lane_op(a.ops, lane);
     if (op == LANE_HOLD) return;                     // held lane: skipped for the whole clip
     const bool first = a.first || op == LANE_FIRST;  // the lane's first frame is the clip's first frame
+    const Butter blo = LANE ? a.lane[lane].lo : a.lo, bhi = LANE ? a.lane[lane].hi : a.hi;
+    const bool rebuild_old = LANE ? a.lane[lane].rebuild_old != 0 : a.rebuild_old != 0;
     const int x0 = blockIdx.x * RT_W, y0 = blockIdx.y * RT_H;
     const Level l = a.l;
     const bool tma = USE_TMA && x0 >= 4 && x0 + RT_W + 4 <= l.w && y0 >= 2 && y0 + RT_H + 2 <= l.h;   // CTA-uniform
@@ -414,15 +421,15 @@ __global__ void __launch_bounds__(256) k_riesz_phase_clip(const PhaseClipArgs a,
             riesz_pair(s, y, x + 2, tail, rx, ry);
             const size_t o = vplane * l.plane + (size_t)gy * l.pitch + gx;
             if (a.rx) { a.rx[o] = rx; a.ry[o] = ry; }
-            if (t == 0 && a.rebuild_old) { plow[j] = low; prx[j] = rx; pry[j] = ry; }
+            if (t == 0 && rebuild_old) { plow[j] = low; prx[j] = rx; pry[j] = ry; }
             float pd_c, pd_s, amp;
             phase_difference(low, rx, ry, plow[j], prx[j], pry[j], pd_c, pd_s, amp);
             pc[j] = addr(pc[j], pd_c);
             ps[j] = addr(ps[j], pd_s);
-            const float lo_c = iir_step(pc[j], lr0c[j], lr1c[j], a.lo);
-            const float lo_s = iir_step(ps[j], lr0s[j], lr1s[j], a.lo);
-            const float hi_c = iir_step(pc[j], hr0c[j], hr1c[j], a.hi);
-            const float hi_s = iir_step(ps[j], hr0s[j], hr1s[j], a.hi);
+            const float lo_c = iir_step(pc[j], lr0c[j], lr1c[j], blo);
+            const float lo_s = iir_step(ps[j], lr0s[j], lr1s[j], blo);
+            const float hi_c = iir_step(pc[j], hr0c[j], hr1c[j], bhi);
+            const float hi_s = iir_step(ps[j], hr0s[j], hr1s[j], bhi);
             if (a.amp) {
                 a.amp[o] = amp;
                 a.t_c[o] = normalize_change(hi_c, lo_c, amp);
@@ -454,6 +461,8 @@ struct AmpArgs {
     Gauss13 g;
     float alpha, thresh;
     const uint8_t* ops;                    // LaneOp per lane or null: only RUN lanes are amplified
+    const RieszLane* lane;                 // (virtual) lane v's alpha / thresh are lane[v % lanes]'s; or null
+    int lanes;
 };
 
 // Tile 64 x 16, thread strip 1 x 4 (same row dealing as the 9x9 kernels is not needed here).  Row pass:
@@ -475,6 +484,7 @@ __global__ void __launch_bounds__(256) k_riesz_amplify(const AmpArgs a) {
     __shared__ __align__(16) float sr[3][GA_H][GA_TW];
     const int plane = blockIdx.z;
     if (lane_op(a.ops, plane) != LANE_RUN) return;
+    const float alpha = a.lane ? a.lane[plane % a.lanes].alpha : a.alpha, thresh = a.lane ? a.lane[plane % a.lanes].thresh : a.thresh;
     const int x0 = blockIdx.x * GA_TW, y0 = blockIdx.y * GA_TH;
     const Level l = a.l;
     const size_t pb = (size_t)plane * l.plane;
@@ -538,8 +548,8 @@ __global__ void __launch_bounds__(256) k_riesz_amplify(const AmpArgs a) {
         // normalize() tail + amplify() (RieszPyramid.cpp:125-143)
         const float tc = __fdiv_rn(b[1][p], b[0][p]), ts = __fdiv_rn(b[2][p], b[0][p]);
         const float mag = __fsqrt_rn(addr(mulr(tc, tc), mulr(ts, ts)));
-        float m2 = mulr(mag, a.alpha);
-        m2 = (m2 > a.thresh) ? a.thresh : m2;                 // THRESH_TRUNC
+        float m2 = mulr(mag, alpha);
+        m2 = (m2 > thresh) ? thresh : m2;                 // THRESH_TRUNC
         float pc, ps;
         sincosf(m2, &ps, &pc);
         float pair = __fdiv_rn(addr(mulr(rxv[p], tc), mulr(ryv[p], ts)), mag);
@@ -679,6 +689,9 @@ void RieszMode::reset() {
     lab16_frame = false;
     clip.arena.release();
     clip = Clip{};
+    design.clear();
+    d_rows = nullptr;
+    rows_dev.clear();
     allocated = false;
 }
 
@@ -717,7 +730,7 @@ mc_status RieszMode::build_pyramid(const ModeCtx& ctx, const FrameIO& io, int16_
 
 // amplify (RieszPyramid.cpp:248-252) of band level i over n lanes: the blurred amplitude a and (hiIIR - loIIR) *
 // amplitude tc / ts shift the phase of the band low and its Riesz pair rx / ry into `out`
-mc_status RieszMode::amplify(const ModeCtx& ctx, const mc_params& p, int i, int n, const uint8_t* ops, const float* a, const float* tc,
+mc_status RieszMode::amplify(const ModeCtx& ctx, const RieszLane* tab, int i, int n, const uint8_t* ops, const float* a, const float* tc,
                              const float* ts, const float* low, const float* rx, const float* ry, float* out) {
     AmpArgs m;
     m.l = lv[(size_t)i];
@@ -725,9 +738,10 @@ mc_status RieszMode::amplify(const ModeCtx& ctx, const mc_params& p, int i, int 
     m.low = low; m.rx = rx; m.ry = ry;
     m.out = out;
     gaussian_kernel_13_3(m.g.k);
-    m.alpha = (float)p.amplification;
-    m.thresh = (float)(p.coWavelength * (3.14159265358979323846 / 100.0));  // PI_PERCENT, :214,:269
+    m.alpha = rows[0].alpha;
+    m.thresh = rows[0].thresh;
     m.ops = ops;
+    m.lane = tab; m.lanes = lanes;
     dim3 grid(cdiv(m.l.w, GA_TW), cdiv(m.l.h, GA_TH), n);
     KLAUNCH("riesz_amplify", i, k_riesz_amplify<<<grid, 256, 0, ctx.stream>>>(m));
     return MC_OK;
@@ -753,27 +767,83 @@ mc_status RieszMode::collapse_egress(const ModeCtx& ctx, const FrameIO& io, cons
     return MC_OK;
 }
 
-// Cutoff changes re-design the filter, zero both filters' registers and rebuild `old` from this frame (:243-254).
-mc_status RieszMode::apply_cutoffs(const ModeCtx& ctx, const mc_params& p, bool* rebuild_old) {
-    auto zero_state = [&]() -> mc_status {
-        *ctx.held_lost = true;   // every lane's registers are zeroed and `old` is rebuilt: a held lane restarts on release
+static const mc_params& lane_params(const ModeCtx& ctx, const mc_params& p, int k) { return ctx.lane_params ? ctx.lane_params[k] : p; }
+
+static RieszMode::Design make_design(const mc_params& q, double framerate) {
+    RieszMode::Design d;
+    d.lo_freq = q.coLow; d.hi_freq = q.coHigh; d.framerate = framerate;
+    design_filter(d.lo_freq, framerate, d.loA, d.loB);
+    design_filter(d.hi_freq, framerate, d.hiA, d.hiB);
+    return d;
+}
+
+// Cutoff changes, lane by lane: a lane whose cutoffs changed re-designs its filter at its framerate, its registers are
+// zeroed and its `old` is rebuilt from this frame (:243-254); rebuild[k] says which.  A held lane among them restarts
+// on release.  The other lanes are untouched.
+mc_status RieszMode::apply_cutoffs(const ModeCtx& ctx, const mc_params& p, std::vector<uint8_t>& rebuild) {
+    rebuild.assign((size_t)lanes, 0);
+    for (int k = 0; k < lanes; ++k) {
+        Design& d = design[(size_t)k];
+        const mc_params& q = lane_params(ctx, p, k);
+        if (d.lo_freq != q.coLow) {
+            d.lo_freq = q.coLow;
+            design_filter(d.lo_freq, d.framerate, d.loA, d.loB);
+            rebuild[(size_t)k] = 1;
+        }
+        if (d.hi_freq != q.coHigh) {
+            d.hi_freq = q.coHigh;
+            design_filter(d.hi_freq, d.framerate, d.hiA, d.hiB);
+            rebuild[(size_t)k] = 1;
+        }
+        if (rebuild[(size_t)k]) ctx.lane_lost[k] = 1;
+    }
+    return for_each_run((size_t)lanes, [&](size_t k) { return rebuild[k] != 0; }, [&](size_t a, size_t b) -> mc_status {
         for (auto* v : {&phase_c, &phase_s, &lo_r0c, &lo_r0s, &lo_r1c, &lo_r1s, &hi_r0c, &hi_r0s, &hi_r1c, &hi_r1s})
             for (int i = 0; i < levels - 1; ++i)
-                MCK(cudaMemsetAsync((*v)[(size_t)i], 0, (size_t)lanes * lv[(size_t)i].plane * sizeof(float), ctx.stream));
+                MCK(cudaMemsetAsync((*v)[(size_t)i] + a * lv[(size_t)i].plane, 0, (b - a) * lv[(size_t)i].plane * sizeof(float), ctx.stream));
         return MC_OK;
+    });
+}
+
+// Rows of the per-lane table: the lane's filters, amplification (PI_PERCENT clip, :214, :269) and rebuild flag.  When
+// every row equals row 0 the kernels take row 0's values as scalars (*d = null); otherwise the table is uploaded on the
+// handle's stream when its contents changed (the kernels of earlier frames precede the copy in stream order).
+mc_status RieszMode::lane_table(const ModeCtx& ctx, const mc_params& p, const std::vector<uint8_t>& rebuild, const RieszLane** d) {
+    auto butter = [](const double* A, const double* B) { return Butter{B[0], B[1], B[2], A[1], A[2]}; };
+    auto same = [](const RieszLane& x, const RieszLane& y) {
+        return std::memcmp(&x.lo, &y.lo, sizeof(Butter)) == 0 && std::memcmp(&x.hi, &y.hi, sizeof(Butter)) == 0 &&
+               std::memcmp(&x.alpha, &y.alpha, sizeof(float)) == 0 && std::memcmp(&x.thresh, &y.thresh, sizeof(float)) == 0 &&
+               x.rebuild_old == y.rebuild_old;
     };
-    if (lo_freq != p.coLow) {
-        lo_freq = p.coLow;
-        design_filter(lo_freq, framerate, loA, loB);
-        MCK_ST(zero_state());
-        *rebuild_old = true;
+    rows.resize((size_t)lanes);
+    bool uniform = true;
+    for (int k = 0; k < lanes; ++k) {
+        const Design& g = design[(size_t)k];
+        const mc_params& q = lane_params(ctx, p, k);
+        RieszLane& r = rows[(size_t)k];
+        r.lo = butter(g.loA, g.loB);
+        r.hi = butter(g.hiA, g.hiB);
+        r.alpha = (float)q.amplification;
+        r.thresh = (float)(q.coWavelength * (3.14159265358979323846 / 100.0));
+        r.rebuild_old = rebuild.empty() ? 0 : rebuild[(size_t)k];
+        uniform = uniform && same(r, rows[0]);
     }
-    if (hi_freq != p.coHigh) {
-        hi_freq = p.coHigh;
-        design_filter(hi_freq, framerate, hiA, hiB);
-        MCK_ST(zero_state());
-        *rebuild_old = true;
+    *d = nullptr;
+    if (uniform) return MC_OK;
+    if (!d_rows) {
+        void* v = nullptr;
+        MCK(arena.alloc_bytes(&v, sizeof(RieszLane) * (size_t)lanes));
+        d_rows = (RieszLane*)v;
+        rows_dev.clear();
     }
+    bool changed = rows_dev.size() != rows.size();
+    for (size_t k = 0; !changed && k < rows.size(); ++k) changed = !same(rows[k], rows_dev[k]);
+    if (changed) {
+        // pageable source: staged before the call returns
+        MCK(cudaMemcpyAsync(d_rows, rows.data(), sizeof(RieszLane) * (size_t)lanes, cudaMemcpyHostToDevice, ctx.stream));
+        rows_dev = rows;
+    }
+    *d = d_rows;
     return MC_OK;
 }
 
@@ -817,9 +887,11 @@ mc_status RieszMode::allocate(const ModeCtx& ctx, const FrameIO& io, const mc_pa
     void* lp = nullptr;
     MCK(arena.alloc_bytes(&lp, (size_t)lanes * 3 * plane16 * sizeof(int16_t)));
     lab16 = (int16_t*)lp;
-    lo_freq = p.coLow; hi_freq = p.coHigh; framerate = p.framerate;
-    design_filter(lo_freq, framerate, loA, loB);
-    design_filter(hi_freq, framerate, hiA, hiB);
+    design.resize((size_t)lanes);
+    for (int k = 0; k < lanes; ++k) {
+        const mc_params& q = lane_params(ctx, p, k);
+        design[(size_t)k] = make_design(q, q.framerate);
+    }
     allocated = true;
     return MC_OK;
 }
@@ -832,18 +904,32 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_
     }
     // Per-lane ops: lanes without state take their first frame while the others run, held lanes are skipped.  When every
     // lane is on its first frame the handle's state is rebuilt from scratch, as for the reference's first frame.
-    const bool fresh = !allocated || std::isnan(loA[0]) || std::isnan(hiA[0]);  // :226
-    plan.make(ctx.lane_ops, lanes, fresh);
+    // A filter design that is not finite makes every frame a first frame (:226): when no lane's design is finite the
+    // handle's state is rebuilt from scratch, as for the reference's first frame; otherwise such a lane (unless held)
+    // takes a first frame with a design made afresh from its parameters, at their framerate.
+    bool any_finite = false;
+    for (const Design& d : design) any_finite = any_finite || d.finite();
+    const bool fresh = !allocated || !any_finite;
+    lane_ops.assign(ctx.lane_ops, ctx.lane_ops + lanes);
+    for (int k = 0; !fresh && k < lanes; ++k)
+        if (lane_ops[(size_t)k] != LANE_HOLD && !design[(size_t)k].finite()) {
+            lane_ops[(size_t)k] = LANE_FIRST;
+            const mc_params& q = lane_params(ctx, p, k);
+            design[(size_t)k] = make_design(q, q.framerate);
+        }
+    plan.make(lane_ops.data(), lanes, fresh);
     if (plan.n_hold == lanes) return MC_OK;   // every lane held: nothing to do
     const bool first = fresh || plan.n_first == lanes;
     if (frames > 1) {
-        // A filter design that is not finite makes every frame a first frame (:226).  Such a clip runs as frame calls;
-        // the design the clip's first frame leaves behind is known here: the parameters' own, at the framerate it uses.
-        double A[3], B[3], C[3], D[3];
-        const double fr = first ? p.framerate : framerate;
-        design_filter(p.coLow, fr, A, B);
-        design_filter(p.coHigh, fr, C, D);
-        if (std::isnan(A[0]) || std::isnan(C[0])) return frame_loop(ctx, io_in, p, nlevels, produced, frames);
+        // Such a clip runs as frame calls; the design the clip's first frame leaves behind is known here: each lane's
+        // parameters', at the framerate it uses.  So does a clip with a NaN cutoff: it never equals the stored one, so
+        // every frame call re-designs the lane's filter and rebuilds its `old`, which the clip kernel does at frame 0 only.
+        for (int k = 0; k < lanes; ++k) {
+            if (plan.op[(size_t)k] == LANE_HOLD) continue;
+            const mc_params& q = lane_params(ctx, p, k);
+            if (std::isnan(q.coLow) || std::isnan(q.coHigh) || !make_design(q, first ? q.framerate : design[(size_t)k].framerate).finite())
+                return frame_loop(ctx, io_in, p, nlevels, produced, frames);
+        }
     }
     if (first) {
         if (allocated) *ctx.held_lost = true;
@@ -861,24 +947,27 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_
         for (int i = 0; i < levels - 1; ++i) std::swap(cur_low[(size_t)i], old_low[(size_t)i]);
         return MC_OK;
     }
-    bool rebuild_old = false;
-    MCK_ST(apply_cutoffs(ctx, p, &rebuild_old));
+    std::vector<uint8_t> rebuild;
+    MCK_ST(apply_cutoffs(ctx, p, rebuild));
+    const RieszLane* tab = nullptr;
+    MCK_ST(lane_table(ctx, p, rebuild, &tab));
     const int nb = levels - 1;
     for (int i = 0; i < nb; ++i) {
         PhaseArgs a;
         a.l = lv[(size_t)i];
         a.low = cur_low[(size_t)i];
-        a.plow = rebuild_old ? nullptr : old_low[(size_t)i];
+        a.plow = !tab && rows[0].rebuild_old ? nullptr : old_low[(size_t)i];
         a.prx = old_rx[(size_t)i]; a.pry = old_ry[(size_t)i];
         a.rx = cur_rx[(size_t)i]; a.ry = cur_ry[(size_t)i];
         a.ph_c = phase_c[(size_t)i]; a.ph_s = phase_s[(size_t)i];
         a.lo_r0c = lo_r0c[(size_t)i]; a.lo_r0s = lo_r0s[(size_t)i]; a.lo_r1c = lo_r1c[(size_t)i]; a.lo_r1s = lo_r1s[(size_t)i];
         a.hi_r0c = hi_r0c[(size_t)i]; a.hi_r0s = hi_r0s[(size_t)i]; a.hi_r1c = hi_r1c[(size_t)i]; a.hi_r1s = hi_r1s[(size_t)i];
         a.amp = amp[(size_t)i]; a.t_c = t_c[(size_t)i]; a.t_s = t_s[(size_t)i];
-        a.lo = Butter{loB[0], loB[1], loB[2], loA[1], loA[2]};
-        a.hi = Butter{hiB[0], hiB[1], hiB[2], hiA[1], hiA[2]};
+        a.lo = rows[0].lo;
+        a.hi = rows[0].hi;
         a.cur_low = cur_low[(size_t)i];
         a.ops = io.ops;
+        a.lane = tab;
         dim3 grid(cdiv(a.l.w, RT_W), cdiv(a.l.h, RT_H), lanes);
         KLAUNCH("riesz_phase", i, k_riesz_phase<<<grid, 256, 0, ctx.stream>>>(a));
     }
@@ -896,7 +985,7 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_
     if (plan.n_run == 0) return MC_OK;   // only first frames (passthrough) and held lanes
     // this frame's band/pair now live in the old_* buffers
     for (int i = nb - 1; i >= 0; --i)
-        MCK_ST(amplify(ctx, p, i, lanes, io.ops, amp[(size_t)i], t_c[(size_t)i], t_s[(size_t)i], old_low[(size_t)i], old_rx[(size_t)i],
+        MCK_ST(amplify(ctx, tab, i, lanes, io.ops, amp[(size_t)i], t_c[(size_t)i], t_s[(size_t)i], old_low[(size_t)i], old_rx[(size_t)i],
                        old_ry[(size_t)i], low_amp[(size_t)i]));
     MCK_ST(collapse_egress(ctx, io, lab16, oct[(size_t)levels - 1], low_amp, res, tm_band, tm_valid, ctx.float_out));
     frame_taps = TAPS_SYNTH;
@@ -956,8 +1045,10 @@ mc_status RieszMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_p
         }
         return MC_OK;
     }));
-    bool rebuild_old = false;
-    if (!first) MCK_ST(apply_cutoffs(ctx, p, &rebuild_old));
+    std::vector<uint8_t> rebuild;
+    if (!first) MCK_ST(apply_cutoffs(ctx, p, rebuild));
+    const RieszLane* tab = nullptr;
+    MCK_ST(lane_table(ctx, p, rebuild, &tab));
     const uint8_t* ops0 = nullptr;   // per-lane ops of the clip's first frame (null when uniform)
     MCK(plan.upload(ctx, &ops0));
     FrameIO io = io0;   // every frame of every lane
@@ -979,20 +1070,22 @@ mc_status RieszMode::run_clip(const ModeCtx& ctx, const FrameIO& io0, const mc_p
         a.ph_c = phase_c[(size_t)i]; a.ph_s = phase_s[(size_t)i];
         a.lo_r0c = lo_r0c[(size_t)i]; a.lo_r0s = lo_r0s[(size_t)i]; a.lo_r1c = lo_r1c[(size_t)i]; a.lo_r1s = lo_r1s[(size_t)i];
         a.hi_r0c = hi_r0c[(size_t)i]; a.hi_r0s = hi_r0s[(size_t)i]; a.hi_r1c = hi_r1c[(size_t)i]; a.hi_r1s = hi_r1s[(size_t)i];
-        a.lo = Butter{loB[0], loB[1], loB[2], loA[1], loA[2]};
-        a.hi = Butter{hiB[0], hiB[1], hiB[2], hiA[1], hiA[2]};
+        a.lo = rows[0].lo;
+        a.hi = rows[0].hi;
         a.first = first ? 1 : 0;
-        a.rebuild_old = rebuild_old ? 1 : 0;
+        a.rebuild_old = rows[0].rebuild_old;
         a.ops = ops0;
+        a.lane = tab;
         dim3 grid(cdiv(a.l.w, RT_W), cdiv(a.l.h, RT_H), lanes);
         const CUtensorMap& tm = *reinterpret_cast<const CUtensorMap*>(&clip.tm_band[(size_t)i]);
-        if (ctx.opt.use_tma && clip.tm_valid[(size_t)i])
-            KLAUNCH("riesz_phase_clip", i, k_riesz_phase_clip<true><<<grid, 256, 0, ctx.stream>>>(a, frames, lanes, tm));
-        else
-            KLAUNCH("riesz_phase_clip", i, k_riesz_phase_clip<false><<<grid, 256, 0, ctx.stream>>>(a, frames, lanes, tm));
+        const bool tma = ctx.opt.use_tma && clip.tm_valid[(size_t)i];
+        if (tma && tab) KLAUNCH("riesz_phase_clip", i, k_riesz_phase_clip<true, true><<<grid, 256, 0, ctx.stream>>>(a, frames, lanes, tm));
+        else if (tma) KLAUNCH("riesz_phase_clip", i, k_riesz_phase_clip<true, false><<<grid, 256, 0, ctx.stream>>>(a, frames, lanes, tm));
+        else if (tab) KLAUNCH("riesz_phase_clip", i, k_riesz_phase_clip<false, true><<<grid, 256, 0, ctx.stream>>>(a, frames, lanes, tm));
+        else KLAUNCH("riesz_phase_clip", i, k_riesz_phase_clip<false, false><<<grid, 256, 0, ctx.stream>>>(a, frames, lanes, tm));
         if (ctx.opt.analysis_only) continue;
         // the amplified band overwrites the Riesz pair's rx, point for point
-        MCK_ST(amplify(ctx, p, i, vl, io.ops, clip.amp, clip.t_c, clip.t_s, clip.band[(size_t)i], clip.rx[(size_t)i], clip.ry[(size_t)i],
+        MCK_ST(amplify(ctx, tab, i, vl, io.ops, clip.amp, clip.t_c, clip.t_s, clip.band[(size_t)i], clip.rx[(size_t)i], clip.ry[(size_t)i],
                        clip.rx[(size_t)i]));
     }
     if (ctx.opt.analysis_only) return MC_OK;   // state-carry pass: nothing is produced

@@ -176,6 +176,17 @@ class MagnificationProcessor(IProcessor):
         (a stream without a new frame this step).  Holds survive reset()."""
         self._check(self._lib.mc_hold_lane(self._h, int(lane), int(bool(hold))))
 
+    def set_lane_params(self, lane: int, params: Optional[MagnificationParams]) -> None:
+        """From the next frame call or submit on, `lane` runs with the six non-structural fields of `params`
+        (amplification, coWavelength, coLow, coHigh, chromAttenuation, framerate) in place of the call's; mode, levels
+        and preprocess still come from the call.  None: the lane follows the call's parameters again.  An override
+        survives reset()."""
+        lp = None
+        if params is not None:
+            lp = C.byref(capi.McLaneParams(float(params.amplification), float(params.coWavelength), float(params.coLow),
+                                           float(params.coHigh), float(params.chromAttenuation), float(params.framerate)))
+        self._check(self._lib.mc_set_lane_params(self._h, int(lane), lp))
+
     def lane_produced(self) -> np.ndarray:
         """-> bool[lanes]: which lanes produced an output in the most recent frame call (or collect())."""
         a = np.zeros(self.lanes, np.uint8)
@@ -419,6 +430,10 @@ class ProcessingChainB200:
     def reset(self) -> None:
         """ProcessingChain's recovery path resets every stage (ProcessingChain.cpp:50-62); only the magnifier has state."""
         self.magnifier.reset()
+
+    def set_lane_params(self, lane: int, params: Optional[MagnificationParams]) -> None:
+        """MagnificationProcessor.set_lane_params of the chain's magnifier."""
+        self.magnifier.set_lane_params(lane, params)
 
     @staticmethod
     def geometry(cfg: ProcessorConfig, w: int, h: int, c: int) -> "capi.McChainInfo":

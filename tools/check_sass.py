@@ -90,16 +90,17 @@ def main():
     tma = [k for k in body if k.startswith("void k_level<0, true>")]
     need(len(tma) == 1 and count(tma[0], "UTMALDG") == 3 and count(tma[0], "SYNCS") >= 2,
          "k_level<f32, TMA>: three cp.async.bulk.tensor copies (UTMALDG: input window + both state tiles) + mbarrier (SYNCS)")
-    clip = [k for k in body if k.startswith("void k_level_clip<0, true>")]
-    need(len(clip) == 1 and count(clip[0], "UTMALDG") >= 1 and count(clip[0], "SYNCS") >= 2,
-         "k_level_clip<f32, TMA>: double-buffered cp.async.bulk.tensor (UTMALDG) + mbarrier (SYNCS)")
+    # one instance for the launch's coefficients and one for per-lane coefficients (mc_set_lane_params)
+    clip = [k for k in body if k.startswith("void k_level_clip<0, true,")]
+    need(len(clip) == 2 and all(count(k, "UTMALDG") >= 1 and count(k, "SYNCS") >= 2 for k in clip),
+         "k_level_clip<f32, TMA, *>: double-buffered cp.async.bulk.tensor (UTMALDG) + mbarrier (SYNCS), 2 instances")
     spills = clip_spills()
     need(bool(spills) and all(s == (0, 0) for s in spills.values()), f"k_level_clip<*>: no local-memory spills (ptxas -v, {len(spills)} instances)")
-    pclip = [k for k in body if k.startswith("void k_riesz_phase_clip<true>")]
-    need(len(pclip) == 1 and count(pclip[0], "UTMALDG") >= 1 and count(pclip[0], "SYNCS") >= 2,
-         "k_riesz_phase_clip<TMA>: double-buffered cp.async.bulk.tensor (UTMALDG) + mbarrier (SYNCS)")
+    pclip = [k for k in body if k.startswith("void k_riesz_phase_clip<true,")]
+    need(len(pclip) == 2 and all(count(k, "UTMALDG") >= 1 and count(k, "SYNCS") >= 2 for k in pclip),
+         "k_riesz_phase_clip<TMA, *>: double-buffered cp.async.bulk.tensor (UTMALDG) + mbarrier (SYNCS), 2 instances")
     pspills = clip_spills("k_riesz_phase_clip", "mc_riesz")
-    need(len(pspills) == 2 and all(s == (0, 0) for s in pspills.values()),
+    need(len(pspills) == 4 and all(s == (0, 0) for s in pspills.values()),
          f"k_riesz_phase_clip<*>: no local-memory spills (ptxas -v, {len(pspills)} instances)")
     r9 = [k for k in body if k.startswith("k_riesz_analysis(") or k.startswith("k_riesz_collapse(")]
     need(len(r9) == 2 and all(count(k, "UTMALDG") == 1 and count(k, "SYNCS") >= 2 for k in r9), "k_riesz_analysis / k_riesz_collapse: 9x9 input tile by one bulk-tensor copy")
