@@ -291,7 +291,8 @@ mc_status mc_collect(mc_handle* h, int* produced);
  *   Errors, returned before any copy or kernel is enqueued, with the handle's state and the frames in flight unchanged:
  *     MC_ERR_INVALID for a full pipeline, slot buffers that would have to grow while frames are in flight ("pipeline
  *     geometry changed"), and every argument error of the matching device chain call (a NULL `out` where the call would
- *     write it included); MC_ERR_UNSUPPORTED for Color's multi-lane refusals.  Clips are not submitted.
+ *     write it included); MC_ERR_UNSUPPORTED for Color's multi-lane refusals.  A chain submit takes one frame
+ *     per lane; clips are submitted through the compose submits (mc_chain_compose_submit, after the 4:2:2 section).
  * mc_chain_submit_nv12 and mc_chain_submit_yuv422 follow the NV12 and 4:2:2 sections below. */
 mc_status mc_chain_submit(mc_handle* h, const uint8_t* in, int width, int height, int channels, size_t in_step,
                           const mc_params* p, int grayscale, uint8_t* out, size_t out_step, uint8_t* original,
@@ -479,6 +480,51 @@ mc_status mc_chain_process_yuv422(mc_handle* h, const mc_yuv422* in, int width, 
  * and both frames come back, as every chain call on a 4:2:2 source writes them. */
 mc_status mc_chain_submit_yuv422(mc_handle* h, const mc_yuv422* in, int width, int height, const mc_params* p, int grayscale,
                                  uint8_t* out, size_t out_step, uint8_t* original, size_t original_step, mc_chain_info* info);
+
+/* --- the export canvas from host clips, pipelined (an exporter that decodes to host memory) ---------------------------
+ * mc_chain_compose_device / _nv12_device / _yuv422_device on host memory, submitted and collected as mc_submit is: one
+ * call submits a clip of `frames` consecutive frames of every lane, and mc_collect collects it, in strict FIFO order with
+ * mc_submit, mc_submit_nv12, the chain submits and the other compose submits on the handle.  An exporter submits T decoded
+ * frames and collects T finished canvases in file order, with the uploads, kernels and downloads of up to
+ * mc_pipeline_depth() clips overlapped.
+ *   Memory: `in` and `canvas` have the layout of the matching device compose call, on host memory: virtual lane
+ *     v = t * lanes + k has its input at v * height * in_step (NV12 and 4:2:2 frames: at v * lane_stride) and its canvas
+ *     (BGR, or both NV12 planes) at v * canvas->lane_stride.  Each buffer may be pinned or pageable, independently of the
+ *     others.  All of them must stay valid until the submit is collected, and `in` must also stay unchanged until then.
+ *   Equivalence: for any sequence of compose submits, with restarts, holds, mc_set_lane_params, mc_set_overlay, parameter,
+ *     ROI or levels changes between them and mixed with the other submits, every byte of every canvas, the produced
+ *     flags, mc_lane_produced and the temporal state after each collect equal, bit for bit, those of the matching device
+ *     compose call on the same frames uploaded by the caller.  Lifecycle, lane parameters and the overlay are taken at
+ *     submit (for a clip, at its first frame, as in the device clip calls); frames in flight keep what they were
+ *     submitted with.
+ *   What is written: that of the device compose call.  The canvas of every virtual lane that is not held is downloaded;
+ *     held lanes, row padding and the canvases of a 0 x 0 geometry are left untouched.
+ *   produced: frames * lanes host bytes, [t][lane], written by the mc_collect that collects the submit, and valid until
+ *     then.  *produced of that mc_collect is "at least one virtual lane produced"; mc_lane_produced then reports the
+ *     flags of the clip's last frame (a submit does not change it before it is collected).
+ *   info: filled by the submit, final when it returns, with magnified 0 (the collected flags carry that fact).
+ *   Errors, returned before any copy or kernel is enqueued, with the handle's state and the frames in flight unchanged:
+ *     MC_ERR_INVALID for every argument error of the matching device compose call (overlay geometry included): frames <
+ *     1, frames * lanes > MC_MAX_LANES and a NULL produced among them; for a full pipeline; and for slot buffers that
+ *     would have to grow while frames are in flight ("pipeline geometry changed").  MC_ERR_UNSUPPORTED for Color's
+ *     multi-lane refusals.  The device clip calls keep refusing while submitted frames are in flight.
+ *   Memory per pipeline slot (mc_pipeline_depth() slots, each grown, never shrunk, only while nothing is in flight):
+ *     device memory for the clip's input (frames * lanes * its bytes per frame: width * height * channels, NV12 1.5 and
+ *     4:2:2 2 bytes per pixel) and for the canvases of this frame size and split without a crop or downscale (frames *
+ *     lanes * cw * ch * 3 bytes for BGR, * 1.5 for NV12 canvases), so that a ROI or downscale change and an export's
+ *     last, shorter clip fit in the slots that are there.  At T = 16, 1080p BGR in and a left/right BGR canvas that is
+ *     about 100 MB in plus 200 MB out per slot.  Pinned host staging for a submit's input or canvas bytes is allocated
+ *     (per slot, grow-only) only when that buffer is pageable; pinned buffers are copied straight to and from device
+ *     memory, and pageable ones cost two host copies of every byte on the calling thread. */
+mc_status mc_chain_compose_submit(mc_handle* h, const uint8_t* in, int frames, int width, int height, int channels,
+                                  size_t in_step, const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                                  uint8_t* produced, mc_chain_info* info);
+mc_status mc_chain_compose_submit_nv12(mc_handle* h, const mc_nv12* in, int frames, int width, int height,
+                                       const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                                       uint8_t* produced, mc_chain_info* info);
+mc_status mc_chain_compose_submit_yuv422(mc_handle* h, const mc_yuv422* in, int frames, int width, int height,
+                                         const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                                         uint8_t* produced, mc_chain_info* info);
 
 /* Pinned host memory for frames (so FramePool buffers can be DMA'd directly). */
 void* mc_host_alloc(size_t bytes);

@@ -54,7 +54,8 @@ MC_CANVAS_BGR, MC_CANVAS_NV12 = 0, 1
 
 
 class McCanvas(C.Structure):
-    """mc_canvas: the export canvases of a chain compose call (plane pointers are device addresses as integers)."""
+    """mc_canvas: the export canvases of a chain compose call (plane pointers are device addresses as integers, or host
+    addresses for the compose submits)."""
     _fields_ = [("format", C.c_int32), ("data", C.c_void_p), ("uv", C.c_void_p), ("pitch", C.c_size_t),
                 ("lane_stride", C.c_size_t)]
 
@@ -129,6 +130,12 @@ SIGNATURES = {
                                        C.POINTER(McChainInfo)]),
     "mc_chain_submit_yuv422": (C.c_int, [_vp, _YV, C.c_int, C.c_int, _PP, C.c_int, _vp, C.c_size_t, _vp, C.c_size_t,
                                          C.POINTER(McChainInfo)]),
+    "mc_chain_compose_submit": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, C.c_int, C.c_int, _CV,
+                                          _u8p, C.POINTER(McChainInfo)]),
+    "mc_chain_compose_submit_nv12": (C.c_int, [_vp, _NV, C.c_int, C.c_int, C.c_int, _PP, C.c_int, C.c_int, _CV, _u8p,
+                                               C.POINTER(McChainInfo)]),
+    "mc_chain_compose_submit_yuv422": (C.c_int, [_vp, _YV, C.c_int, C.c_int, C.c_int, _PP, C.c_int, C.c_int, _CV, _u8p,
+                                                 C.POINTER(McChainInfo)]),
     "mc_process_nv12_device": (C.c_int, [_vp, _NV, C.c_int, C.c_int, _PP, _NV, C.POINTER(C.c_int)]),
     "mc_process_clip_nv12_device": (C.c_int, [_vp, _NV, C.c_int, C.c_int, C.c_int, _PP, _NV, _u8p]),
     "mc_submit_nv12": (C.c_int, [_vp, _NV, C.c_int, C.c_int, _PP, _NV]),

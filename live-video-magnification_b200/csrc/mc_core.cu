@@ -40,6 +40,25 @@ struct DeviceBuffer {
     }
 };
 
+// A grow-only pinned host buffer, freed with its owner.  grow(need) frees the old allocation before it allocates the
+// larger one.
+struct PinnedBuffer {
+    uint8_t* p = nullptr;
+    size_t n = 0;
+    PinnedBuffer() = default;
+    PinnedBuffer(const PinnedBuffer&) = delete;
+    PinnedBuffer& operator=(const PinnedBuffer&) = delete;
+    ~PinnedBuffer() { if (p) cudaFreeHost(p); }
+    cudaError_t grow(size_t need) {
+        if (need <= n) return cudaSuccess;
+        if (p) cudaFreeHost(p);
+        p = nullptr; n = 0;
+        const cudaError_t e = cudaHostAlloc((void**)&p, need, cudaHostAllocDefault);
+        if (e == cudaSuccess) n = need;
+        return e;
+    }
+};
+
 // A frame set: one plane per lane (BGR or gray: height rows of w * c bytes) or two (NV12: height luma rows and height / 2
 // Cb,Cr rows of w bytes).  Rows hold `row` bytes and are `pitch` apart; lane l starts l * lane_stride after lane 0.
 struct Planes {
@@ -73,18 +92,20 @@ Planes yuv422_planes(const mc_yuv422& f, int w, int hh) {
 // out_ofs(k) in the slot's device output and in its pinned output staging.
 constexpr int kOutSets = 2;
 
-struct Slot {  // one in-flight frame of the pinned pipeline; frees what it holds
-    uint8_t *h_in = nullptr, *h_out = nullptr;   // pinned staging (lanes frames, packed): input bytes, output bytes
+// One in-flight frame set of the pinned pipeline: one frame of every lane, or a clip of `frames` frames of every lane
+// (virtual lane v = t * lanes + k).  The per-lane arrays hold frames * lanes entries.  Frees what it holds.
+struct Slot {
+    PinnedBuffer h_in, h_out;                    // pinned staging (packed), grown only for pageable inputs / outputs
     DeviceBuffer<> d_in, d_out;                  // device frames (packed)
     cudaEvent_t ev_in = nullptr, ev_k = nullptr, ev_done = nullptr;
     int produced = 0;
-    std::vector<uint8_t> lane_produced;          // per lane: the magnifier produced
+    std::vector<uint8_t> lane_produced;          // per virtual lane: the magnifier produced
+    uint8_t* flags_out = nullptr;                // the caller's copy of lane_produced, written by mc_collect (null: none)
     Planes out[kOutSets];                        // the caller's destinations (base null: none)
     size_t out_ofs[kOutSets] = {};
-    std::vector<uint8_t> written[kOutSets];      // per set and lane: its bytes of out[k] are written
-    bool direct_out[kOutSets] = {};              // D2H went straight into out[k] (pinned)
+    std::vector<uint8_t> written[kOutSets];      // per set and virtual lane: its bytes of out[k] are written
+    bool direct_out[kOutSets] = {};              // D2H goes straight into out[k] (pinned)
     ~Slot() {
-        for (uint8_t* p : {h_in, h_out}) if (p) cudaFreeHost(p);
         for (cudaEvent_t e : {ev_in, ev_k, ev_done}) if (e) cudaEventDestroy(e);
     }
 };
@@ -243,8 +264,9 @@ void free_slots(mc_handle* h) {
     h->next_slot = 0;
 }
 
-// Slots for `in_bytes` of input and `out_bytes` of output per frame set.  They are reallocated, never below their current
-// sizes, only while nothing is in flight.
+// Slots with device buffers for `in_bytes` of input and `out_bytes` of output per frame set.  They are reallocated, never
+// below their current sizes, only while nothing is in flight.  Their pinned staging is grown by submit_impl when a
+// submit's buffers are pageable.
 mc_status ensure_slots(mc_handle* h, size_t in_bytes, size_t out_bytes) {
     const bool have = (int)h->slots.size() == h->depth;
     if (have && h->slots[0].d_in.n >= in_bytes && h->slots[0].d_out.n >= out_bytes) return MC_OK;
@@ -259,10 +281,6 @@ mc_status ensure_slots(mc_handle* h, size_t in_bytes, size_t out_bytes) {
     free_slots(h);
     h->slots = std::vector<Slot>((size_t)h->depth);
     for (auto& s : h->slots) {
-        s.lane_produced.assign((size_t)h->lanes, 0);
-        for (auto& w : s.written) w.assign((size_t)h->lanes, 0);
-        CK(cudaHostAlloc((void**)&s.h_in, in_bytes, cudaHostAllocDefault));
-        CK(cudaHostAlloc((void**)&s.h_out, out_bytes, cudaHostAllocDefault));
         CK(s.d_in.grow(in_bytes));
         CK(s.d_out.grow(out_bytes));
         CK(cudaEventCreateWithFlags(&s.ev_in, cudaEventDisableTiming));
@@ -348,6 +366,16 @@ const mc_params* effective_params(mc_handle* h, const mc_params& p, mc_params* q
     return same ? nullptr : h->lane_eff.data();
 }
 
+// Color lanes whose effective parameters differ need option color_lane_lifecycle: MC_ERR_UNSUPPORTED otherwise.
+mc_status lane_params_check(mc_handle* h, const mc_params& p) {
+    mc_params q;
+    if (p.mode == MC_MODE_COLOR && !h->opt.color_lane_lifecycle && effective_params(h, p, &q)) {
+        h->err = "Color lanes with different parameters (mc_set_lane_params) need option color_lane_lifecycle";
+        return MC_ERR_UNSUPPORTED;
+    }
+    return MC_OK;
+}
+
 // The body of MagnificationProcessor::process on device-resident frames.
 // lane_produced: `lanes` per-lane flags (written).  frames > 1: a clip of that many consecutive
 // frames of every lane, [t][lane] in the lane stride, with frames * lanes flags.
@@ -374,12 +402,10 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
     const int max_levels = calculate_max_levels(w, hh);  // :32-33
     if (max_levels < 1) return MC_OK;
     const int levels = std::min(std::max((int)p->levels, 1), max_levels);  // :34
+    mc_status st = lane_params_check(h, *p);
+    if (st != MC_OK) return st;
     mc_params q;
     const mc_params* lane_params = effective_params(h, *p, &q);
-    if (lane_params && p->mode == MC_MODE_COLOR && !h->opt.color_lane_lifecycle) {
-        h->err = "Color lanes with different parameters (mc_set_lane_params) need option color_lane_lifecycle";
-        return MC_ERR_UNSUPPORTED;
-    }
     p = &q;
     if (p->mode == MC_MODE_COLOR) {
         // A held 1-lane handle skips the call: its window stays as it is.
@@ -412,7 +438,6 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
                       .prof = opt.profile_kernels ? &h->prof : nullptr,
                       .lane_ops = h->ops.data(), .d_lane_ops = h->d_ops, .lane_produced = lane_produced, .held_lost = &held_lost,
                       .lane_params = lane_params, .lane_lost = h->lane_lost.data()};
-    mc_status st = MC_OK;
     switch (p->mode) {
         case MC_MODE_LAPLACE: st = h->motion.process(ctx, io, *p, levels, produced, frames); break;
         case MC_MODE_COLOR: st = h->color.process(ctx, io, *p, levels, produced, frames); break;
@@ -435,42 +460,55 @@ mc_status process_device_impl(mc_handle* h, const uint8_t* d_in, int w, int hh, 
     return st;
 }
 
-// One frame set into the pipeline.  `in` is uploaded on the input stream into the next slot's packed device copy:
-// directly when it is pinned, through the slot's pinned staging when not.  `run(d_in, d_out, produced, lane_produced,
-// written)` then fills the slot's packed output sets d_out[k] (the shapes of out[k], which may differ from `in`'s) on the
-// handle's stream (with no buffers when `in` is empty: the identity), and says per set which lanes it wrote.  Only those
-// lanes are downloaded on the output stream, one copy per run of consecutive ones, into out[k] when it is pinned and into
-// the staging, which mc_collect copies out, when not; the other lanes' bytes of out[k] stay as they are.  The slot's d_in
-// is not overwritten before its kernels ran: the next upload into it follows mc_collect of this frame, which waits on
-// ev_done.  The slots' output holds at least out_reserve bytes.
+// One frame set into the pipeline: one frame of every lane, or with frames > 1 a clip of `frames` frames of every lane
+// (virtual lane v = t * lanes + k at v * lane_stride of `in` and of each out[k]).  `in` is uploaded on the input stream
+// into the next slot's packed device copy: directly when it is pinned, through the slot's pinned staging when not.
+// `run(d_in, d_out, produced, lane_produced, written)` then fills the slot's packed output sets d_out[k] (the shapes of
+// out[k], which may differ from `in`'s) on the handle's stream (with no buffers when `in` is empty: the identity), and
+// says per set which virtual lanes it wrote.  Only those are downloaded on the output stream, one copy per run of
+// consecutive ones, into out[k] when it is pinned and into the staging, which mc_collect copies out, when not; the other
+// lanes' bytes of out[k] stay as they are.  The slot's d_in and d_out are not overwritten before its copies and kernels
+// ran: the next upload into them follows mc_collect of this frame set, which waits on ev_done.  The slots' output holds
+// at least out_reserve bytes.  flags_out (frames * lanes bytes, or null) gets lane_produced at mc_collect.
 template <class Run>
-mc_status submit_impl(mc_handle* h, const Planes& in, const Planes (&out)[kOutSets], Run run, size_t out_reserve = 0) {
-    const size_t lanes = (size_t)h->lanes, bytes = in.lane_bytes() * lanes;
+mc_status submit_impl(mc_handle* h, const Planes& in, const Planes (&out)[kOutSets], Run run, size_t out_reserve = 0,
+                      int frames = 1, uint8_t* flags_out = nullptr) {
+    const size_t vl = (size_t)frames * h->lanes, bytes = in.lane_bytes() * vl;
     size_t ofs[kOutSets], out_bytes = 0;
     for (int k = 0; k < kOutSets; ++k) {
         if (out[k].base[0] && out[k].pitch < out[k].row) { h->err = "out_step too small"; return MC_ERR_INVALID; }
         ofs[k] = out_bytes;
-        out_bytes += (out[k].lane_bytes() * lanes + 255) / 256 * 256;   // each set 256-byte aligned
+        out_bytes += (out[k].lane_bytes() * vl + 255) / 256 * 256;   // each set 256-byte aligned
     }
     mc_status st = ensure_slots(h, std::max<size_t>(bytes, 1), std::max<size_t>({out_bytes, out_reserve, 1}));
     if (st != MC_OK) return st;
     const int si = h->next_slot;
     Slot& s = h->slots[(size_t)si];
+    // pinned staging only for what is pageable
+    const bool pinned_in = bytes && is_pinned(in);
+    if (bytes && !pinned_in) CK(s.h_in.grow(bytes));
+    bool staged_out = false;
+    for (int k = 0; k < kOutSets; ++k) {
+        s.direct_out[k] = out[k].base[0] && is_pinned(out[k]);
+        staged_out |= out[k].base[0] && !s.direct_out[k];
+    }
+    if (staged_out) CK(s.h_out.grow(out_bytes));
     s.produced = 0;
+    s.lane_produced.assign(vl, 0);
+    s.flags_out = flags_out;
     const Planes none;
     Planes d_out[kOutSets];
     for (int k = 0; k < kOutSets; ++k) {
-        s.out[k] = out[k]; s.out_ofs[k] = ofs[k]; s.direct_out[k] = false;
-        std::fill(s.written[k].begin(), s.written[k].end(), (uint8_t)0);
+        s.out[k] = out[k]; s.out_ofs[k] = ofs[k];
+        s.written[k].assign(vl, 0);
         d_out[k] = out[k].lane_bytes() ? out[k].packed(s.d_out.p + ofs[k]) : none;
     }
     const Planes d_in = bytes ? in.packed(s.d_in.p) : none;
     if (bytes) {
-        const bool pinned = is_pinned(in);
-        const Planes src = pinned ? in : in.packed(s.h_in);
-        if (!pinned)
-            for (size_t l = 0; l < lanes; ++l) host_copy(src, in, l);
-        if ((st = copy_planes(h, d_in, src, 0, lanes, cudaMemcpyHostToDevice, h->s_in)) != MC_OK) return st;
+        const Planes src = pinned_in ? in : in.packed(s.h_in.p);
+        if (!pinned_in)
+            for (size_t l = 0; l < vl; ++l) host_copy(src, in, l);
+        if ((st = copy_planes(h, d_in, src, 0, vl, cudaMemcpyHostToDevice, h->s_in)) != MC_OK) return st;
         CK(cudaEventRecord(s.ev_in, h->s_in));
         CK(cudaStreamWaitEvent(h->stream, s.ev_in, 0));
     }
@@ -485,9 +523,8 @@ mc_status submit_impl(mc_handle* h, const Planes& in, const Planes (&out)[kOutSe
         CK(cudaStreamWaitEvent(h->s_out, s.ev_k, 0));
         for (int k = 0; k < kOutSets; ++k) {
             if (!out[k].base[0]) continue;
-            s.direct_out[k] = is_pinned(out[k]);
-            const Planes dst = s.direct_out[k] ? out[k] : out[k].packed(s.h_out + ofs[k]);
-            st = for_each_run(lanes, [&](size_t l) { return s.written[k][l] != 0; }, [&](size_t a, size_t b) {
+            const Planes dst = s.direct_out[k] ? out[k] : out[k].packed(s.h_out.p + ofs[k]);
+            st = for_each_run(vl, [&](size_t l) { return s.written[k][l] != 0; }, [&](size_t a, size_t b) {
                 return copy_planes(h, dst, d_out[k], a, b, cudaMemcpyDeviceToHost, h->s_out);
             });
             if (st != MC_OK) return st;
@@ -775,11 +812,13 @@ mc_status mc_collect(mc_handle* h, int* produced) try {
     Slot& s = h->slots[(size_t)si];
     CK(cudaEventSynchronize(s.ev_done));
     *produced = s.produced;
-    h->lane_produced = s.lane_produced;
+    const size_t vl = s.lane_produced.size();   // a clip's last frame gives mc_lane_produced
+    std::copy(s.lane_produced.end() - h->lanes, s.lane_produced.end(), h->lane_produced.begin());
+    if (s.flags_out) std::memcpy(s.flags_out, s.lane_produced.data(), vl);
     for (int k = 0; k < kOutSets; ++k) {
         if (s.direct_out[k] || !s.out[k].base[0]) continue;
-        const Planes staged = s.out[k].packed(s.h_out + s.out_ofs[k]);
-        for (size_t l = 0; l < (size_t)h->lanes; ++l)
+        const Planes staged = s.out[k].packed(s.h_out.p + s.out_ofs[k]);
+        for (size_t l = 0; l < vl; ++l)
             if (s.written[k][l]) host_copy(s.out[k], staged, l);
     }
     return MC_OK;
@@ -901,13 +940,14 @@ extern "C" mc_status mc_profile_read(mc_handle* h, char* buf, size_t cap) try {
 
 // ---- clips: `frames` consecutive frames of every lane in one call ----------------------------------------------------
 namespace {
-// The argument errors of a clip call, before anything changes.
-mc_status check_clip(mc_handle* h, int frames, const uint8_t* produced) {
+// The argument errors of a clip call, before anything changes.  A blocking or device clip call (not `submitted`) also
+// refuses while pipelined frames are in flight.
+mc_status check_clip(mc_handle* h, int frames, const uint8_t* produced, bool submitted = false) {
     if (frames < 1) { h->err = "frames must be >= 1"; return MC_ERR_INVALID; }
     // frames * lanes * channels becomes a grid.z extent of the batched ingest / egress
     if ((long long)frames * h->lanes > MC_MAX_LANES) { h->err = "frames * lanes exceeds MC_MAX_LANES"; return MC_ERR_INVALID; }
     if (!produced) { h->err = "produced is null"; return MC_ERR_INVALID; }
-    if (!h->inflight.empty()) { h->err = "clip called with pipelined frames in flight"; return MC_ERR_INVALID; }
+    if (!submitted && !h->inflight.empty()) { h->err = "clip called with pipelined frames in flight"; return MC_ERR_INVALID; }
     return MC_OK;
 }
 
@@ -1642,6 +1682,93 @@ extern "C" mc_status mc_chain_submit_yuv422(mc_handle* h, const mc_yuv422* in, i
     CK(cudaSetDevice(h->device));
     if (!in) { h->err = "YUYV frame is null"; return MC_ERR_INVALID; }
     return chain_submit(h, nullptr, 0, nullptr, in, width, height, 3, p, grayscale, out, out_step, original, original_step, info);
+} catch (...) { return on_exception(h); }
+
+// ---- the export canvas from host clips: compose submits, collected by mc_collect -----------------------------------------
+namespace {
+// The planes of the canvases of a cw x ch canvas geometry (BGR, or NV12 luma and Cb,Cr), virtual lane v at v * lane_stride.
+Planes canvas_planes(const mc_canvas& c, int cw, int ch) {
+    if (c.format == MC_CANVAS_NV12) return Planes{{c.data, c.uv}, {(size_t)ch, (size_t)ch / 2}, (size_t)cw, c.pitch, c.lane_stride};
+    return Planes{{c.data, nullptr}, {(size_t)ch, 0}, (size_t)cw * 3, c.pitch, c.lane_stride};
+}
+
+// The body of the compose submits: every check of the matching device compose call (without its refusal while frames are
+// in flight), then one slot of the pipeline whose run is chain_run with a ComposeReq on the slot's buffers.  The compose
+// kernel writes the canvases into the slot's own output, never into handle scratch that the next submit reuses, and the
+// canvases of the lanes that are not held come back from there.  `produced` (frames * lanes) is written by the mc_collect
+// of this submit.
+mc_status compose_submit(mc_handle* h, const uint8_t* in, size_t in_step, const mc_nv12* nv, const mc_yuv422* yv, int frames,
+                         int w, int hh, int channels, const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                         uint8_t* produced, mc_chain_info* info) {
+    if ((int)h->inflight.size() >= h->depth) { h->err = "pipeline full: call mc_collect first"; return MC_ERR_INVALID; }
+    mc_status st = check_clip(h, frames, produced, true);
+    if (st != MC_OK) return st;
+    const ComposeReq cmp{split, canvas};
+    ChainGeom g;
+    if ((st = chain_check(h, in, in_step, nv, yv, frames, w, hh, channels, p, grayscale, false, 0, false, 0, info, &cmp, g)) != MC_OK)
+        return st;
+    const bool empty = chain_empty(in, nv, yv, w, hh);
+    // the device call's magnifier refuses Color lanes with different parameters only once its front ran: here, before any copy
+    if (!empty && calculate_max_levels(g.dw, g.dh) >= 1 && (st = lane_params_check(h, *p)) != MC_OK) return st;
+    int cw, ch;
+    canvas_size(g, split, cw, ch);
+    Planes src, dst[kOutSets];
+    if (!empty) {
+        src = nv ? nv12_planes(*nv, w, hh) : yv ? yuv422_planes(*yv, w, hh) : bgr_planes(in, w, hh, channels, in_step);
+        if (cw > 0) dst[0] = canvas_planes(*canvas, cw, ch);
+    }
+    // Room for the canvases of this frame size without a crop or downscale, so that a ROI or downscale change with clips in
+    // flight does not have to grow the slots; a shorter clip fits in a longer one's.
+    ChainGeom full;
+    full.dw = empty ? 0 : w; full.dh = empty ? 0 : hh;
+    int fw, fh;
+    canvas_size(full, split, fw, fh);
+    const size_t reserve = ((size_t)fw * fh * (canvas->format == MC_CANVAS_NV12 ? 3 : 6) / 2 * frames * h->lanes + 255) / 256 * 256;
+    const int order = yv ? yv->order : 0;
+    const size_t lanes = (size_t)h->lanes, vl = (size_t)frames * lanes;
+    return submit_impl(h, src, dst, [&](const Planes& d_in, const Planes* d_out, int* any, uint8_t* flags,
+                                        std::vector<uint8_t>* written) {
+        const mc_nv12 dnv = nv12_of(d_in);
+        const mc_yuv422 dyv{d_in.base[0], d_in.pitch, d_in.lane_stride, order};
+        const mc_canvas dcv{canvas->format, d_out[0].base[0], d_out[0].base[1], d_out[0].pitch, d_out[0].lane_stride};
+        const ComposeReq dcmp{split, &dcv};
+        const mc_status rs = chain_run(h, g, d_in.base[0], d_in.pitch, nv ? &dnv : nullptr, yv ? &dyv : nullptr, frames, w, hh,
+                                       channels, p, nullptr, 0, nullptr, 0, flags, &dcmp);
+        if (rs != MC_OK) return rs;
+        *any = std::any_of(flags, flags + vl, [](uint8_t x) { return x != 0; });
+        for (size_t v = 0; v < vl; ++v) written[0][v] = cw > 0 && !h->hold[v % lanes];   // what the compose kernel wrote
+        return MC_OK;
+    }, reserve, frames, produced);
+}
+}  // namespace
+
+// The pipelined exporter: a clip of every lane through the chain and compose per submit, collected by mc_collect in
+// submit order with every other submit.
+extern "C" mc_status mc_chain_compose_submit(mc_handle* h, const uint8_t* in, int frames, int width, int height, int channels,
+                                             size_t in_step, const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                                             uint8_t* produced, mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    return compose_submit(h, in, in_step, nullptr, nullptr, frames, width, height, channels, p, grayscale, split, canvas, produced,
+                          info);
+} catch (...) { return on_exception(h); }
+
+extern "C" mc_status mc_chain_compose_submit_nv12(mc_handle* h, const mc_nv12* in, int frames, int width, int height,
+                                                  const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                                                  uint8_t* produced, mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    if (!in) { h->err = "NV12 plane is null"; return MC_ERR_INVALID; }
+    return compose_submit(h, nullptr, 0, in, nullptr, frames, width, height, 3, p, grayscale, split, canvas, produced, info);
+} catch (...) { return on_exception(h); }
+
+extern "C" mc_status mc_chain_compose_submit_yuv422(mc_handle* h, const mc_yuv422* in, int frames, int width, int height,
+                                                    const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                                                    uint8_t* produced, mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    if (!in) { h->err = "YUYV frame is null"; return MC_ERR_INVALID; }
+    return compose_submit(h, nullptr, 0, nullptr, in, frames, width, height, 3, p, grayscale, split, canvas, produced, info);
 } catch (...) { return on_exception(h); }
 
 /* test hooks, not declared in the public header: the two conversion kernels alone on device buffers (default stream,

@@ -11,6 +11,7 @@ the H100 behind the C ABI (include/magcore_b200.h).
 """
 from __future__ import annotations
 
+import collections
 import ctypes as C
 import enum
 from dataclasses import dataclass, field, replace
@@ -420,12 +421,15 @@ class ProcessingChainB200:
     ``run_chain_once(frame, cfg) -> (cur, original)`` returns the *same* frame object wherever the reference
     returns the same FrameRef (identity stages / passthrough); it needs ``lanes == 1``.  ``process_device`` and
     ``process_nv12_device`` / ``process_yuv422_device`` run the chain on device frames of every lane, for one frame or a
-    clip; ``submit`` / ``submit_nv12`` / ``submit_yuv422`` pipeline host frames of every lane, and ``collect`` returns them
-    in order; ``run_chain_once`` of a ``Frame`` whose format is "YUYV" or "UYVY" takes a camera's packed 4:2:2 bytes."""
+    clip; ``submit`` / ``submit_nv12`` / ``submit_yuv422`` pipeline host frames of every lane, ``compose_submit`` and its
+    ``_nv12`` / ``_yuv422`` forms pipeline host clips into export canvases, and ``collect`` returns them in order;
+    ``run_chain_once`` of a ``Frame`` whose format is "YUYV" or "UYVY" takes a camera's packed 4:2:2 bytes."""
 
     def __init__(self, device: int = 0, lanes: int = 1):
         self.magnifier = MagnificationProcessor(device=device, lanes=lanes)
         self.lanes = lanes
+        # the flag arrays of the latest compose submits: every submit in flight is among the last 16 (the deepest pipeline)
+        self._pending_flags = collections.deque(maxlen=16)
 
     def reset(self) -> None:
         """ProcessingChain's recovery path resets every stage (ProcessingChain.cpp:50-62); only the magnifier has state."""
@@ -502,8 +506,43 @@ class ProcessingChainB200:
                                                out_step, original_ptr or None, original_step, C.byref(info)))
         return info
 
+    # -- pipelined export canvases from host clips (mc_chain_compose_submit*, collected by collect()) ------------------------
+    def _compose_submit(self, fn, src, frames: int, *args, split: int, canvas: capi.McCanvas):
+        m, info = self.magnifier, capi.McChainInfo()
+        flags = np.zeros((int(frames), self.lanes), np.uint8)
+        m._check(fn(m._h, src, int(frames), *args, int(split), C.byref(canvas), flags.ctypes.data_as(C.POINTER(C.c_uint8)),
+                    C.byref(info)))
+        self._pending_flags.append(flags)   # the core writes it at collect: kept alive until then
+        return info, flags
+
+    def compose_submit(self, in_ptr: int, frames: int, w: int, h: int, c: int, in_step: int, cfg: ProcessorConfig, split: int,
+                       canvas: capi.McCanvas):
+        """mc_chain_compose_submit: a clip of `frames` BGR or gray host frames of every lane (virtual lane t * lanes + k at
+        its index * h * in_step; pinned or pageable) through the chain and the export canvas into host canvases ->
+        (McChainInfo with magnified 0, u8 [frames, lanes] produced flags, filled by the collect() of this submit).  The
+        input and the canvases must stay valid, and the input unchanged, until then."""
+        m, p = self.magnifier, _to_mc(cfg)
+        return self._compose_submit(m._lib.mc_chain_compose_submit, in_ptr or None, frames, w, h, c, in_step, C.byref(p),
+                                    int(cfg.grayscale), split=split, canvas=canvas)
+
+    def compose_submit_nv12(self, in_planes: capi.McNv12, frames: int, w: int, h: int, cfg: ProcessorConfig, split: int,
+                            canvas: capi.McCanvas):
+        """mc_chain_compose_submit_nv12: compose_submit() on NV12 host planes (virtual lane v at v * lane_stride)."""
+        m, p = self.magnifier, _to_mc(cfg)
+        return self._compose_submit(m._lib.mc_chain_compose_submit_nv12, C.byref(in_planes), frames, w, h, C.byref(p),
+                                    int(cfg.grayscale), split=split, canvas=canvas)
+
+    def compose_submit_yuv422(self, in_frame: capi.McYuv422, frames: int, w: int, h: int, cfg: ProcessorConfig, split: int,
+                              canvas: capi.McCanvas):
+        """mc_chain_compose_submit_yuv422: compose_submit() on packed YUYV / UYVY host frames (virtual lane v at
+        v * lane_stride)."""
+        m, p = self.magnifier, _to_mc(cfg)
+        return self._compose_submit(m._lib.mc_chain_compose_submit_yuv422, C.byref(in_frame), frames, w, h, C.byref(p),
+                                    int(cfg.grayscale), split=split, canvas=canvas)
+
     def collect(self) -> np.ndarray:
-        """mc_collect of the oldest frame in flight -> bool[lanes]: which lanes magnified it."""
+        """mc_collect of the oldest frame in flight -> bool[lanes]: which lanes magnified it (of a compose submit's clip:
+        its last frame; the flags of every frame are in the array compose_submit returned)."""
         self.magnifier.collect()
         return self.magnifier.lane_produced()
 
