@@ -8,6 +8,7 @@
 #include <deque>
 #include <initializer_list>
 #include <new>
+#include <optional>
 #include <string>
 #include <vector>
 
@@ -84,9 +85,58 @@ Planes nv12_planes(const mc_nv12& f, int w, int hh) {
 }
 mc_nv12 nv12_of(const Planes& f) { return mc_nv12{f.base[0], f.base[1], f.pitch, f.lane_stride}; }
 
-Planes yuv422_planes(const mc_yuv422& f, int w, int hh) {
-    return Planes{{f.data, nullptr}, {(size_t)hh, 0}, (size_t)2 * w, f.pitch, f.lane_stride};
-}
+// The source frames of a call: u8 BGR or gray, NV12 planes or packed 4:2:2 frames, virtual lane v at v *
+// planes.lane_stride.  Only these helpers tell the formats apart.
+struct Source {
+    static constexpr int kBadOrder = FRONT_UYVY + 1;   // a 4:2:2 frame of an order out of range: refused by check()
+    int kind = FRONT_BGR;                               // FrontSrc, the front's `src`
+    int w = 0, hh = 0, channels = 3;                    // NV12 and 4:2:2 frames stand for BGR ones
+    Planes planes;
+    const char* missing = nullptr;   // the call's mc_nv12 / mc_yuv422 is NULL: its error comes before every other check
+
+    static Source bgr(const uint8_t* in, int w, int hh, int c, size_t step) {
+        return Source{c == 3 ? FRONT_BGR : FRONT_GRAY, w, hh, c, bgr_planes(in, w, hh, c, step)};
+    }
+    static Source nv12(const mc_nv12* f, int w, int hh) {
+        return f ? Source{FRONT_NV12, w, hh, 3, nv12_planes(*f, w, hh)} : Source{FRONT_NV12, w, hh, 3, {}, "NV12 plane is null"};
+    }
+    static Source yuv422(const mc_yuv422* f, int w, int hh) {
+        if (!f) return Source{FRONT_YUYV, w, hh, 3, {}, "YUYV frame is null"};
+        const int kind = f->order == MC_YUV422_YUYV || f->order == MC_YUV422_UYVY ? FRONT_YUYV + f->order : kBadOrder;
+        return Source{kind, w, hh, 3, Planes{{f->data, nullptr}, {(size_t)hh, 0}, (size_t)2 * w, f->pitch, f->lane_stride}};
+    }
+
+    // BGR or gray frames, which the magnifier reads where they are
+    bool bgr_or_gray() const { return kind == FRONT_BGR || kind == FRONT_GRAY; }
+    // the identity: no BGR or gray frame (NV12 and 4:2:2 frames are checked instead)
+    bool empty() const { return bgr_or_gray() && (!planes.base[0] || w <= 0 || hh <= 0); }
+    // the 4:2:2 conversion is a front stage that always runs: the front writes its BGR frame where a BGR source would
+    // leave the result to the input
+    bool converts() const { return kind >= FRONT_YUYV; }
+    // the source's argument errors for `vl` virtual lanes -> an error text, or null
+    const char* check(size_t vl) const {
+        if (kind == FRONT_NV12) {
+            if (w < 2 || hh < 2 || (w & 1) || (hh & 1)) return "NV12 width and height must be even and >= 2";
+            if (!planes.base[0] || !planes.base[1]) return "NV12 plane is null";
+            if (planes.pitch < (size_t)w) return "NV12 pitch < width";
+            if (vl > 1 && planes.lane_stride < planes.pitch * hh) return "NV12 lane_stride < pitch * height";
+            return nullptr;
+        }
+        if (converts()) {
+            if (!planes.base[0]) return "YUYV frame is null";
+            if (kind == kBadOrder) return "YUYV order out of range";
+            if (w < 2 || (w & 1) || hh < 1) return "YUYV width must be even and >= 2, height >= 1";
+            if (planes.pitch < (size_t)2 * w) return "YUYV pitch < 2 * width";
+            if (vl > 1 && planes.lane_stride < planes.pitch * hh) return "YUYV lane_stride < pitch * height";
+            return nullptr;
+        }
+        return !empty() && planes.pitch < planes.row ? "step too small" : nullptr;
+    }
+    // the frames as the front and the compose kernel read them
+    PaneSrc pane() const { return PaneSrc{planes.base[0], planes.base[1], planes.pitch, planes.lane_stride, kind}; }
+    // the same frames at `p` (a pipeline slot's packed device copy)
+    Source on(const Planes& p) const { Source s = *this; s.planes = p; return s; }
+};
 
 // A slot's output frame sets: the processed frames and, for chain submits, the original tap.  Set k sits at
 // out_ofs(k) in the slot's device output and in its pinned output staging.
@@ -1022,11 +1072,8 @@ extern "C" mc_status mc_process_clip(mc_handle* h, const uint8_t* in, int frames
 namespace {
 mc_status check_nv12(mc_handle* h, std::initializer_list<const mc_nv12*> frame_sets, int w, int hh, int vlanes, const mc_params* p) {
     if (!p) { h->err = "params is null"; return MC_ERR_INVALID; }
-    if (w < 2 || hh < 2 || (w & 1) || (hh & 1)) { h->err = "NV12 width and height must be even and >= 2"; return MC_ERR_INVALID; }
     for (const mc_nv12* f : frame_sets) {
-        if (!f || !f->y || !f->uv) { h->err = "NV12 plane is null"; return MC_ERR_INVALID; }
-        if (f->pitch < (size_t)w) { h->err = "NV12 pitch < width"; return MC_ERR_INVALID; }
-        if (vlanes > 1 && f->lane_stride < f->pitch * hh) { h->err = "NV12 lane_stride < pitch * height"; return MC_ERR_INVALID; }
+        if (const char* e = Source::nv12(f, w, hh).check((size_t)vlanes)) { h->err = e; return MC_ERR_INVALID; }
     }
     return MC_OK;
 }
@@ -1230,111 +1277,92 @@ const char* check_compose(const ComposeReq& c, const ChainGeom& g, size_t vl, co
     return nullptr;
 }
 
-const char* check_yuv422(const mc_yuv422& f, int w, int hh, size_t vl) {
-    if (!f.data) return "YUYV frame is null";
-    if (f.order != MC_YUV422_YUYV && f.order != MC_YUV422_UYVY) return "YUYV order out of range";
-    if (w < 2 || (w & 1) || hh < 1) return "YUYV width must be even and >= 2, height >= 1";
-    if (f.pitch < (size_t)2 * w) return "YUYV pitch < 2 * width";
-    if (vl > 1 && f.lane_stride < f.pitch * hh) return "YUYV lane_stride < pitch * height";
-    return nullptr;
-}
-
-bool chain_empty(const uint8_t* in, const mc_nv12* nv, const mc_yuv422* yv, int w, int hh) {
-    return !nv && !yv && (in == nullptr || w <= 0 || hh <= 0);
-}
+// Where a chain call's results go: the processed frames and the original tap (null: not wanted), or with cmp the export
+// canvases instead.
+struct ChainDst {
+    uint8_t* out = nullptr; size_t out_step = 0;     // the processed frames
+    uint8_t* orig = nullptr; size_t orig_step = 0;   // the original tap
+    std::optional<ComposeReq> cmp;
+};
 
 // The argument errors of a chain call on `frames` consecutive frames of every lane, before anything changes, and its
-// geometry g and info.  Only the pointers' nullness is read, so host and device frame sets are checked alike: in (u8 BGR
-// or gray, in_step), or NV12 planes nv, or a packed 4:2:2 frame yv; out_given / orig_given: the processed frames' and
-// the original tap's destinations are not NULL.  A 4:2:2 source's conversion is a front stage that always runs: the
-// front writes its BGR frame where a BGR source would leave the result to the input, and info says so.
-mc_status chain_check(mc_handle* h, const uint8_t* in, size_t in_step, const mc_nv12* nv, const mc_yuv422* yv, int frames, int w,
-                      int hh, int channels, const mc_params* p, int grayscale, bool out_given, size_t out_step, bool orig_given,
-                      size_t orig_step, mc_chain_info* info, const ComposeReq* cmp, ChainGeom& g) {
+// geometry g and info.  Only the pointers' nullness is read, so host and device frame sets are checked alike.
+// out_optional: a NULL d.out is not an error.
+mc_status chain_check(mc_handle* h, const Source& s, int frames, const mc_params* p, int grayscale, const ChainDst& d,
+                      mc_chain_info* info, ChainGeom& g, bool out_optional = false) {
     if (!p || !info) { h->err = "params or info is null"; return MC_ERR_INVALID; }
-    const bool empty = chain_empty(in, nv, yv, w, hh);
-    if (const char* e = chain_geometry(p, empty ? 0 : w, empty ? 0 : hh, channels, grayscale, g, info)) {
+    const bool empty = s.empty();
+    if (const char* e = chain_geometry(p, empty ? 0 : s.w, empty ? 0 : s.hh, s.channels, grayscale, g, info)) {
         h->err = e;
         return MC_ERR_INVALID;
     }
-    const bool pre = g.pre || yv, front = g.front() || yv;
-    if (yv) {
+    const bool pre = g.pre || s.converts(), front = g.front() || s.converts();
+    const size_t lanes = (size_t)h->lanes, vl = (size_t)frames * lanes;
+    if (s.converts()) {   // info says where the conversion went; the frame's errors come before the canvas's
         info->orig_is_input = 0; info->orig_w = g.dw; info->orig_h = g.dh; info->orig_channels = 3;
         info->cur_is_input = 0; info->out_w = g.dw; info->out_h = g.dh; info->out_channels = g.cc;
+        if (const char* e = s.check(vl)) { h->err = e; return MC_ERR_INVALID; }
     }
-    const size_t lanes = (size_t)h->lanes, vl = (size_t)frames * lanes;
-    if (yv) {
-        if (const char* e = check_yuv422(*yv, w, hh, vl)) { h->err = e; return MC_ERR_INVALID; }
-    }
-    if (cmp) {
-        if (const char* e = check_compose(*cmp, g, vl, h->ov)) { h->err = e; return MC_ERR_INVALID; }
+    if (d.cmp) {
+        if (const char* e = check_compose(*d.cmp, g, vl, h->ov)) { h->err = e; return MC_ERR_INVALID; }
     }
     if (empty) return MC_OK;   // the identity
-    mc_status st;
-    if (nv) {
-        if ((st = check_nv12(h, {nv}, w, hh, (int)vl, p)) != MC_OK) return st;
-    } else if (!yv && in_step < (size_t)w * channels) {
-        h->err = "step too small";
-        return MC_ERR_INVALID;
-    }
+    if (const char* e = s.converts() ? nullptr : s.check(vl)) { h->err = e; return MC_ERR_INVALID; }
     if (p->mode < 0 || p->mode > MC_MODE_NONE) { h->err = "bad mode"; return MC_ERR_INVALID; }
-    if (!cmp && (front || p->mode != MC_MODE_NONE)) {
-        if (!out_given) { h->err = "output pointer is null"; return MC_ERR_INVALID; }
-        if (out_step < (size_t)g.dw * g.cc) { h->err = "out_step too small"; return MC_ERR_INVALID; }
+    if (!d.cmp && (front || p->mode != MC_MODE_NONE)) {
+        if (!d.out && !out_optional) { h->err = "output pointer is null"; return MC_ERR_INVALID; }
+        if (d.out_step < (size_t)g.dw * g.cc) { h->err = "out_step too small"; return MC_ERR_INVALID; }
     }
-    if (!cmp && pre && orig_given && orig_step < (size_t)g.dw * channels) {
+    if (!d.cmp && pre && d.orig && d.orig_step < (size_t)g.dw * s.channels) {
         h->err = "original_step too small";
         return MC_ERR_INVALID;
     }
     const int max_levels = calculate_max_levels(g.dw, g.dh);
     if (p->mode == MC_MODE_COLOR && max_levels >= 1 && !(lanes == 1 && h->hold[0])) {
         const int levels = std::min(std::max((int)p->levels, 1), max_levels);
-        if ((st = color_lane_check(h, p, levels, g.cc, g.dw, g.dh)) != MC_OK) return st;
+        return color_lane_check(h, p, levels, g.cc, g.dw, g.dh);
     }
     return MC_OK;
 }
 
 // runChainOnce for every lane and `frames` consecutive frames, on device frame sets that passed chain_check (which gave
-// g).  One front launch writes the preprocessed frames (d_orig, or staging) and the magnifier's input (the same frames or
-// their gray), the magnifier writes d_out, and the frames it did not produce get the front's output.  produced: frames *
-// lanes flags.  With cmp, the call composes instead: d_out / d_orig are not the caller's, the magnifier writes h->x_mag,
-// the preprocessed frames stay in h->f_pre when the canvas shows them, and one compose launch reads every pane where it is.
+// g).  One front launch writes the preprocessed frames (d.orig, or staging) and the magnifier's input (the same frames or
+// their gray), the magnifier writes d.out, and the frames it did not produce get the front's output.  produced: frames *
+// lanes flags.  With d.cmp, the call composes instead: the magnifier writes h->x_mag, the preprocessed frames stay in
+// h->f_pre when the canvas shows them, and one compose launch reads every pane where it is.
 // Everything it uses of the handle's chain scratch (f_pre, f_gray, f_flags, f_tabs, n_in, x_mag, x_ops and the host
 // copies) is written and read on the handle's stream only, so pipelined frames may share it in submit order.
-mc_status chain_run(mc_handle* h, const ChainGeom& g, const uint8_t* d_in, size_t in_step, const mc_nv12* nv, const mc_yuv422* yv,
-                    int frames, int w, int hh, int channels, const mc_params* p, uint8_t* d_out, size_t out_step, uint8_t* d_orig,
-                    size_t orig_step, uint8_t* produced, const ComposeReq* cmp = nullptr) {
+mc_status chain_run(mc_handle* h, const ChainGeom& g, const Source& s, int frames, const mc_params* p, ChainDst d, uint8_t* produced) {
     const size_t lanes = (size_t)h->lanes, vl = (size_t)frames * lanes;
-    if (chain_empty(d_in, nv, yv, w, hh)) return clip_run(h, nullptr, frames, 0, 0, channels, 0, p, nullptr, 0, produced);
-    const bool pre = g.pre || yv, front = g.front() || yv;
+    if (s.empty()) return clip_run(h, nullptr, frames, 0, 0, s.channels, 0, p, nullptr, 0, produced);
+    const bool pre = g.pre || s.converts(), front = g.front() || s.converts();
     const size_t out_row = (size_t)g.dw * g.cc;
     mc_status st;
-    if (cmp) {
+    if (d.cmp) {
         if (p->mode != MC_MODE_NONE) {
             CK(h->x_mag.grow(out_row * g.dh * vl));
-            d_out = h->x_mag.p; out_step = out_row;
+            d.out = h->x_mag.p; d.out_step = out_row;
         }
-        d_orig = nullptr;
-        if (g.pre && cmp->split != MC_SPLIT_NONE) {
-            orig_step = (size_t)g.dw * channels;
-            CK(h->f_pre.grow(orig_step * g.dh * vl));
-            d_orig = h->f_pre.p;
+        d.orig = nullptr;
+        if (g.pre && d.cmp->split != MC_SPLIT_NONE) {
+            d.orig_step = (size_t)g.dw * s.channels;
+            CK(h->f_pre.grow(d.orig_step * g.dh * vl));
+            d.orig = h->f_pre.p;
         }
     }
-    const bool tap = pre && d_orig;
+    const bool tap = pre && d.orig;
     // ---- the front: one launch over the virtual lanes; held lanes are skipped
-    const uint8_t* mag_in = d_in;
-    size_t mag_step = in_step;
+    const PaneSrc input = s.pane();
+    const uint8_t* mag_in = input.p;
+    size_t mag_step = input.step;
     if (front) {
         FrontArgs a;
-        if (nv) { a.src = nv->y; a.uv = nv->uv; a.step = nv->pitch; a.lane_stride = nv->lane_stride; }
-        else if (yv) { a.src = yv->data; a.step = yv->pitch; a.lane_stride = yv->lane_stride; }
-        else { a.src = d_in; a.step = in_step; a.lane_stride = in_step * hh; }
+        a.src = input.p; a.uv = input.uv; a.step = input.step; a.lane_stride = input.lane_stride;
         a.rx = g.rx; a.ry = g.ry; a.dw = g.dw; a.dh = g.dh; a.kind = g.kind; a.isx = g.isx; a.isy = g.isy;
         if (tap) {
-            a.dst = d_orig; a.dst_step = orig_step;
+            a.dst = d.orig; a.dst_step = d.orig_step;
         } else if (pre && !g.gray) {   // the preprocessed frames are the magnifier's input
-            a.dst_step = (size_t)g.dw * channels;
+            a.dst_step = (size_t)g.dw * s.channels;
             CK(h->f_pre.grow(a.dst_step * g.dh * vl));
             a.dst = h->f_pre.p;
         }
@@ -1351,28 +1379,24 @@ mc_status chain_run(mc_handle* h, const ChainGeom& g, const uint8_t* d_in, size_
             CK(cudaMemcpyAsync(h->f_flags.p, h->f_flags_host.data(), vl, cudaMemcpyHostToDevice, h->stream));
             a.flags = h->f_flags.p;
         }
-        const int src = nv ? FRONT_NV12 : yv ? FRONT_YUYV + yv->order : channels == 3 ? FRONT_BGR : FRONT_GRAY;
-        if ((st = launch_counted(h, "chain_front", [&] { return launch_chain_front(a, src, (int)vl, h->stream); })) != MC_OK) return st;
+        if ((st = launch_counted(h, "chain_front", [&] { return launch_chain_front(a, input.kind, (int)vl, h->stream); })) != MC_OK) return st;
         mag_in = g.gray ? a.gray : a.dst;
         mag_step = g.gray ? (size_t)g.dw : a.dst_step;
-    } else if (nv && p->mode != MC_MODE_NONE) {   // a plain NV12 -> BGR conversion
-        if ((st = nv12_ingest(h, *nv, w, hh, (int)vl, p, false)) != MC_OK) return st;
+    } else if (!s.bgr_or_gray() && p->mode != MC_MODE_NONE) {   // NV12 without a front stage: a plain NV12 -> BGR conversion
+        if ((st = nv12_ingest(h, nv12_of(s.planes), s.w, s.hh, (int)vl, p, false)) != MC_OK) return st;
         mag_in = h->n_in.p;
-        mag_step = bgr_step_of(w);
+        mag_step = bgr_step_of(s.w);
     }
 
-    // ---- the magnifier, straight into d_out; then the canvases, or the front's output for the frames it did not produce
-    if ((st = clip_run(h, mag_in, frames, g.dw, g.dh, g.cc, mag_step, p, d_out, out_step, produced)) != MC_OK) return st;
-    if (cmp) {
+    // ---- the magnifier, straight into d.out; then the canvases, or the front's output for the frames it did not produce
+    if ((st = clip_run(h, mag_in, frames, g.dw, g.dh, g.cc, mag_step, p, d.out, d.out_step, produced)) != MC_OK) return st;
+    if (d.cmp) {
         ComposeArgs a;
         a.w = g.dw & ~1; a.h = g.dh & ~1;
         if (a.w <= 0 || a.h <= 0) return MC_OK;   // a 0 x 0 canvas
-        const int in_kind = channels == 3 ? FRONT_BGR : FRONT_GRAY, out_kind = g.cc == 3 ? FRONT_BGR : FRONT_GRAY;
-        const PaneSrc input = nv   ? PaneSrc{nv->y, nv->uv, nv->pitch, nv->lane_stride, FRONT_NV12}
-                              : yv ? PaneSrc{yv->data, nullptr, yv->pitch, yv->lane_stride, FRONT_YUYV + yv->order}
-                                   : PaneSrc{d_in, nullptr, in_step, in_step * hh, in_kind};
-        a.src[0] = tap ? PaneSrc{d_orig, nullptr, orig_step, orig_step * g.dh, in_kind} : input;
-        a.src[1] = PaneSrc{d_out, nullptr, out_step, out_step * g.dh, out_kind};
+        const int in_kind = s.channels == 3 ? FRONT_BGR : FRONT_GRAY, out_kind = g.cc == 3 ? FRONT_BGR : FRONT_GRAY;
+        a.src[0] = tap ? PaneSrc{d.orig, nullptr, d.orig_step, d.orig_step * g.dh, in_kind} : input;
+        a.src[1] = PaneSrc{d.out, nullptr, d.out_step, d.out_step * g.dh, out_kind};
         a.src[2] = front ? PaneSrc{mag_in, nullptr, mag_step, mag_step * g.dh, out_kind} : input;
         // the pane choice of every virtual lane goes to the device on the handle's stream, as the front's flags do
         h->x_ops_host.resize(vl);   // lives on the handle: the copy is asynchronous
@@ -1381,8 +1405,8 @@ mc_status chain_run(mc_handle* h, const ChainGeom& g, const uint8_t* d_in, size_
         CK(h->x_ops.grow(vl));
         CK(cudaMemcpyAsync(h->x_ops.p, h->x_ops_host.data(), vl, cudaMemcpyHostToDevice, h->stream));
         a.ops = h->x_ops.p;
-        a.split = cmp->split;
-        const mc_canvas& cv = *cmp->canvas;
+        a.split = d.cmp->split;
+        const mc_canvas& cv = *d.cmp->canvas;
         a.nv12 = cv.format == MC_CANVAS_NV12;
         a.data = cv.data; a.uv = cv.uv; a.pitch = cv.pitch; a.lane_stride = cv.lane_stride;
         if (h->ov.set) {
@@ -1396,9 +1420,9 @@ mc_status chain_run(mc_handle* h, const ChainGeom& g, const uint8_t* d_in, size_
         return launch_counted(h, "compose", [&] { return launch_compose(a, (int)vl, h->stream); });
     }
     if (!front) return MC_OK;
-    const size_t in_lane = mag_step * g.dh, out_lane = out_step * g.dh;
+    const size_t in_lane = mag_step * g.dh, out_lane = d.out_step * g.dh;
     return for_each_run(vl, [&](size_t v) { return !produced[v] && !h->hold[v % lanes]; }, [&](size_t a, size_t b) -> mc_status {
-        CK(cudaMemcpy2DAsync(d_out + a * out_lane, out_step, mag_in + a * in_lane, mag_step, out_row, (b - a) * g.dh,
+        CK(cudaMemcpy2DAsync(d.out + a * out_lane, d.out_step, mag_in + a * in_lane, mag_step, out_row, (b - a) * g.dh,
                              cudaMemcpyDeviceToDevice, h->stream));
         return MC_OK;
     });
@@ -1406,18 +1430,14 @@ mc_status chain_run(mc_handle* h, const ChainGeom& g, const uint8_t* d_in, size_
 
 // A device chain call: checked (with the pipelined frames' refusal), run, and its last frame's flags are
 // mc_lane_produced's.
-mc_status chain_impl(mc_handle* h, const uint8_t* d_in, size_t in_step, const mc_nv12* nv, const mc_yuv422* yv, int frames,
-                     int w, int hh, int channels, const mc_params* p, int grayscale, uint8_t* d_out, size_t out_step,
-                     uint8_t* d_orig, size_t orig_step, uint8_t* produced, mc_chain_info* info,
-                     const ComposeReq* cmp = nullptr) {
+mc_status chain_impl(mc_handle* h, const Source& s, int frames, const mc_params* p, int grayscale, const ChainDst& d,
+                     uint8_t* produced, mc_chain_info* info) {
+    if (s.missing) { h->err = s.missing; return MC_ERR_INVALID; }
     mc_status st = check_clip(h, frames, produced);
     if (st != MC_OK) return st;
     ChainGeom g;
-    if ((st = chain_check(h, d_in, in_step, nv, yv, frames, w, hh, channels, p, grayscale, d_out != nullptr, out_step,
-                          d_orig != nullptr, orig_step, info, cmp, g)) != MC_OK)
-        return st;
-    st = chain_run(h, g, d_in, in_step, nv, yv, frames, w, hh, channels, p, d_out, out_step, d_orig, orig_step, produced, cmp);
-    if (st != MC_OK) return st;
+    if ((st = chain_check(h, s, frames, p, grayscale, d, info, g)) != MC_OK) return st;
+    if ((st = chain_run(h, g, s, frames, p, d, produced)) != MC_OK) return st;
     const size_t lanes = (size_t)h->lanes, vl = (size_t)frames * lanes;
     std::memcpy(h->lane_produced.data(), produced + vl - lanes, lanes);
     info->magnified = std::any_of(produced, produced + vl, [](uint8_t x) { return x != 0; });
@@ -1438,8 +1458,8 @@ extern "C" mc_status mc_chain_process_device(mc_handle* h, const uint8_t* d_in, 
                                              mc_chain_info* info) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    return chain_impl(h, d_in, in_step, nullptr, nullptr, frames, width, height, channels, p, grayscale, d_out, out_step, d_original,
-                      original_step, produced, info);
+    return chain_impl(h, Source::bgr(d_in, width, height, channels, in_step), frames, p, grayscale,
+                      ChainDst{d_out, out_step, d_original, original_step}, produced, info);
 } catch (...) { return on_exception(h); }
 
 extern "C" mc_status mc_chain_process_nv12_device(mc_handle* h, const mc_nv12* in, int frames, int width, int height,
@@ -1448,8 +1468,7 @@ extern "C" mc_status mc_chain_process_nv12_device(mc_handle* h, const mc_nv12* i
                                                   mc_chain_info* info) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    if (!in) { h->err = "NV12 plane is null"; return MC_ERR_INVALID; }
-    return chain_impl(h, nullptr, 0, in, nullptr, frames, width, height, 3, p, grayscale, d_out, out_step, d_original, original_step,
+    return chain_impl(h, Source::nv12(in, width, height), frames, p, grayscale, ChainDst{d_out, out_step, d_original, original_step},
                       produced, info);
 } catch (...) { return on_exception(h); }
 
@@ -1519,9 +1538,8 @@ extern "C" mc_status mc_chain_compose_device(mc_handle* h, const uint8_t* d_in, 
                                              uint8_t* produced, mc_chain_info* info) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    const ComposeReq c{split, canvas};
-    return chain_impl(h, d_in, in_step, nullptr, nullptr, frames, width, height, channels, p, grayscale, nullptr, 0, nullptr, 0, produced,
-                      info, &c);
+    return chain_impl(h, Source::bgr(d_in, width, height, channels, in_step), frames, p, grayscale,
+                      ChainDst{.cmp = ComposeReq{split, canvas}}, produced, info);
 } catch (...) { return on_exception(h); }
 
 extern "C" mc_status mc_chain_compose_nv12_device(mc_handle* h, const mc_nv12* in, int frames, int width, int height,
@@ -1529,9 +1547,8 @@ extern "C" mc_status mc_chain_compose_nv12_device(mc_handle* h, const mc_nv12* i
                                                   uint8_t* produced, mc_chain_info* info) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    if (!in) { h->err = "NV12 plane is null"; return MC_ERR_INVALID; }
-    const ComposeReq c{split, canvas};
-    return chain_impl(h, nullptr, 0, in, nullptr, frames, width, height, 3, p, grayscale, nullptr, 0, nullptr, 0, produced, info, &c);
+    return chain_impl(h, Source::nv12(in, width, height), frames, p, grayscale, ChainDst{.cmp = ComposeReq{split, canvas}}, produced,
+                      info);
 } catch (...) { return on_exception(h); }
 
 extern "C" mc_status mc_chain_process_yuv422_device(mc_handle* h, const mc_yuv422* in, int frames, int width, int height,
@@ -1540,9 +1557,8 @@ extern "C" mc_status mc_chain_process_yuv422_device(mc_handle* h, const mc_yuv42
                                                     mc_chain_info* info) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    if (!in) { h->err = "YUYV frame is null"; return MC_ERR_INVALID; }
-    return chain_impl(h, nullptr, 0, nullptr, in, frames, width, height, 3, p, grayscale, d_out, out_step, d_original,
-                      original_step, produced, info);
+    return chain_impl(h, Source::yuv422(in, width, height), frames, p, grayscale, ChainDst{d_out, out_step, d_original, original_step},
+                      produced, info);
 } catch (...) { return on_exception(h); }
 
 extern "C" mc_status mc_chain_compose_yuv422_device(mc_handle* h, const mc_yuv422* in, int frames, int width, int height,
@@ -1550,42 +1566,36 @@ extern "C" mc_status mc_chain_compose_yuv422_device(mc_handle* h, const mc_yuv42
                                                     uint8_t* produced, mc_chain_info* info) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    if (!in) { h->err = "YUYV frame is null"; return MC_ERR_INVALID; }
-    const ComposeReq c{split, canvas};
-    return chain_impl(h, nullptr, 0, nullptr, in, frames, width, height, 3, p, grayscale, nullptr, 0, nullptr, 0, produced, info,
-                      &c);
+    return chain_impl(h, Source::yuv422(in, width, height), frames, p, grayscale, ChainDst{.cmp = ComposeReq{split, canvas}},
+                      produced, info);
 } catch (...) { return on_exception(h); }
 
 namespace {
 // The body of the chain submits and of the blocking host chain calls: chain_check on the host frame set, then one slot of
-// the pipeline whose run is chain_run on the slot's buffers.  The processed frames go to `out` (lane k at k * out_h *
-// out_step) and the original tap to `original` (lane k at k * orig_h * original_step).  out_optional: a NULL `out` is
-// not an error; the processed frames are then not downloaded.
-mc_status chain_submit(mc_handle* h, const uint8_t* in, size_t in_step, const mc_nv12* nv, const mc_yuv422* yv, int w, int hh,
-                       int channels, const mc_params* p, int grayscale, uint8_t* out, size_t out_step, uint8_t* original,
-                       size_t original_step, mc_chain_info* info, bool out_optional = false) {
+// the pipeline whose run is chain_run on the slot's buffers.  The processed frames go to d.out (lane k at k * out_h *
+// out_step) and the original tap to d.orig (lane k at k * orig_h * orig_step).  out_optional: a NULL d.out is not an
+// error; the processed frames are then not downloaded.
+mc_status chain_submit(mc_handle* h, const Source& s, const mc_params* p, int grayscale, const ChainDst& d, mc_chain_info* info,
+                       bool out_optional = false) {
+    if (s.missing) { h->err = s.missing; return MC_ERR_INVALID; }
     if ((int)h->inflight.size() >= h->depth) { h->err = "pipeline full: call mc_collect first"; return MC_ERR_INVALID; }
     ChainGeom g;
-    mc_status st = chain_check(h, in, in_step, nv, yv, 1, w, hh, channels, p, grayscale, out || out_optional, out_step,
-                               original != nullptr, original_step, info, nullptr, g);
+    mc_status st = chain_check(h, s, 1, p, grayscale, d, info, g, out_optional);
     if (st != MC_OK) return st;
-    const bool empty = chain_empty(in, nv, yv, w, hh), front = g.front() || yv, tap = (g.pre || yv) && original;
+    const bool empty = s.empty(), front = g.front() || s.converts(), tap = (g.pre || s.converts()) && d.orig;
     Planes src, dst[kOutSets];
     if (!empty) {
-        src = nv ? nv12_planes(*nv, w, hh) : yv ? yuv422_planes(*yv, w, hh) : bgr_planes(in, w, hh, channels, in_step);
-        dst[0] = bgr_planes(out, g.dw, g.dh, g.cc, out_step);
-        if (tap) dst[1] = bgr_planes(original, g.dw, g.dh, channels, original_step);
+        src = s.planes;
+        dst[0] = bgr_planes(d.out, g.dw, g.dh, g.cc, d.out_step);
+        if (tap) dst[1] = bgr_planes(d.orig, g.dw, g.dh, s.channels, d.orig_step);
     }
     // Room for the largest outputs of this frame size (no crop or downscale, no gray), so that a ROI, downscale or grayscale
     // change with frames in flight does not have to grow the slots.
-    const size_t full = empty ? 0 : ((size_t)w * hh * (yv ? 3 : channels) * h->lanes + 255) / 256 * 256;
-    const int order = yv ? yv->order : 0;
+    const size_t full = empty ? 0 : ((size_t)s.w * s.hh * s.channels * h->lanes + 255) / 256 * 256;
     return submit_impl(h, src, dst, [&](const Planes& d_in, const Planes* d_out, int* produced, uint8_t* lane_produced,
                                         std::vector<uint8_t>* written) {
-        const mc_nv12 dnv = nv12_of(d_in);
-        const mc_yuv422 dyv{d_in.base[0], d_in.pitch, d_in.lane_stride, order};
-        const mc_status rs = chain_run(h, g, d_in.base[0], d_in.pitch, nv ? &dnv : nullptr, yv ? &dyv : nullptr, 1, w, hh, channels,
-                                       p, d_out[0].base[0], d_out[0].pitch, d_out[1].base[0], d_out[1].pitch, lane_produced);
+        const ChainDst slot{d_out[0].base[0], d_out[0].pitch, d_out[1].base[0], d_out[1].pitch};
+        const mc_status rs = chain_run(h, g, s.on(d_in), 1, p, slot, lane_produced);
         if (rs != MC_OK) return rs;
         *produced = std::any_of(lane_produced, lane_produced + h->lanes, [](uint8_t x) { return x != 0; });
         for (size_t l = 0; l < (size_t)h->lanes; ++l) {   // what chain_run wrote: see mc_chain_process_device
@@ -1593,34 +1603,33 @@ mc_status chain_submit(mc_handle* h, const uint8_t* in, size_t in_step, const mc
             written[1][l] = tap && !h->hold[l];
         }
         return MC_OK;
-    }, original ? 2 * full : full);
+    }, d.orig ? 2 * full : full);
 }
 
-// The blocking 1-lane host calls: chain_submit + mc_collect into tight buffers.  yuv: the source is the 4:2:2 frame yv,
-// whose conversion always runs, so a buffer too small for its frame is refused before anything runs.  A BGR or gray
-// frame's buffer that turns out too small for what the chain wrote is not downloaded, and the call returns
-// MC_ERR_INVALID once the frame ran.
-mc_status chain_host_call(mc_handle* h, const char* name, const uint8_t* in, size_t in_step, bool yuv, const mc_yuv422* yv, int w,
-                          int hh, int channels, const mc_params* p, int grayscale, uint8_t* out, size_t out_bytes, uint8_t* original,
-                          size_t original_bytes, mc_chain_info* info) {
+// The blocking 1-lane host calls: chain_submit + mc_collect into tight buffers.  A source that converts (4:2:2) always
+// writes both frames, so a buffer too small for its frame is refused before anything runs.  A BGR or gray frame's buffer
+// that turns out too small for what the chain wrote is not downloaded, and the call returns MC_ERR_INVALID once the frame
+// ran.
+mc_status chain_host_call(mc_handle* h, const char* name, const Source& s, const mc_params* p, int grayscale, uint8_t* out,
+                          size_t out_bytes, uint8_t* original, size_t original_bytes, mc_chain_info* info) {
     std::memset(info, 0, sizeof(*info));
     info->cur_is_input = 1; info->orig_is_input = 1;
     if (h->lanes != 1) { h->err = std::string(name) + " needs a 1-lane handle"; return MC_ERR_INVALID; }
     if (!h->inflight.empty()) { h->err = std::string(name) + " called with pipelined frames in flight"; return MC_ERR_INVALID; }
     if (h->hold[0]) { h->err = std::string(name) + " called while lane 0 is held"; return MC_ERR_INVALID; }
-    if (yuv && !yv) { h->err = "YUYV frame is null"; return MC_ERR_INVALID; }
+    if (s.missing) { h->err = s.missing; return MC_ERR_INVALID; }
     ChainGeom g;
-    const bool have = !chain_empty(in, nullptr, yv, w, hh);
-    if (const char* e = chain_geometry(p, have ? w : 0, have ? hh : 0, channels, grayscale, g, info)) {
+    const bool empty = s.empty();
+    if (const char* e = chain_geometry(p, empty ? 0 : s.w, empty ? 0 : s.hh, s.channels, grayscale, g, info)) {
         h->err = e;
         return MC_ERR_INVALID;
     }
-    const size_t out_frame = (size_t)g.dw * g.dh * g.cc, orig_frame = (size_t)g.dw * g.dh * channels;
+    const size_t out_frame = (size_t)g.dw * g.dh * g.cc, orig_frame = (size_t)g.dw * g.dh * s.channels;
     const bool out_fits = out && out_bytes >= out_frame, orig_fits = original && original_bytes >= orig_frame;
-    if (yuv && out && !out_fits) { h->err = "out buffer too small"; return MC_ERR_INVALID; }
-    if (yuv && original && !orig_fits) { h->err = "original buffer too small"; return MC_ERR_INVALID; }
-    mc_status st = chain_submit(h, in, in_step, nullptr, yv, w, hh, channels, p, grayscale, out_fits ? out : nullptr,
-                                (size_t)g.dw * g.cc, orig_fits ? original : nullptr, (size_t)g.dw * channels, info, true);
+    if (s.converts() && out && !out_fits) { h->err = "out buffer too small"; return MC_ERR_INVALID; }
+    if (s.converts() && original && !orig_fits) { h->err = "original buffer too small"; return MC_ERR_INVALID; }
+    const ChainDst tight{out_fits ? out : nullptr, (size_t)g.dw * g.cc, orig_fits ? original : nullptr, (size_t)g.dw * s.channels};
+    mc_status st = chain_submit(h, s, p, grayscale, tight, info, true);
     if (st != MC_OK) return st;
     int produced = 0;
     if ((st = mc_collect(h, &produced)) != MC_OK) return st;
@@ -1640,7 +1649,7 @@ extern "C" mc_status mc_chain_process(mc_handle* h, const uint8_t* in, int width
                                       size_t original_bytes, mc_chain_info* info) try {
     if (!h || !p || !info) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    return chain_host_call(h, "mc_chain_process", in, in_step, false, nullptr, width, height, channels, p, grayscale, out, out_bytes,
+    return chain_host_call(h, "mc_chain_process", Source::bgr(in, width, height, channels, in_step), p, grayscale, out, out_bytes,
                            original, original_bytes, info);
 } catch (...) { return on_exception(h); }
 
@@ -1651,8 +1660,8 @@ extern "C" mc_status mc_chain_process_yuv422(mc_handle* h, const mc_yuv422* in, 
                                              size_t original_bytes, mc_chain_info* info) try {
     if (!h || !p || !info) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    return chain_host_call(h, "mc_chain_process_yuv422", nullptr, 0, true, in, width, height, 3, p, grayscale, out, out_bytes,
-                           original, original_bytes, info);
+    return chain_host_call(h, "mc_chain_process_yuv422", Source::yuv422(in, width, height), p, grayscale, out, out_bytes, original,
+                           original_bytes, info);
 } catch (...) { return on_exception(h); }
 
 // The pipelined host chain: one frame of every lane per submit, collected by mc_collect in submit order with mc_submit and
@@ -1662,8 +1671,8 @@ extern "C" mc_status mc_chain_submit(mc_handle* h, const uint8_t* in, int width,
                                      size_t original_step, mc_chain_info* info) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    return chain_submit(h, in, in_step, nullptr, nullptr, width, height, channels, p, grayscale, out, out_step, original,
-                        original_step, info);
+    return chain_submit(h, Source::bgr(in, width, height, channels, in_step), p, grayscale,
+                        ChainDst{out, out_step, original, original_step}, info);
 } catch (...) { return on_exception(h); }
 
 extern "C" mc_status mc_chain_submit_nv12(mc_handle* h, const mc_nv12* in, int width, int height, const mc_params* p, int grayscale,
@@ -1671,8 +1680,7 @@ extern "C" mc_status mc_chain_submit_nv12(mc_handle* h, const mc_nv12* in, int w
                                           mc_chain_info* info) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    if (!in) { h->err = "NV12 plane is null"; return MC_ERR_INVALID; }
-    return chain_submit(h, nullptr, 0, in, nullptr, width, height, 3, p, grayscale, out, out_step, original, original_step, info);
+    return chain_submit(h, Source::nv12(in, width, height), p, grayscale, ChainDst{out, out_step, original, original_step}, info);
 } catch (...) { return on_exception(h); }
 
 extern "C" mc_status mc_chain_submit_yuv422(mc_handle* h, const mc_yuv422* in, int width, int height, const mc_params* p,
@@ -1680,8 +1688,7 @@ extern "C" mc_status mc_chain_submit_yuv422(mc_handle* h, const mc_yuv422* in, i
                                             mc_chain_info* info) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    if (!in) { h->err = "YUYV frame is null"; return MC_ERR_INVALID; }
-    return chain_submit(h, nullptr, 0, nullptr, in, width, height, 3, p, grayscale, out, out_step, original, original_step, info);
+    return chain_submit(h, Source::yuv422(in, width, height), p, grayscale, ChainDst{out, out_step, original, original_step}, info);
 } catch (...) { return on_exception(h); }
 
 // ---- the export canvas from host clips: compose submits, collected by mc_collect -----------------------------------------
@@ -1697,43 +1704,37 @@ Planes canvas_planes(const mc_canvas& c, int cw, int ch) {
 // kernel writes the canvases into the slot's own output, never into handle scratch that the next submit reuses, and the
 // canvases of the lanes that are not held come back from there.  `produced` (frames * lanes) is written by the mc_collect
 // of this submit.
-mc_status compose_submit(mc_handle* h, const uint8_t* in, size_t in_step, const mc_nv12* nv, const mc_yuv422* yv, int frames,
-                         int w, int hh, int channels, const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+mc_status compose_submit(mc_handle* h, const Source& s, int frames, const mc_params* p, int grayscale, const ComposeReq& cmp,
                          uint8_t* produced, mc_chain_info* info) {
+    if (s.missing) { h->err = s.missing; return MC_ERR_INVALID; }
     if ((int)h->inflight.size() >= h->depth) { h->err = "pipeline full: call mc_collect first"; return MC_ERR_INVALID; }
     mc_status st = check_clip(h, frames, produced, true);
     if (st != MC_OK) return st;
-    const ComposeReq cmp{split, canvas};
     ChainGeom g;
-    if ((st = chain_check(h, in, in_step, nv, yv, frames, w, hh, channels, p, grayscale, false, 0, false, 0, info, &cmp, g)) != MC_OK)
-        return st;
-    const bool empty = chain_empty(in, nv, yv, w, hh);
+    if ((st = chain_check(h, s, frames, p, grayscale, ChainDst{.cmp = cmp}, info, g)) != MC_OK) return st;
+    const bool empty = s.empty();
     // the device call's magnifier refuses Color lanes with different parameters only once its front ran: here, before any copy
     if (!empty && calculate_max_levels(g.dw, g.dh) >= 1 && (st = lane_params_check(h, *p)) != MC_OK) return st;
     int cw, ch;
-    canvas_size(g, split, cw, ch);
+    canvas_size(g, cmp.split, cw, ch);
     Planes src, dst[kOutSets];
     if (!empty) {
-        src = nv ? nv12_planes(*nv, w, hh) : yv ? yuv422_planes(*yv, w, hh) : bgr_planes(in, w, hh, channels, in_step);
-        if (cw > 0) dst[0] = canvas_planes(*canvas, cw, ch);
+        src = s.planes;
+        if (cw > 0) dst[0] = canvas_planes(*cmp.canvas, cw, ch);
     }
     // Room for the canvases of this frame size without a crop or downscale, so that a ROI or downscale change with clips in
     // flight does not have to grow the slots; a shorter clip fits in a longer one's.
     ChainGeom full;
-    full.dw = empty ? 0 : w; full.dh = empty ? 0 : hh;
+    full.dw = empty ? 0 : s.w; full.dh = empty ? 0 : s.hh;
     int fw, fh;
-    canvas_size(full, split, fw, fh);
-    const size_t reserve = ((size_t)fw * fh * (canvas->format == MC_CANVAS_NV12 ? 3 : 6) / 2 * frames * h->lanes + 255) / 256 * 256;
-    const int order = yv ? yv->order : 0;
+    canvas_size(full, cmp.split, fw, fh);
+    const size_t reserve =
+        ((size_t)fw * fh * (cmp.canvas->format == MC_CANVAS_NV12 ? 3 : 6) / 2 * frames * h->lanes + 255) / 256 * 256;
     const size_t lanes = (size_t)h->lanes, vl = (size_t)frames * lanes;
     return submit_impl(h, src, dst, [&](const Planes& d_in, const Planes* d_out, int* any, uint8_t* flags,
                                         std::vector<uint8_t>* written) {
-        const mc_nv12 dnv = nv12_of(d_in);
-        const mc_yuv422 dyv{d_in.base[0], d_in.pitch, d_in.lane_stride, order};
-        const mc_canvas dcv{canvas->format, d_out[0].base[0], d_out[0].base[1], d_out[0].pitch, d_out[0].lane_stride};
-        const ComposeReq dcmp{split, &dcv};
-        const mc_status rs = chain_run(h, g, d_in.base[0], d_in.pitch, nv ? &dnv : nullptr, yv ? &dyv : nullptr, frames, w, hh,
-                                       channels, p, nullptr, 0, nullptr, 0, flags, &dcmp);
+        const mc_canvas slot{cmp.canvas->format, d_out[0].base[0], d_out[0].base[1], d_out[0].pitch, d_out[0].lane_stride};
+        const mc_status rs = chain_run(h, g, s.on(d_in), frames, p, ChainDst{.cmp = ComposeReq{cmp.split, &slot}}, flags);
         if (rs != MC_OK) return rs;
         *any = std::any_of(flags, flags + vl, [](uint8_t x) { return x != 0; });
         for (size_t v = 0; v < vl; ++v) written[0][v] = cw > 0 && !h->hold[v % lanes];   // what the compose kernel wrote
@@ -1749,8 +1750,8 @@ extern "C" mc_status mc_chain_compose_submit(mc_handle* h, const uint8_t* in, in
                                              uint8_t* produced, mc_chain_info* info) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    return compose_submit(h, in, in_step, nullptr, nullptr, frames, width, height, channels, p, grayscale, split, canvas, produced,
-                          info);
+    return compose_submit(h, Source::bgr(in, width, height, channels, in_step), frames, p, grayscale, ComposeReq{split, canvas},
+                          produced, info);
 } catch (...) { return on_exception(h); }
 
 extern "C" mc_status mc_chain_compose_submit_nv12(mc_handle* h, const mc_nv12* in, int frames, int width, int height,
@@ -1758,8 +1759,7 @@ extern "C" mc_status mc_chain_compose_submit_nv12(mc_handle* h, const mc_nv12* i
                                                   uint8_t* produced, mc_chain_info* info) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    if (!in) { h->err = "NV12 plane is null"; return MC_ERR_INVALID; }
-    return compose_submit(h, nullptr, 0, in, nullptr, frames, width, height, 3, p, grayscale, split, canvas, produced, info);
+    return compose_submit(h, Source::nv12(in, width, height), frames, p, grayscale, ComposeReq{split, canvas}, produced, info);
 } catch (...) { return on_exception(h); }
 
 extern "C" mc_status mc_chain_compose_submit_yuv422(mc_handle* h, const mc_yuv422* in, int frames, int width, int height,
@@ -1767,8 +1767,7 @@ extern "C" mc_status mc_chain_compose_submit_yuv422(mc_handle* h, const mc_yuv42
                                                     uint8_t* produced, mc_chain_info* info) try {
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
-    if (!in) { h->err = "YUYV frame is null"; return MC_ERR_INVALID; }
-    return compose_submit(h, nullptr, 0, nullptr, in, frames, width, height, 3, p, grayscale, split, canvas, produced, info);
+    return compose_submit(h, Source::yuv422(in, width, height), frames, p, grayscale, ComposeReq{split, canvas}, produced, info);
 } catch (...) { return on_exception(h); }
 
 /* test hooks, not declared in the public header: the two conversion kernels alone on device buffers (default stream,
