@@ -157,6 +157,48 @@ typedef struct mc_lane_params {
  * MC_ERR_INVALID for a NULL handle or a lane out of range. */
 mc_status mc_set_lane_params(mc_handle* h, int lane, const mc_lane_params* lp);
 
+/* --- lane state: save one lane's temporal state as host bytes, and load it into a lane of any handle ------------------
+ * A running stream moves (to another lane, handle, GPU, process or a file) without the visible restart of its temporal
+ * filters: save its lane on the source, load the blob into the destination lane, then restart or hold the source lane.
+ *   Equivalence: lane k of handle A is saved after some call, and the blob is loaded into lane j of handle B (any lane
+ *     count, the same or another device, or A itself).  Fed lane k's next frames with the same effective parameters,
+ *     through any mix of frame, clip, chain, compose, NV12, 4:2:2 and submit calls, lane j then gives, bit for bit, what
+ *     lane k would have given: the output bytes, the produced flags, mc_lane_produced and the temporal state afterwards.
+ *     B's other lanes equal, bit for bit, those of a twin of B without the load, and A those of a twin of A without the
+ *     save: a save only reads.
+ *   What travels: temporal state only.  The lane's "has state" bit: a lane without state saves a valid blob (without
+ *     planes), and loading it is mc_restart_lane.  Laplace: hi / lo of every kept level (levels 0 and `levels` too with
+ *     faithful_level0), and whether the state is bounded (a loaded unbounded state turns L-only synthesis off for B,
+ *     DESIGN.md §4).  Phase: the 13 planes of every band level (those mc_get_state names) and the lane's filter design:
+ *     its cutoffs, the framerate it was designed at and its coefficients, so a lane designed at 25 fps keeps that design
+ *     in a handle whose other lanes run at 30 fps.  Color: the window's length, the physical slot of its oldest column,
+ *     its ring size and its slots as they lie (not rotated into logical order: the filter's rounding follows the slots).
+ *   What stays: configuration belongs to the destination lane: its hold, its mc_set_lane_params override and the handle's
+ *     overlay and options.  Move an override yourself.  The read-only taps ("gauss", "lab16", "oct", "window", ...)
+ *     describe the last frame call and are not changed by a load.  A held lane stays held and runs from the loaded state
+ *     when it is released.
+ *   Key: the blob records the structural key (mode, clamped levels, width, height, channels, the preprocess fingerprint)
+ *     and, for Laplace, faithful_level0.  If B holds state (after a frame call of some mode), the blob's key must be its
+ *     key; if it holds none (new, after mc_reset, a structural reset, mode None or a failed frame), the load takes the
+ *     blob's key and allocates the mode's state as a frame call with that key would: every other lane has no state.  A
+ *     later frame call with another key resets structurally, as always.
+ *   Blocking: a save waits for the work enqueued on the handle, and a load has finished when it returns (src may be freed).
+ *     Pageable buffers go through the handle's pinned staging (grow-only: the largest blob's planes); pinned ones are
+ *     copied directly.
+ *   Blob: opaque, stable within a blob version: a header (magic, version, total size, key, the mode's scalars), then the
+ *     planes as dense rows.  Saving right after a load gives the same bytes.  1080p colour: Laplace at 6 levels 16.6 MB,
+ *     Phase at 6 levels 143.6 MB, Color at 3 levels with a 64-slot window 24.9 MB.
+ *   Errors, with no state, flag or configuration changed: MC_ERR_INVALID for a NULL handle, `bytes` or src; a lane out of
+ *     range; cap smaller than the blob; a blob that is truncated (`bytes` is not its size) or of another magic or version;
+ *     a key or faithful_level0 that differs from B's; submitted frames in flight.  MC_ERR_UNSUPPORTED for a load into a
+ *     Color handle (or of a Color blob) with lanes > 1 without option "color_lane_lifecycle".  A CUDA failure while the
+ *     planes are copied in drops B's state, as a failed frame does. */
+/* Save lane `lane`'s temporal state into dst (host memory, pinned or pageable).  dst == NULL: only *bytes is set, to
+ * the size needed.  Otherwise cap must be >= that size; *bytes receives the bytes written. */
+mc_status mc_save_lane(mc_handle* h, int lane, void* dst, size_t cap, size_t* bytes);
+/* Make lane `lane`'s temporal state the one saved in src (host memory, `bytes` long).  The other lanes are untouched. */
+mc_status mc_load_lane(mc_handle* h, int lane, const void* src, size_t bytes);
+
 /* Per-lane produced flags (n == lanes) of the frame most recently returned by mc_process / mc_process_device /
  * mc_chain_process, or collected by mc_collect.  The `*produced` of those calls is "at least one lane produced", and
  * a lane's bytes of `out` are written only when its flag is 1.  MC_ERR_INVALID if n != lanes. */

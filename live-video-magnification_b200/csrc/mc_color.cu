@@ -325,6 +325,101 @@ void ColorMode::reset() {
     tap_frame = -1;
 }
 
+mc_status ColorMode::allocate(const ModeCtx& ctx, int width, int height, int nchannels, int nlevels) {
+    reset();
+    levels = nlevels; channels = nchannels; w = width; h = height;
+    const int planes = lanes * channels;
+    lv.resize((size_t)levels + 1);
+    int cw = w, ch = h;
+    for (int l = 0; l <= levels; ++l) {
+        lv[(size_t)l] = make_level(cw, ch);
+        cw = (cw + 1) / 2; ch = (ch + 1) / 2;
+    }
+    G.assign((size_t)levels + 1, nullptr);
+    for (int l = 0; l <= levels; ++l) MCK(arena.alloc(&G[(size_t)l], (size_t)planes * lv[(size_t)l].plane));
+    const Level& ls = lv[(size_t)levels];
+    small_rows = ls.w * ls.h;
+    ulv.resize((size_t)levels + 1);
+    U.assign((size_t)levels + 2, nullptr);
+    int uw = ls.w, uh = ls.h;
+    for (int i = 0; i <= levels; ++i) {
+        ulv[(size_t)i] = make_level(uw, uh);
+        MCK(arena.alloc(&U[(size_t)i], (size_t)planes * ulv[(size_t)i].plane));
+        uw *= 2; uh *= 2;
+    }
+    if (ulv[(size_t)levels].w != w || ulv[(size_t)levels].h != h)
+        MCK(arena.alloc(&U[(size_t)levels + 1], (size_t)planes * lv[0].plane));
+    void* mmv = nullptr;
+    MCK(arena.alloc_bytes(&mmv, sizeof(unsigned) * 4 * (size_t)lanes));
+    minmax = (float*)mmv;
+    void* tv = nullptr;
+    MCK(arena.alloc_bytes(&tv, sizeof(ColorLane) * (size_t)lanes));
+    d_table = (ColorLane*)tv;
+    count.assign((size_t)lanes, 0); head.assign((size_t)lanes, 0); mod.assign((size_t)lanes, 0);
+    table.assign((size_t)lanes, ColorLane{});
+    allocated = true;
+    return MC_OK;
+}
+
+// Grows the ring to `need` slots (grow) or swaps it with `work` (a rotation); with `relayout`, lane k's slot t < copy_n
+// of the new ring takes slot (src_head + t) % src_mod of the old one (d_rows[k], on the device).
+mc_status ColorMode::reshape_ring(const ModeCtx& ctx, int need, bool grow, bool relayout, const ColorLane* d_rows) {
+    const size_t S = slot_signals();
+    float* dst = work;
+    float* nwork = nullptr;
+    void* nspec = nullptr;
+    if (grow) {
+        MCK(arena.alloc(&dst, (size_t)need * S));
+        MCK(arena.alloc(&nwork, (size_t)need * S));
+        MCK(arena.alloc_bytes(&nspec, sizeof(cufftComplex) * (size_t)(need / 2 + 1) * S));
+    }
+    if (relayout) {
+        const bool pp = ctx.prof && ctx.prof->begin("ring_relayout", 0, ctx.stream);
+        k_ring_relayout<<<dim3(gs_blocks(lane_sig()), (unsigned)lanes), 256, 0, ctx.stream>>>(ring, dst, S, lane_sig(), lane_stride(), d_rows);
+        if (pp) ctx.prof->end(ctx.stream);
+        MCK(cudaGetLastError());
+        ++*ctx.launches;
+    }
+    if (grow) {
+        if (ring) {   // cudaFree orders itself after the relayout above (it synchronises the device)
+            // the "filtered" tap of the last frame moves along (a load grows the ring between frames)
+            MCK(cudaMemcpyAsync(nwork, work, (size_t)ring_cap * S * sizeof(float), cudaMemcpyDeviceToDevice, ctx.stream));
+            arena.free_block(ring); arena.free_block(work); arena.free_block(spec);
+        }
+        ring = dst; work = nwork; spec = (cufftComplex*)nspec;
+        ring_cap = need;
+    } else {
+        std::swap(ring, work);
+    }
+    return MC_OK;
+}
+
+// A load (mc_load_lane) whose window is longer than the ring: the ring grows as process() grows it, and every lane's
+// window is copied to the slots it occupies (source slot t -> slot t), so each lane keeps its physical layout.
+mc_status ColorMode::reserve_ring(const ModeCtx& ctx, int need) {
+    need = std::max(need, 2);
+    if (ring && ring_cap >= need) return MC_OK;
+    bool has_data = false;
+    std::vector<ColorLane> rows((size_t)lanes, ColorLane{});
+    for (int k = 0; k < lanes; ++k) {
+        need = std::max(need, mod[(size_t)k]);
+        rows[(size_t)k].src_head = 0;
+        rows[(size_t)k].src_mod = std::max(mod[(size_t)k], 1);
+        rows[(size_t)k].copy_n = count[(size_t)k];   // head == 0 or count == mod: slots 0 .. count-1 hold the window
+        has_data |= count[(size_t)k] > 0;
+    }
+    // pageable source: staged before the call returns; the kernels of every earlier frame that read d_table precede it
+    if (has_data) MCK(cudaMemcpyAsync(d_table, rows.data(), sizeof(ColorLane) * (size_t)lanes, cudaMemcpyHostToDevice, ctx.stream));
+    return reshape_ring(ctx, need, true, has_data, d_table);
+}
+
+void ColorMode::lane_planes(int lane, int lane_mod, std::vector<LanePlane>& out) const {
+    out.clear();
+    if (!allocated || lane_mod <= 0) return;
+    // slot t of the lane is its block at t * S + lane * lstride: one 2D block of lane_mod rows
+    out.push_back(LanePlane{ring + (size_t)lane * lane_stride(), slot_signals() * sizeof(float), lane_sig() * sizeof(float), (size_t)lane_mod});
+}
+
 // Grows the clip scratch to `vl` virtual lanes and `work_floats` floats of filtered windows.  The float tap is written in
 // place by the last frame's egress, so the scratch holds none.
 mc_status ColorMode::alloc_clip(const ModeCtx& ctx, int vl, size_t work_floats) {
@@ -598,50 +693,11 @@ mc_status ColorMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_par
     want_cap.resize((size_t)lanes);
     for (int k = 0; k < lanes; ++k)   // MagnifyCore.hpp:176, from each lane's own frame rate
         want_cap[(size_t)k] = optimal_buffer_size((int)(ctx.lane_params ? ctx.lane_params[k] : p).framerate);
-    const int C = io.channels;
-    const int planes = lanes * C;
-    if (!allocated) {
-        reset();
-        levels = nlevels; channels = C; w = io.w; h = io.h;
-        lv.resize((size_t)levels + 1);
-        int cw = w, ch = h;
-        for (int l = 0; l <= levels; ++l) {
-            lv[(size_t)l] = make_level(cw, ch);
-            cw = (cw + 1) / 2; ch = (ch + 1) / 2;
-        }
-        G.assign((size_t)levels + 1, nullptr);
-        for (int l = 0; l <= levels; ++l) MCK(arena.alloc(&G[(size_t)l], (size_t)planes * lv[(size_t)l].plane));
-        const Level& ls = lv[(size_t)levels];
-        small_rows = ls.w * ls.h;
-        ulv.resize((size_t)levels + 1);
-        U.assign((size_t)levels + 2, nullptr);
-        int uw = ls.w, uh = ls.h;
-        for (int i = 0; i <= levels; ++i) {
-            ulv[(size_t)i] = make_level(uw, uh);
-            MCK(arena.alloc(&U[(size_t)i], (size_t)planes * ulv[(size_t)i].plane));
-            uw *= 2; uh *= 2;
-        }
-        if (ulv[(size_t)levels].w != w || ulv[(size_t)levels].h != h)
-            MCK(arena.alloc(&U[(size_t)levels + 1], (size_t)planes * lv[0].plane));
-        void* mmv = nullptr;
-        MCK(arena.alloc_bytes(&mmv, sizeof(unsigned) * 4 * (size_t)lanes));
-        minmax = (float*)mmv;
-        void* tv = nullptr;
-        MCK(arena.alloc_bytes(&tv, sizeof(ColorLane) * (size_t)lanes));
-        d_table = (ColorLane*)tv;
-        count.assign((size_t)lanes, 0); head.assign((size_t)lanes, 0); mod.assign((size_t)lanes, 0);
-        table.assign((size_t)lanes, ColorLane{});
-        allocated = true;
-    }
+    const int planes = lanes * io.channels;
+    if (!allocated) MCK_ST(allocate(ctx, io.w, io.h, io.channels, nlevels));
     plan.make(ctx.lane_ops, lanes, false);
     if (plan.n_hold == lanes) return MC_OK;   // nothing to append, nothing produced
-    // One lane's block of a slot is lane_sig signals (pixels x channels).  cuFFT takes a lane's block as the base pointer
-    // of a one-lane transform, which must be 8-byte aligned: on a multi-lane handle an odd block is followed by one
-    // padding signal.
-    const size_t lane_sig = (size_t)C * small_rows;
-    const int pad = lanes > 1 ? (int)(lane_sig & 1) : 0;
-    const size_t lstride = lane_sig + pad;
-    const size_t S = (size_t)lanes * lstride;            // signals of a slot
+    const size_t S = slot_signals();
 
     // Ring geometry, lane by lane.  A lane's `mod` is its LOGICAL ring size (its slots are taken modulo it), `ring_cap`
     // the allocation.  It follows the window cap the frame rate asks for; when that changes (rare: a UI action) the
@@ -693,32 +749,7 @@ mc_status ColorMode::process(const ModeCtx& ctx, const FrameIO& io, const mc_par
     if (frames > 1 || relayout || !s1.uniform)
         MCK(cudaMemcpyAsync(dtab, rows, sizeof(ColorLane) * (size_t)vl, cudaMemcpyHostToDevice, ctx.stream));
 
-    if (grow || rotate) {
-        float* dst = work;
-        float* nwork = nullptr;
-        void* nspec = nullptr;
-        if (grow) {
-            MCK(arena.alloc(&dst, (size_t)need * S));
-            MCK(arena.alloc(&nwork, (size_t)need * S));
-            MCK(arena.alloc_bytes(&nspec, sizeof(cufftComplex) * (size_t)(need / 2 + 1) * S));
-        }
-        if (relayout) {
-            const bool pp = ctx.prof && ctx.prof->begin("ring_relayout", 0, ctx.stream);
-            k_ring_relayout<<<dim3(gs_blocks(lane_sig), (unsigned)lanes), 256, 0, ctx.stream>>>(ring, dst, S, lane_sig, lstride, dtab);
-            if (pp) ctx.prof->end(ctx.stream);
-            MCK(cudaGetLastError());
-            ++*ctx.launches;
-        }
-        if (grow) {
-            if (ring) {   // cudaFree orders itself after the relayout above (it synchronises the device)
-                arena.free_block(ring); arena.free_block(work); arena.free_block(spec);
-            }
-            ring = dst; work = nwork; spec = (cufftComplex*)nspec;
-            ring_cap = need;
-        } else {
-            std::swap(ring, work);
-        }
-    }
+    if (grow || rotate) MCK_ST(reshape_ring(ctx, need, grow, relayout, dtab));
 
     if (frames == 1) {
         tap_frame = -1;

@@ -228,6 +228,8 @@ struct mc_handle {
     int n_lane_lp = 0;
     std::vector<mc_params> lane_eff;
     std::vector<uint8_t> lane_lost;   // per frame call: lanes whose state the mode dropped
+    // mc_save_lane / mc_load_lane: pinned staging of a blob's planes when the caller's buffer is pageable (grow-only)
+    PinnedBuffer lane_stage;
 };
 
 namespace {
@@ -588,6 +590,63 @@ mc_status submit_impl(mc_handle* h, const Planes& in, const Planes (&out)[kOutSe
     return MC_OK;
 }
 
+// ---- lane state blobs (mc_save_lane / mc_load_lane) ----------------------------------------------------------------
+constexpr char kBlobMagic[8] = {'M', 'C', 'L', 'A', 'N', 'E', 0, 0};
+constexpr uint32_t kBlobVersion = 1;
+// A blob's header.  The lane's state planes follow it, in the order the mode lists them (lane_planes), as dense rows.
+struct LaneBlob {
+    char magic[8];
+    uint32_t version;
+    uint32_t has_state;   // the lane's "has state" bit; a blob without state has no planes
+    uint64_t bytes;       // the whole blob: header + planes
+    // the structural key (tracker_changes) and, for Laplace, faithful_level0
+    int32_t mode, levels, w, h, channels, pre_down, pre_roi, faithful;
+    float roi[4];
+    int32_t ab_bounded;   // Laplace: the handle's ab_bounded (L-only synthesis, DESIGN §4)
+    int32_t count, head, mod;   // Color: the lane's window
+    double design[15];    // Phase: the lane's RieszMode::Design (lo_freq, hi_freq, framerate, loA, loB, hiA, hiB)
+};
+static_assert(sizeof(LaneBlob) == 208, "no padding: every byte of a header is defined");
+static_assert(sizeof(RieszMode::Design) == sizeof(LaneBlob::design), "Design is 15 doubles");
+
+mc_params blob_key(const LaneBlob& b) {
+    mc_params p{};
+    p.mode = b.mode; p.pre_downscale = b.pre_down; p.pre_roiEnabled = b.pre_roi;
+    p.pre_roiX = b.roi[0]; p.pre_roiY = b.roi[1]; p.pre_roiW = b.roi[2]; p.pre_roiH = b.roi[3];
+    return p;
+}
+
+// Lane `lane`'s state planes for the blob's mode (Color: a window of the blob's length) -> their bytes
+size_t lane_planes(mc_handle* h, const LaneBlob& b, int lane, std::vector<LanePlane>& out) {
+    out.clear();
+    if (b.has_state) {
+        if (b.mode == MC_MODE_LAPLACE) h->motion.lane_planes(lane, out);
+        else if (b.mode == MC_MODE_PHASE) h->riesz.lane_planes(lane, out);
+        else if (b.mode == MC_MODE_COLOR) h->color.lane_planes(lane, b.mod, out);
+    }
+    size_t total = 0;
+    for (const LanePlane& p : out) total += p.row_bytes * p.rows;
+    return total;
+}
+
+// The planes between the device and `host` (the blob's plane bytes, dense) on the handle's stream, through the pinned
+// staging when `host` is pageable; complete when it returns.
+mc_status copy_lane_planes(mc_handle* h, const std::vector<LanePlane>& planes, size_t total, uint8_t* host, bool save) {
+    const bool pinned = is_pinned(host);
+    if (!pinned) CK(h->lane_stage.grow(total));
+    uint8_t* base = pinned ? host : h->lane_stage.p;
+    if (!pinned && !save) std::memcpy(base, host, total);
+    size_t ofs = 0;
+    for (const LanePlane& p : planes) {
+        if (save) CK(cudaMemcpy2DAsync(base + ofs, p.row_bytes, p.ptr, p.pitch, p.row_bytes, p.rows, cudaMemcpyDeviceToHost, h->stream));
+        else CK(cudaMemcpy2DAsync(p.ptr, p.pitch, base + ofs, p.row_bytes, p.row_bytes, p.rows, cudaMemcpyHostToDevice, h->stream));
+        ofs += p.row_bytes * p.rows;
+    }
+    CK(cudaStreamSynchronize(h->stream));
+    if (!pinned && save) std::memcpy(host, base, total);
+    return MC_OK;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -781,6 +840,131 @@ mc_status mc_set_lane_params(mc_handle* h, int lane, const mc_lane_params* lp) t
     h->n_lane_lp += (lp != nullptr) - (h->lane_lp_set[(size_t)lane] != 0);
     h->lane_lp_set[(size_t)lane] = lp != nullptr;
     if (lp) h->lane_lp[(size_t)lane] = *lp;   // taken into the next frame call; frames in flight are not affected
+    return MC_OK;
+} catch (...) { return on_exception(h); }
+
+mc_status mc_save_lane(mc_handle* h, int lane, void* dst, size_t cap, size_t* bytes) try {
+    if (!h || !bytes) return MC_ERR_INVALID;
+    if (lane < 0 || lane >= h->lanes) { h->err = "lane out of range"; return MC_ERR_INVALID; }
+    if (!h->inflight.empty()) { h->err = "mc_save_lane with pipelined frames in flight"; return MC_ERR_INVALID; }
+    CK(cudaSetDevice(h->device));
+    LaneBlob b;
+    std::memset(&b, 0, sizeof(b));
+    std::memcpy(b.magic, kBlobMagic, sizeof(b.magic));
+    b.version = kBlobVersion;
+    b.has_state = h->has_state[(size_t)lane] != 0;
+    b.mode = h->t_mode; b.levels = h->t_levels; b.w = h->t_w; b.h = h->t_h; b.channels = h->t_channels;
+    b.pre_down = h->t_down; b.pre_roi = h->t_roi;
+    b.roi[0] = h->t_rx; b.roi[1] = h->t_ry; b.roi[2] = h->t_rw; b.roi[3] = h->t_rh;
+    if (b.has_state) {
+        if (b.mode == MC_MODE_LAPLACE) {
+            b.faithful = h->motion.faithful;
+            b.ab_bounded = h->motion.ab_bounded;
+        } else if (b.mode == MC_MODE_COLOR) {
+            b.count = h->color.count[(size_t)lane]; b.head = h->color.head[(size_t)lane]; b.mod = h->color.mod[(size_t)lane];
+        } else if (b.mode == MC_MODE_PHASE && h->riesz.allocated) {
+            std::memcpy(b.design, &h->riesz.design[(size_t)lane], sizeof(b.design));
+        }
+    }
+    std::vector<LanePlane> planes;
+    const size_t total = lane_planes(h, b, lane, planes);
+    b.bytes = sizeof(b) + total;
+    *bytes = b.bytes;
+    if (!dst) return MC_OK;
+    if (cap < b.bytes) { h->err = "mc_save_lane: cap is smaller than the blob"; return MC_ERR_INVALID; }
+    std::memcpy(dst, &b, sizeof(b));
+    return copy_lane_planes(h, planes, total, (uint8_t*)dst + sizeof(b), true);
+} catch (...) { return on_exception(h); }
+
+mc_status mc_load_lane(mc_handle* h, int lane, const void* src, size_t bytes) try {
+    if (!h || !src) return MC_ERR_INVALID;
+    if (lane < 0 || lane >= h->lanes) { h->err = "lane out of range"; return MC_ERR_INVALID; }
+    if (!h->inflight.empty()) { h->err = "mc_load_lane with pipelined frames in flight"; return MC_ERR_INVALID; }
+    LaneBlob b;
+    if (bytes < sizeof(b)) { h->err = "lane blob truncated"; return MC_ERR_INVALID; }
+    std::memcpy(&b, src, sizeof(b));
+    if (std::memcmp(b.magic, kBlobMagic, sizeof(b.magic)) != 0 || b.version != kBlobVersion) {
+        h->err = "not a lane blob of this version";
+        return MC_ERR_INVALID;
+    }
+    if (b.bytes != bytes) { h->err = "lane blob size differs from its header (truncated?)"; return MC_ERR_INVALID; }
+    // the rule of single-lane restarts (color_lane_check), for the mode the lane has after the load
+    auto color_refused = [&](int mode) {
+        if (mode != MC_MODE_COLOR || h->lanes == 1 || h->opt.color_lane_lifecycle) return false;
+        h->err = "Color mode loads one lane of a multi-lane handle only with option color_lane_lifecycle";
+        return true;
+    };
+    CK(cudaSetDevice(h->device));
+    if (!b.has_state) return color_refused(h->t_mode) ? MC_ERR_UNSUPPORTED : mc_restart_lane(h, lane);
+    const bool mode_ok = b.mode == MC_MODE_LAPLACE || b.mode == MC_MODE_PHASE || b.mode == MC_MODE_COLOR;
+    if (!mode_ok || (b.channels != 1 && b.channels != 3) || b.w <= 0 || b.h <= 0 || b.levels < 1 ||
+        b.levels > calculate_max_levels(b.w, b.h) ||
+        (b.mode == MC_MODE_COLOR && (b.mod < 2 || b.count < 1 || b.count > b.mod || b.head < 0 || b.head >= b.mod ||
+                                     (b.head != 0 && b.count != b.mod)))) {
+        h->err = "lane blob: bad key or window";
+        return MC_ERR_INVALID;
+    }
+    const mc_params key = blob_key(b);
+    const bool fresh = h->t_mode == MC_MODE_NONE;   // the handle holds no state: the load takes the blob's key
+    if (!fresh && tracker_changes(h, &key, b.levels, b.channels, b.w, b.h)) {
+        h->err = "lane blob: its key (mode, levels, size, channels, preprocess) differs from the handle's state";
+        return MC_ERR_INVALID;
+    }
+    if (b.mode == MC_MODE_LAPLACE && ((b.faithful != 0) != h->opt.faithful_level0 ||
+                                      (h->motion.allocated && h->motion.faithful != (b.faithful != 0)))) {
+        h->err = "lane blob: faithful_level0 differs from the handle's";
+        return MC_ERR_INVALID;
+    }
+    if (color_refused(b.mode)) return MC_ERR_UNSUPPORTED;
+    Options opt = h->opt;
+    if (opt.profile_kernels) opt.lane_groups = 1;
+    const ModeCtx ctx{.stream = h->stream, .tables = &h->tables, .launches = &h->launches, .err = &h->err, .opt = opt,
+                      .float_out = nullptr, .prof = nullptr};
+    // The mode's state for the key, allocated as a frame call allocates it (every other lane then has no state).  An
+    // allocation made here is undone when the blob turns out not to fit it.
+    bool allocated_here = false;
+    mc_status st = MC_OK;
+    if (fresh) tracker_update(h, &key, b.levels, b.channels, b.w, b.h);
+    if (b.mode == MC_MODE_LAPLACE && !h->motion.allocated) {
+        allocated_here = true;
+        st = h->motion.allocate(ctx, b.w, b.h, b.channels, b.levels);
+    } else if (b.mode == MC_MODE_PHASE && b.channels == 3 && !h->riesz.allocated) {
+        allocated_here = true;
+        st = h->riesz.allocate(ctx, b.w, b.h, nullptr, b.levels);
+    } else if (b.mode == MC_MODE_COLOR && !h->color.allocated) {
+        allocated_here = true;
+        st = h->color.allocate(ctx, b.w, b.h, b.channels, b.levels);
+    }
+    std::vector<LanePlane> planes;
+    const size_t total = st == MC_OK ? lane_planes(h, b, lane, planes) : 0;
+    if (st != MC_OK || sizeof(b) + total != b.bytes) {
+        if (allocated_here) {
+            h->motion.reset(); h->riesz.reset(); h->color.reset();   // nothing else was allocated (a fresh or unallocated mode)
+        }
+        if (fresh) tracker_disable(h);
+        if (st == MC_OK) { h->err = "lane blob size does not match its key"; st = MC_ERR_INVALID; }
+        return st;
+    }
+    // From here a failure is a CUDA error: the state may be half-written, so it is dropped as after a failed frame.
+    if (b.mode == MC_MODE_COLOR) {
+        st = h->color.reserve_ring(ctx, b.mod);
+        if (st == MC_OK) lane_planes(h, b, lane, planes);   // the ring may have moved
+    }
+    if (st == MC_OK) st = copy_lane_planes(h, planes, total, (uint8_t*)src + sizeof(b), false);
+    if (st != MC_OK) {
+        reset_modes(h);
+        tracker_reset(h);
+        return st;
+    }
+    if (b.mode == MC_MODE_LAPLACE) {
+        h->motion.empty = false;
+        h->motion.ab_bounded = h->motion.ab_bounded && b.ab_bounded;   // an unbounded state must not run L-only synthesis
+    } else if (b.mode == MC_MODE_PHASE && h->riesz.allocated) {
+        std::memcpy(&h->riesz.design[(size_t)lane], b.design, sizeof(b.design));
+    } else if (b.mode == MC_MODE_COLOR) {
+        h->color.count[(size_t)lane] = b.count; h->color.head[(size_t)lane] = b.head; h->color.mod[(size_t)lane] = b.mod;
+    }
+    h->has_state[(size_t)lane] = 1;
     return MC_OK;
 } catch (...) { return on_exception(h); }
 

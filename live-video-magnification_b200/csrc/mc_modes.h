@@ -145,6 +145,13 @@ inline void lab16_state(const int16_t* lab16, bool current, int w, int h, int pi
     out.ptr16 = lab16; out.rows = h; out.cols = w; out.channels = 3; out.pitch = pitch16; out.plane_stride = plane16;
 }
 
+// One block of a lane's temporal state as mc_save_lane / mc_load_lane copy it: `rows` rows of `row_bytes` bytes,
+// `pitch` bytes apart, from `ptr` (device).  A blob holds the rows dense.
+struct LanePlane {
+    void* ptr = nullptr;
+    size_t pitch = 0, row_bytes = 0, rows = 0;
+};
+
 // Simple owner of cudaMalloc'ed float buffers (freed together on reset()).
 struct DeviceArena {
     std::vector<void*> blocks;
@@ -255,9 +262,12 @@ struct MotionMode {
     // holds frames * lanes flags
     mc_status process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced, int frames = 1);
     void find_state(const char* name, int level, StateRef& out);
+    // the state of every lane for this key, as a frame call allocates it (every lane's next frame is its first)
+    mc_status allocate(const ModeCtx& ctx, int w, int h, int channels, int levels);
+    // lane `lane`'s state: hi then lo of every kept level, all channels of a plane set in one block
+    void lane_planes(int lane, std::vector<LanePlane>& out) const;
 
 private:
-    mc_status allocate(const ModeCtx& ctx, const FrameIO& io, int levels);
     mc_status make_groups(const ModeCtx& ctx);
     void drop_groups();
     bool luma_only(const ModeCtx& ctx) const;
@@ -359,8 +369,22 @@ struct ColorMode {
     // holds frames * lanes flags
     mc_status process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced, int frames = 1);
     void find_state(const char* name, int level, StateRef& out);
+    // the planes of this key with every window empty, as a frame call allocates them (the ring follows on the first frame)
+    mc_status allocate(const ModeCtx& ctx, int w, int h, int channels, int levels);
+    // lane `lane`'s window of `mod` slots as it lies in the ring: its block of physical slots 0 .. mod-1
+    void lane_planes(int lane, int lane_mod, std::vector<LanePlane>& out) const;
+    // makes the ring hold at least `need` slots, every lane's window in the slots it occupies (mc_load_lane)
+    mc_status reserve_ring(const ModeCtx& ctx, int need);
 
 private:
+    // A slot's layout.  One lane's block of a slot is lane_sig() signals (pixels x channels).  cuFFT takes a lane's block
+    // as the base pointer of a one-lane transform, which must be 8-byte aligned: on a multi-lane handle an odd block is
+    // followed by one padding signal.
+    size_t lane_sig() const { return (size_t)channels * small_rows; }
+    size_t lane_stride() const { return lane_sig() + (lanes > 1 ? (lane_sig() & 1) : 0); }
+    size_t slot_signals() const { return (size_t)lanes * lane_stride(); }
+    // the ring grown to `need` slots (grow) or rotated; with `relayout` the lanes' windows move by d_rows' relayout fields
+    mc_status reshape_ring(const ModeCtx& ctx, int need, bool grow, bool relayout, const ColorLane* d_rows);
     mc_status fft_plan(const ModeCtx& ctx, int n, bool one_lane, FftPlans** out);
     mc_status alloc_clip(const ModeCtx& ctx, int vlanes, size_t work_floats);
     // the append and filter rules of one frame: writes its `lanes` rows of a lane table, moves count / head
@@ -430,9 +454,14 @@ struct RieszMode {
     // holds frames * lanes flags
     mc_status process(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels, int* produced, int frames = 1);
     void find_state(const char* name, int level, StateRef& out);
+    // The handle's state for `levels` levels at w x h, the filters designed from p (each lane's params) or, with p null,
+    // not designed (not finite: the lane's next frame designs them, as a first frame)
+    mc_status allocate(const ModeCtx& ctx, int w, int h, const mc_params* p, int levels);
+    // lane `lane`'s state: the 13 planes of every band level, plane by plane (old.lowpass, old.rx, old.ry, phase.c,
+    // phase.s, lo.r0.c, lo.r0.s, lo.r1.c, lo.r1.s, hi.r0.c, hi.r0.s, hi.r1.c, hi.r1.s)
+    void lane_planes(int lane, std::vector<LanePlane>& out) const;
 
 private:
-    mc_status allocate(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int levels);
     mc_status apply_cutoffs(const ModeCtx& ctx, const mc_params& p, std::vector<uint8_t>& rebuild);
     // the per-lane table of this frame (null when every lane's row is lane 0's: the scalars of row 0), uploaded on change
     mc_status lane_table(const ModeCtx& ctx, const mc_params& p, const std::vector<uint8_t>& rebuild, const RieszLane** d);

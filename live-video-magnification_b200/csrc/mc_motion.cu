@@ -133,9 +133,9 @@ static bool luma_params(const mc_params& p, const std::vector<float>& g) {
     return true;
 }
 
-mc_status MotionMode::allocate(const ModeCtx& ctx, const FrameIO& io, int nlevels) {
+mc_status MotionMode::allocate(const ModeCtx& ctx, int width, int height, int nchannels, int nlevels) {
     reset();
-    levels = nlevels; channels = io.channels; w = io.w; h = io.h;
+    levels = nlevels; channels = nchannels; w = width; h = height;
     faithful = ctx.opt.faithful_level0;
     from_state = ctx.opt.band_from_state;
     const size_t planes = (size_t)lanes * channels;
@@ -179,7 +179,7 @@ mc_status MotionMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc
     *produced = 0;
     if (!allocated || faithful != ctx.opt.faithful_level0 || from_state != ctx.opt.band_from_state) {
         if (allocated) *ctx.held_lost = true;
-        mc_status st = allocate(ctx, io_in, nlevels);
+        mc_status st = allocate(ctx, io_in.w, io_in.h, io_in.channels, nlevels);
         if (st != MC_OK) return st;
     } else if (groups_req != ctx.opt.lane_groups) {
         mc_status st = make_groups(ctx);
@@ -488,6 +488,18 @@ void MotionMode::find_state(const char* name, int level, StateRef& out) {
     if (!p) return;
     const Level& l = lv[(size_t)level];
     out.ptr = p; out.rows = l.h; out.cols = l.w; out.channels = channels; out.pitch = l.pitch; out.plane_stride = l.plane;
+}
+
+void MotionMode::lane_planes(int lane, std::vector<LanePlane>& out) const {
+    out.clear();
+    if (!allocated) return;
+    for (int l = 0; l <= levels; ++l) {
+        const Level& L = lv[(size_t)l];
+        for (float* p : {hi[(size_t)l], lo[(size_t)l]})
+            if (p)   // a lane's channels are consecutive planes of h rows `pitch` apart: one block of channels * h rows
+                out.push_back(LanePlane{p + (size_t)lane * channels * L.plane, (size_t)L.pitch * sizeof(float), (size_t)L.w * sizeof(float),
+                                        (size_t)channels * L.h});
+    }
 }
 
 }  // namespace mc

@@ -847,11 +847,11 @@ mc_status RieszMode::lane_table(const ModeCtx& ctx, const mc_params& p, const st
     return MC_OK;
 }
 
-// The handle's state for `nlevels` levels at io's size, the filters designed from p; the Riesz pair of `old`, the phases
-// and the IIR registers start at zero.
-mc_status RieszMode::allocate(const ModeCtx& ctx, const FrameIO& io, const mc_params& p, int nlevels) {
+// The handle's state for `nlevels` levels at width x height, the filters designed from p; the Riesz pair of `old`, the
+// phases and the IIR registers start at zero.
+mc_status RieszMode::allocate(const ModeCtx& ctx, int width, int height, const mc_params* p, int nlevels) {
     reset();
-    levels = nlevels; w = io.w; h = io.h;
+    levels = nlevels; w = width; h = height;
     lv.resize((size_t)levels);
     int cw = w, ch = h;
     for (int i = 0; i < levels; ++i) {
@@ -889,11 +889,27 @@ mc_status RieszMode::allocate(const ModeCtx& ctx, const FrameIO& io, const mc_pa
     lab16 = (int16_t*)lp;
     design.resize((size_t)lanes);
     for (int k = 0; k < lanes; ++k) {
-        const mc_params& q = lane_params(ctx, p, k);
+        if (!p) {
+            design[(size_t)k].loA[0] = design[(size_t)k].hiA[0] = NAN;
+            continue;
+        }
+        const mc_params& q = lane_params(ctx, *p, k);
         design[(size_t)k] = make_design(q, q.framerate);
     }
     allocated = true;
     return MC_OK;
+}
+
+void RieszMode::lane_planes(int lane, std::vector<LanePlane>& out) const {
+    out.clear();
+    if (!allocated) return;
+    for (const auto* v : {&old_low, &old_rx, &old_ry, &phase_c, &phase_s, &lo_r0c, &lo_r0s, &lo_r1c, &lo_r1s, &hi_r0c, &hi_r0s, &hi_r1c,
+                          &hi_r1s})
+        for (int i = 0; i < levels - 1; ++i) {
+            const Level& l = lv[(size_t)i];
+            out.push_back(LanePlane{(*v)[(size_t)i] + (size_t)lane * l.plane, (size_t)l.pitch * sizeof(float), (size_t)l.w * sizeof(float),
+                                    (size_t)l.h});
+        }
 }
 
 mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_params& p, int nlevels, int* produced, int frames) {
@@ -933,7 +949,7 @@ mc_status RieszMode::process(const ModeCtx& ctx, const FrameIO& io_in, const mc_
     }
     if (first) {
         if (allocated) *ctx.held_lost = true;
-        MCK_ST(allocate(ctx, io_in, p, nlevels));
+        MCK_ST(allocate(ctx, io_in.w, io_in.h, &p, nlevels));
     }
     lab16_frame = false;   // a clip converts into its own scratch; a frame call rewrites lab16 below
     if (frames > 1) return run_clip(ctx, io_in, p, frames, first, produced);

@@ -188,6 +188,19 @@ class MagnificationProcessor(IProcessor):
                                            float(params.coHigh), float(params.chromAttenuation), float(params.framerate)))
         self._check(self._lib.mc_set_lane_params(self._h, int(lane), lp))
 
+    def save_lane(self, lane: int) -> bytes:
+        """The lane's temporal state as an opaque blob (mc_save_lane), for load_lane on any lane of any processor."""
+        n = C.c_size_t(0)
+        self._check(self._lib.mc_save_lane(self._h, int(lane), None, 0, C.byref(n)))
+        buf = C.create_string_buffer(n.value)
+        self._check(self._lib.mc_save_lane(self._h, int(lane), buf, n.value, C.byref(n)))
+        return buf.raw[:n.value]
+
+    def load_lane(self, lane: int, blob: bytes) -> None:
+        """Makes the lane's temporal state the one saved in `blob` (mc_load_lane); the lane's hold and parameters stay
+        its own, and the other lanes are untouched."""
+        self._check(self._lib.mc_load_lane(self._h, int(lane), C.c_char_p(bytes(blob)), len(blob)))
+
     def lane_produced(self) -> np.ndarray:
         """-> bool[lanes]: which lanes produced an output in the most recent frame call (or collect())."""
         a = np.zeros(self.lanes, np.uint8)
@@ -438,6 +451,14 @@ class ProcessingChainB200:
     def set_lane_params(self, lane: int, params: Optional[MagnificationParams]) -> None:
         """MagnificationProcessor.set_lane_params of the chain's magnifier."""
         self.magnifier.set_lane_params(lane, params)
+
+    def save_lane(self, lane: int) -> bytes:
+        """MagnificationProcessor.save_lane of the chain's magnifier (the front stages have no state)."""
+        return self.magnifier.save_lane(lane)
+
+    def load_lane(self, lane: int, blob: bytes) -> None:
+        """MagnificationProcessor.load_lane of the chain's magnifier."""
+        self.magnifier.load_lane(lane, blob)
 
     @staticmethod
     def geometry(cfg: ProcessorConfig, w: int, h: int, c: int) -> "capi.McChainInfo":
