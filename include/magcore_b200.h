@@ -393,16 +393,17 @@ mc_status mc_chain_process_nv12_device(mc_handle* h, const mc_nv12* in, int fram
  *   MC_SPLIT_NONE        the processed pane alone: w x h
  *   MC_SPLIT_LEFT_RIGHT  the original pane left of the processed one: 2w x h
  *   MC_SPLIT_TOP_BOTTOM  the original pane above the processed one: w x 2h
- * A canvas is packed BGR (pitch >= 3 * its width) or NV12 (pitch >= its width; cvtColor(COLOR_BGR2YUV_I420) of the BGR
- * canvas with Cb,Cr interleaved, as the NV12 calls write).  Its dimensions are always even, so an NV12 canvas always
- * exists when the BGR one does. */
+ * A canvas is packed BGR (pitch >= 3 * its width), NV12 (pitch >= its width; cvtColor(COLOR_BGR2YUV_I420) of the BGR
+ * canvas with Cb,Cr interleaved, as the NV12 calls write) or I420 (the planes cvtColor(COLOR_BGR2YUV_I420) returns; see
+ * the planar 4:2:0 section).  Its dimensions are always even, so a 4:2:0 canvas always exists when the BGR one does. */
 typedef enum mc_split { MC_SPLIT_NONE = 0, MC_SPLIT_LEFT_RIGHT = 1, MC_SPLIT_TOP_BOTTOM = 2 } mc_split; /* livim::SplitMode */
-typedef enum mc_canvas_format { MC_CANVAS_BGR = 0, MC_CANVAS_NV12 = 1 } mc_canvas_format;
+typedef enum mc_canvas_format { MC_CANVAS_BGR = 0, MC_CANVAS_NV12 = 1, MC_CANVAS_I420 = 2 } mc_canvas_format;
 typedef struct mc_canvas {
     int32_t format;       /* mc_canvas_format */
-    uint8_t* data;        /* BGR: canvas of virtual lane 0; NV12: its luma plane */
-    uint8_t* uv;          /* NV12: interleaved Cb,Cr plane (need not follow the luma); BGR: unused */
-    size_t pitch;         /* bytes per row (both NV12 planes) */
+    uint8_t* data;        /* BGR: canvas of virtual lane 0; NV12 / I420: its luma plane */
+    uint8_t* uv;          /* NV12: interleaved Cb,Cr plane (need not follow the luma); I420: Cb plane, with the Cr plane
+                             at uv + (pitch / 2) * (canvas_h / 2); BGR: unused */
+    size_t pitch;         /* bytes per row (both NV12 planes; the I420 luma plane, whose chroma rows are pitch / 2 apart) */
     size_t lane_stride;   /* bytes from one virtual lane's canvas (planes) to the next */
 } mc_canvas;
 
@@ -449,8 +450,8 @@ mc_status mc_chain_compose_nv12_device(mc_handle* h, const mc_nv12* in, int fram
  *   Stream order: mc_set_overlay copies the overlay to device memory in stream order on mc_stream().  Compose calls
  *     enqueued before it use the previous overlay, calls after it the new one.  The caller's buffers may be freed as
  *     soon as it returns.
- *   Every compose call (BGR, NV12 and YUYV sources; BGR and NV12 canvases; frames, clips and lanes) maps each canvas it
- *     writes: a canvas pixel inside a rect becomes map[index][v] in each of its channels, before the NV12 conversion (a
+ *   Every compose call (BGR, NV12, YUYV and I420 sources; BGR, NV12 and I420 canvases; frames, clips and lanes) maps each
+ *     canvas it writes: a canvas pixel inside a rect becomes map[index][v] in each of its channels, before the 4:2:0 conversion (a
  *     2x2 block whose top-left pixel is labelled takes its Cb,Cr from the labelled value).  Held lanes and 0 x 0
  *     canvases stay untouched, as without an overlay.  Chain calls that do not compose ignore it.
  *   Errors, MC_ERR_INVALID: mc_set_overlay with canvas_w or canvas_h < 1, rects or maps out of range, a NULL map or
@@ -567,6 +568,54 @@ mc_status mc_chain_compose_submit_nv12(mc_handle* h, const mc_nv12* in, int fram
 mc_status mc_chain_compose_submit_yuv422(mc_handle* h, const mc_yuv422* in, int frames, int width, int height,
                                          const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
                                          uint8_t* produced, mc_chain_info* info);
+
+/* --- planar 4:2:0 frames (I420 / YV12): the hand-off format of software decoders and encoders -------------------------
+ * FFmpeg's software decoders and encoders (libx264, FFV1, MJPEG; AV_PIX_FMT_YUV420P) and cv::VideoCapture / VideoWriter
+ * exchange 4:2:0 YCbCr in three planes: a luma plane and a Cb and a Cr plane of height/2 rows of width/2 bytes, one Cb and
+ * one Cr per 2x2 pixel block.  BT.601 limited range, as NV12: OpenCV converts I420 and YV12 with the fixed point of its
+ * NV12 conversion, and the core converts them on the device with the same arithmetic.
+ *   Equivalence, input: let X be any I420 input.  Every call on X equals, bit for bit, the NV12 call on the frame with X's
+ *     Y plane and its U, V planes interleaved, and therefore the BGR call on cv2.cvtColor(X, COLOR_YUV2BGR_I420) (_YV12
+ *     when the planes are YV12's): the processed frames, the original tap, `info`, the produced flags, mc_lane_produced
+ *     and the temporal state afterwards.  I420, NV12, 4:2:2 and BGR calls of the same geometry interleave on one handle
+ *     without a structural reset (the tracker sees channels 3).  A ROI at an odd column or row still takes each pixel's
+ *     chroma from its own 2x2 block of the frame.
+ *   Equivalence, canvas: an MC_CANVAS_I420 canvas's Y, Cb and Cr planes equal the NV12 canvas of the same call with its
+ *     chroma de-interleaved, which is cv2.cvtColor(bgr_canvas, COLOR_BGR2YUV_I420), labels included (a 2x2 block whose
+ *     top-left pixel is labelled takes its Cb,Cr from the labelled value).  Every compose call accepts it: BGR, gray,
+ *     NV12, 4:2:2 and I420 sources; device and submit; frames, clips and lanes.  Held lanes, 0 x 0 canvases and row
+ *     padding stay untouched, the bytes between canvas_w / 2 and pitch / 2 of each chroma row included.  The layout is
+ *     that of av_image_alloc / x264_picture_alloc buffers whose chroma linesize is half the luma's.
+ *   Errors, returned before any kernel or copy runs, with no caller buffer, state or frame in flight changed:
+ *     MC_ERR_INVALID for a NULL descriptor or plane, width or height odd or < 2, pitch < width, chroma_pitch < width / 2,
+ *     lane_stride < pitch * height with more than one virtual lane, and every argument error of the NV12 twin.  An I420
+ *     canvas: MC_ERR_INVALID for a NULL data or uv, an odd pitch or pitch < canvas_w.
+ *   Memory: staging and pipeline slots follow the NV12 rules, 1.5 B/px for frames and canvases.  Pageable planes go
+ *     through pinned staging; pinned planes are copied directly. */
+typedef struct mc_yuv420p {
+    uint8_t* y;            /* luma plane of (virtual) lane 0: height rows of width bytes */
+    uint8_t* u;            /* Cb plane: height/2 rows of width/2 bytes */
+    uint8_t* v;            /* Cr plane: height/2 rows of width/2 bytes; YV12 is passed with u / v at its Cb / Cr planes */
+    size_t pitch;          /* luma bytes per row (AVFrame linesize[0]) */
+    size_t chroma_pitch;   /* Cb and Cr bytes per row (linesize[1] == linesize[2]) */
+    size_t lane_stride;    /* bytes from one virtual lane's planes to the next, the same for all three */
+} mc_yuv420p;
+/* mc_chain_process_nv12_device on I420 device planes (frame t of lane k is virtual lane t * lanes + k) */
+mc_status mc_chain_process_yuv420p_device(mc_handle* h, const mc_yuv420p* in, int frames, int width, int height,
+                                          const mc_params* p, int grayscale, uint8_t* d_out, size_t out_step,
+                                          uint8_t* d_original, size_t original_step, uint8_t* produced, mc_chain_info* info);
+/* mc_chain_compose_nv12_device on I420 device planes */
+mc_status mc_chain_compose_yuv420p_device(mc_handle* h, const mc_yuv420p* in, int frames, int width, int height,
+                                          const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                                          uint8_t* produced, mc_chain_info* info);
+/* mc_chain_submit_nv12 on I420 host planes: 1.5 B/px cross PCIe upwards */
+mc_status mc_chain_submit_yuv420p(mc_handle* h, const mc_yuv420p* in, int width, int height, const mc_params* p, int grayscale,
+                                  uint8_t* out, size_t out_step, uint8_t* original, size_t original_step, mc_chain_info* info);
+/* mc_chain_compose_submit_nv12 on I420 host planes: an exporter that decodes and encodes I420 in software submits its
+ * decoded frames and collects canvases its encoder takes as they are */
+mc_status mc_chain_compose_submit_yuv420p(mc_handle* h, const mc_yuv420p* in, int frames, int width, int height,
+                                          const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                                          uint8_t* produced, mc_chain_info* info);
 
 /* Pinned host memory for frames (so FramePool buffers can be DMA'd directly). */
 void* mc_host_alloc(size_t bytes);

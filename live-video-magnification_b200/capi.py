@@ -49,8 +49,15 @@ class McYuv422(C.Structure):
     _fields_ = [("data", C.c_void_p), ("pitch", C.c_size_t), ("lane_stride", C.c_size_t), ("order", C.c_int32)]
 
 
+class McYuv420p(C.Structure):
+    """mc_yuv420p: one planar 4:2:0 frame set (I420; YV12 with u / v at its Cb / Cr planes); plane pointers are host or
+    device addresses as integers."""
+    _fields_ = [("y", C.c_void_p), ("u", C.c_void_p), ("v", C.c_void_p), ("pitch", C.c_size_t), ("chroma_pitch", C.c_size_t),
+                ("lane_stride", C.c_size_t)]
+
+
 MC_SPLIT_NONE, MC_SPLIT_LEFT_RIGHT, MC_SPLIT_TOP_BOTTOM = 0, 1, 2
-MC_CANVAS_BGR, MC_CANVAS_NV12 = 0, 1
+MC_CANVAS_BGR, MC_CANVAS_NV12, MC_CANVAS_I420 = 0, 1, 2
 
 
 class McCanvas(C.Structure):
@@ -80,6 +87,7 @@ _PP = C.POINTER(McParams)
 _NV = C.POINTER(McNv12)
 _CV = C.POINTER(McCanvas)
 _YV = C.POINTER(McYuv422)
+_YP = C.POINTER(McYuv420p)
 SIGNATURES = {
     "mc_abi_version": (C.c_int, []),
     "mc_device_count": (C.c_int, []),
@@ -138,6 +146,14 @@ SIGNATURES = {
                                                C.POINTER(McChainInfo)]),
     "mc_chain_compose_submit_yuv422": (C.c_int, [_vp, _YV, C.c_int, C.c_int, C.c_int, _PP, C.c_int, C.c_int, _CV, _u8p,
                                                  C.POINTER(McChainInfo)]),
+    "mc_chain_process_yuv420p_device": (C.c_int, [_vp, _YP, C.c_int, C.c_int, C.c_int, _PP, C.c_int, _vp, C.c_size_t, _vp,
+                                                  C.c_size_t, _u8p, C.POINTER(McChainInfo)]),
+    "mc_chain_compose_yuv420p_device": (C.c_int, [_vp, _YP, C.c_int, C.c_int, C.c_int, _PP, C.c_int, C.c_int, _CV, _u8p,
+                                                  C.POINTER(McChainInfo)]),
+    "mc_chain_submit_yuv420p": (C.c_int, [_vp, _YP, C.c_int, C.c_int, _PP, C.c_int, _vp, C.c_size_t, _vp, C.c_size_t,
+                                          C.POINTER(McChainInfo)]),
+    "mc_chain_compose_submit_yuv420p": (C.c_int, [_vp, _YP, C.c_int, C.c_int, C.c_int, _PP, C.c_int, C.c_int, _CV, _u8p,
+                                                  C.POINTER(McChainInfo)]),
     "mc_process_nv12_device": (C.c_int, [_vp, _NV, C.c_int, C.c_int, _PP, _NV, C.POINTER(C.c_int)]),
     "mc_process_clip_nv12_device": (C.c_int, [_vp, _NV, C.c_int, C.c_int, C.c_int, _PP, _NV, _u8p]),
     "mc_submit_nv12": (C.c_int, [_vp, _NV, C.c_int, C.c_int, _PP, _NV]),

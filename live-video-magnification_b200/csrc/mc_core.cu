@@ -60,39 +60,70 @@ struct PinnedBuffer {
     }
 };
 
-// A frame set: one plane per lane (BGR or gray: height rows of w * c bytes) or two (NV12: height luma rows and height / 2
-// Cb,Cr rows of w bytes).  Rows hold `row` bytes and are `pitch` apart; lane l starts l * lane_stride after lane 0.
+// A frame set: one plane per lane (BGR or gray: height rows of w * c bytes), two (NV12: height luma rows and height / 2
+// Cb,Cr rows of w bytes) or three (I420: height luma rows of w bytes, height / 2 rows of w / 2 bytes in each chroma plane).
+// Plane k's rows hold row[k] bytes and are pitch[k] apart; lane l starts l * lane_stride after lane 0, in every plane.
 struct Planes {
-    uint8_t* base[2] = {nullptr, nullptr};
-    size_t rows[2] = {0, 0};   // rows per lane; 0: no second plane
-    size_t row = 0, pitch = 0, lane_stride = 0;
+    static constexpr int kMax = 3;
+    uint8_t* base[kMax] = {};
+    size_t rows[kMax] = {};   // rows per lane; 0: no such plane
+    size_t row[kMax] = {}, pitch[kMax] = {};
+    size_t lane_stride = 0;
 
-    size_t lane_rows() const { return rows[0] + rows[1]; }
-    size_t lane_bytes() const { return lane_rows() * row; }
-    // the same shape packed at `p`: no row padding, the second plane right after the first, lanes back to back
-    Planes packed(uint8_t* p) const { return Planes{{p, p + rows[0] * row}, {rows[0], rows[1]}, row, row, lane_bytes()}; }
-    // `lanes` consecutive lanes are one run of lanes * lane_rows() rows `pitch` apart
+    size_t lane_rows() const { return rows[0] + rows[1] + rows[2]; }
+    size_t lane_bytes() const { return rows[0] * row[0] + rows[1] * row[1] + rows[2] * row[2]; }
+    // the same shape packed at `p`: no row padding, each plane right after the one before, lanes back to back
+    Planes packed(uint8_t* p) const {
+        Planes q;
+        for (int k = 0; k < kMax && rows[k]; ++k) {
+            q.base[k] = p; q.rows[k] = rows[k]; q.row[k] = q.pitch[k] = row[k];
+            p += rows[k] * row[k];
+        }
+        q.lane_stride = lane_bytes();
+        return q;
+    }
+    // `lanes` consecutive lanes are one run of lanes * lane_rows() rows of row[0] bytes, pitch[0] apart
     bool one_run(size_t lanes) const {
-        return (!rows[1] || base[1] == base[0] + rows[0] * pitch) && (lanes == 1 || lane_stride == lane_rows() * pitch);
+        size_t at = 0;
+        for (int k = 0; k < kMax && rows[k]; ++k) {
+            if (row[k] != row[0] || pitch[k] != pitch[0] || base[k] != base[0] + at) return false;
+            at += rows[k] * pitch[0];
+        }
+        return lanes == 1 || lane_stride == at;
+    }
+    // the bytes of `lanes` consecutive lanes lie back to back without a gap: one linear copy moves them
+    bool dense(size_t lanes) const {
+        size_t at = 0;
+        for (int k = 0; k < kMax && rows[k]; ++k) {
+            if (pitch[k] != row[k] || base[k] != base[0] + at) return false;
+            at += rows[k] * row[k];
+        }
+        return lanes == 1 || lane_stride == at;
     }
 };
 
 Planes bgr_planes(const uint8_t* p, int w, int hh, int c, size_t step) {
-    return Planes{{const_cast<uint8_t*>(p), nullptr}, {(size_t)hh, 0}, (size_t)w * c, step, step * hh};
+    return Planes{{const_cast<uint8_t*>(p)}, {(size_t)hh}, {(size_t)w * c}, {step}, step * hh};
 }
 Planes nv12_planes(const mc_nv12& f, int w, int hh) {
-    return Planes{{f.y, f.uv}, {(size_t)hh, (size_t)hh / 2}, (size_t)w, f.pitch, f.lane_stride};
+    return Planes{{f.y, f.uv}, {(size_t)hh, (size_t)hh / 2}, {(size_t)w, (size_t)w}, {f.pitch, f.pitch}, f.lane_stride};
 }
-mc_nv12 nv12_of(const Planes& f) { return mc_nv12{f.base[0], f.base[1], f.pitch, f.lane_stride}; }
+mc_nv12 nv12_of(const Planes& f) { return mc_nv12{f.base[0], f.base[1], f.pitch[0], f.lane_stride}; }
+// the luma plane and chroma addressing (mc_internal.h) of 4:2:0 planes: NV12 with two planes, I420 with three
+Nv12Planes yuv420_of(const Planes& f) {
+    if (!f.rows[2]) return Nv12Planes{f.base[0], f.base[1], f.base[1] + 1, f.pitch[0], f.pitch[0], f.lane_stride, kNv12ChromaStep};
+    return Nv12Planes{f.base[0], f.base[1], f.base[2], f.pitch[0], f.pitch[1], f.lane_stride, kI420ChromaStep};
+}
 
-// The source frames of a call: u8 BGR or gray, NV12 planes or packed 4:2:2 frames, virtual lane v at v *
-// planes.lane_stride.  Only these helpers tell the formats apart.
+// The source frames of a call: u8 BGR or gray, 4:2:0 planes (NV12, or I420 with three planes) or packed 4:2:2 frames,
+// virtual lane v at v * planes.lane_stride.  Only these helpers tell the formats apart.
 struct Source {
     static constexpr int kBadOrder = FRONT_UYVY + 1;   // a 4:2:2 frame of an order out of range: refused by check()
     int kind = FRONT_BGR;                               // FrontSrc, the front's `src`
-    int w = 0, hh = 0, channels = 3;                    // NV12 and 4:2:2 frames stand for BGR ones
+    int w = 0, hh = 0, channels = 3;                    // 4:2:0 and 4:2:2 frames stand for BGR ones
     Planes planes;
-    const char* missing = nullptr;   // the call's mc_nv12 / mc_yuv422 is NULL: its error comes before every other check
+    const char* missing = nullptr;   // the call's mc_nv12 / mc_yuv420p / mc_yuv422 is NULL: its error comes first
+    bool i420 = false;               // 4:2:0 in three planes (mc_yuv420p)
 
     static Source bgr(const uint8_t* in, int w, int hh, int c, size_t step) {
         return Source{c == 3 ? FRONT_BGR : FRONT_GRAY, w, hh, c, bgr_planes(in, w, hh, c, step)};
@@ -100,10 +131,18 @@ struct Source {
     static Source nv12(const mc_nv12* f, int w, int hh) {
         return f ? Source{FRONT_NV12, w, hh, 3, nv12_planes(*f, w, hh)} : Source{FRONT_NV12, w, hh, 3, {}, "NV12 plane is null"};
     }
+    static Source yuv420p(const mc_yuv420p* f, int w, int hh) {
+        if (!f) return Source{FRONT_NV12, w, hh, 3, {}, "I420 frame is null", true};
+        const size_t ch = (size_t)std::max(hh, 0) / 2, cw = (size_t)std::max(w, 0) / 2;
+        return Source{FRONT_NV12, w, hh, 3,
+                      Planes{{f->y, f->u, f->v}, {(size_t)std::max(hh, 0), ch, ch}, {(size_t)std::max(w, 0), cw, cw},
+                             {f->pitch, f->chroma_pitch, f->chroma_pitch}, f->lane_stride},
+                      nullptr, true};
+    }
     static Source yuv422(const mc_yuv422* f, int w, int hh) {
         if (!f) return Source{FRONT_YUYV, w, hh, 3, {}, "YUYV frame is null"};
         const int kind = f->order == MC_YUV422_YUYV || f->order == MC_YUV422_UYVY ? FRONT_YUYV + f->order : kBadOrder;
-        return Source{kind, w, hh, 3, Planes{{f->data, nullptr}, {(size_t)hh, 0}, (size_t)2 * w, f->pitch, f->lane_stride}};
+        return Source{kind, w, hh, 3, Planes{{f->data}, {(size_t)hh}, {(size_t)2 * w}, {f->pitch}, f->lane_stride}};
     }
 
     // BGR or gray frames, which the magnifier reads where they are
@@ -115,25 +154,37 @@ struct Source {
     bool converts() const { return kind >= FRONT_YUYV; }
     // the source's argument errors for `vl` virtual lanes -> an error text, or null
     const char* check(size_t vl) const {
+        if (i420) {
+            if (w < 2 || hh < 2 || (w & 1) || (hh & 1)) return "I420 width and height must be even and >= 2";
+            if (!planes.base[0] || !planes.base[1] || !planes.base[2]) return "I420 plane is null";
+            if (planes.pitch[0] < (size_t)w) return "I420 pitch < width";
+            if (planes.pitch[1] < (size_t)w / 2) return "I420 chroma_pitch < width / 2";
+            if (vl > 1 && planes.lane_stride < planes.pitch[0] * hh) return "I420 lane_stride < pitch * height";
+            return nullptr;
+        }
         if (kind == FRONT_NV12) {
             if (w < 2 || hh < 2 || (w & 1) || (hh & 1)) return "NV12 width and height must be even and >= 2";
             if (!planes.base[0] || !planes.base[1]) return "NV12 plane is null";
-            if (planes.pitch < (size_t)w) return "NV12 pitch < width";
-            if (vl > 1 && planes.lane_stride < planes.pitch * hh) return "NV12 lane_stride < pitch * height";
+            if (planes.pitch[0] < (size_t)w) return "NV12 pitch < width";
+            if (vl > 1 && planes.lane_stride < planes.pitch[0] * hh) return "NV12 lane_stride < pitch * height";
             return nullptr;
         }
         if (converts()) {
             if (!planes.base[0]) return "YUYV frame is null";
             if (kind == kBadOrder) return "YUYV order out of range";
             if (w < 2 || (w & 1) || hh < 1) return "YUYV width must be even and >= 2, height >= 1";
-            if (planes.pitch < (size_t)2 * w) return "YUYV pitch < 2 * width";
-            if (vl > 1 && planes.lane_stride < planes.pitch * hh) return "YUYV lane_stride < pitch * height";
+            if (planes.pitch[0] < (size_t)2 * w) return "YUYV pitch < 2 * width";
+            if (vl > 1 && planes.lane_stride < planes.pitch[0] * hh) return "YUYV lane_stride < pitch * height";
             return nullptr;
         }
-        return !empty() && planes.pitch < planes.row ? "step too small" : nullptr;
+        return !empty() && planes.pitch[0] < planes.row[0] ? "step too small" : nullptr;
     }
     // the frames as the front and the compose kernel read them
-    PaneSrc pane() const { return PaneSrc{planes.base[0], planes.base[1], planes.pitch, planes.lane_stride, kind}; }
+    PaneSrc pane() const {
+        if (kind != FRONT_NV12) return PaneSrc{planes.base[0], nullptr, planes.pitch[0], planes.lane_stride, kind};
+        const Nv12Planes f = yuv420_of(planes);
+        return PaneSrc{f.y, f.cb, f.pitch, f.lane_stride, kind, f.cr, f.cpitch, f.cstep};
+    }
     // the same frames at `p` (a pipeline slot's packed device copy)
     Source on(const Planes& p) const { Source s = *this; s.planes = p; return s; }
 };
@@ -350,31 +401,38 @@ bool is_pinned(const void* p) {
     }
     return at.type == cudaMemoryTypeHost;
 }
-bool is_pinned(const Planes& f) { return is_pinned(f.base[0]) && (!f.rows[1] || is_pinned(f.base[1])); }
+bool is_pinned(const Planes& f) {
+    for (int k = 0; k < Planes::kMax && f.rows[k]; ++k)
+        if (!is_pinned(f.base[k])) return false;
+    return true;
+}
 
 // Lane l of every plane, host to host, row by row.
 void host_copy(const Planes& dst, const Planes& src, size_t l) {
-    for (int k = 0; k < 2; ++k)
+    for (int k = 0; k < Planes::kMax; ++k)
         for (size_t r = 0; r < src.rows[k]; ++r)
-            std::memcpy(dst.base[k] + l * dst.lane_stride + r * dst.pitch, src.base[k] + l * src.lane_stride + r * src.pitch, src.row);
+            std::memcpy(dst.base[k] + l * dst.lane_stride + r * dst.pitch[k], src.base[k] + l * src.lane_stride + r * src.pitch[k],
+                        src.row[k]);
 }
 
-// Lanes [a, b) of every plane between host and device: one copy when both sides hold them as one run of rows (a plain
-// copy when neither side pads its rows), otherwise one 2D copy per plane and lane.
+// Lanes [a, b) of every plane between host and device: one plain copy when neither side has a gap between their bytes,
+// one 2D copy when both sides hold them as one run of rows of one width, otherwise one 2D copy per plane and lane.
 mc_status copy_planes(mc_handle* h, const Planes& dst, const Planes& src, size_t a, size_t b, cudaMemcpyKind kind, cudaStream_t s) {
+    uint8_t* d = dst.base[0] + a * dst.lane_stride;
+    const uint8_t* from = src.base[0] + a * src.lane_stride;
+    if (dst.dense(b - a) && src.dense(b - a)) {
+        CK(cudaMemcpyAsync(d, from, (b - a) * src.lane_bytes(), kind, s));
+        return MC_OK;
+    }
     if (dst.one_run(b - a) && src.one_run(b - a)) {
-        uint8_t* d = dst.base[0] + a * dst.lane_stride;
-        const uint8_t* from = src.base[0] + a * src.lane_stride;
-        const size_t rows = (b - a) * src.lane_rows();
-        if (dst.pitch == src.row && src.pitch == src.row) CK(cudaMemcpyAsync(d, from, rows * src.row, kind, s));
-        else CK(cudaMemcpy2DAsync(d, dst.pitch, from, src.pitch, src.row, rows, kind, s));
+        CK(cudaMemcpy2DAsync(d, dst.pitch[0], from, src.pitch[0], src.row[0], (b - a) * src.lane_rows(), kind, s));
         return MC_OK;
     }
     for (size_t l = a; l < b; ++l)
-        for (int k = 0; k < 2; ++k)
+        for (int k = 0; k < Planes::kMax; ++k)
             if (src.rows[k])
-                CK(cudaMemcpy2DAsync(dst.base[k] + l * dst.lane_stride, dst.pitch, src.base[k] + l * src.lane_stride, src.pitch, src.row,
-                                     src.rows[k], kind, s));
+                CK(cudaMemcpy2DAsync(dst.base[k] + l * dst.lane_stride, dst.pitch[k], src.base[k] + l * src.lane_stride, src.pitch[k],
+                                     src.row[k], src.rows[k], kind, s));
     return MC_OK;
 }
 
@@ -528,7 +586,7 @@ mc_status submit_impl(mc_handle* h, const Planes& in, const Planes (&out)[kOutSe
     const size_t vl = (size_t)frames * h->lanes, bytes = in.lane_bytes() * vl;
     size_t ofs[kOutSets], out_bytes = 0;
     for (int k = 0; k < kOutSets; ++k) {
-        if (out[k].base[0] && out[k].pitch < out[k].row) { h->err = "out_step too small"; return MC_ERR_INVALID; }
+        if (out[k].base[0] && out[k].pitch[0] < out[k].row[0]) { h->err = "out_step too small"; return MC_ERR_INVALID; }
         ofs[k] = out_bytes;
         out_bytes += (out[k].lane_bytes() * vl + 255) / 256 * 256;   // each set 256-byte aligned
     }
@@ -1030,8 +1088,8 @@ mc_status mc_submit(mc_handle* h, const uint8_t* in, int width, int height, int 
     return submit_impl(h, have ? bgr_planes(in, width, height, channels, in_step) : none,
                        {have ? bgr_planes(out, width, height, channels, out_step) : none, none},
                        [&](const Planes& d_in, const Planes* d_out, int* produced, uint8_t* lane_produced, std::vector<uint8_t>* written) {
-                           const mc_status st = process_device_impl(h, d_in.base[0], width, height, channels, d_in.pitch, p,
-                                                                    d_out[0].base[0], d_out[0].pitch, produced, lane_produced);
+                           const mc_status st = process_device_impl(h, d_in.base[0], width, height, channels, d_in.pitch[0], p,
+                                                                    d_out[0].base[0], d_out[0].pitch[0], produced, lane_produced);
                            std::copy(lane_produced, lane_produced + h->lanes, written[0].begin());
                            return st;
                        });
@@ -1233,13 +1291,13 @@ extern "C" mc_status mc_process_clip(mc_handle* h, const uint8_t* in, int frames
     if (!(in != nullptr && width > 0 && height > 0 && (channels == 1 || channels == 3)))
         return clip_impl(h, nullptr, frames, 0, 0, channels, 0, p, nullptr, 0, produced);   // the identity
     const Planes src = bgr_planes(in, width, height, channels, in_step), dst = bgr_planes(out, width, height, channels, out_step);
-    if (in_step < src.row || (out && out_step < src.row)) { h->err = "step too small"; return MC_ERR_INVALID; }
+    if (in_step < src.row[0] || (out && out_step < src.row[0])) { h->err = "step too small"; return MC_ERR_INVALID; }
     const size_t vl = (size_t)frames * h->lanes;
     CK(h->k_in.grow(src.lane_bytes() * vl));
     CK(h->k_out.grow(src.lane_bytes() * vl));
     const Planes d_in = src.packed(h->k_in.p), d_out = src.packed(h->k_out.p);
     if ((st = copy_planes(h, d_in, src, 0, vl, cudaMemcpyHostToDevice, h->stream)) != MC_OK) return st;
-    st = clip_impl(h, d_in.base[0], frames, width, height, channels, d_in.pitch, p, d_out.base[0], d_out.pitch, produced);
+    st = clip_impl(h, d_in.base[0], frames, width, height, channels, d_in.pitch[0], p, d_out.base[0], d_out.pitch[0], produced);
     if (st != MC_OK) return st;
     // only the frames that produced are downloaded, one copy per run of consecutive ones ([t][lane] order); the bytes of
     // the others in `out` are left as they are
@@ -1262,7 +1320,7 @@ mc_status check_nv12(mc_handle* h, std::initializer_list<const mc_nv12*> frame_s
     return MC_OK;
 }
 
-Nv12Planes planes_of(const mc_nv12& f) { return Nv12Planes{f.y, f.uv, f.pitch, f.lane_stride}; }
+Nv12Planes planes_of(const mc_nv12& f) { return Nv12Planes{f.y, f.uv, f.uv + 1, f.pitch, f.pitch, f.lane_stride, kNv12ChromaStep}; }
 
 // Row pitch of the BGR staging: 16-byte rows keep the conversions on their 64-bit path.
 size_t bgr_step_of(int w) { return (size_t)round_up(3 * w, 16); }
@@ -1279,15 +1337,15 @@ mc_status launch_counted(mc_handle* h, const char* name, Launch launch) {
     return MC_OK;
 }
 
-// `in` -> h->n_in (BGR, bgr_step_of(w)) for `vlanes` virtual lanes, and h->n_out sized for the magnifier's BGR output
-// unless the caller writes it elsewhere (bgr_out false).  Mode None does not read its input: no launch.
-mc_status nv12_ingest(mc_handle* h, const mc_nv12& in, int w, int hh, int vlanes, const mc_params* p, bool bgr_out = true) {
+// `in` (NV12 or I420) -> h->n_in (BGR, bgr_step_of(w)) for `vlanes` virtual lanes, and h->n_out sized for the magnifier's
+// BGR output unless the caller writes it elsewhere (bgr_out false).  Mode None does not read its input: no launch.
+mc_status nv12_ingest(mc_handle* h, const Nv12Planes& in, int w, int hh, int vlanes, const mc_params* p, bool bgr_out = true) {
     const size_t bytes = bgr_step_of(w) * hh * vlanes;
     CK(h->n_in.grow(bytes));
     if (bgr_out) CK(h->n_out.grow(bytes));
     if (p->mode == MC_MODE_NONE) return MC_OK;
     return launch_counted(h, "nv12_to_bgr", [&] {
-        return launch_nv12_to_bgr(planes_of(in), w, hh, vlanes, h->n_in.p, bgr_step_of(w), h->stream);
+        return launch_nv12_to_bgr(in, w, hh, vlanes, h->n_in.p, bgr_step_of(w), h->stream);
     });
 }
 
@@ -1311,7 +1369,7 @@ mc_status nv12_egress(mc_handle* h, const mc_nv12& out, int w, int hh, int vlane
 // One frame call on NV12 device planes: nv12_ingest -> the magnifier on the BGR staging -> nv12_egress.
 mc_status nv12_frame(mc_handle* h, const mc_nv12& in, const mc_nv12& out, int w, int hh, const mc_params* p, int* produced,
                      uint8_t* lane_produced) {
-    mc_status st = nv12_ingest(h, in, w, hh, h->lanes, p);
+    mc_status st = nv12_ingest(h, planes_of(in), w, hh, h->lanes, p);
     if (st != MC_OK) return st;
     const size_t step = bgr_step_of(w);
     if ((st = process_device_impl(h, h->n_in.p, w, hh, 3, step, p, h->n_out.p, step, produced, lane_produced)) != MC_OK) return st;
@@ -1337,7 +1395,7 @@ extern "C" mc_status mc_process_clip_nv12_device(mc_handle* h, const mc_nv12* in
     if (st != MC_OK) return st;
     const int vlanes = frames * h->lanes;
     if ((st = check_nv12(h, {in, out}, width, height, vlanes, p)) != MC_OK) return st;
-    if ((st = nv12_ingest(h, *in, width, height, vlanes, p)) != MC_OK) return st;
+    if ((st = nv12_ingest(h, planes_of(*in), width, height, vlanes, p)) != MC_OK) return st;
     const size_t step = bgr_step_of(width);
     st = clip_impl(h, h->n_in.p, frames, width, height, 3, step, p, h->n_out.p, step, produced);
     if (st != MC_OK) return st;
@@ -1451,8 +1509,9 @@ struct ComposeReq {
 const char* check_compose(const ComposeReq& c, const ChainGeom& g, size_t vl, const mc_handle::Overlay& ov) {
     if (c.split < MC_SPLIT_NONE || c.split > MC_SPLIT_TOP_BOTTOM) return "split out of range";
     const mc_canvas* cv = c.canvas;
-    if (!cv || (cv->format != MC_CANVAS_BGR && cv->format != MC_CANVAS_NV12)) return "canvas is null or of an unknown format";
-    if (!cv->data || (cv->format == MC_CANVAS_NV12 && !cv->uv)) return "canvas plane is null";
+    if (!cv || cv->format < MC_CANVAS_BGR || cv->format > MC_CANVAS_I420) return "canvas is null or of an unknown format";
+    if (!cv->data || (cv->format != MC_CANVAS_BGR && !cv->uv)) return "canvas plane is null";
+    if (cv->format == MC_CANVAS_I420 && cv->pitch % 2) return "I420 canvas pitch is odd";
     int cw, ch;
     canvas_size(g, c.split, cw, ch);
     if (ov.set && cw > 0 && (cw != ov.cw || ch != ov.ch)) return "canvas geometry differs from the overlay's";
@@ -1541,7 +1600,8 @@ mc_status chain_run(mc_handle* h, const ChainGeom& g, const Source& s, int frame
     size_t mag_step = input.step;
     if (front) {
         FrontArgs a;
-        a.src = input.p; a.uv = input.uv; a.step = input.step; a.lane_stride = input.lane_stride;
+        a.src = input.p; a.step = input.step; a.lane_stride = input.lane_stride;
+        a.cb = input.cb; a.cr = input.cr; a.cpitch = input.cpitch; a.cstep = input.cstep;
         a.rx = g.rx; a.ry = g.ry; a.dw = g.dw; a.dh = g.dh; a.kind = g.kind; a.isx = g.isx; a.isy = g.isy;
         if (tap) {
             a.dst = d.orig; a.dst_step = d.orig_step;
@@ -1566,8 +1626,8 @@ mc_status chain_run(mc_handle* h, const ChainGeom& g, const Source& s, int frame
         if ((st = launch_counted(h, "chain_front", [&] { return launch_chain_front(a, input.kind, (int)vl, h->stream); })) != MC_OK) return st;
         mag_in = g.gray ? a.gray : a.dst;
         mag_step = g.gray ? (size_t)g.dw : a.dst_step;
-    } else if (!s.bgr_or_gray() && p->mode != MC_MODE_NONE) {   // NV12 without a front stage: a plain NV12 -> BGR conversion
-        if ((st = nv12_ingest(h, nv12_of(s.planes), s.w, s.hh, (int)vl, p, false)) != MC_OK) return st;
+    } else if (!s.bgr_or_gray() && p->mode != MC_MODE_NONE) {   // 4:2:0 without a front stage: a plain 4:2:0 -> BGR conversion
+        if ((st = nv12_ingest(h, yuv420_of(s.planes), s.w, s.hh, (int)vl, p, false)) != MC_OK) return st;
         mag_in = h->n_in.p;
         mag_step = bgr_step_of(s.w);
     }
@@ -1591,8 +1651,13 @@ mc_status chain_run(mc_handle* h, const ChainGeom& g, const Source& s, int frame
         a.ops = h->x_ops.p;
         a.split = d.cmp->split;
         const mc_canvas& cv = *d.cmp->canvas;
-        a.nv12 = cv.format == MC_CANVAS_NV12;
+        a.nv12 = cv.format != MC_CANVAS_BGR;
         a.data = cv.data; a.uv = cv.uv; a.pitch = cv.pitch; a.lane_stride = cv.lane_stride;
+        if (cv.format == MC_CANVAS_I420) {   // the Cr plane follows the Cb plane's canvas_h / 2 rows of pitch / 2 bytes
+            int cw, ch;
+            canvas_size(g, a.split, cw, ch);
+            a.cr = cv.uv + cv.pitch / 2 * (size_t)(ch / 2);
+        }
         if (h->ov.set) {
             a.ov_rects = h->ov.rects;
             a.ov_map = h->ov_dev.p;
@@ -1754,6 +1819,25 @@ extern "C" mc_status mc_chain_compose_yuv422_device(mc_handle* h, const mc_yuv42
                       produced, info);
 } catch (...) { return on_exception(h); }
 
+extern "C" mc_status mc_chain_process_yuv420p_device(mc_handle* h, const mc_yuv420p* in, int frames, int width, int height,
+                                                     const mc_params* p, int grayscale, uint8_t* d_out, size_t out_step,
+                                                     uint8_t* d_original, size_t original_step, uint8_t* produced,
+                                                     mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    return chain_impl(h, Source::yuv420p(in, width, height), frames, p, grayscale,
+                      ChainDst{d_out, out_step, d_original, original_step}, produced, info);
+} catch (...) { return on_exception(h); }
+
+extern "C" mc_status mc_chain_compose_yuv420p_device(mc_handle* h, const mc_yuv420p* in, int frames, int width, int height,
+                                                     const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                                                     uint8_t* produced, mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    return chain_impl(h, Source::yuv420p(in, width, height), frames, p, grayscale, ChainDst{.cmp = ComposeReq{split, canvas}},
+                      produced, info);
+} catch (...) { return on_exception(h); }
+
 namespace {
 // The body of the chain submits and of the blocking host chain calls: chain_check on the host frame set, then one slot of
 // the pipeline whose run is chain_run on the slot's buffers.  The processed frames go to d.out (lane k at k * out_h *
@@ -1778,7 +1862,7 @@ mc_status chain_submit(mc_handle* h, const Source& s, const mc_params* p, int gr
     const size_t full = empty ? 0 : ((size_t)s.w * s.hh * s.channels * h->lanes + 255) / 256 * 256;
     return submit_impl(h, src, dst, [&](const Planes& d_in, const Planes* d_out, int* produced, uint8_t* lane_produced,
                                         std::vector<uint8_t>* written) {
-        const ChainDst slot{d_out[0].base[0], d_out[0].pitch, d_out[1].base[0], d_out[1].pitch};
+        const ChainDst slot{d_out[0].base[0], d_out[0].pitch[0], d_out[1].base[0], d_out[1].pitch[0]};
         const mc_status rs = chain_run(h, g, s.on(d_in), 1, p, slot, lane_produced);
         if (rs != MC_OK) return rs;
         *produced = std::any_of(lane_produced, lane_produced + h->lanes, [](uint8_t x) { return x != 0; });
@@ -1875,12 +1959,26 @@ extern "C" mc_status mc_chain_submit_yuv422(mc_handle* h, const mc_yuv422* in, i
     return chain_submit(h, Source::yuv422(in, width, height), p, grayscale, ChainDst{out, out_step, original, original_step}, info);
 } catch (...) { return on_exception(h); }
 
+extern "C" mc_status mc_chain_submit_yuv420p(mc_handle* h, const mc_yuv420p* in, int width, int height, const mc_params* p,
+                                             int grayscale, uint8_t* out, size_t out_step, uint8_t* original, size_t original_step,
+                                             mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    return chain_submit(h, Source::yuv420p(in, width, height), p, grayscale, ChainDst{out, out_step, original, original_step},
+                        info);
+} catch (...) { return on_exception(h); }
+
 // ---- the export canvas from host clips: compose submits, collected by mc_collect -----------------------------------------
 namespace {
-// The planes of the canvases of a cw x ch canvas geometry (BGR, or NV12 luma and Cb,Cr), virtual lane v at v * lane_stride.
+// The planes of the canvases of a cw x ch canvas geometry (BGR; NV12 luma and Cb,Cr; I420 luma, Cb and Cr), virtual lane v at
+// v * lane_stride.  Only the canvas_w (chroma: canvas_w / 2) bytes of each row are copied.
 Planes canvas_planes(const mc_canvas& c, int cw, int ch) {
-    if (c.format == MC_CANVAS_NV12) return Planes{{c.data, c.uv}, {(size_t)ch, (size_t)ch / 2}, (size_t)cw, c.pitch, c.lane_stride};
-    return Planes{{c.data, nullptr}, {(size_t)ch, 0}, (size_t)cw * 3, c.pitch, c.lane_stride};
+    const size_t w = (size_t)cw, hh = (size_t)ch;
+    if (c.format == MC_CANVAS_NV12) return Planes{{c.data, c.uv}, {hh, hh / 2}, {w, w}, {c.pitch, c.pitch}, c.lane_stride};
+    if (c.format == MC_CANVAS_I420)
+        return Planes{{c.data, c.uv, c.uv + c.pitch / 2 * (hh / 2)}, {hh, hh / 2, hh / 2}, {w, w / 2, w / 2},
+                      {c.pitch, c.pitch / 2, c.pitch / 2}, c.lane_stride};
+    return Planes{{c.data}, {hh}, {w * 3}, {c.pitch}, c.lane_stride};
 }
 
 // The body of the compose submits: every check of the matching device compose call (without its refusal while frames are
@@ -1913,11 +2011,11 @@ mc_status compose_submit(mc_handle* h, const Source& s, int frames, const mc_par
     int fw, fh;
     canvas_size(full, cmp.split, fw, fh);
     const size_t reserve =
-        ((size_t)fw * fh * (cmp.canvas->format == MC_CANVAS_NV12 ? 3 : 6) / 2 * frames * h->lanes + 255) / 256 * 256;
+        ((size_t)fw * fh * (cmp.canvas->format == MC_CANVAS_BGR ? 6 : 3) / 2 * frames * h->lanes + 255) / 256 * 256;
     const size_t lanes = (size_t)h->lanes, vl = (size_t)frames * lanes;
     return submit_impl(h, src, dst, [&](const Planes& d_in, const Planes* d_out, int* any, uint8_t* flags,
                                         std::vector<uint8_t>* written) {
-        const mc_canvas slot{cmp.canvas->format, d_out[0].base[0], d_out[0].base[1], d_out[0].pitch, d_out[0].lane_stride};
+        const mc_canvas slot{cmp.canvas->format, d_out[0].base[0], d_out[0].base[1], d_out[0].pitch[0], d_out[0].lane_stride};
         const mc_status rs = chain_run(h, g, s.on(d_in), frames, p, ChainDst{.cmp = ComposeReq{cmp.split, &slot}}, flags);
         if (rs != MC_OK) return rs;
         *any = std::any_of(flags, flags + vl, [](uint8_t x) { return x != 0; });
@@ -1952,6 +2050,14 @@ extern "C" mc_status mc_chain_compose_submit_yuv422(mc_handle* h, const mc_yuv42
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
     return compose_submit(h, Source::yuv422(in, width, height), frames, p, grayscale, ComposeReq{split, canvas}, produced, info);
+} catch (...) { return on_exception(h); }
+
+extern "C" mc_status mc_chain_compose_submit_yuv420p(mc_handle* h, const mc_yuv420p* in, int frames, int width, int height,
+                                                     const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                                                     uint8_t* produced, mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    return compose_submit(h, Source::yuv420p(in, width, height), frames, p, grayscale, ComposeReq{split, canvas}, produced, info);
 } catch (...) { return on_exception(h); }
 
 /* test hooks, not declared in the public header: the two conversion kernels alone on device buffers (default stream,

@@ -161,13 +161,20 @@ cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16
                           bool luma_only = false, const float* lane_chroma = nullptr, int chroma_lanes = 1);
 
 // PreprocessProcessor + GrayscaleProcessor on the device (mc_preprocess.cu): one launch over `vlanes` virtual lanes.
-// FRONT_YUYV + mc_yuv422_order is the packed 4:2:2 source of that byte order.
+// FRONT_YUYV + mc_yuv422_order is the packed 4:2:2 source of that byte order.  FRONT_NV12 is any 4:2:0 source, NV12 or
+// I420 / YV12, told apart only by its chroma addressing (cb, cr, cpitch, cstep below).
 enum FrontSrc { FRONT_BGR = 0, FRONT_GRAY = 1, FRONT_NV12 = 2, FRONT_YUYV = 3, FRONT_UYVY = 4 };
 enum FrontKind { FRONT_COPY = 0, FRONT_AREA_FAST = 1, FRONT_AREA = 2 };   // crop only / integer INTER_AREA / general INTER_AREA
+// The chroma of a 4:2:0 frame: the Cb and Cr of its 2x2 block (bx, by) are at cb[by * cpitch + bx * cstep] and
+// cr[by * cpitch + bx * cstep].  NV12: cr = cb + 1, cstep 2, cpitch = the luma pitch; I420: two planes, cstep 1.
+constexpr int kNv12ChromaStep = 2, kI420ChromaStep = 1;
 struct FrontArgs {
-    const uint8_t* src = nullptr;   // lane 0's frame (BGR / gray / YUYV / UYVY) or luma plane (NV12)
-    const uint8_t* uv = nullptr;    // NV12: lane 0's Cb,Cr plane
-    size_t step = 0, lane_stride = 0;   // row pitch and virtual-lane stride of the source (both NV12 planes)
+    const uint8_t* src = nullptr;   // lane 0's frame (BGR / gray / YUYV / UYVY) or luma plane (4:2:0)
+    const uint8_t* cb = nullptr;    // 4:2:0: lane 0's chroma, addressed as above
+    const uint8_t* cr = nullptr;
+    size_t cpitch = 0;
+    int cstep = kNv12ChromaStep;
+    size_t step = 0, lane_stride = 0;   // row pitch and virtual-lane stride of the source (the same for every plane)
     int rx = 0, ry = 0;             // ROI origin in the source
     int dw = 0, dh = 0;             // output size
     int kind = FRONT_COPY, isx = 1, isy = 1;
@@ -180,15 +187,17 @@ struct FrontArgs {
 };
 cudaError_t launch_chain_front(const FrontArgs& a, int src, int vlanes, cudaStream_t s);
 
-// NV12 hand-off (mc_preprocess.cu).  An NV12 frame set: `lanes` frames, lane k's luma plane at y + k * lane_stride (h rows of
-// w bytes) and its interleaved Cb,Cr plane at uv + k * lane_stride (h / 2 rows); both planes `pitch` bytes per row.
-// BGR frames are packed u8 BGR, lane k at bgr + k * bgr_step * h.  w and h are even.
+// NV12 hand-off (mc_preprocess.cu).  A 4:2:0 frame set: `lanes` frames, lane k's luma plane at y + k * lane_stride (h rows of
+// w bytes, `pitch` apart) and its chroma at cb / cr + k * lane_stride, addressed as FrontArgs describes (h / 2 rows): NV12
+// (interleaved Cb,Cr) or I420.  BGR frames are packed u8 BGR, lane k at bgr + k * bgr_step * h.  w and h are even.
 struct Nv12Planes {
     const uint8_t* y = nullptr;
-    const uint8_t* uv = nullptr;
-    size_t pitch = 0, lane_stride = 0;
+    const uint8_t* cb = nullptr;
+    const uint8_t* cr = nullptr;
+    size_t pitch = 0, cpitch = 0, lane_stride = 0;
+    int cstep = kNv12ChromaStep;
 };
-// cvtColor(YUV2BGR_NV12) of every lane
+// cvtColor(YUV2BGR_NV12) (I420: YUV2BGR_I420, the same arithmetic) of every lane
 cudaError_t launch_nv12_to_bgr(const Nv12Planes& in, int w, int h, int lanes, uint8_t* bgr, size_t bgr_step, cudaStream_t s);
 // cvtColor(BGR2YUV_I420) of every lane whose flag is set (flags: one byte per lane, or null for all), chroma interleaved
 cudaError_t launch_bgr_to_nv12(const uint8_t* bgr, size_t bgr_step, int w, int h, int lanes, const uint8_t* flags,
@@ -196,12 +205,16 @@ cudaError_t launch_bgr_to_nv12(const uint8_t* bgr, size_t bgr_step, int w, int h
 
 // The export canvas (mc_preprocess.cu): Exporter.cpp's compose(original, cur, split) over virtual lanes, its labels as
 // the handle's overlay (mc_set_overlay): per-pixel u8 tone maps inside at most kOverlayRects disjoint canvas rects.
-// A pane source holds virtual lane v's frame at p + v * lane_stride (NV12: its Cb,Cr plane at uv + v * lane_stride).
+// A pane source holds virtual lane v's frame at p + v * lane_stride (4:2:0: its chroma at cb / cr + v * lane_stride,
+// addressed as FrontArgs describes).
 struct PaneSrc {
     const uint8_t* p = nullptr;
-    const uint8_t* uv = nullptr;
+    const uint8_t* cb = nullptr;
     size_t step = 0, lane_stride = 0;
-    int kind = FRONT_BGR;           // FrontSrc: BGR, gray (expanded as GRAY2BGR), NV12 or YUYV / UYVY (converted as cvtColor)
+    int kind = FRONT_BGR;           // FrontSrc: BGR, gray (expanded as GRAY2BGR), 4:2:0 or YUYV / UYVY (converted as cvtColor)
+    const uint8_t* cr = nullptr;
+    size_t cpitch = 0;
+    int cstep = kNv12ChromaStep;
 };
 // Which frame is virtual lane v's `cur` pane
 enum ComposeOp : uint8_t { COMPOSE_SKIP = 0, COMPOSE_MAGNIFIED = 1, COMPOSE_FALLBACK = 2 };
@@ -215,9 +228,10 @@ struct ComposeArgs {
     const uint8_t* ops = nullptr;   // ComposeOp per virtual lane; null: every lane MAGNIFIED
     int split = 0;                  // mc_split: the original pane is read only when it is not MC_SPLIT_NONE
     int w = 0, h = 0;               // pane size: even and > 0
-    int nv12 = 0;                   // canvas format: packed BGR (0) or NV12 (1)
-    uint8_t* data = nullptr;        // BGR canvas or NV12 luma plane of virtual lane 0
-    uint8_t* uv = nullptr;          // NV12: Cb,Cr plane of virtual lane 0
+    int nv12 = 0;                   // canvas format: packed BGR (0) or 4:2:0 (1: NV12, or I420 when cr is set)
+    uint8_t* data = nullptr;        // BGR canvas or luma plane of virtual lane 0
+    uint8_t* uv = nullptr;          // NV12: Cb,Cr plane of virtual lane 0; I420: its Cb plane
+    uint8_t* cr = nullptr;          // I420: Cr plane of virtual lane 0, rows pitch / 2 apart in both chroma planes; NV12: null
     size_t pitch = 0, lane_stride = 0;
     int ov_rects = 0;               // the overlay: 0 .. kOverlayRects rects; 0 leaves every canvas as composed
     OverlayRect ov[kOverlayRects];

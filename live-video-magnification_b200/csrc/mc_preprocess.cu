@@ -1,9 +1,9 @@
 // Front of the reference chain fused onto the device (SURVEY.md 8f-1): PreprocessProcessor (normalised ROI crop +
 // INTER_AREA 1/2..1/8 downscale, reference src/processing/PreprocessProcessor.cpp:10-51) and GrayscaleProcessor
 // (BGR2GRAY, src/processing/GrayscaleProcessor.cpp:7-16), bit-exact with OpenCV's u8 paths (mc_math.cuh), in one kernel
-// over every virtual lane whose source is u8 BGR, u8 gray, NV12 planes or a packed 4:2:2 camera frame (YUYV / UYVY; an
-// NV12 or 4:2:2 pixel is converted as cvtColor converts it inside the tap walk, so no full-resolution BGR frame needs to
-// be stored); and the NV12
+// over every virtual lane whose source is u8 BGR, u8 gray, 4:2:0 planes (NV12 or I420 / YV12) or a packed 4:2:2 camera
+// frame (YUYV / UYVY; a 4:2:0 or 4:2:2 pixel is converted as cvtColor converts it inside the tap walk, so no
+// full-resolution BGR frame needs to be stored); and the NV12
 // conversions around the magnifier for the video decoder / encoder hand-off, and the export canvas built from the chain's
 // two taps (the exporter's compose, SURVEY.md 8f-2).
 #include "../../include/magcore_b200.h"
@@ -36,6 +36,19 @@ template <> struct FrontPx<FRONT_NV12> {   // cvtColor(YUV2BGR_NV12) of the pixe
         v[0] = b; v[1] = g; v[2] = r;
     }
 };
+// cvtColor(YUV2BGR_I420) of the pixel: the same arithmetic, its block's Cb and Cr from two planes `cpitch` bytes per row.
+// The FRONT_NV12 instance walks its taps with this functor when the chroma is planar (FrontArgs::cstep), so the NV12 walk
+// keeps the address arithmetic of an interleaved pair.
+struct I420Px {
+    const uint8_t* y; const uint8_t* u; const uint8_t* w; size_t pitch, cpitch; int ox, oy;
+    __device__ void operator()(int sx, int sy, int (&v)[3]) const {
+        const int ax = ox + sx, ay = oy + sy;
+        const size_t c = (size_t)(ay >> 1) * cpitch + (ax >> 1);
+        uint8_t b, g, r;
+        nv12_to_bgr_px(__ldg(y + (size_t)ay * pitch + ax), __ldg(u + c), __ldg(w + c), b, g, r);
+        v[0] = b; v[1] = g; v[2] = r;
+    }
+};
 // cvtColor(YUV2BGR_YUYV / _UYVY) of the pixel: its Y and its group's Cb,Cr, the group read as one 32-bit word when every
 // group is 4-byte aligned (vec), else byte by byte.  p is the ROI's first row; the group of a pixel follows from its
 // column in the frame (ox + sx), so a crop at an odd column still pairs the frame's pixels.
@@ -55,6 +68,13 @@ template <bool UYVY> struct Yuv422Px {
 template <> struct FrontPx<FRONT_YUYV> : Yuv422Px<false> {};
 template <> struct FrontPx<FRONT_UYVY> : Yuv422Px<true> {};
 
+// The preprocessed pixel (x, y): its ROI tap, or its INTER_AREA taps, read through px.
+template <int CN, class Px>
+__device__ __forceinline__ void front_walk(const FrontArgs& a, const Px& px, int x, int y, int (&o)[CN]) {
+    if (a.kind == FRONT_COPY) px(x, y, o);
+    else resize_area_px<CN>(px, y, x, a.isx, a.isy, a.kind == FRONT_AREA_FAST, a.xtab, a.xofs, a.ytab, a.yofs, o);
+}
+
 // One thread per output pixel of one virtual lane (blockIdx.z): every channel of the preprocessed pixel and its gray
 // byte from one walk over the pixel's source taps.
 template <int SRC>
@@ -63,17 +83,20 @@ __global__ void __launch_bounds__(256) k_chain_front(const FrontArgs a) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
     const size_t v = blockIdx.z;
     if (x >= a.dw || (a.flags && !a.flags[v])) return;
-    FrontPx<SRC> px;
-    if constexpr (SRC == FRONT_NV12) {
-        px = FrontPx<SRC>{a.src + v * a.lane_stride, a.uv + v * a.lane_stride, a.step, a.rx, a.ry};
-    } else if constexpr (SRC == FRONT_YUYV || SRC == FRONT_UYVY) {
-        px.p = a.src + v * a.lane_stride + (size_t)a.ry * a.step; px.pitch = a.step; px.ox = a.rx; px.vec = a.vec != 0;
-    } else {
-        px = FrontPx<SRC>{a.src + v * a.lane_stride + (size_t)a.ry * a.step + (size_t)CN * a.rx, a.step};
-    }
     int o[CN];
-    if (a.kind == FRONT_COPY) px(x, y, o);
-    else resize_area_px<CN>(px, y, x, a.isx, a.isy, a.kind == FRONT_AREA_FAST, a.xtab, a.xofs, a.ytab, a.yofs, o);
+    if constexpr (SRC == FRONT_NV12) {   // one uniform branch on the chroma layout
+        const size_t l = v * a.lane_stride;
+        if (a.cstep == kNv12ChromaStep) front_walk(a, FrontPx<SRC>{a.src + l, a.cb + l, a.step, a.rx, a.ry}, x, y, o);
+        else front_walk(a, I420Px{a.src + l, a.cb + l, a.cr + l, a.step, a.cpitch, a.rx, a.ry}, x, y, o);
+    } else {
+        FrontPx<SRC> px;
+        if constexpr (SRC == FRONT_YUYV || SRC == FRONT_UYVY) {
+            px.p = a.src + v * a.lane_stride + (size_t)a.ry * a.step; px.pitch = a.step; px.ox = a.rx; px.vec = a.vec != 0;
+        } else {
+            px = FrontPx<SRC>{a.src + v * a.lane_stride + (size_t)a.ry * a.step + (size_t)CN * a.rx, a.step};
+        }
+        front_walk(a, px, x, y, o);
+    }
     if (a.dst) {
         uint8_t* d = a.dst + v * a.dst_lane_stride + (size_t)y * a.dst_step + (size_t)CN * x;
 #pragma unroll
@@ -104,11 +127,12 @@ cudaError_t launch_chain_front(const FrontArgs& args, int src, int vlanes, cudaS
 // conversions to and from the packed BGR frames the modes work on, bit-exact with OpenCV's u8 fixed point
 // (nv12_to_bgr_px / bgr_to_ycc_px in mc_math.cuh); and the export canvas of Exporter.cpp:25-34, 53-88 (labels as the
 // handle's overlay of per-pixel tone maps),
-// whose panes are BGR, gray (GRAY2BGR) or NV12 sources and whose canvas is BGR or NV12.  All three kernels are
-// bandwidth-bound: 1.5 B/px of NV12 and 3 B/px of BGR per pixel.  A thread owns a 2-row x 8-column block: one 64-bit load
-// or store per luma or gray row, one for the 4 Cb,Cr pairs of the block, and three per BGR row (24 bytes); rows or
-// pointers that are not 8-byte aligned, a canvas block that does not start on an 8-byte boundary, and the last columns
-// of a row whose width is not a multiple of 8, take the byte path.  The compose kernel with one BGR pane does
+// whose panes are BGR, gray (GRAY2BGR), 4:2:0 or 4:2:2 sources and whose canvas is BGR, NV12 or I420.  All three kernels
+// are bandwidth-bound: 1.5 B/px of 4:2:0 and 3 B/px of BGR per pixel.  A thread owns a 2-row x 8-column block: one 64-bit
+// load or store per luma or gray row, one for the 4 Cb,Cr pairs of the block (I420: one 32-bit access per chroma plane),
+// and three per BGR row (24 bytes); rows or pointers that are not 8-byte aligned (I420 chroma: 4-byte), a canvas block
+// that does not start on an 8-byte boundary, and the last columns of a row whose width is not a multiple of 8, take the
+// byte path.  NV12 and I420 differ only in the chroma addressing (FrontArgs in mc_internal.h), one uniform branch.  The compose kernel with one BGR pane does
 // k_bgr_to_nv12's job, but measured 3.64 against 3.45 us per 1080p frame on an H100 (tools/bench_nv12.py), so the NV12
 // egress keeps its own kernel.
 
@@ -117,13 +141,11 @@ namespace {
 constexpr int kBlockX = 32, kBlockY = 4;   // threads: 32 column groups of 8 x 4 row pairs
 
 struct ToBgrArgs {
-    const uint8_t* y;
-    const uint8_t* uv;
-    size_t pitch, lane_stride;
+    Nv12Planes in;
     uint8_t* bgr;
     size_t bgr_step;
     int w, h;
-    int vec_in, vec_out;   // the NV12 planes / the BGR rows allow 64-bit accesses
+    int vec_in, vec_out;   // the 4:2:0 planes / the BGR rows allow 64-bit (I420 chroma: 32-bit) accesses
 };
 
 struct ToNv12Args {
@@ -151,9 +173,38 @@ __device__ __forceinline__ void load8(const uint8_t* __restrict__ p, bool vec, i
     }
 }
 
+__device__ __forceinline__ void load4(const uint8_t* __restrict__ p, bool vec, int n, uint8_t (&v)[4]) {
+    if (vec) {
+        const unsigned q = __ldg(reinterpret_cast<const unsigned*>(p));
+#pragma unroll
+        for (int i = 0; i < 4; ++i) v[i] = (uint8_t)(q >> (8 * i));
+    } else {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) v[i] = i < n ? __ldg(p + i) : (uint8_t)0;
+    }
+}
+
+// The Cb (u) and Cr (w) of the n / 2 2x2 blocks from column x0 (even) in chroma row r of a 4:2:0 frame's lane: one 64-bit
+// load of the interleaved pairs (NV12) or one 32-bit load per plane (I420).
+__device__ __forceinline__ void load_chroma(const uint8_t* cb, const uint8_t* cr, size_t cpitch, int cstep, bool vec, int x0,
+                                            int r, int n, uint8_t (&u)[4], uint8_t (&w)[4]) {
+    const size_t o = (size_t)r * cpitch + (size_t)(x0 >> 1) * cstep;
+    if (cstep == kNv12ChromaStep) {
+        uint8_t c[8];
+        load8(cb + o, vec, n, c);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { u[i] = c[2 * i]; w[i] = c[2 * i + 1]; }
+    } else {
+        load4(cb + o, vec, n / 2, u);
+        load4(cr + o, vec, n / 2, w);
+    }
+}
+
 template <int N>
 __device__ __forceinline__ void store(uint8_t* __restrict__ p, bool vec, int n, const uint8_t (&v)[N]) {
-    if (vec) {
+    if (vec && N == 4) {   // one 32-bit store (an I420 chroma row of a block)
+        *reinterpret_cast<unsigned*>(p) = (unsigned)v[0] | (unsigned)v[1] << 8 | (unsigned)v[2] << 16 | (unsigned)v[3] << 24;
+    } else if (vec) {
 #pragma unroll
         for (int j = 0; j < N / 8; ++j) {
             uint2 q;
@@ -175,15 +226,17 @@ __global__ void __launch_bounds__(kBlockX * kBlockY) k_nv12_to_bgr(const ToBgrAr
     const size_t lane = blockIdx.z;
     const int n = min(8, a.w - x0);                     // even: w is
     const bool full = n == 8;
-    const uint8_t* yp = a.y + lane * a.lane_stride + (size_t)(2 * r) * a.pitch + x0;
-    uint8_t y0[8], y1[8], c[8];
+    const Nv12Planes& in = a.in;
+    const uint8_t* yp = in.y + lane * in.lane_stride + (size_t)(2 * r) * in.pitch + x0;
+    uint8_t y0[8], y1[8], cu[4], cv[4];
     load8(yp, full && a.vec_in, n, y0);
-    load8(yp + a.pitch, full && a.vec_in, n, y1);
-    load8(a.uv + lane * a.lane_stride + (size_t)r * a.pitch + x0, full && a.vec_in, n, c);
+    load8(yp + in.pitch, full && a.vec_in, n, y1);
+    load_chroma(in.cb + lane * in.lane_stride, in.cr + lane * in.lane_stride, in.cpitch, in.cstep, full && a.vec_in, x0, r, n,
+                cu, cv);
     uint8_t o0[24], o1[24];
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-        const int u = c[i & ~1], v = c[i | 1];
+        const int u = cu[i >> 1], v = cv[i >> 1];
         nv12_to_bgr_px(y0[i], u, v, o0[3 * i], o0[3 * i + 1], o0[3 * i + 2]);
         nv12_to_bgr_px(y1[i], u, v, o1[3 * i], o1[3 * i + 1], o1[3 * i + 2]);
     }
@@ -225,19 +278,19 @@ __global__ void __launch_bounds__(kBlockX * kBlockY) k_bgr_to_nv12(const ToNv12A
     store(a.uv + lane * a.lane_stride + (size_t)r * a.pitch + x0, full && a.vec_out, n, c);
 }
 // Two rows (2r, 2r + 1) of n <= 8 pixels from column x0 of virtual lane v's frame in a pane source, as BGR bytes: gray
-// expanded as GRAY2BGR, NV12 and YUYV / UYVY converted as cvtColor does (x0 and n are even, so the Cb,Cr pairs and the
-// 4:2:2 groups are whole).
+// expanded as GRAY2BGR, NV12 / I420 and YUYV / UYVY converted as cvtColor does (x0 and n are even, so the Cb,Cr pairs and
+// the 4:2:2 groups are whole).
 __device__ __forceinline__ void load_pane(const PaneSrc& s, bool vec, size_t v, int x0, int r, int n, uint8_t (&o0)[24],
                                           uint8_t (&o1)[24]) {
     const uint8_t* row = s.p + v * s.lane_stride + (size_t)(2 * r) * s.step;
     if (s.kind == FRONT_NV12) {
-        uint8_t y0[8], y1[8], c[8];
+        uint8_t y0[8], y1[8], cu[4], cv[4];
         load8(row + x0, vec, n, y0);
         load8(row + s.step + x0, vec, n, y1);
-        load8(s.uv + v * s.lane_stride + (size_t)r * s.step + x0, vec, n, c);
+        load_chroma(s.cb + v * s.lane_stride, s.cr + v * s.lane_stride, s.cpitch, s.cstep, vec, x0, r, n, cu, cv);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-            const int u = c[i & ~1], w = c[i | 1];
+            const int u = cu[i >> 1], w = cv[i >> 1];
             nv12_to_bgr_px(y0[i], u, w, o0[3 * i], o0[3 * i + 1], o0[3 * i + 2]);
             nv12_to_bgr_px(y1[i], u, w, o1[3 * i], o1[3 * i + 1], o1[3 * i + 2]);
         }
@@ -353,7 +406,16 @@ __global__ void __launch_bounds__(kBlockX * kBlockY, 8) k_compose(const ComposeA
         }
         store(row + cx, vec, n, y0);
         store(row + a.pitch + cx, vec, n, y1);
-        store(a.uv + v * a.lane_stride + (size_t)(cy / 2) * a.pitch + cx, vec, n, c);
+        if (a.cr) {   // I420: the block's 4 Cb and 4 Cr bytes into their planes, rows pitch / 2 apart
+            uint8_t cu[4], cv[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) { cu[k] = c[2 * k]; cv[k] = c[2 * k + 1]; }
+            const size_t o = v * a.lane_stride + (size_t)(cy / 2) * (a.pitch / 2) + cx / 2;
+            store(a.uv + o, vec, n / 2, cu);
+            store(a.cr + o, vec, n / 2, cv);
+        } else {
+            store(a.uv + v * a.lane_stride + (size_t)(cy / 2) * a.pitch + cx, vec, n, c);
+        }
     } else {
         store(row + (size_t)3 * cx, vec, 3 * n, p0);
         if (ov) overlay_row(a, cx, cy + 1, p1);
@@ -362,6 +424,13 @@ __global__ void __launch_bounds__(kBlockX * kBlockY, 8) k_compose(const ComposeA
 }
 
 bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
+bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
+
+// The chroma of a 4:2:0 frame allows the vector accesses of load_chroma / the compose kernel's chroma stores: 8-byte
+// interleaved pairs (NV12; the luma checks cover the pitch) or 4-byte rows of both planes (I420).
+bool chroma_vec(const uint8_t* cb, const uint8_t* cr, size_t cpitch, int cstep) {
+    return cstep == kNv12ChromaStep ? aligned8(cb) : aligned4(cb) && aligned4(cr) && cpitch % 4 == 0;
+}
 
 dim3 grid_of(int w, int h, int lanes) {
     const int groups = (w + 7) / 8;
@@ -372,9 +441,10 @@ dim3 grid_of(int w, int h, int lanes) {
 
 cudaError_t launch_nv12_to_bgr(const Nv12Planes& in, int w, int h, int lanes, uint8_t* bgr, size_t bgr_step, cudaStream_t s) {
     ToBgrArgs a;
-    a.y = in.y; a.uv = in.uv; a.pitch = in.pitch; a.lane_stride = in.lane_stride;
+    a.in = in;
     a.bgr = bgr; a.bgr_step = bgr_step; a.w = w; a.h = h;
-    a.vec_in = aligned8(in.y) && aligned8(in.uv) && in.pitch % 8 == 0 && (lanes == 1 || in.lane_stride % 8 == 0);
+    a.vec_in = aligned8(in.y) && chroma_vec(in.cb, in.cr, in.cpitch, in.cstep) && in.pitch % 8 == 0 &&
+               (lanes == 1 || in.lane_stride % 8 == 0);
     a.vec_out = aligned8(bgr) && bgr_step % 8 == 0;
     k_nv12_to_bgr<<<grid_of(w, h, lanes), dim3(kBlockX, kBlockY), 0, s>>>(a);
     return cudaGetLastError();
@@ -385,11 +455,12 @@ cudaError_t launch_compose(ComposeArgs a, int vlanes, cudaStream_t s) {
     a.vec_src = 0;
     for (int i = 0; i < 3; ++i) {
         const PaneSrc& p = a.src[i];
-        const bool vec = p.p && aligned8(p.p) && (p.kind != FRONT_NV12 || aligned8(p.uv)) && p.step % 8 == 0 &&
-                         (lane_vec || p.lane_stride % 8 == 0);
+        const bool vec = p.p && aligned8(p.p) && (p.kind != FRONT_NV12 || chroma_vec(p.cb, p.cr, p.cpitch, p.cstep)) &&
+                         p.step % 8 == 0 && (lane_vec || p.lane_stride % 8 == 0);
         a.vec_src |= (int)vec << i;
     }
-    a.vec_out = aligned8(a.data) && (!a.nv12 || aligned8(a.uv)) && a.pitch % 8 == 0 && (lane_vec || a.lane_stride % 8 == 0);
+    a.vec_out = aligned8(a.data) && (!a.nv12 || (a.cr ? aligned4(a.uv) && aligned4(a.cr) : aligned8(a.uv))) && a.pitch % 8 == 0 &&
+                (lane_vec || a.lane_stride % 8 == 0);
     const int panes = a.split == MC_SPLIT_NONE ? 1 : 2;
     dim3 grid = grid_of(a.w, a.h, vlanes);
     a.pane_blocks = (int)grid.y;
