@@ -395,15 +395,21 @@ mc_status mc_chain_process_nv12_device(mc_handle* h, const mc_nv12* in, int fram
  *   MC_SPLIT_TOP_BOTTOM  the original pane above the processed one: w x 2h
  * A canvas is packed BGR (pitch >= 3 * its width), NV12 (pitch >= its width; cvtColor(COLOR_BGR2YUV_I420) of the BGR
  * canvas with Cb,Cr interleaved, as the NV12 calls write) or I420 (the planes cvtColor(COLOR_BGR2YUV_I420) returns; see
- * the planar 4:2:0 section).  Its dimensions are always even, so a 4:2:0 canvas always exists when the BGR one does. */
+ * the planar 4:2:0 section), or RGB: packed R,G,B (MC_CANVAS_RGB, pitch >= 3 * its width) or three planes R, G, B
+ * (MC_CANVAS_RGB_PLANAR; see the RGB section).  Its dimensions are always even, so a 4:2:0 canvas always exists when the
+ * BGR one does. */
 typedef enum mc_split { MC_SPLIT_NONE = 0, MC_SPLIT_LEFT_RIGHT = 1, MC_SPLIT_TOP_BOTTOM = 2 } mc_split; /* livim::SplitMode */
-typedef enum mc_canvas_format { MC_CANVAS_BGR = 0, MC_CANVAS_NV12 = 1, MC_CANVAS_I420 = 2 } mc_canvas_format;
+typedef enum mc_canvas_format {
+    MC_CANVAS_BGR = 0, MC_CANVAS_NV12 = 1, MC_CANVAS_I420 = 2, MC_CANVAS_RGB = 3, MC_CANVAS_RGB_PLANAR = 4
+} mc_canvas_format;
 typedef struct mc_canvas {
     int32_t format;       /* mc_canvas_format */
-    uint8_t* data;        /* BGR: canvas of virtual lane 0; NV12 / I420: its luma plane */
+    uint8_t* data;        /* BGR / RGB: canvas of virtual lane 0; NV12 / I420: its luma plane; RGB_PLANAR: its R plane,
+                             with the G and B planes at data + pitch * canvas_h and data + 2 * pitch * canvas_h */
     uint8_t* uv;          /* NV12: interleaved Cb,Cr plane (need not follow the luma); I420: Cb plane, with the Cr plane
-                             at uv + (pitch / 2) * (canvas_h / 2); BGR: unused */
-    size_t pitch;         /* bytes per row (both NV12 planes; the I420 luma plane, whose chroma rows are pitch / 2 apart) */
+                             at uv + (pitch / 2) * (canvas_h / 2); BGR, RGB, RGB_PLANAR: unused */
+    size_t pitch;         /* bytes per row (both NV12 planes; the I420 luma plane, whose chroma rows are pitch / 2 apart;
+                             each RGB_PLANAR plane) */
     size_t lane_stride;   /* bytes from one virtual lane's canvas (planes) to the next */
 } mc_canvas;
 
@@ -450,8 +456,9 @@ mc_status mc_chain_compose_nv12_device(mc_handle* h, const mc_nv12* in, int fram
  *   Stream order: mc_set_overlay copies the overlay to device memory in stream order on mc_stream().  Compose calls
  *     enqueued before it use the previous overlay, calls after it the new one.  The caller's buffers may be freed as
  *     soon as it returns.
- *   Every compose call (BGR, NV12, YUYV and I420 sources; BGR, NV12 and I420 canvases; frames, clips and lanes) maps each
- *     canvas it writes: a canvas pixel inside a rect becomes map[index][v] in each of its channels, before the 4:2:0 conversion (a
+ *   Every compose call (BGR, NV12, YUYV, I420 and RGB sources; BGR, NV12, I420 and RGB canvases; frames, clips and lanes)
+ *     maps each canvas it writes: a canvas pixel inside a rect becomes map[index][v] in each of its channels, before the
+ *     4:2:0 conversion or the RGB channel order (a
  *     2x2 block whose top-left pixel is labelled takes its Cb,Cr from the labelled value).  Held lanes and 0 x 0
  *     canvases stay untouched, as without an overlay.  Chain calls that do not compose ignore it.
  *   Errors, MC_ERR_INVALID: mc_set_overlay with canvas_w or canvas_h < 1, rects or maps out of range, a NULL map or
@@ -616,6 +623,63 @@ mc_status mc_chain_submit_yuv420p(mc_handle* h, const mc_yuv420p* in, int width,
 mc_status mc_chain_compose_submit_yuv420p(mc_handle* h, const mc_yuv420p* in, int frames, int width, int height,
                                           const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
                                           uint8_t* produced, mc_chain_info* info);
+
+/* --- RGB frames (packed RGB, RGBA / BGRA, planar RGB): PyTorch tensors, Python image libraries and desktop capture ------
+ * torchvision's decode_jpeg(device="cuda") returns planar RGB (3, H, W) u8 tensors and image models take (N, 3, H, W)
+ * batches; PyAV's to_ndarray(format="rgb24"), PIL and imageio hand out packed RGB; desktop and GPU capture (Media
+ * Foundation RGB32, CoreVideo 32BGRA, GStreamer BGRx / RGBA, GL readbacks) hand out 32-bit BGRA / RGBA pixels.  The core
+ * reads every such frame where it is and swaps its channels on the device.
+ *   Equivalence, input: let X be any RGB input and B = cv2.cvtColor(X, COLOR_RGB2BGR / COLOR_RGBA2BGR / COLOR_BGRA2BGR)
+ *     (planar X: cv2.merge([B_plane, G_plane, R_plane])).  Every call on X equals, bit for bit, the BGR call on B: the
+ *     processed frames, the original tap, the produced flags, mc_lane_produced and the temporal state afterwards.  The
+ *     conversion is a front stage that always runs, as for 4:2:2: `info` has cur_is_input = orig_is_input = 0, and
+ *     d_out / d_original receive B (or its BGR2GRAY under grayscale) where a BGR call would leave the result to the
+ *     input.  RGB, BGR, NV12, 4:2:2 and I420 calls of one geometry interleave on a handle without a structural reset
+ *     (the tracker sees channels 3).  The 4th byte of an RGBA / BGRA pixel is never read.
+ *   Equivalence, canvas: an MC_CANVAS_RGB canvas is cv2.cvtColor(bgr_canvas, COLOR_BGR2RGB) of the BGR canvas of the
+ *     same call, labels included (the overlay's tone maps act on each channel alike); an MC_CANVAS_RGB_PLANAR canvas is
+ *     that BGR canvas's channels 2, 1, 0 as planes, one CHW tensor per virtual lane.  Every compose call accepts both:
+ *     BGR, gray, NV12, 4:2:2, I420 and RGB sources; device and submit; frames, clips and lanes.  Held lanes, 0 x 0
+ *     canvases, row padding and the padding after each plane stay untouched.
+ *   Errors, returned before any kernel or copy runs, with no caller buffer, state or frame in flight changed:
+ *     MC_ERR_INVALID for a NULL descriptor, data or (planar) g / b, a layout out of range, width or height < 1, pitch <
+ *     width * bytes per pixel (planar: < width), lane_stride < pitch * height with more than one virtual lane, and every
+ *     argument error of the BGR twin.  An RGB canvas: MC_ERR_INVALID for a NULL data, pitch < 3 * canvas_w (planar: <
+ *     canvas_w) and, with more than one virtual lane, lane_stride < pitch * canvas_h (planar: < 3 * pitch * canvas_h).
+ *     Color's multi-lane refusals stay MC_ERR_UNSUPPORTED.
+ *   Memory: only width * bytes per pixel of each row crosses PCIe (3 B/px; RGBA / BGRA 4 B/px), and canvases come back
+ *     at 3 B/px.  Pageable frames go through pinned staging; pinned ones are copied directly. */
+typedef enum mc_rgb_layout {
+    MC_RGB_RGB = 0,      /* packed R,G,B, 3 bytes per pixel (rgb24, HWC RGB arrays and tensors) */
+    MC_RGB_RGBA = 1,     /* packed R,G,B,A (or X), 4 bytes per pixel; the 4th byte is never read */
+    MC_RGB_BGRA = 2,     /* packed B,G,R,A (or X), 4 bytes per pixel; the 4th byte is never read */
+    MC_RGB_PLANAR = 3    /* three planes R, G, B of width bytes per row (CHW / NCHW tensors) */
+} mc_rgb_layout;
+typedef struct mc_rgb {
+    uint8_t* data;        /* packed: frame of (virtual) lane 0; planar: its R plane */
+    uint8_t* g;           /* planar: G plane; packed: unused */
+    uint8_t* b;           /* planar: B plane; packed: unused */
+    size_t pitch;         /* bytes per row (every plane) */
+    size_t lane_stride;   /* bytes from one virtual lane's frame (planes) to the next */
+    int32_t layout;       /* mc_rgb_layout */
+} mc_rgb;
+/* mc_chain_process_device on RGB device frames (frame t of lane k is virtual lane t * lanes + k) */
+mc_status mc_chain_process_rgb_device(mc_handle* h, const mc_rgb* in, int frames, int width, int height, const mc_params* p,
+                                      int grayscale, uint8_t* d_out, size_t out_step, uint8_t* d_original,
+                                      size_t original_step, uint8_t* produced, mc_chain_info* info);
+/* mc_chain_compose_device on RGB device frames: e.g. the planes of an (N, 3, H, W) CUDA tensor in, planar RGB canvases
+ * of another tensor out */
+mc_status mc_chain_compose_rgb_device(mc_handle* h, const mc_rgb* in, int frames, int width, int height, const mc_params* p,
+                                      int grayscale, int split, const mc_canvas* canvas, uint8_t* produced,
+                                      mc_chain_info* info);
+/* mc_chain_submit on RGB host frames */
+mc_status mc_chain_submit_rgb(mc_handle* h, const mc_rgb* in, int width, int height, const mc_params* p, int grayscale,
+                              uint8_t* out, size_t out_step, uint8_t* original, size_t original_step, mc_chain_info* info);
+/* mc_chain_compose_submit on RGB host frames: an exporter that decodes rgb24 or captures BGRA submits its frames as
+ * they are */
+mc_status mc_chain_compose_submit_rgb(mc_handle* h, const mc_rgb* in, int frames, int width, int height, const mc_params* p,
+                                      int grayscale, int split, const mc_canvas* canvas, uint8_t* produced,
+                                      mc_chain_info* info);
 
 /* Pinned host memory for frames (so FramePool buffers can be DMA'd directly). */
 void* mc_host_alloc(size_t bytes);

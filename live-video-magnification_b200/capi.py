@@ -56,8 +56,18 @@ class McYuv420p(C.Structure):
                 ("lane_stride", C.c_size_t)]
 
 
+MC_RGB_RGB, MC_RGB_RGBA, MC_RGB_BGRA, MC_RGB_PLANAR = 0, 1, 2, 3
+
+
+class McRgb(C.Structure):
+    """mc_rgb: one RGB frame set (packed RGB, RGBA / BGRA, or planar R, G, B planes); pointers are host or device
+    addresses as integers."""
+    _fields_ = [("data", C.c_void_p), ("g", C.c_void_p), ("b", C.c_void_p), ("pitch", C.c_size_t), ("lane_stride", C.c_size_t),
+                ("layout", C.c_int32)]
+
+
 MC_SPLIT_NONE, MC_SPLIT_LEFT_RIGHT, MC_SPLIT_TOP_BOTTOM = 0, 1, 2
-MC_CANVAS_BGR, MC_CANVAS_NV12, MC_CANVAS_I420 = 0, 1, 2
+MC_CANVAS_BGR, MC_CANVAS_NV12, MC_CANVAS_I420, MC_CANVAS_RGB, MC_CANVAS_RGB_PLANAR = 0, 1, 2, 3, 4
 
 
 class McCanvas(C.Structure):
@@ -88,6 +98,7 @@ _NV = C.POINTER(McNv12)
 _CV = C.POINTER(McCanvas)
 _YV = C.POINTER(McYuv422)
 _YP = C.POINTER(McYuv420p)
+_RG = C.POINTER(McRgb)
 SIGNATURES = {
     "mc_abi_version": (C.c_int, []),
     "mc_device_count": (C.c_int, []),
@@ -154,6 +165,14 @@ SIGNATURES = {
                                           C.POINTER(McChainInfo)]),
     "mc_chain_compose_submit_yuv420p": (C.c_int, [_vp, _YP, C.c_int, C.c_int, C.c_int, _PP, C.c_int, C.c_int, _CV, _u8p,
                                                   C.POINTER(McChainInfo)]),
+    "mc_chain_process_rgb_device": (C.c_int, [_vp, _RG, C.c_int, C.c_int, C.c_int, _PP, C.c_int, _vp, C.c_size_t, _vp,
+                                              C.c_size_t, _u8p, C.POINTER(McChainInfo)]),
+    "mc_chain_compose_rgb_device": (C.c_int, [_vp, _RG, C.c_int, C.c_int, C.c_int, _PP, C.c_int, C.c_int, _CV, _u8p,
+                                              C.POINTER(McChainInfo)]),
+    "mc_chain_submit_rgb": (C.c_int, [_vp, _RG, C.c_int, C.c_int, _PP, C.c_int, _vp, C.c_size_t, _vp, C.c_size_t,
+                                      C.POINTER(McChainInfo)]),
+    "mc_chain_compose_submit_rgb": (C.c_int, [_vp, _RG, C.c_int, C.c_int, C.c_int, _PP, C.c_int, C.c_int, _CV, _u8p,
+                                              C.POINTER(McChainInfo)]),
     "mc_process_nv12_device": (C.c_int, [_vp, _NV, C.c_int, C.c_int, _PP, _NV, C.POINTER(C.c_int)]),
     "mc_process_clip_nv12_device": (C.c_int, [_vp, _NV, C.c_int, C.c_int, C.c_int, _PP, _NV, _u8p]),
     "mc_submit_nv12": (C.c_int, [_vp, _NV, C.c_int, C.c_int, _PP, _NV]),

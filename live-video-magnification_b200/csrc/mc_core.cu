@@ -115,15 +115,20 @@ Nv12Planes yuv420_of(const Planes& f) {
     return Nv12Planes{f.base[0], f.base[1], f.base[2], f.pitch[0], f.pitch[1], f.lane_stride, kI420ChromaStep};
 }
 
-// The source frames of a call: u8 BGR or gray, 4:2:0 planes (NV12, or I420 with three planes) or packed 4:2:2 frames,
-// virtual lane v at v * planes.lane_stride.  Only these helpers tell the formats apart.
+// The source frames of a call: u8 BGR or gray, 4:2:0 planes (NV12, or I420 with three planes), packed 4:2:2 frames or
+// RGB frames (packed in one plane, planar in three), virtual lane v at v * planes.lane_stride.  Only these helpers tell
+// the formats apart.
 struct Source {
-    static constexpr int kBadOrder = FRONT_UYVY + 1;   // a 4:2:2 frame of an order out of range: refused by check()
+    static constexpr int kBadOrder = FRONT_RGB + 1;    // a 4:2:2 frame of an order out of range: refused by check()
     int kind = FRONT_BGR;                               // FrontSrc, the front's `src`
     int w = 0, hh = 0, channels = 3;                    // 4:2:0 and 4:2:2 frames stand for BGR ones
     Planes planes;
-    const char* missing = nullptr;   // the call's mc_nv12 / mc_yuv420p / mc_yuv422 is NULL: its error comes first
+    const char* missing = nullptr;   // the call's mc_nv12 / mc_yuv420p / mc_yuv422 / mc_rgb is NULL: its error comes first
     bool i420 = false;               // 4:2:0 in three planes (mc_yuv420p)
+    int layout = MC_RGB_RGB;         // FRONT_RGB: the mc_rgb_layout
+
+    // bytes per pixel of an RGB layout's plane: 3 or 4 packed, 1 planar (an out-of-range layout is refused by check())
+    static int rgb_pstep(int layout) { return layout == MC_RGB_RGB ? 3 : layout == MC_RGB_PLANAR ? 1 : 4; }
 
     static Source bgr(const uint8_t* in, int w, int hh, int c, size_t step) {
         return Source{c == 3 ? FRONT_BGR : FRONT_GRAY, w, hh, c, bgr_planes(in, w, hh, c, step)};
@@ -139,6 +144,17 @@ struct Source {
                              {f->pitch, f->chroma_pitch, f->chroma_pitch}, f->lane_stride},
                       nullptr, true};
     }
+    static Source rgb(const mc_rgb* f, int w, int hh) {
+        if (!f) return Source{FRONT_RGB, w, hh, 3, {}, "RGB frame is null"};
+        const size_t rows = (size_t)std::max(hh, 0), row = (size_t)std::max(w, 0) * rgb_pstep(f->layout);
+        Source s{FRONT_RGB, w, hh, 3};
+        s.layout = f->layout;
+        if (f->layout == MC_RGB_PLANAR)
+            s.planes = Planes{{f->data, f->g, f->b}, {rows, rows, rows}, {row, row, row}, {f->pitch, f->pitch, f->pitch}, f->lane_stride};
+        else
+            s.planes = Planes{{f->data}, {rows}, {row}, {f->pitch}, f->lane_stride};
+        return s;
+    }
     static Source yuv422(const mc_yuv422* f, int w, int hh) {
         if (!f) return Source{FRONT_YUYV, w, hh, 3, {}, "YUYV frame is null"};
         const int kind = f->order == MC_YUV422_YUYV || f->order == MC_YUV422_UYVY ? FRONT_YUYV + f->order : kBadOrder;
@@ -149,9 +165,12 @@ struct Source {
     bool bgr_or_gray() const { return kind == FRONT_BGR || kind == FRONT_GRAY; }
     // the identity: no BGR or gray frame (NV12 and 4:2:2 frames are checked instead)
     bool empty() const { return bgr_or_gray() && (!planes.base[0] || w <= 0 || hh <= 0); }
-    // the 4:2:2 conversion is a front stage that always runs: the front writes its BGR frame where a BGR source would
-    // leave the result to the input
+    // the 4:2:2 and RGB conversions are a front stage that always runs: the front writes its BGR frame where a BGR source
+    // would leave the result to the input
     bool converts() const { return kind >= FRONT_YUYV; }
+    // the compose kernel reads the original pane from the front's BGR tap rather than from the frames: RGB, whose channel
+    // swap does not fit the kernel's registers (the tap is the frame the front writes for the magnifier anyway)
+    bool composes_from_tap() const { return kind == FRONT_RGB; }
     // the source's argument errors for `vl` virtual lanes -> an error text, or null
     const char* check(size_t vl) const {
         if (i420) {
@@ -169,6 +188,15 @@ struct Source {
             if (vl > 1 && planes.lane_stride < planes.pitch[0] * hh) return "NV12 lane_stride < pitch * height";
             return nullptr;
         }
+        if (kind == FRONT_RGB) {
+            if (!planes.base[0]) return "RGB data is null";
+            if (layout < MC_RGB_RGB || layout > MC_RGB_PLANAR) return "RGB layout out of range";
+            if (layout == MC_RGB_PLANAR && (!planes.base[1] || !planes.base[2])) return "RGB plane is null";
+            if (w < 1 || hh < 1) return "RGB width and height must be >= 1";
+            if (planes.pitch[0] < planes.row[0]) return "RGB pitch < width * bytes per pixel";
+            if (vl > 1 && planes.lane_stride < planes.pitch[0] * hh) return "RGB lane_stride < pitch * height";
+            return nullptr;
+        }
         if (converts()) {
             if (!planes.base[0]) return "YUYV frame is null";
             if (kind == kBadOrder) return "YUYV order out of range";
@@ -181,6 +209,14 @@ struct Source {
     }
     // the frames as the front and the compose kernel read them
     PaneSrc pane() const {
+        if (kind == FRONT_RGB) {   // the B, G and R channel bases (mc_internal.h)
+            uint8_t* const* b = planes.base;
+            const size_t pitch = planes.pitch[0];
+            if (layout == MC_RGB_PLANAR) return PaneSrc{b[2], b[1], pitch, planes.lane_stride, kind, b[0], pitch, 1};
+            const bool bgra = layout == MC_RGB_BGRA;
+            return PaneSrc{b[0] + (bgra ? 0 : 2), b[0] + 1, pitch, planes.lane_stride, kind, b[0] + (bgra ? 2 : 0), pitch,
+                           rgb_pstep(layout)};
+        }
         if (kind != FRONT_NV12) return PaneSrc{planes.base[0], nullptr, planes.pitch[0], planes.lane_stride, kind};
         const Nv12Planes f = yuv420_of(planes);
         return PaneSrc{f.y, f.cb, f.pitch, f.lane_stride, kind, f.cr, f.cpitch, f.cstep};
@@ -1509,14 +1545,17 @@ struct ComposeReq {
 const char* check_compose(const ComposeReq& c, const ChainGeom& g, size_t vl, const mc_handle::Overlay& ov) {
     if (c.split < MC_SPLIT_NONE || c.split > MC_SPLIT_TOP_BOTTOM) return "split out of range";
     const mc_canvas* cv = c.canvas;
-    if (!cv || cv->format < MC_CANVAS_BGR || cv->format > MC_CANVAS_I420) return "canvas is null or of an unknown format";
-    if (!cv->data || (cv->format != MC_CANVAS_BGR && !cv->uv)) return "canvas plane is null";
+    if (!cv || cv->format < MC_CANVAS_BGR || cv->format > MC_CANVAS_RGB_PLANAR) return "canvas is null or of an unknown format";
+    const bool yuv420 = cv->format == MC_CANVAS_NV12 || cv->format == MC_CANVAS_I420;
+    if (!cv->data || (yuv420 && !cv->uv)) return "canvas plane is null";
     if (cv->format == MC_CANVAS_I420 && cv->pitch % 2) return "I420 canvas pitch is odd";
     int cw, ch;
     canvas_size(g, c.split, cw, ch);
     if (ov.set && cw > 0 && (cw != ov.cw || ch != ov.ch)) return "canvas geometry differs from the overlay's";
-    if (cv->pitch < (size_t)cw * (cv->format == MC_CANVAS_BGR ? 3 : 1)) return "canvas pitch < canvas row";
-    if (vl > 1 && cv->lane_stride < cv->pitch * ch) return "canvas lane_stride < pitch * canvas height";
+    if (cv->pitch < (size_t)cw * (cv->format == MC_CANVAS_BGR || cv->format == MC_CANVAS_RGB ? 3 : 1))
+        return "canvas pitch < canvas row";
+    const size_t planes = cv->format == MC_CANVAS_RGB_PLANAR ? 3 : 1;
+    if (vl > 1 && cv->lane_stride < planes * cv->pitch * ch) return "canvas lane_stride < pitch * canvas height (per plane)";
     return nullptr;
 }
 
@@ -1587,7 +1626,7 @@ mc_status chain_run(mc_handle* h, const ChainGeom& g, const Source& s, int frame
             d.out = h->x_mag.p; d.out_step = out_row;
         }
         d.orig = nullptr;
-        if (g.pre && d.cmp->split != MC_SPLIT_NONE) {
+        if ((g.pre || s.composes_from_tap()) && d.cmp->split != MC_SPLIT_NONE) {
             d.orig_step = (size_t)g.dw * s.channels;
             CK(h->f_pre.grow(d.orig_step * g.dh * vl));
             d.orig = h->f_pre.p;
@@ -1651,12 +1690,15 @@ mc_status chain_run(mc_handle* h, const ChainGeom& g, const Source& s, int frame
         a.ops = h->x_ops.p;
         a.split = d.cmp->split;
         const mc_canvas& cv = *d.cmp->canvas;
-        a.nv12 = cv.format != MC_CANVAS_BGR;
+        a.format = cv.format;
         a.data = cv.data; a.uv = cv.uv; a.pitch = cv.pitch; a.lane_stride = cv.lane_stride;
+        int cw, ch;
+        canvas_size(g, a.split, cw, ch);
         if (cv.format == MC_CANVAS_I420) {   // the Cr plane follows the Cb plane's canvas_h / 2 rows of pitch / 2 bytes
-            int cw, ch;
-            canvas_size(g, a.split, cw, ch);
             a.cr = cv.uv + cv.pitch / 2 * (size_t)(ch / 2);
+        } else if (cv.format == MC_CANVAS_RGB_PLANAR) {   // the G and B planes follow the R plane's canvas_h rows
+            a.uv = cv.data + cv.pitch * (size_t)ch;
+            a.cr = cv.data + 2 * cv.pitch * (size_t)ch;
         }
         if (h->ov.set) {
             a.ov_rects = h->ov.rects;
@@ -1838,6 +1880,25 @@ extern "C" mc_status mc_chain_compose_yuv420p_device(mc_handle* h, const mc_yuv4
                       produced, info);
 } catch (...) { return on_exception(h); }
 
+extern "C" mc_status mc_chain_process_rgb_device(mc_handle* h, const mc_rgb* in, int frames, int width, int height,
+                                                 const mc_params* p, int grayscale, uint8_t* d_out, size_t out_step,
+                                                 uint8_t* d_original, size_t original_step, uint8_t* produced,
+                                                 mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    return chain_impl(h, Source::rgb(in, width, height), frames, p, grayscale, ChainDst{d_out, out_step, d_original, original_step},
+                      produced, info);
+} catch (...) { return on_exception(h); }
+
+extern "C" mc_status mc_chain_compose_rgb_device(mc_handle* h, const mc_rgb* in, int frames, int width, int height,
+                                                 const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                                                 uint8_t* produced, mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    return chain_impl(h, Source::rgb(in, width, height), frames, p, grayscale, ChainDst{.cmp = ComposeReq{split, canvas}},
+                      produced, info);
+} catch (...) { return on_exception(h); }
+
 namespace {
 // The body of the chain submits and of the blocking host chain calls: chain_check on the host frame set, then one slot of
 // the pipeline whose run is chain_run on the slot's buffers.  The processed frames go to d.out (lane k at k * out_h *
@@ -1968,16 +2029,27 @@ extern "C" mc_status mc_chain_submit_yuv420p(mc_handle* h, const mc_yuv420p* in,
                         info);
 } catch (...) { return on_exception(h); }
 
+extern "C" mc_status mc_chain_submit_rgb(mc_handle* h, const mc_rgb* in, int width, int height, const mc_params* p, int grayscale,
+                                         uint8_t* out, size_t out_step, uint8_t* original, size_t original_step,
+                                         mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    return chain_submit(h, Source::rgb(in, width, height), p, grayscale, ChainDst{out, out_step, original, original_step}, info);
+} catch (...) { return on_exception(h); }
+
 // ---- the export canvas from host clips: compose submits, collected by mc_collect -----------------------------------------
 namespace {
-// The planes of the canvases of a cw x ch canvas geometry (BGR; NV12 luma and Cb,Cr; I420 luma, Cb and Cr), virtual lane v at
-// v * lane_stride.  Only the canvas_w (chroma: canvas_w / 2) bytes of each row are copied.
+// The planes of the canvases of a cw x ch canvas geometry (BGR or RGB; NV12 luma and Cb,Cr; I420 luma, Cb and Cr; planar R,
+// G and B), virtual lane v at v * lane_stride.  Only the canvas_w (chroma: canvas_w / 2) bytes of each row are copied.
 Planes canvas_planes(const mc_canvas& c, int cw, int ch) {
     const size_t w = (size_t)cw, hh = (size_t)ch;
     if (c.format == MC_CANVAS_NV12) return Planes{{c.data, c.uv}, {hh, hh / 2}, {w, w}, {c.pitch, c.pitch}, c.lane_stride};
     if (c.format == MC_CANVAS_I420)
         return Planes{{c.data, c.uv, c.uv + c.pitch / 2 * (hh / 2)}, {hh, hh / 2, hh / 2}, {w, w / 2, w / 2},
                       {c.pitch, c.pitch / 2, c.pitch / 2}, c.lane_stride};
+    if (c.format == MC_CANVAS_RGB_PLANAR)
+        return Planes{{c.data, c.data + c.pitch * hh, c.data + 2 * c.pitch * hh}, {hh, hh, hh}, {w, w, w},
+                      {c.pitch, c.pitch, c.pitch}, c.lane_stride};
     return Planes{{c.data}, {hh}, {w * 3}, {c.pitch}, c.lane_stride};
 }
 
@@ -2011,7 +2083,8 @@ mc_status compose_submit(mc_handle* h, const Source& s, int frames, const mc_par
     int fw, fh;
     canvas_size(full, cmp.split, fw, fh);
     const size_t reserve =
-        ((size_t)fw * fh * (cmp.canvas->format == MC_CANVAS_BGR ? 6 : 3) / 2 * frames * h->lanes + 255) / 256 * 256;
+        ((size_t)fw * fh * (cmp.canvas->format == MC_CANVAS_NV12 || cmp.canvas->format == MC_CANVAS_I420 ? 3 : 6) / 2 * frames *
+             h->lanes + 255) / 256 * 256;
     const size_t lanes = (size_t)h->lanes, vl = (size_t)frames * lanes;
     return submit_impl(h, src, dst, [&](const Planes& d_in, const Planes* d_out, int* any, uint8_t* flags,
                                         std::vector<uint8_t>* written) {
@@ -2058,6 +2131,14 @@ extern "C" mc_status mc_chain_compose_submit_yuv420p(mc_handle* h, const mc_yuv4
     if (!h) return MC_ERR_INVALID;
     CK(cudaSetDevice(h->device));
     return compose_submit(h, Source::yuv420p(in, width, height), frames, p, grayscale, ComposeReq{split, canvas}, produced, info);
+} catch (...) { return on_exception(h); }
+
+extern "C" mc_status mc_chain_compose_submit_rgb(mc_handle* h, const mc_rgb* in, int frames, int width, int height,
+                                                 const mc_params* p, int grayscale, int split, const mc_canvas* canvas,
+                                                 uint8_t* produced, mc_chain_info* info) try {
+    if (!h) return MC_ERR_INVALID;
+    CK(cudaSetDevice(h->device));
+    return compose_submit(h, Source::rgb(in, width, height), frames, p, grayscale, ComposeReq{split, canvas}, produced, info);
 } catch (...) { return on_exception(h); }
 
 /* test hooks, not declared in the public header: the two conversion kernels alone on device buffers (default stream,

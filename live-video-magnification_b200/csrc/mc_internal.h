@@ -162,8 +162,11 @@ cudaError_t launch_egress(const FrameIO& io, const DeviceTables& tb, const int16
 
 // PreprocessProcessor + GrayscaleProcessor on the device (mc_preprocess.cu): one launch over `vlanes` virtual lanes.
 // FRONT_YUYV + mc_yuv422_order is the packed 4:2:2 source of that byte order.  FRONT_NV12 is any 4:2:0 source, NV12 or
-// I420 / YV12, told apart only by its chroma addressing (cb, cr, cpitch, cstep below).
-enum FrontSrc { FRONT_BGR = 0, FRONT_GRAY = 1, FRONT_NV12 = 2, FRONT_YUYV = 3, FRONT_UYVY = 4 };
+// I420 / YV12, told apart only by its chroma addressing (cb, cr, cpitch, cstep below).  FRONT_RGB is any RGB-family
+// source (packed RGB, RGBA / BGRA, planar RGB): the B, G and R bytes of its pixel (x, y) are at src / cb / cr +
+// y * step + x * cstep, cstep 3 or 4 for packed pixels and 1 for planes.  The front's FRONT_BGR instance walks every
+// 3-channel packed or planar source this way, BGR itself with the bases src, src + 1, src + 2 and cstep 3.
+enum FrontSrc { FRONT_BGR = 0, FRONT_GRAY = 1, FRONT_NV12 = 2, FRONT_YUYV = 3, FRONT_UYVY = 4, FRONT_RGB = 5 };
 enum FrontKind { FRONT_COPY = 0, FRONT_AREA_FAST = 1, FRONT_AREA = 2 };   // crop only / integer INTER_AREA / general INTER_AREA
 // The chroma of a 4:2:0 frame: the Cb and Cr of its 2x2 block (bx, by) are at cb[by * cpitch + bx * cstep] and
 // cr[by * cpitch + bx * cstep].  NV12: cr = cb + 1, cstep 2, cpitch = the luma pitch; I420: two planes, cstep 1.
@@ -206,12 +209,13 @@ cudaError_t launch_bgr_to_nv12(const uint8_t* bgr, size_t bgr_step, int w, int h
 // The export canvas (mc_preprocess.cu): Exporter.cpp's compose(original, cur, split) over virtual lanes, its labels as
 // the handle's overlay (mc_set_overlay): per-pixel u8 tone maps inside at most kOverlayRects disjoint canvas rects.
 // A pane source holds virtual lane v's frame at p + v * lane_stride (4:2:0: its chroma at cb / cr + v * lane_stride,
-// addressed as FrontArgs describes).
+// addressed as FrontArgs describes; RGB: its B, G and R channel bases at p, cb and cr + v * lane_stride, pixel step cstep).
 struct PaneSrc {
     const uint8_t* p = nullptr;
     const uint8_t* cb = nullptr;
     size_t step = 0, lane_stride = 0;
-    int kind = FRONT_BGR;           // FrontSrc: BGR, gray (expanded as GRAY2BGR), 4:2:0 or YUYV / UYVY (converted as cvtColor)
+    int kind = FRONT_BGR;           // FrontSrc: BGR, gray (expanded as GRAY2BGR), 4:2:0 or YUYV / UYVY (converted as cvtColor);
+                                    // RGB for the front only (the compose kernel reads an RGB source's BGR tap)
     const uint8_t* cr = nullptr;
     size_t cpitch = 0;
     int cstep = kNv12ChromaStep;
@@ -228,10 +232,11 @@ struct ComposeArgs {
     const uint8_t* ops = nullptr;   // ComposeOp per virtual lane; null: every lane MAGNIFIED
     int split = 0;                  // mc_split: the original pane is read only when it is not MC_SPLIT_NONE
     int w = 0, h = 0;               // pane size: even and > 0
-    int nv12 = 0;                   // canvas format: packed BGR (0) or 4:2:0 (1: NV12, or I420 when cr is set)
-    uint8_t* data = nullptr;        // BGR canvas or luma plane of virtual lane 0
-    uint8_t* uv = nullptr;          // NV12: Cb,Cr plane of virtual lane 0; I420: its Cb plane
-    uint8_t* cr = nullptr;          // I420: Cr plane of virtual lane 0, rows pitch / 2 apart in both chroma planes; NV12: null
+    int format = 0;                 // mc_canvas_format; NV12 and I420 are told apart by cr
+    uint8_t* data = nullptr;        // BGR / RGB canvas, luma plane or R plane of virtual lane 0
+    uint8_t* uv = nullptr;          // NV12: Cb,Cr plane of virtual lane 0; I420: its Cb plane; RGB_PLANAR: its G plane
+    uint8_t* cr = nullptr;          // I420: Cr plane of virtual lane 0, rows pitch / 2 apart in both chroma planes;
+                                    // RGB_PLANAR: its B plane; NV12: null
     size_t pitch = 0, lane_stride = 0;
     int ov_rects = 0;               // the overlay: 0 .. kOverlayRects rects; 0 leaves every canvas as composed
     OverlayRect ov[kOverlayRects];

@@ -15,13 +15,6 @@ namespace {
 
 // Source pixels as the front kernel reads them: (sx, sy) relative to the ROI origin (ox, oy) of virtual lane v.
 template <int SRC> struct FrontPx;
-template <> struct FrontPx<FRONT_BGR> {
-    const uint8_t* p; size_t step;
-    __device__ void operator()(int sx, int sy, int (&v)[3]) const {
-        const uint8_t* q = p + (size_t)sy * step + (size_t)3 * sx;
-        v[0] = __ldg(q); v[1] = __ldg(q + 1); v[2] = __ldg(q + 2);
-    }
-};
 template <> struct FrontPx<FRONT_GRAY> {
     const uint8_t* p; size_t step;
     __device__ void operator()(int sx, int sy, int (&v)[1]) const { v[0] = __ldg(p + (size_t)sy * step + sx); }
@@ -67,6 +60,16 @@ template <bool UYVY> struct Yuv422Px {
 };
 template <> struct FrontPx<FRONT_YUYV> : Yuv422Px<false> {};
 template <> struct FrontPx<FRONT_UYVY> : Yuv422Px<true> {};
+// A BGR pixel, or COLOR_RGB2BGR / RGBA2BGR / BGRA2BGR (planar: a merge of the B, G, R planes) of an RGB one: its three
+// channel bytes at b / g / r + sy * pitch + sx * pstep, the bases already at the ROI origin.  One functor serves BGR and
+// all four RGB layouts.
+struct RgbPx {
+    const uint8_t* b; const uint8_t* g; const uint8_t* r; size_t pitch; int pstep;
+    __device__ void operator()(int sx, int sy, int (&v)[3]) const {
+        const size_t o = (size_t)sy * pitch + (size_t)sx * pstep;
+        v[0] = __ldg(b + o); v[1] = __ldg(g + o); v[2] = __ldg(r + o);
+    }
+};
 
 // The preprocessed pixel (x, y): its ROI tap, or its INTER_AREA taps, read through px.
 template <int CN, class Px>
@@ -88,14 +91,15 @@ __global__ void __launch_bounds__(256) k_chain_front(const FrontArgs a) {
         const size_t l = v * a.lane_stride;
         if (a.cstep == kNv12ChromaStep) front_walk(a, FrontPx<SRC>{a.src + l, a.cb + l, a.step, a.rx, a.ry}, x, y, o);
         else front_walk(a, I420Px{a.src + l, a.cb + l, a.cr + l, a.step, a.cpitch, a.rx, a.ry}, x, y, o);
-    } else {
+    } else if constexpr (SRC == FRONT_YUYV || SRC == FRONT_UYVY) {
         FrontPx<SRC> px;
-        if constexpr (SRC == FRONT_YUYV || SRC == FRONT_UYVY) {
-            px.p = a.src + v * a.lane_stride + (size_t)a.ry * a.step; px.pitch = a.step; px.ox = a.rx; px.vec = a.vec != 0;
-        } else {
-            px = FrontPx<SRC>{a.src + v * a.lane_stride + (size_t)a.ry * a.step + (size_t)CN * a.rx, a.step};
-        }
+        px.p = a.src + v * a.lane_stride + (size_t)a.ry * a.step; px.pitch = a.step; px.ox = a.rx; px.vec = a.vec != 0;
         front_walk(a, px, x, y, o);
+    } else if constexpr (SRC == FRONT_BGR) {   // BGR and every RGB layout: three channel bases
+        const size_t l = v * a.lane_stride + (size_t)a.ry * a.step + (size_t)a.rx * a.cstep;
+        front_walk(a, RgbPx{a.src + l, a.cb + l, a.cr + l, a.step, a.cstep}, x, y, o);
+    } else {
+        front_walk(a, FrontPx<SRC>{a.src + v * a.lane_stride + (size_t)a.ry * a.step + (size_t)CN * a.rx, a.step}, x, y, o);
     }
     if (a.dst) {
         uint8_t* d = a.dst + v * a.dst_lane_stride + (size_t)y * a.dst_step + (size_t)CN * x;
@@ -114,7 +118,10 @@ cudaError_t launch_chain_front(const FrontArgs& args, int src, int vlanes, cudaS
     a.vec = (reinterpret_cast<uintptr_t>(a.src) & 3) == 0 && a.step % 4 == 0 && (vlanes == 1 || a.lane_stride % 4 == 0);
     const dim3 grid((unsigned)((a.dw + 255) / 256), (unsigned)a.dh, (unsigned)vlanes);
     switch (src) {
-        case FRONT_BGR: k_chain_front<FRONT_BGR><<<grid, 256, 0, s>>>(a); break;
+        case FRONT_BGR:   // the B, G, R channel bases of a BGR frame, the RGB family's fifth layout
+            a.cb = a.src + 1; a.cr = a.src + 2; a.cstep = 3;
+            [[fallthrough]];
+        case FRONT_RGB: k_chain_front<FRONT_BGR><<<grid, 256, 0, s>>>(a); break;
         case FRONT_GRAY: k_chain_front<FRONT_GRAY><<<grid, 256, 0, s>>>(a); break;
         case FRONT_YUYV: k_chain_front<FRONT_YUYV><<<grid, 256, 0, s>>>(a); break;
         case FRONT_UYVY: k_chain_front<FRONT_UYVY><<<grid, 256, 0, s>>>(a); break;
@@ -353,6 +360,26 @@ __device__ __forceinline__ void overlay_row(const ComposeArgs& a, int cx, int y,
     }
 }
 
+__device__ __forceinline__ void swap_rb(uint8_t (&p)[24]) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const uint8_t t = p[3 * k];
+        p[3 * k] = p[3 * k + 2];
+        p[3 * k + 2] = t;
+    }
+}
+
+// The R, G and B bytes of a canvas row's 8 BGR pixels p into the planes of a planar RGB canvas, `o` bytes from each base.
+__device__ __forceinline__ void store_planes(const ComposeArgs& a, size_t o, bool vec, int n, const uint8_t (&p)[24]) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        uint8_t q[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) q[k] = p[3 * k + 2 - c];
+        store((c == 0 ? a.data : c == 1 ? a.uv : a.cr) + o, vec, n, q);
+    }
+}
+
 // Whether the canvas box [x0, x0 + w) x [y0, y0 + h) meets a rect of the overlay.
 __device__ __forceinline__ bool overlay_meets(const ComposeArgs& a, int x0, int y0, int w, int h) {
     bool hit = false;
@@ -368,9 +395,11 @@ __device__ __forceinline__ bool overlay_meets(const ComposeArgs& a, int x0, int 
 // pane 0, then those of pane 1, so a CTA stays inside one pane and reads one source.  A CTA whose canvas box meets an
 // overlay rect maps its pixels in registers before they are stored or converted; the others take one uniform branch.
 // Each row is mapped just before it is stored or converted, and 8 CTAs per SM (64 registers) keep the occupancy of the
-// kernel without an overlay path, with no spills (-Xptxas -v).
-template <bool NV12_OUT>
-__global__ void __launch_bounds__(kBlockX * kBlockY, 8) k_compose(const ComposeArgs a) {
+// kernel without an overlay path, with no spills (-Xptxas -v).  OUT is the canvas format; MC_CANVAS_NV12 stands for both
+// 4:2:0 canvases, NV12 and I420 (cr set).  The planar RGB canvas regathers both rows' bytes into three planes, which
+// spills at 64 registers in every order tried (-Xptxas -v): its instance runs 6 CTAs per SM (80 registers) instead.
+template <int OUT>
+__global__ void __launch_bounds__(kBlockX * kBlockY, OUT == MC_CANVAS_RGB_PLANAR ? 6 : 8) k_compose(const ComposeArgs a) {
     const size_t v = blockIdx.z;
     const int op = a.ops ? a.ops[v] : COMPOSE_MAGNIFIED;
     if (op == COMPOSE_SKIP) return;
@@ -390,7 +419,7 @@ __global__ void __launch_bounds__(kBlockX * kBlockY, 8) k_compose(const ComposeA
     if (ov) overlay_row(a, cx, cy, p0);
     const bool vec = full && a.vec_out && cx % 8 == 0;
     uint8_t* row = a.data + v * a.lane_stride + (size_t)cy * a.pitch;
-    if constexpr (NV12_OUT) {
+    if constexpr (OUT == MC_CANVAS_NV12) {
         uint8_t y0[8], y1[8], c[8];
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
@@ -416,9 +445,16 @@ __global__ void __launch_bounds__(kBlockX * kBlockY, 8) k_compose(const ComposeA
         } else {
             store(a.uv + v * a.lane_stride + (size_t)(cy / 2) * a.pitch + cx, vec, n, c);
         }
-    } else {
+    } else if constexpr (OUT == MC_CANVAS_RGB_PLANAR) {   // one row store of n bytes per plane: R at data, G at uv, B at cr
+        const size_t o = v * a.lane_stride + (size_t)cy * a.pitch + cx;
+        store_planes(a, o, vec, n, p0);
+        if (ov) overlay_row(a, cx, cy + 1, p1);
+        store_planes(a, o + a.pitch, vec, n, p1);
+    } else {   // BGR, or RGB: the BGR store with bytes 0 and 2 of each pixel exchanged
+        if constexpr (OUT == MC_CANVAS_RGB) swap_rb(p0);
         store(row + (size_t)3 * cx, vec, 3 * n, p0);
         if (ov) overlay_row(a, cx, cy + 1, p1);
+        if constexpr (OUT == MC_CANVAS_RGB) swap_rb(p1);
         store(row + a.pitch + (size_t)3 * cx, vec, 3 * n, p1);
     }
 }
@@ -431,6 +467,7 @@ bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0;
 bool chroma_vec(const uint8_t* cb, const uint8_t* cr, size_t cpitch, int cstep) {
     return cstep == kNv12ChromaStep ? aligned8(cb) : aligned4(cb) && aligned4(cr) && cpitch % 4 == 0;
 }
+
 
 dim3 grid_of(int w, int h, int lanes) {
     const int groups = (w + 7) / 8;
@@ -459,14 +496,21 @@ cudaError_t launch_compose(ComposeArgs a, int vlanes, cudaStream_t s) {
                          p.step % 8 == 0 && (lane_vec || p.lane_stride % 8 == 0);
         a.vec_src |= (int)vec << i;
     }
-    a.vec_out = aligned8(a.data) && (!a.nv12 || (a.cr ? aligned4(a.uv) && aligned4(a.cr) : aligned8(a.uv))) && a.pitch % 8 == 0 &&
-                (lane_vec || a.lane_stride % 8 == 0);
+    const bool yuv420 = a.format == MC_CANVAS_NV12 || a.format == MC_CANVAS_I420;
+    const bool planes_vec = yuv420 ? (a.cr ? aligned4(a.uv) && aligned4(a.cr) : aligned8(a.uv))
+                                   : a.format != MC_CANVAS_RGB_PLANAR || (aligned8(a.uv) && aligned8(a.cr));
+    a.vec_out = aligned8(a.data) && planes_vec && a.pitch % 8 == 0 && (lane_vec || a.lane_stride % 8 == 0);
     const int panes = a.split == MC_SPLIT_NONE ? 1 : 2;
     dim3 grid = grid_of(a.w, a.h, vlanes);
     a.pane_blocks = (int)grid.y;
     grid.y *= panes;
-    if (a.nv12) k_compose<true><<<grid, dim3(kBlockX, kBlockY), 0, s>>>(a);
-    else k_compose<false><<<grid, dim3(kBlockX, kBlockY), 0, s>>>(a);
+    const dim3 block(kBlockX, kBlockY);
+    switch (a.format) {
+        case MC_CANVAS_RGB: k_compose<MC_CANVAS_RGB><<<grid, block, 0, s>>>(a); break;
+        case MC_CANVAS_RGB_PLANAR: k_compose<MC_CANVAS_RGB_PLANAR><<<grid, block, 0, s>>>(a); break;
+        case MC_CANVAS_BGR: k_compose<MC_CANVAS_BGR><<<grid, block, 0, s>>>(a); break;
+        default: k_compose<MC_CANVAS_NV12><<<grid, block, 0, s>>>(a); break;
+    }
     return cudaGetLastError();
 }
 

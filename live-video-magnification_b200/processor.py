@@ -378,6 +378,17 @@ class MagnificationProcessor(IProcessor):
                                                               flags.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(info)))
         return flags.astype(bool), info
 
+    def chain_compose_rgb_device(self, d_in: capi.McRgb, frames: int, w: int, h: int, cfg: ProcessorConfig, split: int,
+                                 canvas: capi.McCanvas):
+        """mc_chain_compose_rgb_device on RGB device frames (packed RGB, RGBA / BGRA or planar) -> (produced
+        bool[frames, lanes], McChainInfo)."""
+        p, info = _to_mc(cfg), capi.McChainInfo()
+        flags = np.zeros((int(frames), self.lanes), np.uint8)
+        self._check(self._lib.mc_chain_compose_rgb_device(self._h, C.byref(d_in), int(frames), w, h, C.byref(p), int(cfg.grayscale),
+                                                          int(split), C.byref(canvas), flags.ctypes.data_as(C.POINTER(C.c_uint8)),
+                                                          C.byref(info)))
+        return flags.astype(bool), info
+
     def set_overlay(self, ov) -> None:
         """mc_set_overlay: every later compose call maps its canvases through `ov` (a labels.Overlay or a
         capi.McOverlay), until it is replaced or cleared.  The core copies it; `ov` may be dropped afterwards."""
@@ -443,10 +454,11 @@ class ProcessingChainB200:
 
     ``run_chain_once(frame, cfg) -> (cur, original)`` returns the *same* frame object wherever the reference
     returns the same FrameRef (identity stages / passthrough); it needs ``lanes == 1``.  ``process_device`` and
-    ``process_nv12_device`` / ``process_yuv420p_device`` / ``process_yuv422_device`` run the chain on device frames of every
-    lane, for one frame or a clip; ``submit`` / ``submit_nv12`` / ``submit_yuv420p`` / ``submit_yuv422`` pipeline host
-    frames of every lane, ``compose_submit`` and its ``_nv12`` / ``_yuv420p`` / ``_yuv422`` forms pipeline host clips into
-    export canvases (BGR, NV12 or I420), and ``collect`` returns them in order;
+    ``process_nv12_device`` / ``process_yuv420p_device`` / ``process_yuv422_device`` / ``process_rgb_device`` run the chain
+    on device frames of every lane, for one frame or a clip; ``submit`` / ``submit_nv12`` / ``submit_yuv420p`` /
+    ``submit_yuv422`` / ``submit_rgb`` pipeline host frames of every lane, ``compose_submit`` and its ``_nv12`` /
+    ``_yuv420p`` / ``_yuv422`` / ``_rgb`` forms pipeline host clips into export canvases (BGR, NV12, I420, RGB or planar
+    RGB), and ``collect`` returns them in order;
     ``run_chain_once`` of a ``Frame`` whose format is "YUYV" or "UYVY" takes a camera's packed 4:2:2 bytes."""
 
     def __init__(self, device: int = 0, lanes: int = 1):
@@ -520,6 +532,16 @@ class ProcessingChainB200:
                                                         flags.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(info)))
         return flags.astype(bool), info
 
+    def process_rgb_device(self, d_in: capi.McRgb, frames: int, w: int, h: int, cfg: ProcessorConfig, d_out: int, out_step: int,
+                           d_original: int = 0, original_step: int = 0):
+        """mc_chain_process_rgb_device on RGB device frames -> (produced bool[frames, lanes], McChainInfo)."""
+        m, p, info = self.magnifier, _to_mc(cfg), capi.McChainInfo()
+        flags = np.zeros((int(frames), self.lanes), np.uint8)
+        m._check(m._lib.mc_chain_process_rgb_device(m._h, C.byref(d_in), int(frames), w, h, C.byref(p), int(cfg.grayscale), d_out,
+                                                    out_step, d_original or None, original_step,
+                                                    flags.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(info)))
+        return flags.astype(bool), info
+
     # -- pipelined host frames of every lane (mc_chain_submit*, collected by collect()) -------------------------------------
     def submit(self, in_ptr: int, w: int, h: int, c: int, in_step: int, cfg: ProcessorConfig, out_ptr: int, out_step: int,
                original_ptr: int = 0, original_step: int = 0) -> "capi.McChainInfo":
@@ -554,6 +576,14 @@ class ProcessingChainB200:
         m, p, info = self.magnifier, _to_mc(cfg), capi.McChainInfo()
         m._check(m._lib.mc_chain_submit_yuv420p(m._h, C.byref(in_planes), w, h, C.byref(p), int(cfg.grayscale), out_ptr or None,
                                                 out_step, original_ptr or None, original_step, C.byref(info)))
+        return info
+
+    def submit_rgb(self, in_frame: capi.McRgb, w: int, h: int, cfg: ProcessorConfig, out_ptr: int, out_step: int,
+                   original_ptr: int = 0, original_step: int = 0) -> "capi.McChainInfo":
+        """mc_chain_submit_rgb: submit() on RGB host frames (lane k at k * lane_stride)."""
+        m, p, info = self.magnifier, _to_mc(cfg), capi.McChainInfo()
+        m._check(m._lib.mc_chain_submit_rgb(m._h, C.byref(in_frame), w, h, C.byref(p), int(cfg.grayscale), out_ptr or None,
+                                            out_step, original_ptr or None, original_step, C.byref(info)))
         return info
 
     # -- pipelined export canvases from host clips (mc_chain_compose_submit*, collected by collect()) ------------------------
@@ -596,6 +626,14 @@ class ProcessingChainB200:
         into BGR, NV12 or I420 canvases."""
         m, p = self.magnifier, _to_mc(cfg)
         return self._compose_submit(m._lib.mc_chain_compose_submit_yuv420p, C.byref(in_planes), frames, w, h, C.byref(p),
+                                    int(cfg.grayscale), split=split, canvas=canvas)
+
+    def compose_submit_rgb(self, in_frame: capi.McRgb, frames: int, w: int, h: int, cfg: ProcessorConfig, split: int,
+                           canvas: capi.McCanvas):
+        """mc_chain_compose_submit_rgb: compose_submit() on RGB host frames (virtual lane v at v * lane_stride), into
+        BGR, NV12, I420, RGB or planar RGB canvases."""
+        m, p = self.magnifier, _to_mc(cfg)
+        return self._compose_submit(m._lib.mc_chain_compose_submit_rgb, C.byref(in_frame), frames, w, h, C.byref(p),
                                     int(cfg.grayscale), split=split, canvas=canvas)
 
     def collect(self) -> np.ndarray:
