@@ -157,6 +157,41 @@ typedef struct mc_lane_params {
  * MC_ERR_INVALID for a NULL handle or a lane out of range. */
 mc_status mc_set_lane_params(mc_handle* h, int lane, const mc_lane_params* lp);
 
+/* --- per-lane region of interest: each camera of a multi-lane handle cropped at its own rectangle --------------------- */
+/* roi != NULL: from the next frame call or submit on, `lane` uses the four floats roi[0..3] = {x, y, w, h} (normalised, as
+ * pre_roiX / Y / W / H) in place of the call's ROI fields; pre_roiEnabled, pre_downscale, grayscale, mode and levels still
+ * come from the call.  roi == NULL: the lane follows the call's ROI again.
+ *   Equivalence: lane k's effective params are the call's, with the four ROI fields replaced by lane k's override if it has
+ *     one.  Lane k then gives, bit for bit, what a 1-lane handle gives when fed lane k's frames with those params, under
+ *     the restarts and holds lane k saw: the processed frame and the original tap, the canvas (labels included), `info`,
+ *     the produced flags, mc_lane_produced, and the temporal state afterwards (which a mc_save_lane blob shows byte for
+ *     byte).
+ *   Where it applies: every call.  Chain, compose, clip and submit calls of every source (BGR, gray, NV12, 4:2:2, I420,
+ *     RGB) crop each lane's frames at the lane's own rectangle.  The magnifier-only calls (mc_process*, mc_submit*) do not
+ *     crop, so there the override only enters the lane's structural fingerprint.  A clip takes the override at its first
+ *     frame and a submit at submit time: frames in flight keep what they were submitted with.
+ *   Per-lane structural reset: the fingerprint (mode, levels, size, channels, downscale, pre_roiEnabled and the ROI,
+ *     compared with exact ==) is kept per lane.  A lane whose effective ROI changes while the rest stays restarts alone,
+ *     as its 1-lane twin would; the other lanes continue untouched.  A Phase lane restarted this way re-designs its
+ *     filters at its effective framerate, as its twin's structural reset does (mc_restart_lane keeps the design's
+ *     framerate, see mc_set_lane_params).  A held lane keeps its state while its ROI changes: it is compared when the
+ *     lane is released, which restarts it only if its ROI then differs from the one it ran with.  A change of the
+ *     rest of the fingerprint, or of every lane's ROI at once, still resets every lane.  On a Color handle with lanes > 1,
+ *     restarting some lanes needs option "color_lane_lifecycle": without it the call returns MC_ERR_UNSUPPORTED and
+ *     changes nothing.
+ *   One geometry: in a call that crops (pre_roiEnabled), every lane that runs must get a crop of the same pixel size after
+ *     the rounding (lround) and clamping of PreprocessParams; that size is the call's output geometry.  Otherwise the call
+ *     returns MC_ERR_INVALID before any copy or launch, with nothing changed, and mc_last_error names the lane.  Held lanes
+ *     are checked when they run again.
+ *   Lifetime: an override is configuration.  Like mc_set_lane_params and holds, it survives mc_reset, structural resets
+ *     and failed frames.
+ *   Lane state: a mc_save_lane blob records the saving lane's own fingerprint, ROI included.  A load into a handle that
+ *     holds state must match the destination lane's own fingerprint (MC_ERR_INVALID otherwise); a load into a handle
+ *     without state takes the blob's.  A later call whose effective ROI for that lane differs restarts the lane, as the
+ *     source lane's twin would.
+ * MC_ERR_INVALID for a NULL handle or a lane out of range. */
+mc_status mc_set_lane_roi(mc_handle* h, int lane, const float* roi);
+
 /* --- lane state: save one lane's temporal state as host bytes, and load it into a lane of any handle ------------------
  * A running stream moves (to another lane, handle, GPU, process or a file) without the visible restart of its temporal
  * filters: save its lane on the source, load the blob into the destination lane, then restart or hold the source lane.

@@ -116,6 +116,7 @@ SIGNATURES = {
     "mc_hold_lane": (C.c_int, [_vp, C.c_int, C.c_int]),
     "mc_lane_produced": (C.c_int, [_vp, _u8p, C.c_int]),
     "mc_set_lane_params": (C.c_int, [_vp, C.c_int, C.POINTER(McLaneParams)]),
+    "mc_set_lane_roi": (C.c_int, [_vp, C.c_int, C.POINTER(C.c_float)]),
     "mc_save_lane": (C.c_int, [_vp, C.c_int, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
     "mc_load_lane": (C.c_int, [_vp, C.c_int, _vp, C.c_size_t]),
     "mc_process": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_size_t, _PP, _vp, C.c_size_t, C.POINTER(C.c_int)]),

@@ -2,6 +2,7 @@
 // (reference src/processing/MagnificationProcessor.cpp:10-67) — level clamp, structural reset,
 // mode dispatch, passthrough decisions — plus device memory, streams and the pinned pipeline.
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -246,6 +247,13 @@ struct Slot {
         for (cudaEvent_t e : {ev_in, ev_k, ev_done}) if (e) cudaEventDestroy(e);
     }
 };
+
+// A normalised ROI {x, y, w, h}: pre_roiX / Y / W / H of mc_params
+using Roi = std::array<float, 4>;
+constexpr Roi kFullRoi = {0.f, 0.f, 1.f, 1.f};
+Roi roi_of(const mc_params& p) { return {p.pre_roiX, p.pre_roiY, p.pre_roiW, p.pre_roiH}; }
+// exact != on every field, as the reference's fingerprint compares (IProcessor.hpp:35-39): a NaN never equals
+bool roi_differs(const Roi& a, const Roi& b) { return a[0] != b[0] || a[1] != b[1] || a[2] != b[2] || a[3] != b[3]; }
 }  // namespace
 
 struct mc_handle {
@@ -256,10 +264,12 @@ struct mc_handle {
     std::string err;
     uint64_t launches = 0;
 
-    // StructuralTracker (MagnifyCore.hpp:45-80)
+    // StructuralTracker (MagnifyCore.hpp:45-80): the handle's part of the fingerprint, and per lane the ROI of its
+    // effective params (mc_set_lane_roi), so that a lane whose ROI alone moves restarts alone
     int t_mode = MC_MODE_NONE, t_levels = -1, t_channels = -1, t_w = 0, t_h = 0;
     int t_down = 1, t_roi = 0;
-    float t_rx = 0.f, t_ry = 0.f, t_rw = 1.f, t_rh = 1.f;
+    std::vector<Roi> t_lroi;
+    std::vector<uint8_t> roi_moved;   // per frame call: lanes whose ROI fingerprint changes (tracker_plan)
 
     Options opt;
     Profiler prof;
@@ -315,6 +325,13 @@ struct mc_handle {
     int n_lane_lp = 0;
     std::vector<mc_params> lane_eff;
     std::vector<uint8_t> lane_lost;   // per frame call: lanes whose state the mode dropped
+    // Per-lane ROIs (mc_set_lane_roi): configuration, kept across resets
+    std::vector<Roi> lane_roi;
+    std::vector<uint8_t> lane_roi_set;
+    int n_lane_roi = 0;
+    // chain calls whose lanes crop at different origins: one origin per virtual lane, and its host copy
+    DeviceBuffer<int2> f_org;
+    std::vector<int2> f_org_host;
     // mc_save_lane / mc_load_lane: pinned staging of a blob's planes when the caller's buffer is pageable (grow-only)
     PinnedBuffer lane_stage;
 };
@@ -372,20 +389,47 @@ void tracker_disable(mc_handle* h) {
 }
 void tracker_reset(mc_handle* h) {
     tracker_disable(h);
-    h->t_down = 1; h->t_roi = 0; h->t_rx = 0.f; h->t_ry = 0.f; h->t_rw = 1.f; h->t_rh = 1.f;
+    h->t_down = 1; h->t_roi = 0;
+    h->t_lroi.assign((size_t)h->lanes, kFullRoi);
 }
+// The handle's part of the fingerprint: everything but the ROI rectangle, which each lane keeps (t_lroi).
 bool tracker_changes(const mc_handle* h, const mc_params* p, int lv, int ch, int w, int hh) {
     return p->mode != h->t_mode || lv != h->t_levels || w != h->t_w || hh != h->t_h ||
-           ch != h->t_channels || p->pre_downscale != h->t_down ||
-           (p->pre_roiEnabled != 0) != (h->t_roi != 0) || p->pre_roiX != h->t_rx ||
-           p->pre_roiY != h->t_ry || p->pre_roiW != h->t_rw || p->pre_roiH != h->t_rh;
+           ch != h->t_channels || p->pre_downscale != h->t_down || (p->pre_roiEnabled != 0) != (h->t_roi != 0);
 }
+void tracker_set(mc_handle* h, const mc_params* p, int lv, int ch, int w, int hh) {
+    h->t_mode = p->mode; h->t_levels = lv; h->t_w = w; h->t_h = hh; h->t_channels = ch;
+    h->t_down = p->pre_downscale; h->t_roi = p->pre_roiEnabled != 0;
+}
+// Lane l's effective ROI: its override (mc_set_lane_roi), or the call's.
+Roi lane_roi(const mc_handle* h, const mc_params& p, size_t l) { return h->lane_roi_set[l] ? h->lane_roi[l] : roi_of(p); }
+// The fingerprint's verdict on a call: true when the handle resets structurally, because its own part changed or every
+// lane's ROI did (a change of the call's ROI without overrides, as before lanes had their own).  Otherwise h->roi_moved
+// flags the lanes whose ROI alone changed: each restarts alone, as its 1-lane twin would.  A held lane keeps its state and
+// its fingerprint, because its twin skips the call: it is compared when the lane runs again, so a ROI moved and moved back
+// during a hold restarts nothing.
+bool tracker_plan(mc_handle* h, const mc_params* p, int lv, int ch, int w, int hh) {
+    const size_t lanes = (size_t)h->lanes;
+    h->roi_moved.assign(lanes, 0);
+    if (tracker_changes(h, p, lv, ch, w, hh)) return true;
+    size_t n = 0;
+    for (size_t l = 0; l < lanes; ++l) n += h->roi_moved[l] = roi_differs(lane_roi(h, *p, l), h->t_lroi[l]);
+    if (n == lanes) return true;
+    for (size_t l = 0; l < lanes; ++l) h->roi_moved[l] = h->roi_moved[l] && !h->hold[l];
+    return false;
+}
+// tracker_plan, applied: true for a structural reset (the caller drops every lane's state); a running lane whose ROI alone
+// moved loses its state here, and a Phase lane's next frame re-designs its filters at its framerate, as its twin's
+// structural reset does.
 bool tracker_update(mc_handle* h, const mc_params* p, int lv, int ch, int w, int hh) {
-    const bool change = tracker_changes(h, p, lv, ch, w, hh);
-    if (change) {
-        h->t_mode = p->mode; h->t_levels = lv; h->t_w = w; h->t_h = hh; h->t_channels = ch;
-        h->t_down = p->pre_downscale; h->t_roi = p->pre_roiEnabled != 0;
-        h->t_rx = p->pre_roiX; h->t_ry = p->pre_roiY; h->t_rw = p->pre_roiW; h->t_rh = p->pre_roiH;
+    const bool change = tracker_plan(h, p, lv, ch, w, hh);
+    if (change) tracker_set(h, p, lv, ch, w, hh);
+    for (size_t l = 0; l < (size_t)h->lanes; ++l) {
+        if (!change && !h->roi_moved[l]) continue;
+        h->t_lroi[l] = lane_roi(h, *p, l);
+        if (change) continue;
+        h->has_state[l] = 0;
+        h->riesz.redesign((int)l);
     }
     return change;
 }
@@ -473,12 +517,16 @@ mc_status copy_planes(mc_handle* h, const Planes& dst, const Planes& src, size_t
 }
 
 // Without option "color_lane_lifecycle" a multi-lane Color handle keeps its lanes in lock-step: a frame call while a lane
-// is held, or restarted while others run, is MC_ERR_UNSUPPORTED, checked before any state changes.
+// is held, or restarted while others run (mc_restart_lane, or its own ROI moved), is MC_ERR_UNSUPPORTED, checked before
+// any state changes.
 mc_status color_lane_check(mc_handle* h, const mc_params* p, int levels, int channels, int w, int hh) {
     if (h->opt.color_lane_lifecycle) return MC_OK;
-    const bool change = tracker_changes(h, p, levels, channels, w, hh);
+    const bool change = tracker_plan(h, p, levels, channels, w, hh);
     int n_hold = 0, n_state = 0;
-    for (int l = 0; l < h->lanes; ++l) { n_hold += h->hold[(size_t)l] != 0; n_state += h->has_state[(size_t)l] != 0; }
+    for (size_t l = 0; l < (size_t)h->lanes; ++l) {
+        n_hold += h->hold[l] != 0;
+        n_state += h->has_state[l] && !h->roi_moved[l];
+    }
     if (n_hold) { h->err = "Color mode cannot hold a lane of a multi-lane handle"; return MC_ERR_UNSUPPORTED; }
     if (!change && n_state != 0 && n_state != h->lanes) {
         h->err = "Color mode cannot restart one lane of a multi-lane handle while the others run";
@@ -876,6 +924,9 @@ mc_status mc_create_lanes(int device, int lanes, mc_handle** out) try {
     h->lane_produced.assign((size_t)lanes, 0);
     h->lane_lp.assign((size_t)lanes, mc_lane_params{});
     h->lane_lp_set.assign((size_t)lanes, 0);
+    h->lane_roi.assign((size_t)lanes, kFullRoi);
+    h->lane_roi_set.assign((size_t)lanes, 0);
+    h->t_lroi.assign((size_t)lanes, kFullRoi);
     if ((e = cudaMalloc((void**)&h->d_ops, (size_t)lanes)) != cudaSuccess) return fail("cudaMalloc lane ops", e);
     *out = h;
     return MC_OK;
@@ -937,6 +988,15 @@ mc_status mc_set_lane_params(mc_handle* h, int lane, const mc_lane_params* lp) t
     return MC_OK;
 } catch (...) { return on_exception(h); }
 
+mc_status mc_set_lane_roi(mc_handle* h, int lane, const float* roi) try {
+    if (!h) return MC_ERR_INVALID;
+    if (lane < 0 || lane >= h->lanes) { h->err = "lane out of range"; return MC_ERR_INVALID; }
+    h->n_lane_roi += (roi != nullptr) - (h->lane_roi_set[(size_t)lane] != 0);
+    h->lane_roi_set[(size_t)lane] = roi != nullptr;
+    if (roi) std::copy(roi, roi + 4, h->lane_roi[(size_t)lane].begin());   // taken into the next frame call or submit
+    return MC_OK;
+} catch (...) { return on_exception(h); }
+
 mc_status mc_save_lane(mc_handle* h, int lane, void* dst, size_t cap, size_t* bytes) try {
     if (!h || !bytes) return MC_ERR_INVALID;
     if (lane < 0 || lane >= h->lanes) { h->err = "lane out of range"; return MC_ERR_INVALID; }
@@ -949,7 +1009,7 @@ mc_status mc_save_lane(mc_handle* h, int lane, void* dst, size_t cap, size_t* by
     b.has_state = h->has_state[(size_t)lane] != 0;
     b.mode = h->t_mode; b.levels = h->t_levels; b.w = h->t_w; b.h = h->t_h; b.channels = h->t_channels;
     b.pre_down = h->t_down; b.pre_roi = h->t_roi;
-    b.roi[0] = h->t_rx; b.roi[1] = h->t_ry; b.roi[2] = h->t_rw; b.roi[3] = h->t_rh;
+    std::copy(h->t_lroi[(size_t)lane].begin(), h->t_lroi[(size_t)lane].end(), b.roi);   // the lane's own fingerprint
     if (b.has_state) {
         if (b.mode == MC_MODE_LAPLACE) {
             b.faithful = h->motion.faithful;
@@ -999,9 +1059,10 @@ mc_status mc_load_lane(mc_handle* h, int lane, const void* src, size_t bytes) tr
         return MC_ERR_INVALID;
     }
     const mc_params key = blob_key(b);
+    const Roi key_roi = roi_of(key);
     const bool fresh = h->t_mode == MC_MODE_NONE;   // the handle holds no state: the load takes the blob's key
-    if (!fresh && tracker_changes(h, &key, b.levels, b.channels, b.w, b.h)) {
-        h->err = "lane blob: its key (mode, levels, size, channels, preprocess) differs from the handle's state";
+    if (!fresh && (tracker_changes(h, &key, b.levels, b.channels, b.w, b.h) || roi_differs(key_roi, h->t_lroi[(size_t)lane]))) {
+        h->err = "lane blob: its key (mode, levels, size, channels, preprocess) differs from the lane's state";
         return MC_ERR_INVALID;
     }
     if (b.mode == MC_MODE_LAPLACE && ((b.faithful != 0) != h->opt.faithful_level0 ||
@@ -1018,7 +1079,11 @@ mc_status mc_load_lane(mc_handle* h, int lane, const void* src, size_t bytes) tr
     // allocation made here is undone when the blob turns out not to fit it.
     bool allocated_here = false;
     mc_status st = MC_OK;
-    if (fresh) tracker_update(h, &key, b.levels, b.channels, b.w, b.h);
+    const std::vector<Roi> lroi = h->t_lroi;
+    if (fresh) {   // every lane takes the blob's fingerprint (the others have no state)
+        tracker_set(h, &key, b.levels, b.channels, b.w, b.h);
+        h->t_lroi.assign((size_t)h->lanes, key_roi);
+    }
     if (b.mode == MC_MODE_LAPLACE && !h->motion.allocated) {
         allocated_here = true;
         st = h->motion.allocate(ctx, b.w, b.h, b.channels, b.levels);
@@ -1035,7 +1100,10 @@ mc_status mc_load_lane(mc_handle* h, int lane, const void* src, size_t bytes) tr
         if (allocated_here) {
             h->motion.reset(); h->riesz.reset(); h->color.reset();   // nothing else was allocated (a fresh or unallocated mode)
         }
-        if (fresh) tracker_disable(h);
+        if (fresh) {
+            tracker_disable(h);
+            h->t_lroi = lroi;
+        }
         if (st == MC_OK) { h->err = "lane blob size does not match its key"; st = MC_ERR_INVALID; }
         return st;
     }
@@ -1464,6 +1532,7 @@ struct ChainGeom {
     int rx = 0, ry = 0, rw = 0, rh = 0;                   // the ROI in the frame
     int dw = 0, dh = 0, cc = 0;                           // the magnifier's input: size and channels
     int kind = FRONT_COPY, isx = 1, isy = 1;              // how the ROI becomes dw x dh
+    std::vector<int2> org;                                // per lane: its own ROI origin (mc_set_lane_roi); empty: rx, ry
     bool front() const { return pre || gray; }
 };
 
@@ -1494,6 +1563,41 @@ const char* chain_geometry(const mc_params* p, int w, int hh, int channels, int 
     }
     if (g.front()) { info->cur_is_input = 0; info->out_w = g.dw; info->out_h = g.dh; info->out_channels = g.cc; }
     return nullptr;
+}
+
+// chain_geometry of a call on the handle's lanes, each cropped at its effective ROI (mc_set_lane_roi).  The first lane
+// that runs (lane 0 when every lane is held) gives the geometry and the info; every other running lane must crop a
+// rectangle of the same pixel size, which then starts at the lane's own origin (g.org, left empty when every origin is
+// (g.rx, g.ry)).  Held lanes are not cropped, so they are checked when they run again.
+mc_status chain_lane_geometry(mc_handle* h, const mc_params* p, int w, int hh, int channels, int grayscale, ChainGeom& g,
+                              mc_chain_info* info) {
+    const size_t lanes = (size_t)h->lanes;
+    size_t first = 0;
+    while (first < lanes && h->hold[first]) ++first;
+    if (first == lanes) first = 0;
+    mc_params q = *p;
+    const Roi r0 = lane_roi(h, *p, first);
+    q.pre_roiX = r0[0]; q.pre_roiY = r0[1]; q.pre_roiW = r0[2]; q.pre_roiH = r0[3];
+    if (const char* e = chain_geometry(&q, w, hh, channels, grayscale, g, info)) { h->err = e; return MC_ERR_INVALID; }
+    if (!g.pre || !p->pre_roiEnabled || h->n_lane_roi == 0) return MC_OK;
+    std::vector<int2> org(lanes, make_int2(g.rx, g.ry));
+    bool same = true;
+    for (size_t l = 0; l < lanes; ++l) {
+        if (h->hold[l]) continue;
+        const Roi r = lane_roi(h, *p, l);
+        int x, y, rw, rh;
+        preprocess_roi(w, hh, true, r[0], r[1], r[2], r[3], x, y, rw, rh);
+        if (rw != g.rw || rh != g.rh) {
+            h->err = "lane " + std::to_string(l) + "'s ROI crops " + std::to_string(rw) + "x" + std::to_string(rh) + ", lane " +
+                     std::to_string(first) + "'s " + std::to_string(g.rw) + "x" + std::to_string(g.rh) +
+                     ": the lanes of a call must crop rectangles of one size";
+            return MC_ERR_INVALID;
+        }
+        org[l] = make_int2(x, y);
+        same = same && x == g.rx && y == g.ry;
+    }
+    if (!same) g.org = std::move(org);
+    return MC_OK;
 }
 
 // The general INTER_AREA tap tables of g on the device, in one buffer (x taps, y taps, x offsets, y offsets): built and
@@ -1574,10 +1678,8 @@ mc_status chain_check(mc_handle* h, const Source& s, int frames, const mc_params
                       mc_chain_info* info, ChainGeom& g, bool out_optional = false) {
     if (!p || !info) { h->err = "params or info is null"; return MC_ERR_INVALID; }
     const bool empty = s.empty();
-    if (const char* e = chain_geometry(p, empty ? 0 : s.w, empty ? 0 : s.hh, s.channels, grayscale, g, info)) {
-        h->err = e;
-        return MC_ERR_INVALID;
-    }
+    mc_status st = chain_lane_geometry(h, p, empty ? 0 : s.w, empty ? 0 : s.hh, s.channels, grayscale, g, info);
+    if (st != MC_OK) return st;
     const bool pre = g.pre || s.converts(), front = g.front() || s.converts();
     const size_t lanes = (size_t)h->lanes, vl = (size_t)frames * lanes;
     if (s.converts()) {   // info says where the conversion went; the frame's errors come before the canvas's
@@ -1655,6 +1757,13 @@ mc_status chain_run(mc_handle* h, const ChainGeom& g, const Source& s, int frame
             a.gray = h->f_gray.p;
         }
         if (g.kind == FRONT_AREA && (st = area_tables(h, g, a)) != MC_OK) return st;
+        if (!g.org.empty()) {   // the lanes' own crop origins go up on the handle's stream, as the held-lane flags do
+            h->f_org_host.resize(vl);   // lives on the handle: the copy is asynchronous
+            for (size_t v = 0; v < vl; ++v) h->f_org_host[v] = g.org[v % lanes];
+            CK(h->f_org.grow(vl));
+            CK(cudaMemcpyAsync(h->f_org.p, h->f_org_host.data(), vl * sizeof(int2), cudaMemcpyHostToDevice, h->stream));
+            a.org = h->f_org.p;
+        }
         if (std::any_of(h->hold.begin(), h->hold.end(), [](uint8_t x) { return x != 0; })) {
             h->f_flags_host.resize(vl);   // lives on the handle: the copy is asynchronous
             for (size_t v = 0; v < vl; ++v) h->f_flags_host[v] = !h->hold[v % lanes];
@@ -1949,16 +2058,14 @@ mc_status chain_host_call(mc_handle* h, const char* name, const Source& s, const
     if (s.missing) { h->err = s.missing; return MC_ERR_INVALID; }
     ChainGeom g;
     const bool empty = s.empty();
-    if (const char* e = chain_geometry(p, empty ? 0 : s.w, empty ? 0 : s.hh, s.channels, grayscale, g, info)) {
-        h->err = e;
-        return MC_ERR_INVALID;
-    }
+    mc_status st = chain_lane_geometry(h, p, empty ? 0 : s.w, empty ? 0 : s.hh, s.channels, grayscale, g, info);
+    if (st != MC_OK) return st;
     const size_t out_frame = (size_t)g.dw * g.dh * g.cc, orig_frame = (size_t)g.dw * g.dh * s.channels;
     const bool out_fits = out && out_bytes >= out_frame, orig_fits = original && original_bytes >= orig_frame;
     if (s.converts() && out && !out_fits) { h->err = "out buffer too small"; return MC_ERR_INVALID; }
     if (s.converts() && original && !orig_fits) { h->err = "original buffer too small"; return MC_ERR_INVALID; }
     const ChainDst tight{out_fits ? out : nullptr, (size_t)g.dw * g.cc, orig_fits ? original : nullptr, (size_t)g.dw * s.channels};
-    mc_status st = chain_submit(h, s, p, grayscale, tight, info, true);
+    st = chain_submit(h, s, p, grayscale, tight, info, true);
     if (st != MC_OK) return st;
     int produced = 0;
     if ((st = mc_collect(h, &produced)) != MC_OK) return st;

@@ -179,6 +179,7 @@ struct FrontArgs {
     int cstep = kNv12ChromaStep;
     size_t step = 0, lane_stride = 0;   // row pitch and virtual-lane stride of the source (the same for every plane)
     int rx = 0, ry = 0;             // ROI origin in the source
+    const int2* org = nullptr;      // per virtual lane: its own ROI origin (mc_set_lane_roi) in place of rx / ry; or null
     int dw = 0, dh = 0;             // output size
     int kind = FRONT_COPY, isx = 1, isy = 1;
     const AreaTap* xtab = nullptr; const int* xofs = nullptr; const AreaTap* ytab = nullptr; const int* yofs = nullptr;

@@ -411,6 +411,8 @@ struct RieszMode {
         bool finite() const { return !std::isnan(loA[0]) && !std::isnan(hiA[0]); }
     };
     std::vector<Design> design;
+    // lane k's next frame makes its design afresh at its params' framerate, as a structural reset of the handle would
+    void redesign(int k) { if ((size_t)k < design.size()) design[(size_t)k].loA[0] = NAN; }
     std::vector<RieszLane> rows, rows_dev;   // this frame's per-lane table and the contents of its device copy
     RieszLane* d_rows = nullptr;
     std::vector<uint8_t> lane_ops;           // the handle's ops with lanes of a non-finite design turned FIRST

@@ -79,27 +79,32 @@ __device__ __forceinline__ void front_walk(const FrontArgs& a, const Px& px, int
 }
 
 // One thread per output pixel of one virtual lane (blockIdx.z): every channel of the preprocessed pixel and its gray
-// byte from one walk over the pixel's source taps.
+// byte from one walk over the pixel's source taps.  The per-lane origins cost registers: every instance but the BGR one
+// is held to 32 (8 CTAs per SM, as before them) with no spills (-Xptxas -v).  The BGR instance spills under any bound
+// and runs unbounded at 40, which allocates as the 34 it used before them did (6 CTAs per SM).
 template <int SRC>
-__global__ void __launch_bounds__(256) k_chain_front(const FrontArgs a) {
+__global__ void __launch_bounds__(256, SRC == FRONT_BGR ? 0 : 8) k_chain_front(const FrontArgs a) {
     constexpr int CN = SRC == FRONT_GRAY ? 1 : 3;
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
     const size_t v = blockIdx.z;
     if (x >= a.dw || (a.flags && !a.flags[v])) return;
+    // the lane's crop origin: every lane's rectangle has the size dw x dh maps from, so the tap tables are shared
+    const int2 org = a.org ? a.org[v] : make_int2(a.rx, a.ry);
+    const int rx = org.x, ry = org.y;
     int o[CN];
     if constexpr (SRC == FRONT_NV12) {   // one uniform branch on the chroma layout
         const size_t l = v * a.lane_stride;
-        if (a.cstep == kNv12ChromaStep) front_walk(a, FrontPx<SRC>{a.src + l, a.cb + l, a.step, a.rx, a.ry}, x, y, o);
-        else front_walk(a, I420Px{a.src + l, a.cb + l, a.cr + l, a.step, a.cpitch, a.rx, a.ry}, x, y, o);
+        if (a.cstep == kNv12ChromaStep) front_walk(a, FrontPx<SRC>{a.src + l, a.cb + l, a.step, rx, ry}, x, y, o);
+        else front_walk(a, I420Px{a.src + l, a.cb + l, a.cr + l, a.step, a.cpitch, rx, ry}, x, y, o);
     } else if constexpr (SRC == FRONT_YUYV || SRC == FRONT_UYVY) {
         FrontPx<SRC> px;
-        px.p = a.src + v * a.lane_stride + (size_t)a.ry * a.step; px.pitch = a.step; px.ox = a.rx; px.vec = a.vec != 0;
+        px.p = a.src + v * a.lane_stride + (size_t)ry * a.step; px.pitch = a.step; px.ox = rx; px.vec = a.vec != 0;
         front_walk(a, px, x, y, o);
     } else if constexpr (SRC == FRONT_BGR) {   // BGR and every RGB layout: three channel bases
-        const size_t l = v * a.lane_stride + (size_t)a.ry * a.step + (size_t)a.rx * a.cstep;
+        const size_t l = v * a.lane_stride + (size_t)ry * a.step + (size_t)rx * a.cstep;
         front_walk(a, RgbPx{a.src + l, a.cb + l, a.cr + l, a.step, a.cstep}, x, y, o);
     } else {
-        front_walk(a, FrontPx<SRC>{a.src + v * a.lane_stride + (size_t)a.ry * a.step + (size_t)CN * a.rx, a.step}, x, y, o);
+        front_walk(a, FrontPx<SRC>{a.src + v * a.lane_stride + (size_t)ry * a.step + (size_t)CN * rx, a.step}, x, y, o);
     }
     if (a.dst) {
         uint8_t* d = a.dst + v * a.dst_lane_stride + (size_t)y * a.dst_step + (size_t)CN * x;

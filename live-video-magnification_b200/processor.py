@@ -15,7 +15,7 @@ import collections
 import ctypes as C
 import enum
 from dataclasses import dataclass, field, replace
-from typing import Optional
+from typing import Optional, Tuple
 
 import numpy as np
 
@@ -187,6 +187,16 @@ class MagnificationProcessor(IProcessor):
             lp = C.byref(capi.McLaneParams(float(params.amplification), float(params.coWavelength), float(params.coLow),
                                            float(params.coHigh), float(params.chromAttenuation), float(params.framerate)))
         self._check(self._lib.mc_set_lane_params(self._h, int(lane), lp))
+
+    def set_lane_roi(self, lane: int, roi: Optional[Tuple[float, float, float, float]]) -> None:
+        """From the next frame call or submit on, `lane` crops its frames at the normalised ROI `roi` = (x, y, w, h) in
+        place of the call's (mc_set_lane_roi); pre_roiEnabled, downscale, grayscale, mode and levels still come from the
+        call, and every lane that runs must crop a rectangle of one pixel size.  A lane whose ROI moves restarts alone.
+        None: the lane follows the call's ROI again.  An override survives reset()."""
+        if roi is not None and len(roi) != 4:
+            raise ValueError(f"roi must be (x, y, w, h), got {len(roi)} values")
+        r = None if roi is None else (C.c_float * 4)(*(float(v) for v in roi))
+        self._check(self._lib.mc_set_lane_roi(self._h, int(lane), r))
 
     def save_lane(self, lane: int) -> bytes:
         """The lane's temporal state as an opaque blob (mc_save_lane), for load_lane on any lane of any processor."""
@@ -474,6 +484,10 @@ class ProcessingChainB200:
     def set_lane_params(self, lane: int, params: Optional[MagnificationParams]) -> None:
         """MagnificationProcessor.set_lane_params of the chain's magnifier."""
         self.magnifier.set_lane_params(lane, params)
+
+    def set_lane_roi(self, lane: int, roi: Optional[Tuple[float, float, float, float]]) -> None:
+        """MagnificationProcessor.set_lane_roi: lane `lane` crops at its own ROI (x, y, w, h), or the call's with None."""
+        self.magnifier.set_lane_roi(lane, roi)
 
     def save_lane(self, lane: int) -> bytes:
         """MagnificationProcessor.save_lane of the chain's magnifier (the front stages have no state)."""
